@@ -1,10 +1,10 @@
 # Build everything in-tree (the .so files travel to the GPU box with the snapshot; they are git-ignored).
 #   make            -> product library, host library, oracle
-#   make product    -> deep-prove_b200/libdeepprove_b200.so      (CUDA kernels + C ABI, sm_100a only)
+#   make product    -> deep-prove_b200/libdeepprove_b200.so      (CUDA kernels + C ABI, sm_90a only)
 #   make oracle     -> oracle/libdp_oracle.so                     (CPU restatement: TEST INFRASTRUCTURE)
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -Xptxas -v
 PKG       := deep-prove_b200
 CSRC      := $(PKG)/csrc

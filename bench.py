@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
-"""bench.py -- one JSON line per run (contract in the task statement).
+"""bench.py -- one JSON line per run.
 
 A "step" is one pass of the hot path over one batch of synthetic input.  The headline workload (--workload, default
 dense4m) fills the contract's top-level keys; the other BASELINE.json workloads are measured in the same run and reported
-under "workloads" so ONE driver invocation carries all of them:
+under "workloads" so ONE invocation carries all of them:
   dense4m     BASELINE.json configs[1]: full zkml proof (Prover::prove: witness commits, LogUp-GKR lookups, per-layer
               sumchecks, table proofs, Basefold batch opening; host Poseidon2 Fiat-Shamir) of the Dense-4M MLP of SURVEY.md
               8(d) Cfg 2 -- 4 x [Dense 1024x1024 + bias -> Requant -> ReLU], BIT_LEN 8.  Context::generate (weight commits)
@@ -12,15 +12,18 @@ under "workloads" so ONE driver invocation carries all of them:
   sumcheck20  configs[0] shape: IOPProverState::prove_parallel, nu=20, degree 3, three Base MLEs -> proofs/s, field-ops/s
               and achieved GB/s against the measured HBM peak.
   basefold24  configs[3] on one GPU: Basefold commit+open of 2^24 Base evaluations -> openings/s and Poseidon2
-              permutations/s against the INT32-issue ceiling.
+              permutations/s.
 `value`  : units/s with everything the step reads already resident in HBM; `e2e`: through the host-facing call with HOST
            buffers (inference + witness upload + prove + proof back for the models; upload + prove otherwise).
 `roofline`: per-kernel table taken from a profiled pass of the SAME concurrent batch (per-launch CUDA events on every proving
-           thread's stream), each kernel against the bound that actually limits it (HBM bytes or INT32 issue slots).
+           thread's stream), each kernel against the HBM bound; Poseidon2 kernels as permutations/s (no measured ceiling).
 `cpu_baseline` / `--impl reference`: the CPU path (the C++ oracle port -- the reference itself is Rust with un-vendored
-           dependencies and cannot be built here, DESIGN.md section 3) in latency mode (1 proof x all host threads) AND in
+           dependencies and is not built, DESIGN.md section 3) in latency mode (1 proof x all host threads) AND in
            throughput mode (k concurrent proofs x T/k threads); the better of the two is the value.
 `parity_checked`: the GPU proof and the CPU-arm proof of the same input compared word for word outside the timed region.
+`--dump-outputs DIR`: what the headline workload's last timed step returned (the proof, or the sumcheck messages), one DIR/<name>.npy
+           per array, every u64 word as an exact float64 pair [low 32 bits, high 32 bits]; the inputs are seeded, so two builds can
+           be compared output for output.
 """
 import os
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")   # before torch/CUDA initialise: 16 proof streams + commit pools need more than 8 hardware queues
@@ -117,7 +120,7 @@ class SumcheckWorkload:
     metric, unit = "proofs/sec", "proofs/s"
     name = "sumcheck prove_parallel nu=20 deg=3 3xBase (BASELINE configs[0] shape), host Poseidon2 FS"
     NV = 20
-    NSETS = 8   # 8 x 24 MiB = 192 MiB of inputs > 126 MB L2: a set is evicted before it is reused
+    NSETS = 8   # 8 x 24 MiB = 192 MiB of inputs > 50 MB L2: a set is evicted before it is reused
     units_per_step = 1
     cpu_frac = 1.0
 
@@ -149,6 +152,10 @@ class SumcheckWorkload:
         for m in ms:
             m.free()
         return out
+
+    def outputs(self, last):
+        point, msgs, fin = last
+        return {"point": point, "round_messages": msgs, "final_evals": fin}
 
     def cpu_step(self, O, i):
         mles = [(a, False) for a in self.host_sets[i % self.NSETS]]
@@ -195,7 +202,11 @@ class BasefoldWorkload:
         self.d2h = int(flat.size * 8)
 
     def step_resident(self, i):
-        self.dp.pcs_open(self.mle, self.NV, self.point, cap=1 << 23)
+        return self.dp.pcs_open(self.mle, self.NV, self.point, cap=1 << 23)
+
+    def outputs(self, last):
+        root, flat = last
+        return {"root": root, "proof": flat}
 
     def step_e2e(self, i):
         m = self.dp.Mle.upload(self.evals, False)
@@ -275,11 +286,14 @@ class DenseWorkload:
     def step_e2e(self, i):
         return self.ctx.prove(self.x)
 
-    def run_resident(self, k, device):
-        self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=False)
+    def run_resident(self, k, device, keep_last=False):
+        return self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=False, want_proof=keep_last)
 
-    def run_e2e(self, k, device):
-        self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=True)
+    def run_e2e(self, k, device, keep_last=False):
+        return self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=True, want_proof=keep_last)
+
+    def outputs(self, last):
+        return {"proof": last[1]}
 
     def cpu_step(self, O, i):
         _, ms = O.zkml_prove(self.NL, self.W, self.SEED_MODEL, self.SEED_INPUT, want_proof=False)
@@ -294,7 +308,7 @@ class DenseWorkload:
     cpu_sample = "full proofs of the same model and input (Context::generate not counted)"
     cpu_returns_seconds = True
     l2_note = ("%d proofs in flight per GPU: aggregate working set (~130 MB of weights/codewords/oracles/trees per proof) "
-               "is >> the 126 MB L2; single-stream latency is measured with a 256 MiB L2 flush between proofs" % STREAMS)
+               "is >> the 50 MB L2; single-stream latency is measured with a 256 MiB L2 flush between proofs" % STREAMS)
     flush = True
 
 
@@ -335,11 +349,14 @@ class CnnWorkload:
     def step_e2e(self, i):
         return self.ctx.prove(self.x)
 
-    def run_resident(self, k, device):
-        self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=False)
+    def run_resident(self, k, device, keep_last=False):
+        return self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=False, want_proof=keep_last)
 
-    def run_e2e(self, k, device):
-        self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=True)
+    def run_e2e(self, k, device, keep_last=False):
+        return self.ctx.prove_concurrent(host_workers(self.STREAMS), k * self.units_per_step, device=device, e2e=True, want_proof=keep_last)
+
+    def outputs(self, last):
+        return {"proof": last[1]}
 
     def cpu_step(self, O, i):
         _, ms = O.model_prove(self.desc, self.data, self.x, want_proof=False)
@@ -353,7 +370,7 @@ class CnnWorkload:
 
     cpu_sample = "full proofs of the same model and input (Context::generate not counted)"
     cpu_returns_seconds = True
-    l2_note = ("%d proofs in flight per GPU (aggregate working set >> the 126 MB L2); single-stream latency is measured with a 256 MiB L2 flush between proofs" % STREAMS)
+    l2_note = ("%d proofs in flight per GPU (aggregate working set >> the 50 MB L2); single-stream latency is measured with a 256 MiB L2 flush between proofs" % STREAMS)
     flush = True
 
 
@@ -414,7 +431,7 @@ def load_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "sm_max_mhz": 1965.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "sm_max_mhz": 1980.0}, "H100 SXM data sheet (not measured)"
 
 
 def max_over_ranks(ms, dist, device="cuda"):
@@ -487,37 +504,15 @@ def cpu_arm(wl, O, steps, warm):
             "sample": wl.cpu_sample + " (C++ restatement of the reference algorithm, not the Rust reference; `cores` = threads used = the CPUs this container may run on: min(hardware threads, cgroup cpu.max))"}
 
 
-# ---- facts taken from the committed ncu captures (profiles/ncu_facts.json, written next to the capture summaries) ----
-# The Poseidon2 kernels are bound by the FMA-heavy pipe that executes the 32 x 32 -> 64-bit multiplies (IMAD.WIDE) of the Goldilocks
-# products: ncu (profiles/r02d_ncu_full_k_merkle_up.csv) shows sm__pipe_fmaheavy_cycles_active = 90.65 % at 1.69 Gperm/s, i.e. a
-# ceiling of 1.865 Gperm/s per B200 at 1965 MHz for this formulation (12.85 k thread instructions per permutation).
-P2_INSTR_PER_PERM = 12850.0
-P2_CEILING_GPS, P2_CEILING_MHZ = 1.865, 1965.0
-P2_CEILING_SOURCE = "profiles/r02d_ncu_full_k_merkle_up.csv"
-NCU_TRAFFIC = {
-    ("sumcheck20", "k_sc_round"): (7.69e6, "profiles/r01c_sumcheck20_rounds_ncu.csv: rounds 2-11 of one nu=20 proof, mean per launch (algorithmic 6.6 MB)"),
-    ("dense4m", "k_sc_round"): (7.1e4, "profiles/r01_ncu_full_summary.csv: one small round (latency-bound)"),
-}
-try:
-    _f = json.load(open(os.path.join(ROOT, "profiles", "ncu_facts.json")))
-    P2_INSTR_PER_PERM = float(_f.get("p2_instr_per_perm", P2_INSTR_PER_PERM))
-    P2_CEILING_GPS = float(_f.get("p2_perm_ceiling_gps_at_1965mhz", P2_CEILING_GPS))
-    for k_, v_ in _f.get("traffic", {}).items():
-        NCU_TRAFFIC[tuple(k_.split("/"))] = (v_[0], v_[1])
-except Exception:
-    pass
-
 # BASELINE.md section 1: "Dense 4M proving time 2335 ms" (README.md:18; hardware and exact architecture NOT stated)
 PUBLISHED = {"dense4m": 1.0 / 2.335, "cnn264k": 1.0 / 1.242}   # and "CNN 264k ... proving time 1242 ms" (README.md:17)
 
 
-def kernel_table(prof, peaks, sm_mhz, sm_count=148):
+def kernel_table(prof, peaks):
     """per-kernel rows from dp_profile_read_ex: each kernel against the bound that limits it.
-    Poseidon2 kernels: permutations/s against the FMA-heavy-pipe ceiling measured with ncu (scaled by the SM clock and count);
-    sumcheck rounds: field-ops/s and GB/s against the measured HBM copy bandwidth; everything else: GB/s vs HBM.
+    Poseidon2 kernels: permutations/s (their integer-multiply ceiling has not been measured on H100, so no fraction is given);
+    sumcheck rounds: field-ops/s and GB/s against the HBM bandwidth; everything else: GB/s vs HBM.
     Kernels that process a handful of elements per launch are latency chains and are labelled so (no roofline applies)."""
-    clock = (sm_mhz or peaks.get("sm_max_mhz") or 1965.0)
-    perm_ceiling = P2_CEILING_GPS * 1e9 * (clock / P2_CEILING_MHZ) * (sm_count / 148.0)
     rows = {}
     for name, (cnt, ms, by, units) in prof.items():
         sec = ms * 1e-3
@@ -526,18 +521,18 @@ def kernel_table(prof, peaks, sm_mhz, sm_count=148):
                "hbm_frac": round(by / sec / 1e9 / peaks["hbm_gbs"], 5) if sec > 0 else 0.0}
         if "poseidon2" in name:
             pps = units / sec if sec > 0 else 0.0
-            row.update({"bound": "fma-heavy pipe (IMAD.WIDE of the 64-bit field products)" if cnt and units / cnt > 60000 else "latency (dependent hash chain)",
-                        "perm_per_s": pps, "ceiling_perm_per_s": perm_ceiling, "pipe_frac": round(pps / perm_ceiling, 5)})
+            row.update({"bound": "integer multiplies (IMAD.WIDE of the 64-bit field products)" if cnt and units / cnt > 60000 else "latency (dependent hash chain)",
+                        "perm_per_s": pps})
         elif name.startswith("k_sc_"):
             row.update({"bound": "hbm" if cnt and by / cnt > 4e6 else "latency (one round trip per Fiat-Shamir challenge)",
                         "field_ops_per_s": units / sec if sec > 0 else 0.0})
         else:
             row["bound"] = "hbm" if cnt and by / cnt > 4e6 else "latency"
         rows[name] = row
-    return rows, perm_ceiling
+    return rows
 
 
-def roofline_block(wl_key, rows, ceiling, peaks, peak_kind, source):
+def roofline_block(rows, peaks, peak_kind, source):
     """the dominant THROUGHPUT-bound kernel of a per-kernel table against its own bound (latency chains are listed, not rated)"""
     cand = {k: r for k, r in rows.items() if not k.startswith("k_sc_res") and not r["bound"].startswith("latency")}
     if not cand:
@@ -545,22 +540,21 @@ def roofline_block(wl_key, rows, ceiling, peaks, peak_kind, source):
     name = max(cand, key=lambda k: cand[k]["ms"])
     r = rows[name]
     all_ms = sum(x["ms"] for k, x in rows.items() if not k.startswith("k_sc_res"))
-    traffic = NCU_TRAFFIC.get((wl_key, name.split("(")[0]))
     if "perm_per_s" in r and not r["bound"].startswith("latency"):
-        roof = {"kernel": name, "bound": r["bound"], "achieved": r["perm_per_s"] / 1e9, "peak": ceiling / 1e9, "unit": "Gperm/s", "frac": r["pipe_frac"],
-                "peak_kind": "measured with ncu: the thread-per-hash level kernel reaches 1.69 Gperm/s at sm__pipe_fmaheavy_cycles_active = 90.65 %% (%s); scaled by SM clock" % P2_CEILING_SOURCE}
+        roof = {"kernel": name, "bound": r["bound"], "achieved": r["perm_per_s"] / 1e9, "peak": None, "unit": "Gperm/s", "frac": None,
+                "peak_kind": "not measured on H100"}
     else:
         roof = {"kernel": name, "bound": r["bound"], "achieved": r["GBps"], "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": r["hbm_frac"],
-                "peak_kind": peak_kind + " (MEASURED_PEAKS.json hbm_gbs)"}
+                "peak_kind": peak_kind}
     roof.update({"hbm": {"achieved": r["GBps"], "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": r["hbm_frac"]},
-                 "traffic": traffic[0] if traffic else None, "traffic_source": traffic[1] if traffic else None,
                  "launches": r["launches"], "avg_us": r["avg_us"], "share_of_kernel_time": round(r["ms"] / all_ms, 4) if all_ms > 0 else None,
                  "source": source})
     return roof
 
 
-def run_gpu_workload(env, wl, K, W, full):
-    """time one workload on this rank's GPU; returns the result dict (rank 0 fills the CPU / parity parts when world == 1)"""
+def run_gpu_workload(env, wl, K, W, full, keep_last=False):
+    """time one workload on this rank's GPU; returns the result dict (rank 0 fills the CPU / parity parts when world == 1).
+    wl.last_output: what the last timed step returned (for the batched workloads only with keep_last)"""
     torch, dp, dist = env["torch"], env["dp"], env["dist"]
     rank, world, local_rank = env["rank"], env["world"], env["local_rank"]
     wl.setup_device(dp)
@@ -579,20 +573,21 @@ def run_gpu_workload(env, wl, K, W, full):
         barrier()
         l0 = dp.lib().dp_kernel_launches()
         evs = []
+        last = None
         for i in range(steps):
             if flush_buf is not None:
                 flush_buf.zero_()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            fn(warm + i)
+            last = fn(warm + i)
             e1.record()
             evs.append((e0, e1))
         barrier()
         ms = sum(a.elapsed_time(b) for a, b in evs)
         launches = dp.lib().dp_kernel_launches() - l0
-        return max_over_ranks(ms, dist), launches
+        return max_over_ranks(ms, dist), launches, last
 
-    def timed_many(run, steps, warm):
+    def timed_many(run, steps, warm, keep_last=False):
         """K steps issued as one batch (concurrent proof streams): bracketed by CUDA events recorded on the main stream
         with barrier + synchronize on both sides (the worker streams are drained before the call returns)"""
         if warm:
@@ -601,10 +596,10 @@ def run_gpu_workload(env, wl, K, W, full):
         l0 = dp.lib().dp_kernel_launches()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        run(steps, local_rank)
+        last = run(steps, local_rank, keep_last)
         e1.record()
         barrier()
-        return max_over_ranks(e0.elapsed_time(e1), dist), dp.lib().dp_kernel_launches() - l0
+        return max_over_ranks(e0.elapsed_time(e1), dist), dp.lib().dp_kernel_launches() - l0, last
 
     batched = hasattr(wl, "run_resident")
     latency_ms = None
@@ -612,17 +607,17 @@ def run_gpu_workload(env, wl, K, W, full):
     if batched:
         dp.set_wait_mode(1)      # many proofs in flight: proving threads sleep on the library's poller instead of spinning (DESIGN.md section 5)
         with clk:
-            ms, launches = timed_many(wl.run_resident, K, W)
-        ms_e2e, _ = timed_many(wl.run_e2e, K, 1)
+            ms, launches, wl.last_output = timed_many(wl.run_resident, K, W, keep_last)
+        ms_e2e, _, _ = timed_many(wl.run_e2e, K, 1)
         if full:
             dp.set_wait_mode(0)  # one proof at a time: the single proving thread spins (lowest latency)
-            lat, _ = timed(wl.step_resident, min(K, 10), 2)     # one proof at a time, L2 flushed between proofs
+            lat, _, _ = timed(wl.step_resident, min(K, 10), 2)     # one proof at a time, L2 flushed between proofs
             latency_ms = lat / min(K, 10)
             dp.set_wait_mode(1)
     else:
         with clk:
-            ms, launches = timed(wl.step_resident, K, W)
-        ms_e2e, _ = timed(wl.step_e2e, K, 2)
+            ms, launches, wl.last_output = timed(wl.step_resident, K, W)
+        ms_e2e, _, _ = timed(wl.step_e2e, K, 2)
     clocks = clk.summary()
 
     # per-kernel legs.  (1) the SAME concurrent batch once more with per-launch CUDA events on every proving thread's stream: what runs
@@ -641,7 +636,7 @@ def run_gpu_workload(env, wl, K, W, full):
     prof = dp.profile_read(with_units=True)
     dp.profile_enable(False)
     dp.set_wait_mode(0)
-    rows, ceiling = kernel_table(prof, peaks, clocks.get("sm_mhz"), env["sm_count"])
+    rows = kernel_table(prof, peaks)
     rows_alone = None
     if batched:
         dp.profile_reset(); dp.profile_enable(True)
@@ -650,7 +645,7 @@ def run_gpu_workload(env, wl, K, W, full):
                 flush_buf.zero_()
             wl.step_resident(i)
         torch.cuda.synchronize()
-        rows_alone, _ = kernel_table(dp.profile_read(with_units=True), peaks, clocks.get("sm_mhz"), env["sm_count"])
+        rows_alone = kernel_table(dp.profile_read(with_units=True), peaks)
         dp.profile_enable(False)
 
     ups = getattr(wl, "units_per_step", 1)
@@ -664,23 +659,22 @@ def run_gpu_workload(env, wl, K, W, full):
         res["hbm_frac_whole_proof"] = wl.alg_bytes * v / world / 1e9 / peaks["hbm_gbs"]
     if hasattr(wl, "permutations"):
         res["poseidon2_perm_per_s"] = wl.permutations * v / world
-        res["pipe_frac_whole_step"] = wl.permutations * v / world / ceiling
 
     roof = None
     if rows:
         if batched and rows_alone:
-            roof = roofline_block(wl.key, rows_alone, ceiling, peaks, peak_kind, "profiled pass of single proofs (each kernel alone on the GPU, per-launch CUDA events on the launch stream)")
-            # the whole timed region against the same ceiling: Poseidon2 permutations of all Merkle kernels per second of the batch
+            roof = roofline_block(rows_alone, peaks, peak_kind, "profiled pass of single proofs (each kernel alone on the GPU, per-launch CUDA events on the launch stream)")
+            # the whole timed region: Poseidon2 permutations of all Merkle kernels per second of the batch
             perms = sum(u for n_, (c_, m_, b_, u) in prof.items() if "poseidon2" in n_)
             proofs_profiled = min(K, 2) * ups
             if proofs_profiled:
                 pps = perms / proofs_profiled * v / world
-                roof["whole_step"] = {"poseidon2_perm_per_proof": perms / proofs_profiled, "poseidon2_perm_per_s": pps, "frac_of_pipe_ceiling": round(pps / ceiling, 4),
-                                      "note": "all Merkle kernels of the concurrent timed region: permutations per proof x proofs/s, against the same fma-heavy-pipe ceiling"}
+                roof["whole_step"] = {"poseidon2_perm_per_proof": perms / proofs_profiled, "poseidon2_perm_per_s": pps,
+                                      "note": "all Merkle kernels of the concurrent timed region: permutations per proof x proofs/s"}
             roof["kernels_concurrent_batch"] = dict(sorted(rows.items(), key=lambda kv: -kv[1]["ms"]))
             roof["kernels"] = dict(sorted(rows_alone.items(), key=lambda kv: -kv[1]["ms"]))
         else:
-            roof = roofline_block(wl.key, rows, ceiling, peaks, peak_kind, "profiled pass of the same steps (per-launch CUDA events on the launch stream)")
+            roof = roofline_block(rows, peaks, peak_kind, "profiled pass of the same steps (per-launch CUDA events on the launch stream)")
             roof["kernels"] = dict(sorted(rows.items(), key=lambda kv: -kv[1]["ms"]))
     res["roofline"] = roof
 
@@ -790,6 +784,22 @@ def sharded_basefold(env, nv=24, reps=3):
             "poseidon2_perm_per_s_aggregate": 4.0 * (1 << nv) / (ms * 1e-3)}
 
 
+DUMP_LIMIT_BYTES = 60 << 20     # with the .npy headers, under 64 MB in all
+
+
+def dump_outputs(path, arrays):
+    """u64 words -> float64 pairs [low 32 bits, high 32 bits] (exact), DIR/<name>.npy per array; when the whole would exceed
+    DUMP_LIMIT_BYTES, each array keeps a fixed, seeded sample of its words"""
+    os.makedirs(path, exist_ok=True)
+    words = {name: np.ascontiguousarray(a, dtype=np.uint64).reshape(-1) for name, a in arrays.items()}
+    total = 16 * sum(w.size for w in words.values())
+    rng = np.random.default_rng(0)
+    for name, w in words.items():
+        if total > DUMP_LIMIT_BYTES:
+            w = w[np.sort(rng.choice(w.size, max(1, w.size * DUMP_LIMIT_BYTES // total), replace=False))]
+        np.save(os.path.join(path, name + ".npy"), np.stack([w & np.uint64(0xFFFFFFFF), w >> np.uint64(32)], axis=-1).astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -799,7 +809,11 @@ def main():
     ap.add_argument("--workload", default="dense4m", choices=list(WORKLOADS))
     ap.add_argument("--only", action="store_true", help="measure only --workload (skip the other BASELINE workloads)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step of --workload computed to DIR/<name>.npy (float64, under 64 MB in all)")
     args = ap.parse_args()
+    if args.steps is not None and args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -843,12 +857,13 @@ def main():
     dp.init(local_rank)
     dp.use_torch_stream()
     env = {"torch": torch, "dp": dp, "dist": dist, "rank": rank, "world": world, "local_rank": local_rank, "peaks": load_peaks(),
-           "flush_buf": torch.empty(256 << 20, dtype=torch.uint8, device="cuda"), "no_cpu": args.no_cpu_baseline,
-           "sm_count": torch.cuda.get_device_properties(local_rank).multi_processor_count}
+           "flush_buf": torch.empty(256 << 20, dtype=torch.uint8, device="cuda"), "no_cpu": args.no_cpu_baseline}
 
     wl = WORKLOADS[args.workload]()
     K = args.steps if args.steps is not None else {"dense4m": 6, "cnn264k": 6, "sumcheck20": 20, "basefold24": 5}[args.workload]
-    head = run_gpu_workload(env, wl, K, max(W, 3), True)
+    head = run_gpu_workload(env, wl, K, max(W, 3), True, keep_last=args.dump_outputs is not None)
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(args.dump_outputs, wl.outputs(wl.last_output))
     extra = {}
     for k in others:
         if world > 1 and k in ("sumcheck20", "basefold24"):
@@ -893,7 +908,7 @@ def main():
             "alg_GBps_whole_step": head["alg_GBps_whole_step"],
             "workloads": extra, "sharded": sharded,
         }
-        for k in ("field_ops_per_s", "hbm_frac_whole_proof", "poseidon2_perm_per_s", "pipe_frac_whole_step", "parity_error"):
+        for k in ("field_ops_per_s", "hbm_frac_whole_proof", "poseidon2_perm_per_s", "parity_error"):
             if k in head:
                 out[k] = head[k]
         print(json.dumps(out))

@@ -11,7 +11,7 @@
 struct DpCtx {
     bool ready = false;
     int device = -1;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     cudaMemPool_t pool = nullptr;       // this thread's stream-ordered pool (no cross-stream reuse dependencies)

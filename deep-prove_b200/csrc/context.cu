@@ -102,7 +102,7 @@ static void arena_destroy() {
 // in a PER-THREAD cache (no lock, O(1)); a process-wide pool takes the caches of threads that exit and serves cache misses before the
 // driver is asked (cudaHostAlloc costs ~ms and synchronises the device: never on the proving path once warm).  The first version
 // kept one process-wide list under a mutex and scanned it linearly on every alloc and free: with 48 proving threads and thousands
-// of blocks that was 18 ms of CPU per Dense-4M proof inside dp_sc_create / dp_sc_destroy (profiles/r03a_hostprof.log).
+// of blocks that made dp_sc_create / dp_sc_destroy a large share of a Dense-4M proof's host CPU time.
 static constexpr int PIN_CLASSES = 40;
 struct PinnedPool { std::mutex mu; std::vector<void *> free_[PIN_CLASSES]; };
 static PinnedPool g_pin_pool;
@@ -388,7 +388,7 @@ int dp_profile_read_ex(char (*names)[64], uint64_t *counts, double *total_ms, ui
 int dp_profile_read(char (*names)[64], uint64_t *counts, double *total_ms, uint64_t *bytes, int cap) { return dp_profile_read_ex(names, counts, total_ms, bytes, nullptr, cap); }
 
 const char *dp_last_error(void) { return g_err.c_str(); }
-const char *dp_version(void) { return "deepprove_b200 0.1 (sm_100a)"; }
+const char *dp_version(void) { return "deepprove_b200 0.1 (sm_90a)"; }
 
 int dp_device_count(void) {
     int n = 0;

@@ -1,4 +1,4 @@
-// Goldilocks F = Z/(2^64 - 2^32 + 1) and E = F[X]/(X^2 - 7) for sm_100a device code (and host code
+// Goldilocks F = Z/(2^64 - 2^32 + 1) and E = F[X]/(X^2 - 7) for sm_90a device code (and host code
 // inside the library, for the O(degree)-sized per-round glue).
 // Reference semantics: ff_ext/src/lib.rs:7,13 (p3 Goldilocks / BinomialExtensionField<_,2>, W = 7).
 // All values are canonical (< p) in memory and in registers between operations; E is AoS {c0,c1} so a

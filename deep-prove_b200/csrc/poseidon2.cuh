@@ -167,8 +167,8 @@ __device__ __forceinline__ u64 p2x8_permute(u64 s, int lane8) {
 #pragma unroll 1
     for (int r = 0; r < 4; r++) { s = p2_pow7(w_add_canon(s, c_p2_ext[0][r][lane8])); s = p2x8_mds_light(s, lane8); }
     // Internal rounds: S-box on lane 0, then an 8-lane all-reduce, then the multiply-add.  (A variant that keeps the sum of words 1..7
-    // on every lane and refreshes it in the shadow of the next S-box was measured SLOWER on B200 -- 21.96 vs 20.20 us per compress,
-    // tools/kbench.cu `lat` -- the extra shuffles it issues ahead of the S-box cost more than the all-reduce latency they hide.)
+    // on every lane and refreshes it in the shadow of the next S-box was measured slower per compress with
+    // tools/kbench.cu `lat`: the extra shuffles it issues ahead of the S-box cost more than the all-reduce latency they hide.)
     const u64 dg = c_p2_diag[lane8];
 #pragma unroll 1
     for (int r = 0; r < 22; r++) {

@@ -3,7 +3,7 @@
 // sumcheck_macro/src/lib.rs:46-326 (the per-pair arithmetic), multilinear_extensions/src/mle.rs:631-712
 // (fix_variables_parallel).
 //
-// B200 design: ONE launch per round for the whole VirtualPolynomial.  grid.y = product index, grid.x
+// Design: ONE launch per round for the whole VirtualPolynomial.  grid.y = product index, grid.x
 // tiles the pairs; each operand is streamed once with 16-byte loads.  From round 2 on the fold by the
 // previous challenge is fused into the same pass: a thread reads 4 consecutive elements of the old
 // table, folds them to one adjacent pair, the owning product writes the pair to the (half-size)
@@ -447,7 +447,7 @@ k_sc_lean(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc0
 // SC_RES_TIMEOUT cycles or when the host posts the abort value, and the other CTAs only ever wait on the cluster barrier.
 // Opt-in per handle (dp_sc_set_resident_tail): the caller promises not to wait on other work in the same stream between rounds.
 static constexpr u32 SC_RES_MAXM = 96, SC_RES_MAXP = 48, SC_RES_MAXCTA = 8;
-static constexpr u64 SC_RES_WORK = 2048;                     // resident once sum over products of (pairs this round) <= this (larger rounds are faster in the multi-block kernels: profiles/r02x.log)
+static constexpr u64 SC_RES_WORK = 2048;                     // resident once sum over products of (pairs this round) <= this (larger rounds are faster in the multi-block kernels; 2048 measured best of 1024 / 2048 / 4096 on H100)
 static constexpr long long SC_RES_TIMEOUT = 6000000000LL;   // ~3 s at 1.9 GHz
 static constexpr u64 SC_TAIL_ABORT = ~0ULL, SC_TAIL_FAILED = ~0ULL - 1;
 struct TMle { const void *cur; gle *work; u64 len, len0; u32 is_ext, where; };
@@ -578,8 +578,8 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
         RES_MARK(4);
         if (rank == 0) {                                       // the message first: it is what the host is waiting for
             // few partials per (product, point): one THREAD each (many products run side by side); many (a single product spread over
-            // >= 32 warps): one WARP each, its lanes gather the partials with independent L2 loads -- e3 nu=12: 237 -> 215 us per proof,
-            // while the warp form costs the 6-product LogUp shape 10 % (profiles/r03h.log)
+            // >= 32 warps): one WARP each, its lanes gather the partials with independent L2 loads -- faster for a single wide product,
+            // while the warp form slows the 6-product LogUp shape
             if (G < 32) {
                 for (u32 x = threadIdx.x; x < np * SC_NACC; x += blockDim.x) {
                     const u32 p = x / SC_NACC, t = x % SC_NACC;

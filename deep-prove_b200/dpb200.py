@@ -507,14 +507,18 @@ class ZkmlContext:
         hcheck(host().dph_zkml_prove(self.h, None, 2, label, _ptr(self._out) if want_proof else None, self._out.size, C.byref(n)))
         return self._out[: n.value].copy() if want_proof else None
 
-    def prove_concurrent(self, n_workers, n_proofs, device=0, e2e=False, label=b"m2vec"):
+    def prove_concurrent(self, n_workers, n_proofs, device=0, e2e=False, label=b"m2vec", want_proof=False):
         """n_workers persistent host threads (own stream + device arena each) prove until n_proofs are done; returns wall
-        seconds.  e2e=False: Prover::prove on the stored trace; e2e=True: inference + prove + serialised proof per job."""
+        seconds, or (seconds, flat proof of the last job handed out) when want_proof.  e2e=False: Prover::prove on the stored
+        trace; e2e=True: inference + prove + serialised proof per job."""
         H = host()
-        H.dph_zkml_prove_concurrent.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_int, C.c_char_p, C.POINTER(C.c_double)]
-        sec = C.c_double()
-        hcheck(H.dph_zkml_prove_concurrent(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec)))
-        return sec.value
+        H.dph_zkml_prove_concurrent.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_int, C.c_char_p, C.POINTER(C.c_double),
+                                                C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+        sec, n = C.c_double(), C.c_uint64()
+        out = _ptr(self._out) if want_proof else None
+        hcheck(H.dph_zkml_prove_concurrent(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
+                                           out, self._out.size, C.byref(n)))
+        return (sec.value, self._out[: n.value].copy()) if want_proof else sec.value
 
     def free(self):
         if self.h:

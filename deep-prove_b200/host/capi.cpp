@@ -207,8 +207,9 @@ namespace {
 struct ZkPool {
     std::vector<std::thread> th; std::mutex mu; std::condition_variable cv, done_cv;
     ZkHandle *h = nullptr; int device = 0; bool stop = false; uint64_t pending = 0, inflight = 0; std::string label, err; bool failed = false; bool e2e = false;
+    uint64_t *out = nullptr, out_cap = 0, *out_len = nullptr;   // when set: the flat proof of the call's last job is copied here
     // Identical proofs started together stay in lockstep: all of them sit in the latency-bound layer sumchecks (GPU nearly idle)
-    // and then all of them queue their GPU-filling opening kernels behind each other (CUPTI timeline, profiles/r02k).  So the
+    // and then all of them queue their GPU-filling opening kernels behind each other (CUPTI timeline).  So the
     // workers of one call start `stagger_s` apart (one proof duration spread over the workers; the duration is an average over the
     // proofs this pool has already run -- the first call of a pool is not staggered): latency-bound and GPU-bound phases of
     // different proofs then overlap.  The ramp-up and ramp-down this costs are inside the caller's timed region.
@@ -216,8 +217,8 @@ struct ZkPool {
     void worker(uint32_t idx) {
         bool inited = false; uint64_t seen_gen = 0;
         for (;;) {
-            uint64_t gen; double delay = 0.0;
-            { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || (pending > 0 && idx < active); }); if (stop) break; pending--; inflight++; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } }
+            uint64_t gen; double delay = 0.0; bool keep = false;
+            { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || (pending > 0 && idx < active); }); if (stop) break; pending--; inflight++; keep = pending == 0 && out; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } }
             try {
                 const bool first_ever = !inited;     // grows this thread's device arena: not a representative duration
                 if (!inited) { dp::check(dp_init(device)); inited = true; }
@@ -226,11 +227,17 @@ struct ZkPool {
                 struct timespec cts0; clock_gettime(CLOCK_THREAD_CPUTIME_ID, &cts0);
                 dp::DynTranscript t(label);
                 dp::zkml::Prover<dp::DynTranscript> prover(h->ctx, t);
+                std::vector<uint64_t> flat;
                 if (e2e) {   // from the host input vector: inference, prove, serialised proof in host memory
                     dp::zkml::Proof p = prover.prove(h->trace_input);
-                    std::vector<uint64_t> bytes = p.flatten(h->model.nodes.size());
-                    if (bytes.empty()) throw dp::Error(DP_ERR_STATE, "empty proof");
-                } else { dp::zkml::Proof p = prover.prove(h->trace); (void)p; }
+                    flat = p.flatten(h->model.nodes.size());
+                    if (flat.empty()) throw dp::Error(DP_ERR_STATE, "empty proof");
+                } else { dp::zkml::Proof p = prover.prove(h->trace); if (keep) flat = p.flatten(h->model.nodes.size()); }
+                if (keep) {
+                    std::lock_guard<std::mutex> lk(mu);
+                    if (flat.size() > out_cap) throw dp::Error(DP_ERR_INVALID, "dph_zkml_prove_concurrent: output buffer too small");
+                    memcpy(out, flat.data(), 8 * flat.size()); *out_len = flat.size();
+                }
                 const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
                 if (getenv("DP_HOST_PROF") && idx == 0) { struct timespec cts1; clock_gettime(CLOCK_THREAD_CPUTIME_ID, &cts1);
                     fprintf(stderr, "[worker0] proof wall %.2f ms, thread CPU %.2f ms, transcript permutations %llu\n", sec * 1e3, (cts1.tv_sec - cts0.tv_sec) * 1e3 + (cts1.tv_nsec - cts0.tv_nsec) * 1e-6, (unsigned long long)t.permutations()); }
@@ -246,7 +253,9 @@ struct ZkPool {
 std::mutex g_pools_mu; std::map<void *, std::unique_ptr<ZkPool>> g_pools;
 }
 extern "C" void dph_zkml_pool_free(void *handle) { std::lock_guard<std::mutex> lk(g_pools_mu); g_pools.erase(handle); }
-extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds) {
+// out (optional, cap words): receives the flat proof of the last job handed out, *out_len its length in words.
+extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
+                                         uint64_t *out, uint64_t cap, uint64_t *out_len) {
     DPH_TRY
     ZkHandle *h = (ZkHandle *)handle;
     if (!h->trace.valid()) throw dp::Error(DP_ERR_STATE, "dph_zkml_prove_concurrent: run inference first (mode 1)");
@@ -258,6 +267,7 @@ extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_wo
     {
         std::lock_guard<std::mutex> lk(pool->mu);
         pool->label = label; pool->failed = false; pool->e2e = e2e != 0; pool->pending = n_proofs; pool->active = n_workers; pool->call_gen++;
+        pool->out = out; pool->out_cap = cap; pool->out_len = out_len; if (out_len) *out_len = 0;
         // stagger only when every worker gets several proofs (otherwise the ramps cost more than the overlap gains)
         pool->stagger_s = (!no_stagger && n_workers > 1 && n_proofs >= 3 * n_workers && pool->n_timed > 0) ? pool->avg_proof_s / n_workers : 0.0;
     }

@@ -1,4 +1,4 @@
-/* deepprove_b200 -- C ABI of the B200-native (sm_100a) prover hot path.
+/* deepprove_b200 -- C ABI of the H100-native (sm_90a) prover hot path.
  *
  * This is the drop-in boundary of SURVEY.md section 8(b): the entry points a Rust `-sys` crate would
  * bind so that deep-prove's `sumcheck`, `multilinear_extensions` and `mpcs` crates keep their public

@@ -56,7 +56,7 @@ def main():
     ms = min(r[1] for r in runs)
     point, msgs, fin = runs[-1][0]
     single_ms, same = None, None
-    if rank == 0 and 3 * 8 * n <= 64 << 30:
+    if rank == 0 and 3 * 8 * n <= 32 << 30:      # the inputs plus the first folded tables (as large again) within 80 GB
         full = [splitmix_f(s, n) for s in (1, 2, 3)]
         ts = []
         for _ in range(max(3, reps // 2) + 1):             # first run grows the device arena (cudaMalloc): take the best

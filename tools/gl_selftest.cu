@@ -1,5 +1,5 @@
 // Device-vs-host self test of the field arithmetic and the Poseidon2 permutation (development tool).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -std=c++17 -Iinclude -o gl_selftest_bin tools/gl_selftest.cu   (then: gpurun -- ./gl_selftest_bin)
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -std=c++17 -Iinclude -o gl_selftest_bin tools/gl_selftest.cu   (then run ./gl_selftest_bin on the GPU)
 #include <cstdio>
 #include <vector>
 #include "../deep-prove_b200/csrc/poseidon2.cuh"

@@ -1,6 +1,6 @@
 // Kernel micro-benchmarks (development tool, round 2): candidate formulations of the hot kernels timed with CUDA events on a
-// real B200 before they replace the library versions.  Every candidate is checked against the library formulation first.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Iinclude -o deep-prove_b200/kbench_bin tools/kbench.cu
+// real H100 before they replace the library versions.  Every candidate is checked against the library formulation first.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Iinclude -o deep-prove_b200/kbench_bin tools/kbench.cu
 //   gpurun -- ./deep-prove_b200/kbench_bin [section ...]      sections: perm lat sc
 #include <cstdio>
 #include <cstring>
@@ -461,7 +461,7 @@ int main(int argc, char **argv) {
         };
         printf("[perm] %llu compressions per launch (thread-per-hash level kernel)\n", n_out);
         report("lib k_merkle_up<<<n/128,128>>>", time_ms([&] { k_up_lib<<<(unsigned)(n_out / 128), 128>>>(in, n_out, out); }), out);
-        report("lib, grid 148x8 persistent, 128", time_ms([&] { k_up_lib<<<SM * 8, 128>>>(in, n_out, out); }), out);
+        report("lib, grid SMx8 persistent, 128", time_ms([&] { k_up_lib<<<SM * 8, 128>>>(in, n_out, out); }), out);
 #define RUN_UP(NH, UI, BLOCK, MINB, GRIDMUL) report("v NH=" #NH " UI=" #UI " block=" #BLOCK " minb=" #MINB " grid=SMx" #GRIDMUL, \
             time_ms([&] { k_up_v<NH, UI, BLOCK, MINB><<<SM * GRIDMUL, BLOCK>>>(in, n_out, out); }), out)
         RUN_UP(1, 1, 128, 1, 16); RUN_UP(1, 2, 128, 1, 16); RUN_UP(1, 2, 128, 6, 16); RUN_UP(1, 2, 256, 3, 8); RUN_UP(1, 2, 64, 12, 32);
@@ -513,14 +513,14 @@ int main(int argc, char **argv) {
         auto timed = [&](auto k) { return time_ms([&] { fl(); k(); }) - t_flush; };
         rep1("lib body (2 in flight, canonical acc) 888x256", 888, timed([&] { k_scb3_lib<256><<<888, 256>>>(f[0], f[1], f[2], npairs, part); }));
 #define RUN_B(PPT, BLOCK, MINB, GRID) rep1("lean PPT=" #PPT " block=" #BLOCK " minb=" #MINB " grid=" #GRID, GRID, timed([&] { k_scb3<PPT, BLOCK, MINB><<<GRID, BLOCK>>>(f[0], f[1], f[2], npairs, part); }))
-        RUN_B(1, 256, 1, 2048); RUN_B(2, 256, 1, 1024); RUN_B(4, 256, 1, 512); RUN_B(2, 256, 4, 592); RUN_B(4, 256, 4, 592); RUN_B(4, 256, 3, 444); RUN_B(2, 128, 8, 1184); RUN_B(4, 128, 8, 1184); RUN_B(8, 128, 4, 592);
-        RUN_B(4, 512, 2, 296);
+        RUN_B(1, 256, 1, 2048); RUN_B(2, 256, 1, 1024); RUN_B(4, 256, 1, 512); RUN_B(2, 256, 4, 528); RUN_B(4, 256, 4, 528); RUN_B(4, 256, 3, 396); RUN_B(2, 128, 8, 1056); RUN_B(4, 128, 8, 1056); RUN_B(8, 128, 4, 528);
+        RUN_B(4, 512, 2, 264);
         {
 #define RUN_T(TILE, STAGES, BLOCK, MINB, GRID) do { size_t sm_ = (size_t)STAGES * 3 * 2 * TILE * 8; \
             CK(cudaFuncSetAttribute(k_scb3_tma<TILE, STAGES, BLOCK, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_)); \
             rep1("bulk-async TILE=" #TILE " STAGES=" #STAGES " block=" #BLOCK " minb=" #MINB " grid=" #GRID, GRID, \
                  timed([&] { k_scb3_tma<TILE, STAGES, BLOCK, MINB><<<GRID, BLOCK, sm_>>>(f[0], f[1], f[2], npairs, part); })); } while (0)
-            RUN_T(512, 3, 256, 2, 296); RUN_T(512, 4, 256, 2, 296); RUN_T(256, 4, 256, 4, 592); RUN_T(1024, 3, 512, 1, 148); RUN_T(512, 2, 256, 3, 444); RUN_T(256, 3, 128, 6, 888);
+            RUN_T(512, 3, 256, 2, 264); RUN_T(512, 4, 256, 2, 264); RUN_T(256, 4, 256, 4, 528); RUN_T(1024, 3, 512, 1, 132); RUN_T(512, 2, 256, 3, 396); RUN_T(256, 3, 128, 6, 792);
         }
         // round 2: fold Base -> Ext + message over 2^18 pairs (50.3 MB algorithmic: 25.2 read + 25.2 written)
         gle r = e_make(0x123456789abcdefULL % GL_P, 0xfedcba987654321ULL % GL_P);

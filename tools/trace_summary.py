@@ -2,7 +2,7 @@
 """Summarise a CUPTI kernel timeline (tools/cupti_trace.cpp): per kernel class count / mean duration / share of GPU-resident
 block-time, GPU busy fraction, and how much of the machine's thread slots and registers the running kernels hold over time."""
 import csv, re, sys, collections
-SM, THREADS_PER_SM, REGS_PER_SM = 148, 2048, 65536
+SM, THREADS_PER_SM, REGS_PER_SM = 132, 2048, 65536
 
 def short(n):
     n = re.sub(r"^_Z\d+", "", n)
