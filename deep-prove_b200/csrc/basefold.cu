@@ -786,7 +786,6 @@ static int commit_enqueue(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **o
 }
 
 int dp_pcs_commit(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **out) {
-    DP_HOST_TIMED("dp_pcs_commit");
     DP_REQUIRE_CTX();
     DP_CHECK(poly && out, DP_ERR_INVALID, "dp_pcs_commit: null argument");
     u64 *pin = nullptr;
@@ -834,7 +833,6 @@ static int top_tree_build(DevTree &top, u64 **top_lvl0, const uint64_t *roots, u
 // codeword and the Merkle subtree over that slice; (*out)'s root is the SUBTREE root until dp_pcs_comm_set_shard_roots has been
 // given all ranks' subtree roots (one all-gather of 32 bytes per rank -- the only exchange of the commit).
 int dp_pcs_commit_shard(const dp_mle *poly, uint32_t full_log, uint32_t rank, uint32_t world, dp_pcs_comm **out) {
-    DP_HOST_TIMED("dp_pcs_commit_shard");
     DP_REQUIRE_CTX();
     DP_CHECK(poly && out, DP_ERR_INVALID, "dp_pcs_commit_shard: null argument");
     u32 logG = 0; while ((1u << logG) < world) logG++;
@@ -903,7 +901,6 @@ int dp_pcs_comm_shard_info(const dp_pcs_comm *cm, uint32_t *rank, uint32_t *worl
 // are the batches of values (merkle_tree.rs:68-74,286-312).  Encoding is the per-polynomial pipeline; the leaf level hashes
 // all polynomials' values at an index pair; the levels above are the ordinary tree.
 int dp_pcs_batch_commit(const dp_mle *const *polys, uint32_t n, uint32_t full_log, dp_pcs_comm **out) {
-    DP_HOST_TIMED("dp_pcs_batch_commit");
     DP_REQUIRE_CTX();
     DP_CHECK(polys && out && n >= 1, DP_ERR_INVALID, "cannot batch commit to zero polynomials");      // basefold.rs:367-371
     DP_CHECK(n <= 64, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: at most 64 polynomials per batch");
@@ -976,7 +973,6 @@ static std::vector<StreamSet> g_free_sets; static std::mutex g_sets_mu;
 struct StreamSetReturn { ~StreamSetReturn() { if (!g_pool.empty()) { std::lock_guard<std::mutex> lk(g_sets_mu); g_free_sets.push_back({g_pool, g_pool_ev, g_main_ev}); } } };
 static thread_local StreamSetReturn g_set_return;
 int dp_pcs_commit_many(const dp_mle *const *polys, uint32_t n, uint32_t full_log, dp_pcs_comm **out) {
-    DP_HOST_TIMED("dp_pcs_commit_many");
     DP_REQUIRE_CTX();
     DP_CHECK(polys && out && n > 0, DP_ERR_INVALID, "dp_pcs_commit_many: null argument");
     for (u32 i = 0; i < n; i++) DP_CHECK(polys[i] != nullptr, DP_ERR_INVALID, "dp_pcs_commit_many: null polynomial");
@@ -985,8 +981,7 @@ int dp_pcs_commit_many(const dp_mle *const *polys, uint32_t n, uint32_t full_log
     // streams per host thread for independent commits: 8 are created; a lone proof uses all of them (its 38 witness trees are a pure
     // latency chain each), with many proofs in flight 4 are enough and keep the number of live streams near the 32 hardware queues
     static const u32 SMAX = 8;
-    static const u32 S_ENV = [] { const char *e = getenv("DP_COMMIT_STREAMS"); int v = e ? atoi(e) : 0; return (u32)(v < 0 ? 0 : (v > 8 ? 8 : v)); }();
-    const u32 S = S_ENV ? S_ENV : (dp_wait_mode() == DP_WAIT_BLOCK ? 4u : 8u);
+    const u32 S = dp_wait_mode() == DP_WAIT_BLOCK ? 4u : 8u;
     (void)g_set_return;
     if (g_pool.empty()) {
         std::lock_guard<std::mutex> lk(g_sets_mu);
@@ -1048,7 +1043,6 @@ int dp_pcs_comm_free(dp_pcs_comm *cm) {
 // commit_phase / batch_commit_phase up to and including the first sumcheck message
 int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, uint32_t n_comms, const uint64_t *point, uint32_t num_vars,
                       dp_pcs_open **out, uint64_t first_msg[6]) {
-    DP_HOST_TIMED("dp_pcs_open_begin");
     DP_REQUIRE_CTX();
     DP_CHECK(comms && n_comms >= 1 && point && out && first_msg, DP_ERR_INVALID, "dp_pcs_open_begin: null argument");
     if (int e = bf_prepare()) return e;
@@ -1150,7 +1144,6 @@ int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, u
 // One commit-phase round (commit_phase.rs:85-171 / :253-352): fold the oracle by `challenge`; unless this is
 // the last round return the next sumcheck message and the root of the folded oracle's tree.
 int dp_pcs_open_round(dp_pcs_open *o, const uint64_t challenge[2], uint64_t next_msg[6], uint64_t root[4], int *is_last) {
-    DP_HOST_TIMED("dp_pcs_open_round");
     DP_REQUIRE_CTX();
     DP_CHECK(o && challenge && is_last, DP_ERR_INVALID, "dp_pcs_open_round: null argument");
     DP_CHECK(o->round < o->num_rounds, DP_ERR_STATE, "dp_pcs_open_round: commit phase already finished");
@@ -1255,7 +1248,6 @@ uint64_t dp_pcs_open_query_words(const dp_pcs_open *o) {
 // K13 (query_phase.rs:373-474): for every x index, for every commitment then every round oracle:
 // [p0.c0 p0.c1 p1.c0 p1.c1] + Merkle path without leaf sibling or root (merkle_tree.rs:139-152).
 int dp_pcs_open_query(dp_pcs_open *o, const uint64_t *x_indices, uint32_t n, uint64_t *out) {
-    DP_HOST_TIMED("dp_pcs_open_query");
     DP_REQUIRE_CTX();
     DP_CHECK(o && x_indices && out && n > 0, DP_ERR_INVALID, "dp_pcs_open_query: null argument");
     DP_CHECK(o->have_final, DP_ERR_STATE, "dp_pcs_open_query: commit phase not finished");

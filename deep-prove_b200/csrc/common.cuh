@@ -46,14 +46,6 @@ struct DpProfScope {
     ~DpProfScope() { dp_prof_end(tok); }
 };
 
-// host-side wall-clock accumulators (DP_HOST_PROF=1): where a round-granular call spends its CPU time
-struct DpHostTimer {
-    const char *name; double t0, c0;
-    explicit DpHostTimer(const char *n);
-    ~DpHostTimer();
-};
-#define DP_HOST_TIMED(name) DpHostTimer dp_host_timer_##__LINE__(name)
-
 // ---- waiting for the device -------------------------------------------------------------------------------------------
 // Every round of the prover ends with the host waiting for a word the GPU writes into mapped pinned memory.  Two modes:
 //   DP_WAIT_SPIN  (default): the calling thread spins on the word -- lowest latency, one busy core per proof in flight.

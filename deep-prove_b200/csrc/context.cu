@@ -1,6 +1,5 @@
 // Context, error reporting and memory-pool plumbing of libdeepprove_b200.so.
 #include "common.cuh"
-#include <map>
 #include <cstdlib>
 #include <atomic>
 #include <mutex>
@@ -141,12 +140,8 @@ void dp_pinned_free(void *p) {
 #include <sys/syscall.h>
 #include <unistd.h>
 #include <time.h>
-static std::atomic<int> g_wait_mode{-1};
-int dp_wait_mode() {
-    int m = g_wait_mode.load(std::memory_order_relaxed);
-    if (m < 0) { const char *e = getenv("DP_WAIT_MODE"); m = (e && (e[0] == '1' || e[0] == 'b' || e[0] == 'B')) ? DP_WAIT_BLOCK : DP_WAIT_SPIN; g_wait_mode.store(m); }
-    return m;
-}
+static std::atomic<int> g_wait_mode{DP_WAIT_SPIN};
+int dp_wait_mode() { return g_wait_mode.load(std::memory_order_relaxed); }
 static long futex_call(std::atomic<u32> *addr, int op, u32 val, const struct timespec *ts) { return syscall(SYS_futex, (u32 *)addr, op, val, ts, nullptr, 0); }
 struct WaitSlot {
     std::atomic<u32> state{0};                 // 0 idle, 1 armed (the poller watches it), 3 being fired by the poller, 2 fired
@@ -199,7 +194,6 @@ u64 dp_wait_flag(volatile u64 *flag, u64 want, bool has_fail, u64 fail, double t
     // their round-trip-bound phases) -- never more than about half of the CPUs this process may use.
     {
         static const int spin_limit = [] {
-            if (const char *e = getenv("DP_WAIT_SPINNERS")) return atoi(e);
             double cpus = (double)std::thread::hardware_concurrency();
             if (FILE *f = fopen("/sys/fs/cgroup/cpu.max", "r")) { char q[64]; double per = 0; if (fscanf(f, "%63s %lf", q, &per) == 2 && strcmp(q, "max") != 0 && per > 0) cpus = std::min(cpus, atof(q) / per); fclose(f); }
             // one process per GPU on a shared box (torchrun): this process's share of the CPUs, not the whole container's
@@ -289,18 +283,6 @@ int dp_zero_block_get(void **p) {
 }
 void dp_zero_block_put(void *p) { if (p) g_ctx.zero_blocks.push_back(p); }
 
-static bool g_hostprof = getenv("DP_HOST_PROF") != nullptr;
-struct HostProfAcc { unsigned long long n = 0; double wall_us = 0, cpu_us = 0; };
-static thread_local std::map<std::string, HostProfAcc> g_hostprof_acc;
-static inline double now_us() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-static inline double thread_cpu_us() { struct timespec ts; clock_gettime(CLOCK_THREAD_CPUTIME_ID, &ts); return ts.tv_sec * 1e6 + ts.tv_nsec * 1e-3; }
-DpHostTimer::DpHostTimer(const char *n) : name(n), t0(g_hostprof ? now_us() : 0.0), c0(g_hostprof ? thread_cpu_us() : 0.0) {}
-DpHostTimer::~DpHostTimer() { if (g_hostprof) { auto &a = g_hostprof_acc[name]; a.n++; a.wall_us += now_us() - t0; a.cpu_us += thread_cpu_us() - c0; } }
-extern "C" void dp_hostprof_dump(void) {   // wall = time inside the call, cpu = CPU time this thread burnt inside it (spinning shows up as cpu ~ wall)
-    for (auto &kv : g_hostprof_acc) fprintf(stderr, "[hostprof] %-32s n=%8llu wall=%10.3f ms cpu=%10.3f ms avg wall=%8.2f us cpu=%7.2f us\n", kv.first.c_str(), kv.second.n, kv.second.wall_us / 1e3, kv.second.cpu_us / 1e3, kv.second.wall_us / kv.second.n, kv.second.cpu_us / kv.second.n);
-    g_hostprof_acc.clear();
-}
-
 // ---- per-kernel event timing --------------------------------------------------------------------
 // Process-wide switch and statistics, thread-local event lists: every proving thread brackets its launches with events
 // on ITS stream and folds the elapsed times into the shared table (dp_profile_flush at the end of a proof, or any
@@ -385,7 +367,6 @@ int dp_profile_read_ex(char (*names)[64], uint64_t *counts, double *total_ms, ui
     }
     return i;
 }
-int dp_profile_read(char (*names)[64], uint64_t *counts, double *total_ms, uint64_t *bytes, int cap) { return dp_profile_read_ex(names, counts, total_ms, bytes, nullptr, cap); }
 
 const char *dp_last_error(void) { return g_err.c_str(); }
 const char *dp_version(void) { return "deepprove_b200 0.1 (sm_90a)"; }

@@ -34,58 +34,8 @@ __device__ __forceinline__ u64 gl_reduce128_weak(u64 lo, u64 hi) {
         : "=l"(r) : "l"(lo), "l"(hi));
     return r;
 }
-// 64 x 64 -> 128 bits as four 32 x 32 -> 64 products (IMAD.WIDE) and a carry chain.  `a * b` + `__umul64hi(a, b)` makes the compiler
-// compute the low half twice (6 IMAD.WIDE + 2 IMAD per product); the Poseidon2 kernels run at 90 % of the FMA-heavy pipe that
-// executes IMAD.WIDE (ncu r02d), so the multiplier count is the throughput of every hash kernel.
-#ifndef GL_MULV
-#define GL_MULV 0
-#endif
-__device__ __forceinline__ void gl_mul128(u64 a, u64 b, u64 &lo, u64 &hi) {
-#if GL_MULV == 0
-    lo = a * b; hi = __umul64hi(a, b);
-#else
-    asm("{\n\t.reg .u32 a0, a1, b0, b1, pl, ph, tl, th, ul, uh;\n\t.reg .u64 p, t, u, c;\n\t"
-        "mov.b64 {a0, a1}, %2;\n\tmov.b64 {b0, b1}, %3;\n\t"
-        "mul.wide.u32 p, a0, b0;\n\t"
-        "mov.b64 {pl, ph}, p;\n\t"
-        "cvt.u64.u32 c, ph;\n\t"
-        "mad.wide.u32 t, a0, b1, c;\n\t"             // a0 b1 + hi32(a0 b0) < 2^64
-        "mov.b64 {tl, th}, t;\n\t"
-        "cvt.u64.u32 c, tl;\n\t"
-        "mad.wide.u32 u, a1, b0, c;\n\t"             // a1 b0 + lo32(t) < 2^64
-        "mov.b64 {ul, uh}, u;\n\t"
-        "mov.b64 %0, {pl, ul};\n\t"
-        "cvt.u64.u32 c, th;\n\t"
-        "cvt.u64.u32 t, uh;\n\t"
-        "add.u64 c, c, t;\n\t"
-        "mad.wide.u32 %1, a1, b1, c;\n\t}"           // a1 b1 + hi32(t) + hi32(u) < 2^64
-        : "=l"(lo), "=l"(hi) : "l"(a), "l"(b));
-#endif
-}
-#if GL_MULV == 2
-// the same reduction with the multiplications by 2^32 - 1 done on the integer ALU ((x << 32) - x as a borrow pair; the carry fix-up
-// as a masked add): no IMAD.WIDE left outside the product itself
-__device__ __forceinline__ u64 gl_reduce128_weak_alu(u64 lo, u64 hi) {
-    u64 r;
-    asm("{\n\t.reg .u64 t0, t1, m64;\n\t.reg .u32 hl, hh, m, x0, x1;\n\t"
-        "mov.b64 {hl, hh}, %2;\n\t"
-        "cvt.u64.u32 m64, hh;\n\t"
-        "sub.cc.u64 t0, %1, m64;\n\t"                         // lo - hi_hi
-        "subc.u32 m, 0, 0;\n\t"                               // 0 or 0xFFFFFFFF
-        "cvt.u64.u32 m64, m;\n\t"
-        "sub.u64 t0, t0, m64;\n\t"                            // borrow: - EPS
-        "sub.cc.u32 x0, 0, hl;\n\t"                           // hl * (2^32 - 1) = (hl << 32) - hl
-        "subc.u32 x1, hl, 0;\n\t"
-        "mov.b64 t1, {x0, x1};\n\t"
-        "add.cc.u64 t0, t0, t1;\n\t"
-        "addc.u32 m, 0, 0;\n\t"
-        "sub.u32 m, 0, m;\n\t"                                // carry ? 0xFFFFFFFF : 0
-        "cvt.u64.u32 m64, m;\n\t"
-        "add.u64 %0, t0, m64;\n\t}"                           // + EPS, cannot carry again
-        : "=l"(r) : "l"(lo), "l"(hi));
-    return r;
-}
-#endif
+// 64 x 64 -> 128 bits
+__device__ __forceinline__ void gl_mul128(u64 a, u64 b, u64 &lo, u64 &hi) { lo = a * b; hi = __umul64hi(a, b); }
 __device__ __forceinline__ u64 gl_canon_weak(u64 r) {          // [0, 2^64) -> [0, p)
     u64 t; u32 c;
     asm("{\n\tadd.cc.u64 %0, %2, 0xFFFFFFFF;\n\taddc.u32 %1, 0, 0;\n\t}" : "=l"(t), "=r"(c) : "l"(r));
@@ -113,11 +63,7 @@ __device__ __forceinline__ u64 gl_sub(u64 a, u64 b) {          // a, b < p  ->  
     return d - (u64)m;                                         // borrow: + p == - EPS (mod 2^64)
 }
 __device__ __forceinline__ u64 gl_reduce128(u64 lo, u64 hi) { return gl_canon_weak(gl_reduce128_weak(lo, hi)); }
-#if GL_MULV == 2
-__device__ __forceinline__ u64 gl_mul_weak(u64 a, u64 b) { u64 lo, hi; gl_mul128(a, b, lo, hi); return gl_reduce128_weak_alu(lo, hi); }   // any u64 inputs -> [0, 2^64)
-#else
 __device__ __forceinline__ u64 gl_mul_weak(u64 a, u64 b) { u64 lo, hi; gl_mul128(a, b, lo, hi); return gl_reduce128_weak(lo, hi); }   // any u64 inputs -> [0, 2^64)
-#endif
 __device__ __forceinline__ void gl_mul_wide(u64 a, u64 b, u64 &lo, u64 &hi) { lo = a * b; hi = __umul64hi(a, b); }
 GL_HD u64 gl_neg(u64 a) { return a ? GL_P - a : 0ULL; }
 GL_HD u64 gl_dbl(u64 a) { return gl_add(a, a); }

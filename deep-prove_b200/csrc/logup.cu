@@ -82,7 +82,6 @@ extern "C" {
 // LogUpCircuit::new_lookup_circuit (multiplicities == NULL) / new_table_circuit
 int dp_logup_build(dp_mle *const *columns, uint32_t n_columns, const dp_mle *multiplicities, const uint64_t constant_challenge[2],
                    const uint64_t column_separation_challenge[2], dp_logup **out) {
-    DP_HOST_TIMED("dp_logup_build");
     DP_REQUIRE_CTX();
     DP_CHECK(columns && n_columns >= 1 && n_columns <= 16 && out && constant_challenge && column_separation_challenge, DP_ERR_INVALID, "dp_logup_build: bad argument");
     u64 len = columns[0]->len;

@@ -223,7 +223,6 @@ static int point_from_host(const uint64_t *point, u32 k, gle *out) {
 }
 
 int dp_mle_upload(const uint64_t *evals, uint64_t len, int is_ext, dp_mle **out) {
-    DP_HOST_TIMED("dp_mle_upload");
     DP_REQUIRE_CTX();
     DP_CHECK(out && evals, DP_ERR_INVALID, "dp_mle_upload: null argument");
     DP_CHECK(len > 0 && (len & (len - 1)) == 0, DP_ERR_INVALID, "dp_mle_upload: len must be a power of two");
@@ -333,7 +332,6 @@ int dp_mle_fix_low(const dp_mle *m, const uint64_t *point, uint32_t k, dp_mle **
 }
 
 int dp_mle_evaluate(const dp_mle *m, const uint64_t *point, uint32_t num_vars, uint64_t out[2]) {
-    DP_HOST_TIMED("dp_mle_evaluate");
     DP_REQUIRE_CTX();
     DP_CHECK(m && out, DP_ERR_INVALID, "dp_mle_evaluate: null argument");
     DP_CHECK(num_vars == m->num_vars(), DP_ERR_INVALID, "MLE size does not match the point");  // mle.rs:609-613
@@ -365,7 +363,6 @@ int dp_mle_evaluate(const dp_mle *m, const uint64_t *point, uint32_t num_vars, u
 // evaluate (mle.rs:607-623) for n MLEs with the same num_vars at the same point (e.g. the LogUp output claims,
 // logup_gkr/prover.rs:172-183): out = n x [c0,c1]
 int dp_mle_evaluate_many(const dp_mle *const *mles, uint32_t n, const uint64_t *point, uint32_t num_vars, uint64_t *out) {
-    DP_HOST_TIMED("dp_mle_evaluate_many");
     DP_REQUIRE_CTX();
     DP_CHECK(mles && out && n > 0 && (point || num_vars == 0), DP_ERR_INVALID, "dp_mle_evaluate_many: null argument");
     for (u32 i = 0; i < n; i++) DP_CHECK(mles[i] && mles[i]->num_vars() == num_vars, DP_ERR_INVALID, "MLE size does not match the point");
@@ -395,7 +392,6 @@ int dp_mle_evaluate_many(const dp_mle *const *mles, uint32_t n, const uint64_t *
 }
 
 int dp_eq_build(const uint64_t *point, uint32_t num_vars, dp_mle **outp) {
-    DP_HOST_TIMED("dp_eq_build");
     DP_REQUIRE_CTX();
     DP_CHECK(outp && (point || num_vars == 0), DP_ERR_INVALID, "dp_eq_build: null argument");
     DP_CHECK(num_vars <= 32, DP_ERR_INVALID, "dp_eq_build: num_vars > 32");

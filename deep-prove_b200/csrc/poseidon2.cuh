@@ -25,11 +25,7 @@ static inline cudaError_t p2_upload_constants(const u64 *ext /*64*/, const u64 *
 // reduction.  Only the four digest words are canonicalised at the end.  Every step is exact modular arithmetic,
 // so the digests are bit-identical to the canonical formulation.
 struct p2w { u64 lo; u32 hi; };                                                   // value = lo + hi * 2^64
-#if GL_MULV == 2
-__device__ __forceinline__ u64 w_red(u64 lo, u64 hi) { return gl_reduce128_weak_alu(lo, hi); }
-#else
 __device__ __forceinline__ u64 w_red(u64 lo, u64 hi) { return gl_reduce128_weak(lo, hi); }
-#endif
 __device__ __forceinline__ u64 w_mul(u64 a, u64 b) { u64 lo, hi; gl_mul128(a, b, lo, hi); return w_red(lo, hi); }
 __device__ __forceinline__ u64 w_add_canon(u64 a, u64 c) {                        // a weak, c < p  ->  weak
     u64 r; asm("{\n\t.reg .u32 c;\n\t.reg .u64 t;\n\tadd.cc.u64 t, %1, %2;\n\taddc.u32 c, 0, 0;\n\tmad.wide.u32 %0, c, 0xFFFFFFFF, t;\n\t}" : "=l"(r) : "l"(a), "l"(c));

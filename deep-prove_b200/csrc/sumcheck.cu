@@ -452,7 +452,7 @@ static constexpr long long SC_RES_TIMEOUT = 6000000000LL;   // ~3 s at 1.9 GHz
 static constexpr u64 SC_TAIL_ABORT = ~0ULL, SC_TAIL_FAILED = ~0ULL - 1;
 struct TMle { const void *cur; gle *work; u64 len, len0; u32 is_ext, where; };
 struct TProd { u32 n_idx; u32 idx[5]; };
-struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; long long *dbg; TMle m[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; };   // dbg: optional per-round phase clocks (DP_SC_RES_DEBUG)
+struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; TMle m[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; };
 
 __device__ __forceinline__ u32 cl_rank() { u32 r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ u32 cl_size() { u32 r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
@@ -483,11 +483,9 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
     if (threadIdx.x == 0) for (u32 p = 0; p < np; p++) for (u32 j = 0; j < sp[p].n_idx; j++) { u32 mi = sp[p].idx[j]; if (swriter[mi] == 0xff) swriter[mi] = (unsigned char)p; }
     __syncthreads();
     gle r = r0;
-    long long *const dbg = cfg->dbg;
-#define RES_MARK(ph) do { if (dbg && rank == 0 && threadIdx.x == 0) dbg[k * 8 + (ph)] = clock64(); } while (0)
     // The descriptors of a round depend on the fold bookkeeping only, never on the challenge VALUE: they are rebuilt right after a
-    // round's message has been signalled, i.e. in the shadow of the host's Fiat-Shamir (phase clocks: ~2.2 us per round that used
-    // to sit between the challenge's arrival and the first load).
+    // round's message has been signalled, i.e. in the shadow of the host's Fiat-Shamir, which keeps ~2.2 us per round off the path
+    // from the challenge's arrival to the first load.
     auto build_descs = [&](const bool fold) {
         for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
             bool f = fold && sm[i].len > 1;
@@ -518,7 +516,6 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
     build_descs(cfg->first_has_challenge != 0);
     for (u32 k = 0; k < nr; k++) {
         const u64 seq = seq0 + k;
-        RES_MARK(0);
         if (k > 0) {   // wait for the host's challenge for this round
             if (rank == 0 && threadIdx.x == 0) {
                 long long t0 = clock64(); u64 v, status = 0;
@@ -535,8 +532,6 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
             if (status) { if (rank == 0 && threadIdx.x == 0 && status == 2) { __threadfence_system(); *flag = SC_TAIL_FAILED; } return; }   // uniform over the cluster
             r = e_make(__ldcg(xctl + 1), __ldcg(xctl + 2));
         }
-        RES_MARK(1);
-        RES_MARK(2);
         // work: slot (p, s) = sub-slice s of product p's pairs; warp gw owns slots gw, gw + W, ...
         for (u32 slot = gw; slot < np * G; slot += W) {
             const u32 p = slot / G, s = slot % G;
@@ -573,9 +568,7 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
                 if (lane == 0) __stcg(reinterpret_cast<ulonglong2 *>(xpart + (u64)slot * SC_NACC + t), make_ulonglong2(ws_reduce(v0), ws_reduce(v1)));
             }
         }
-        RES_MARK(3);
         cl_sync();                                             // warp partials and folded tables of every CTA are visible
-        RES_MARK(4);
         if (rank == 0) {                                       // the message first: it is what the host is waiting for
             // few partials per (product, point): one THREAD each (many products run side by side); many (a single product spread over
             // >= 32 warps): one WARP each, its lanes gather the partials with independent L2 loads -- faster for a single wide product,
@@ -613,9 +606,7 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
                 }
                 __syncthreads();
             }
-            RES_MARK(5);
             if (threadIdx.x == 0) { __threadfence_system(); *flag = seq; }
-            RES_MARK(6);
         }
         if (k + 1 < nr) build_descs(true);                     // next round's descriptors while the host hashes
         // CTAs other than 0 run ahead to the next cluster barrier; xpart is not rewritten before it (the work phase follows it)
@@ -667,10 +658,7 @@ struct dp_sc {
     bool tail_enabled = false, tail_active = false; u32 tail_last_round = 0;
     ScTail *h_tail = nullptr; u64 *h_chal = nullptr;
     gle *d_xpart = nullptr; u64 *d_xctl = nullptr;        // resident cluster kernel: warp partials, [status, c0, c1]
-    long long *h_dbg = nullptr; u32 dbg_rounds = 0;
-    u64 last_ops = 0;
     std::vector<gle> challenges;
-    u64 last_bytes = 0;
 };
 
 static u32 ceil_log2_u64(u64 x) { u32 l = 0; while ((1ULL << l) < x) l++; return l; }
@@ -697,15 +685,6 @@ static int sc_free_all(dp_sc *s) {
     dp_dev_free(s->d_xpart); dp_dev_free(s->d_xctl);
     dp_pinned_free(s->h_flag);
     dp_pinned_free(s->h_descs); dp_pinned_free(s->h_out); dp_pinned_free(s->h_fin); dp_pinned_free(s->h_pairs);
-    if (s->h_dbg) {   // DP_SC_RES_DEBUG: device clocks of CTA 0 / thread 0 per round: wait-for-challenge | broadcast | descriptors | work | cluster barrier | sum+store | fence+flag
-        dp_stream_sync(dp_ctx().stream);
-        for (u32 k = 0; k < s->dbg_rounds && k < 64; k++) {
-            const long long *d = s->h_dbg + 8 * k;
-            fprintf(stderr, "[sc_res] round %2u cycles: wait %6lld bcast %5lld desc %5lld work %6lld clsync %5lld sum %5lld signal %5lld | total-excl-wait %6lld\n", k,
-                    d[1] - d[0], 0LL, d[2] - d[1], d[3] - d[2], d[4] - d[3], d[5] - d[4], d[6] - d[5], d[6] - d[1]);
-        }
-        dp_pinned_free(s->h_dbg);
-    }
     dp_pinned_free(s->h_tail); dp_pinned_free(s->h_chal);
     return DP_OK;
 }
@@ -750,7 +729,7 @@ __global__ void k_tail_probe(volatile u64 *mailbox, volatile u64 *result, long l
 static bool sc_tail_supported() {
     static std::once_flag once; static bool supported = false;
     std::call_once(once, [] {
-        if (getenv("DP_SC_NO_TAIL") || getenv("CUDA_INJECTION64_PATH") || getenv("CUDA_INJECTION32_PATH") || getenv("NV_NSIGHT_INJECTION_TRANSPORT_TYPE") ||
+        if (getenv("CUDA_INJECTION64_PATH") || getenv("CUDA_INJECTION32_PATH") || getenv("NV_NSIGHT_INJECTION_TRANSPORT_TYPE") ||
             getenv("NV_NSIGHT_INJECTION_PORT_BASE") || getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR")) return;
         u64 *pin = nullptr;
         if (dp_pinned_alloc((void **)&pin, 128) != DP_OK) return;
@@ -776,8 +755,7 @@ static bool sc_tail_eligible(const dp_sc *s, bool fold) {
     std::vector<char> used(s->n_mles, 0);
     for (auto &pr : s->products) for (u32 j = 0; j < pr.n_idx; j++) used[pr.idx[j]] = 1;
     for (u32 i = 0; i < s->n_mles; i++) if (!used[i] && s->mles[i].len > 1) return false;
-    static const u64 limit = [] { const char *e = getenv("DP_SC_RES_WORK"); return e ? (u64)atoll(e) : SC_RES_WORK; }();
-    return sc_round_work(s, fold) <= limit;
+    return sc_round_work(s, fold) <= SC_RES_WORK;
 }
 template <int DSEL>
 static cudaError_t sc_res_launch(u32 ncta, cudaStream_t st, const ScTail *cfg, gle r, gle *out, gle *pairs, u64 *flag, u64 *chal, u64 seq, gle *xpart, u64 *xctl) {
@@ -805,8 +783,6 @@ static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
         }
         for (u32 p = 0; p < s->n_products; p++) { t.p[p].n_idx = s->products[p].n_idx; for (u32 j = 0; j < 5; j++) t.p[p].idx[j] = s->products[p].idx[j]; }
         s->h_chal[0] = 0;
-        t.dbg = nullptr;
-        if (getenv("DP_SC_RES_DEBUG")) { if (!s->h_dbg && (e = dp_pinned_alloc((void **)&s->h_dbg, sizeof(long long) * 8 * 64))) return e; memset(s->h_dbg, 0, sizeof(long long) * 8 * 64); t.dbg = s->h_dbg; s->dbg_rounds = t.n_rounds; }
         // cluster size by the first resident round's work: ~512 pair-items per CTA, a power of two <= 8 (portable cluster size)
         const u64 work = sc_round_work(s, fold);
         u32 ncta = 1; while (ncta < SC_RES_MAXCTA && (u64)ncta * 512 < work) ncta <<= 1;
@@ -835,12 +811,8 @@ static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
     }
     if (fold) for (auto &m : s->mles) if (m.len > 1) { m.len >>= 1; m.is_ext = true; m.cur = nullptr; m.where = 3; }   // the tables now live in the kernel's bookkeeping
     s->round += 1;
-    s->last_bytes = 0;
-    {
-        DP_HOST_TIMED("dp_sc_round(sync wait)");
-        const bool ok = dp_wait_flag(s->h_flag, s->seq, true, SC_TAIL_FAILED, 8.0) == s->seq;
-        if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(st); DP_CHECK(false, DP_ERR_CUDA, "dp_sc_round: resident kernel timed out waiting for a challenge (other work queued in the same stream?)"); }
-    }
+    const bool ok = dp_wait_flag(s->h_flag, s->seq, true, SC_TAIL_FAILED, 8.0) == s->seq;
+    if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(st); DP_CHECK(false, DP_ERR_CUDA, "dp_sc_round: resident kernel timed out waiting for a challenge (other work queued in the same stream?)"); }
     if (s->round == s->max_nv) s->have_pairs = true;   // written to mapped memory before the flag
     return sc_glue(s, out_evals);
 }
@@ -849,7 +821,6 @@ extern "C" {
 
 int dp_sc_create(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *products, uint32_t n_products,
                  uint32_t max_nv, uint32_t max_deg, dp_sc **out) {
-    DP_HOST_TIMED("dp_sc_create");
     DP_REQUIRE_CTX();
     DP_CHECK(mles && products && out && n_mles > 0 && n_products > 0, DP_ERR_INVALID, "dp_sc_create: null/empty argument");
     DP_CHECK(max_nv != 0, DP_ERR_INVALID, "Attempt to prove a constant.");  // prover.rs:590-593
@@ -906,7 +877,6 @@ int dp_sc_create(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *prod
 }
 
 int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
-    DP_HOST_TIMED("dp_sc_round(total)");
     DP_REQUIRE_CTX();
     DP_CHECK(s && out_evals, DP_ERR_INVALID, "dp_sc_round: null argument");
     DP_CHECK(!s->finished && s->round < s->max_nv, DP_ERR_STATE, "Prover is not active");  // prover.rs:636-639
@@ -987,7 +957,6 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
     // each of the 2 elements a folding operand contributes to a pair
     u64 ops = 0;
     for (u32 p = 0; p < s->n_products; p++) { const ScProd &d = s->h_descs[p]; u64 nf = 0; for (u32 j = 0; j < d.d; j++) if (d.op[j].mode >= OPM_BF) nf++; ops += d.npairs * ((u64)(d.d - 1) * (d.d + 1) + 5 * d.d + 4 + 6 * nf); }
-    s->last_ops = ops;
     // grid sized for THIS round.  lean: Base rounds 256 threads x 2 pairs in flight, folding rounds 128 threads x 1 pair (tools/kbench.cu);
     // general kernel: 2 pairs per thread minimum so small rounds run in a single block
     int gx;
@@ -1038,7 +1007,6 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
         m.cur = dst[i]; m.where = (dst[i] == m.work) ? 1 : 2; m.len >>= 1; m.is_ext = true;
     }
     s->round += 1;
-    s->last_bytes = bytes;
     if (s->round == s->max_nv) {   // last round: bring the (<= 2)-entry tables back together with the message
         bool ok = true;
         for (u32 i = 0; i < s->n_mles; i++) { const ScMle &m = s->mles[i]; if (m.len > 2) ok = false; s->h_fin[i].src = m.cur; s->h_fin[i].mode = m.is_ext ? OPM_E : OPM_B; s->h_fin[i].len = (u32)m.len; }
@@ -1050,21 +1018,17 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
             s->have_pairs = true;
         }
     }
-    {
-        DP_HOST_TIMED("dp_sc_round(sync wait)");
-        if (s->have_pairs) { DP_CUDA(dp_stream_sync(st)); s->round_in_flight = false; }      // last round: the gathered pairs follow the kernel
-        else {
-            volatile u64 *f = s->h_flag;
-            const bool ok = dp_wait_flag(f, s->seq, false, 0, 2.0) == s->seq;
-            if (ok) s->round_in_flight = false;
-            if (!ok) { DP_CUDA(dp_stream_sync(st)); DP_CHECK(*f == s->seq, DP_ERR_CUDA, "dp_sc_round: kernel finished without signalling"); s->round_in_flight = false; }
-        }
+    if (s->have_pairs) { DP_CUDA(dp_stream_sync(st)); s->round_in_flight = false; }      // last round: the gathered pairs follow the kernel
+    else {
+        volatile u64 *f = s->h_flag;
+        const bool ok = dp_wait_flag(f, s->seq, false, 0, 2.0) == s->seq;
+        if (ok) s->round_in_flight = false;
+        if (!ok) { DP_CUDA(dp_stream_sync(st)); DP_CHECK(*f == s->seq, DP_ERR_CUDA, "dp_sc_round: kernel finished without signalling"); s->round_in_flight = false; }
     }
     return sc_glue(s, out_evals);
 }
 
 int dp_sc_finish(dp_sc *s, const uint64_t *last_challenge, uint64_t *out_final) {
-    DP_HOST_TIMED("dp_sc_finish");
     DP_REQUIRE_CTX();
     DP_CHECK(s && last_challenge && out_final, DP_ERR_INVALID, "dp_sc_finish: null argument");
     DP_CHECK(!s->finished && s->round == s->max_nv, DP_ERR_STATE, "dp_sc_finish: rounds not complete");
@@ -1100,7 +1064,6 @@ int dp_sc_finish(dp_sc *s, const uint64_t *last_challenge, uint64_t *out_final) 
 
 int dp_sc_destroy(dp_sc *s) {
     if (!s) return DP_OK;
-    DP_HOST_TIMED("dp_sc_destroy");
     std::lock_guard<std::recursive_mutex> lk(dp_ctx().mu);
     if (dp_ctx().ready) {
         if (s->tail_active && s->round < s->max_nv) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(dp_ctx().stream); }   // release the waiting kernel
@@ -1109,8 +1072,6 @@ int dp_sc_destroy(dp_sc *s) {
     delete s;
     return DP_OK;
 }
-
-uint64_t dp_sc_last_round_bytes(const dp_sc *s) { return s ? s->last_bytes : 0; }
 
 int dp_sc_set_resident_tail(dp_sc *s, int enable) {
     DP_REQUIRE_CTX();

@@ -17,10 +17,10 @@ DP_OK, DP_ERR_INVALID, DP_ERR_CUDA, DP_ERR_NO_DEVICE, DP_ERR_STATE, DP_ERR_UNSUP
 # every symbol include/deepprove_b200.h declares (tests check the .so exports each one)
 ABI_SYMBOLS = [
     "dp_init", "dp_shutdown", "dp_device_count", "dp_last_error", "dp_version", "dp_set_stream", "dp_synchronize",
-    "dp_kernel_launches", "dp_set_wait_mode", "dp_get_wait_mode", "dp_profile_enable", "dp_profile_reset", "dp_profile_read", "dp_profile_read_ex", "dp_profile_flush",
+    "dp_kernel_launches", "dp_set_wait_mode", "dp_get_wait_mode", "dp_profile_enable", "dp_profile_reset", "dp_profile_read_ex", "dp_profile_flush",
     "dp_mle_upload", "dp_mle_wrap_device", "dp_mle_clone", "dp_mle_download", "dp_mle_info", "dp_mle_device_ptr",
     "dp_mle_free", "dp_mle_fix_high", "dp_mle_fix_high_new", "dp_mle_fix_low", "dp_mle_evaluate", "dp_mle_evaluate_many", "dp_eq_build",
-    "dp_sc_create", "dp_sc_round", "dp_sc_finish", "dp_sc_destroy", "dp_sc_last_round_bytes", "dp_sc_current_mle", "dp_sc_set_resident_tail",
+    "dp_sc_create", "dp_sc_round", "dp_sc_finish", "dp_sc_destroy", "dp_sc_current_mle", "dp_sc_set_resident_tail",
     "dp_poseidon2_init", "dp_set_merkle_hasher", "dp_get_merkle_hasher", "dp_pcs_commit", "dp_pcs_commit_many", "dp_pcs_batch_commit", "dp_pcs_comm_num_polys", "dp_pcs_comm_part", "dp_pcs_comm_info", "dp_pcs_comm_codeword", "dp_pcs_comm_bh_evals", "dp_pcs_comm_free",
     "dp_pcs_open_begin", "dp_pcs_open_round", "dp_pcs_open_final_message", "dp_pcs_open_query_words", "dp_pcs_open_query",
     "dp_pcs_open_free", "dp_pcs_commit_shard", "dp_pcs_comm_shard_info", "dp_pcs_comm_set_shard_roots", "dp_pcs_open_set_shard_roots",
@@ -59,9 +59,7 @@ def lib():
         _lib.dp_version.restype = C.c_char_p
         _lib.dp_kernel_launches.restype = C.c_uint64
         _lib.dp_mle_device_ptr.restype = C.c_void_p
-        _lib.dp_sc_last_round_bytes.restype = C.c_uint64
         _lib.dp_mle_device_ptr.argtypes = [C.c_void_p]
-        _lib.dp_sc_last_round_bytes.argtypes = [C.c_void_p]
         _lib.dp_set_stream.argtypes = [C.c_void_p]
         _lib.dp_mle_upload.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_void_p)]
         _lib.dp_mle_wrap_device.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_void_p)]
@@ -324,9 +322,6 @@ class Sumcheck:
         c = _u64(challenge)
         check(lib().dp_sc_finish(self.h, _ptr(c), _ptr(out)))
         return out.reshape(-1, 2)
-
-    def last_round_bytes(self):
-        return lib().dp_sc_last_round_bytes(self.h)
 
     def destroy(self):
         if self.h:

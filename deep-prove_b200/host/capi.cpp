@@ -202,7 +202,6 @@ int dph_zkml_prove(void *handle, const int64_t *input, int mode, const char *lab
 #include <mutex>
 #include <atomic>
 #include <condition_variable>
-extern "C" void dp_hostprof_dump(void);
 namespace {
 struct ZkPool {
     std::vector<std::thread> th; std::mutex mu; std::condition_variable cv, done_cv;
@@ -224,7 +223,6 @@ struct ZkPool {
                 if (!inited) { dp::check(dp_init(device)); inited = true; }
                 if (delay > 0.0) std::this_thread::sleep_for(std::chrono::duration<double>(delay));
                 auto t0 = std::chrono::steady_clock::now();
-                struct timespec cts0; clock_gettime(CLOCK_THREAD_CPUTIME_ID, &cts0);
                 dp::DynTranscript t(label);
                 dp::zkml::Prover<dp::DynTranscript> prover(h->ctx, t);
                 std::vector<uint64_t> flat;
@@ -239,14 +237,12 @@ struct ZkPool {
                     memcpy(out, flat.data(), 8 * flat.size()); *out_len = flat.size();
                 }
                 const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-                if (getenv("DP_HOST_PROF") && idx == 0) { struct timespec cts1; clock_gettime(CLOCK_THREAD_CPUTIME_ID, &cts1);
-                    fprintf(stderr, "[worker0] proof wall %.2f ms, thread CPU %.2f ms, transcript permutations %llu\n", sec * 1e3, (cts1.tv_sec - cts0.tv_sec) * 1e3 + (cts1.tv_nsec - cts0.tv_nsec) * 1e-6, (unsigned long long)t.permutations()); }
                 if (!first_ever) { std::lock_guard<std::mutex> lk(mu); n_timed++; avg_proof_s += (sec - avg_proof_s) / (double)std::min<uint64_t>(n_timed, 64); }
             } catch (const std::exception &e) { std::lock_guard<std::mutex> lk(mu); failed = true; err = e.what(); }
             dp_profile_flush();   // per-kernel timing of the concurrent region (no-op unless dp_profile_enable(1))
             { std::lock_guard<std::mutex> lk(mu); inflight--; if (pending == 0 && inflight == 0) done_cv.notify_all(); }
         }
-        if (inited) { dp_synchronize(); if (getenv("DP_HOST_PROF")) { static std::atomic<int> once{0}; if (!once.exchange(1)) dp_hostprof_dump(); } dp_shutdown(); }
+        if (inited) { dp_synchronize(); dp_shutdown(); }
     }
     ~ZkPool() { { std::lock_guard<std::mutex> lk(mu); stop = true; } cv.notify_all(); for (auto &t : th) t.join(); }
 };
@@ -262,14 +258,13 @@ extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_wo
     ZkPool *pool;
     { std::lock_guard<std::mutex> lk(g_pools_mu); auto &pp = g_pools[handle]; if (!pp) { pp = std::make_unique<ZkPool>(); pp->h = h; pp->device = device; } pool = pp.get(); }
     while (pool->th.size() < n_workers) { const uint32_t idx = (uint32_t)pool->th.size(); pool->th.emplace_back([pool, idx] { pool->worker(idx); }); }
-    static const bool no_stagger = getenv("DP_NO_STAGGER") != nullptr;
     auto t0 = std::chrono::steady_clock::now();
     {
         std::lock_guard<std::mutex> lk(pool->mu);
         pool->label = label; pool->failed = false; pool->e2e = e2e != 0; pool->pending = n_proofs; pool->active = n_workers; pool->call_gen++;
         pool->out = out; pool->out_cap = cap; pool->out_len = out_len; if (out_len) *out_len = 0;
         // stagger only when every worker gets several proofs (otherwise the ramps cost more than the overlap gains)
-        pool->stagger_s = (!no_stagger && n_workers > 1 && n_proofs >= 3 * n_workers && pool->n_timed > 0) ? pool->avg_proof_s / n_workers : 0.0;
+        pool->stagger_s = (n_workers > 1 && n_proofs >= 3 * n_workers && pool->n_timed > 0) ? pool->avg_proof_s / n_workers : 0.0;
     }
     // only the first n_workers threads are woken usefully: notify_all, extra threads just compete for the same jobs
     pool->cv.notify_all();

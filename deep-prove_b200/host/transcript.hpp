@@ -92,17 +92,15 @@ class Sponge {
         if (nin_ || !nout_) duplex();
         return out_[--nout_];
     }
-    u64 permutations() const { return nperm_; }
   private:
     void duplex() {
         for (int i = 0; i < nin_; i++) st_[i] = in_[i];
         nin_ = 0;
-        Poseidon2::permute(st_); nperm_++;
+        Poseidon2::permute(st_);
         memcpy(out_, st_, 32); nout_ = 4;
     }
     u64 st_[8], in_[4], out_[4];
     int nin_ = 0, nout_ = 0;
-    u64 nperm_ = 0;
 };
 
 // trait Transcript<E> as implemented by BasicTranscript<E>
@@ -120,7 +118,6 @@ class BasicTranscript {
     void append_field_element_exts(const ExtVec &v) { for (auto &e : v) append_field_element_ext(e); }
     Ext read_challenge() { u64 a = sp_.sample(); u64 b = sp_.sample(); return Ext(a, b); }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
-    u64 permutations() const { return sp_.permutations(); }
   private:
     Sponge sp_;
 };
@@ -146,17 +143,16 @@ class BlakeTranscript {
     void append_field_element_exts(const ExtVec &v) { for (auto &e : v) append_field_element_ext(e); }
     Ext read_challenge() {
         for (;;) {
-            h_.update("challenge", 9); nfin_++;
+            h_.update("challenge", 9);
             uint8_t o[16]; h_.finalize(o, 16);
             u64 a, b; memcpy(&a, o, 8); memcpy(&b, o + 8, 8);
             if (a < P && b < P) return Ext(a, b);
         }
     }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
-    u64 permutations() const { return nfin_; }    // statistics: finalisations
   private:
     static size_t le(u64 c, uint8_t b[8]) { size_t n = 0; for (int k = 0; k < 8; k++) { b[k] = (uint8_t)(c >> (8 * k)); if (b[k]) n = k + 1; } return n ? n : 1; }
-    dpb3::Hasher h_; u64 nfin_ = 0;
+    dpb3::Hasher h_;
 };
 
 // The transcript the C entry points of the host library build: BasicTranscript, or BlakeTranscript after dph_set_hasher(1)
@@ -173,7 +169,6 @@ class DynTranscript {
     void append_field_element_exts(const ExtVec &v) { for (auto &e : v) append_field_element_ext(e); }
     Ext read_challenge() { return blake_ ? k_.read_challenge() : b_.read_challenge(); }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
-    u64 permutations() const { return blake_ ? k_.permutations() : b_.permutations(); }
   private:
     bool blake_; BasicTranscript b_; BlakeTranscript k_;
 };

@@ -8,7 +8,6 @@
 #pragma once
 #include "mpcs.hpp"
 #include <unordered_map>
-#include <chrono>
 #include <cstdlib>
 #include <cstdio>
 
@@ -338,12 +337,8 @@ class Prover {
         if (tr.outs.size() != m.nodes.size()) throw Error(DP_ERR_INVALID, "prove: the trace does not match the model");
         const std::map<size_t, ConvData> *conv_data = &tr.conv;
         auto node_input = [&](size_t id) -> const DeviceMle & { return id == 0 ? tr.input : tr.outs[id - 1]; };
-        static const bool prof = getenv("DP_HOST_PROF") != nullptr;
-        auto now = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-        double t0 = now();
         ctx_.write_to_transcript(t_);
         instantiate_witness_ctx(m, tr);
-        double t1 = now();
         // output claim (prover.rs:423-436)
         const DeviceMle &fo = tr.outs.back();
         Claim last; for (size_t i = 0, nv = fo.num_vars(); i < nv; i++) last.point.push_back(t_.read_challenge());
@@ -360,12 +355,8 @@ class Prover {
                 last = prove_convolution(id, last, conv_data->at(id));
             }
         }
-        double t2 = now();
         prove_tables();
-        double t3 = now();
         commit_prove();
-        double t4 = now();
-        if (prof) fprintf(stderr, "[zkml] witness+commits %.2f ms | layers %.2f ms | tables %.2f ms | batch_open %.2f ms | FS permutations %llu\n", t1 - t0, t2 - t1, t3 - t2, t4 - t3, (unsigned long long)t_.permutations());
         return std::move(proof_);
     }
 

@@ -49,18 +49,17 @@ uint64_t dp_kernel_launches(void);       /* number of kernels this library launc
 /* How a host thread waits for the device at the end of a round (process-wide).  0 (default) = spin on the completion word:
  * lowest latency, one busy core per proof in flight.  1 = sleep on a futex that ONE poller thread of the library signals:
  * ~5 us more per wait, but waiting proofs cost no CPU, so many more proofs than cores can be in flight per GPU (the
- * reference gets the same effect from rayon's sleeping workers).  Env DP_WAIT_MODE=1 selects it at start-up. */
+ * reference gets the same effect from rayon's sleeping workers). */
 int dp_set_wait_mode(int mode);
 int dp_get_wait_mode(void);
 /* Per-kernel timing with CUDA events recorded on the launch stream around each hot kernel (off by
- * default).  dp_profile_read fills parallel arrays (kernel name, launches, summed ms, summed algorithmic
- * bytes per SURVEY.md 8(d)) and returns the number of distinct kernels. */
+ * default).  dp_profile_read_ex fills parallel arrays (kernel name, launches, summed ms, summed algorithmic
+ * bytes per SURVEY.md 8(d), and, when `units` is not NULL, each kernel's own work unit summed over launches: Poseidon2
+ * permutations for the Merkle kernels, field operations for the sumcheck rounds, 0 elsewhere) and returns the number of
+ * distinct kernels.  The table is process-wide: proving threads fold their launches in with dp_profile_flush(), so a
+ * batch of concurrent proofs is profiled as it runs. */
 int dp_profile_enable(int on);
 int dp_profile_reset(void);
-int dp_profile_read(char (*names)[64], uint64_t *counts, double *total_ms, uint64_t *bytes, int cap);
-/* the same plus each kernel's own work unit summed over launches (Poseidon2 permutations for the Merkle kernels, field
- * operations for the sumcheck rounds; 0 elsewhere).  The table is process-wide: proving threads fold their launches in with
- * dp_profile_flush(), so a batch of concurrent proofs is profiled as it runs. */
 int dp_profile_read_ex(char (*names)[64], uint64_t *counts, double *total_ms, uint64_t *bytes, uint64_t *units, int cap);
 int dp_profile_flush(void);
 
@@ -105,14 +104,15 @@ int dp_sc_create(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *prod
  * previous round's challenge [c0,c1] afterwards.  out_evals receives (max_degree+1) x [c0,c1]:
  * the round polynomial at 0..max_degree, products already scaled, extrapolated and summed. */
 int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals);
-/* Opt in to the resident tail: once every table has <= 128 pairs (the last 8 rounds), ALL remaining rounds are served by one single-block
- * kernel that stays on the device, posts each round message to mapped host memory and polls a mapped mailbox for the next
- * challenge (no launch and no cross-block reduction per round).  Contract: between consecutive dp_sc_round calls on this
+/* Opt in to the resident tail: once a round's pairs, summed over the products, number <= 2048, ALL remaining rounds are served
+ * by one kernel that stays on the device: a thread-block cluster of up to 8 CTAs (~512 pairs each) that posts each round
+ * message to mapped host memory and polls a mapped mailbox for the next challenge (no launch per round).  Handles with more
+ * than 96 MLEs or 48 products keep the per-round kernels.  Contract: between consecutive dp_sc_round calls on this
  * handle the calling thread must not WAIT on other work submitted to the same stream (it would queue behind the
  * resident kernel).  The kernel gives up by itself after ~3 s without a challenge and dp_sc_round reports the error;
- * dp_sc_destroy releases it.  Results are identical with and without it.  Env DP_SC_NO_TAIL=1 disables it globally, and it
- * disables itself under tools that serialise kernel launches (Nsight Compute, compute-sanitizer): a one-time probe checks
- * that a running kernel can see a word the host posts after the launch call returned. */
+ * dp_sc_destroy releases it.  Results are identical with and without it.  It disables itself under tools that serialise
+ * kernel launches (Nsight Compute, compute-sanitizer): a one-time probe checks that a running kernel can see a word the
+ * host posts after the launch call returned. */
 int dp_sc_set_resident_tail(dp_sc *s, int enable);
 /* Tail of prove_parallel (prover.rs:544-568) + get_mle_final_evaluations (:474-490): fixes the last
  * challenge and writes n_mles x [c0,c1]. */
@@ -121,8 +121,6 @@ int dp_sc_destroy(dp_sc *s);
 /* Non-owning view of MLE `idx` as folded so far (valid until the next dp_sc_round / dp_sc_destroy):
  * the state's `poly.flattened_ml_extensions[idx]` after the rounds run so far. */
 int dp_sc_current_mle(dp_sc *s, uint32_t idx, dp_mle **out_view);
-/* Algorithmic HBM bytes moved by the last dp_sc_round (SURVEY.md 8(d) rules), for roofline reports. */
-uint64_t dp_sc_last_round_bytes(const dp_sc *s);
 
 /* ---- zkml lookup: LogUp-GKR fractional-sum circuit (zkml/src/lookup/logup_gkr/circuit.rs) --------------- */
 typedef struct dp_logup dp_logup;

@@ -1,7 +1,8 @@
-"""CPU tests: the C-ABI library loads, exports every symbol include/deepprove_b200.h declares, and
-refuses to compute without a GPU (no CPU fallback)."""
+"""CPU tests: the C-ABI library loads, exports every symbol include/deepprove_b200.h declares (and the host
+library imports no other), and refuses to compute without a GPU (no CPU fallback)."""
 import os
 import re
+import subprocess
 import dpb200
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -20,6 +21,15 @@ def test_every_declared_symbol_is_exported():
     for s in syms:
         assert hasattr(lib, s), "libdeepprove_b200.so does not export %s" % s
     assert sorted(dpb200.ABI_SYMBOLS) == syms, "dpb200.ABI_SYMBOLS out of sync with the header"
+
+
+def test_host_library_links_only_against_the_c_abi():
+    """libdeepprove_host.so calls into libdeepprove_b200.so through the public header alone (DESIGN.md section 1)"""
+    dpb200.host()
+    out = subprocess.run(["nm", "-D", "--undefined-only", dpb200.HOST_LIB_PATH], check=True, capture_output=True, text=True).stdout
+    imported = set(re.findall(r"\bU (dp_[a-z0-9_]+)\b", out))
+    assert imported, "no dp_* import found: nm output not understood"
+    assert sorted(imported - set(header_symbols())) == []
 
 
 def test_no_cpu_fallback_without_gpu():

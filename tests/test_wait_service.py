@@ -26,8 +26,7 @@ def lib():
     L.dp_set_wait_mode(before)
 
 
-def test_blocking_wait_wakes_and_sleeps(lib, monkeypatch):
-    monkeypatch.setenv("DP_WAIT_SPINNERS", "0")
+def test_blocking_wait_wakes_and_sleeps(lib):
     assert lib.dp_set_wait_mode(1) == 0
     words = [C.c_uint64(0) for _ in range(12)]
     out = [None] * 12

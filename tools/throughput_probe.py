@@ -1,7 +1,6 @@
 #!/usr/bin/env python3
 """Where does multi-proof throughput saturate?  Dense-4M proofs/s and kernel launches/s against the number of proving threads
-(each with its own stream + arena) on one GPU.  With DP_HOST_PROF=1 in the environment the first worker's host-side time
-accumulators are dumped when the pool is torn down.   usage: throughput_probe.py [workers ...]"""
+(each with its own stream + arena) on one GPU.   usage: throughput_probe.py [workers ...]"""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "deep-prove_b200"))

@@ -1,20 +1,22 @@
 #!/usr/bin/env python3
 """CUDA runtime API census of W concurrent Dense-4M proofs: calls per proof and time the proving threads spend inside each call
-(CUPTI callbacks; kernel-timeline tracing stays off).  usage: [DP_WAIT_MODE=1] trace_api.py [workers] [proofs]"""
+(CUPTI callbacks; kernel-timeline tracing stays off).  usage: trace_api.py [workers] [proofs] [wait mode: 0 spin (default) | 1 block]
+-> api_w<workers>_mode<mode>.csv in the current directory + a summary"""
 import ctypes as C, os, sys, csv
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "deep-prove_b200"))
 import bench, dpb200 as dp
 W = int(sys.argv[1]) if len(sys.argv) > 1 else 16
 N = int(sys.argv[2]) if len(sys.argv) > 2 else 2 * W
+MODE = int(sys.argv[3]) if len(sys.argv) > 3 else 0
 T = C.CDLL(os.path.join(ROOT, "deep-prove_b200", "libdp_trace.so"))
 T.dp_trace_api_stop.argtypes = [C.c_char_p]
+dp.set_wait_mode(MODE)
 wl = bench.DenseWorkload(); dp.init(0); wl.setup_device(dp)
 wl.ctx.prove_concurrent(W, W)
 assert T.dp_trace_api_start() == 0
 sec = wl.ctx.prove_concurrent(W, N)
-path = os.path.join(ROOT, "gpurun_out", "api_w%d_mode%s.csv" % (W, os.environ.get("DP_WAIT_MODE", "0")))
-os.makedirs(os.path.dirname(path), exist_ok=True)
+path = os.path.abspath("api_w%d_mode%d.csv" % (W, MODE))
 T.dp_trace_api_stop(path.encode())
 rows = sorted(csv.DictReader(open(path)), key=lambda r: -float(r["total_ms"]))
 tot = sum(float(r["total_ms"]) for r in rows)
