@@ -841,6 +841,7 @@ int dp_sc_create(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *prod
         seen_deg = std::max(seen_deg, pr.n_idx);
     }
     DP_CHECK(seen_deg <= max_deg, DP_ERR_INVALID, "dp_sc_create: max_degree smaller than a product's degree");
+    DP_CHECK(max_deg <= 5, DP_ERR_UNSUPPORTED, "do not support degree > 5");  // prover.rs:710; sc_glue's message arrays hold degree 5
     dp_sc *s = new dp_sc();
     s->n_mles = n_mles; s->n_products = n_products; s->max_nv = max_nv; s->max_deg = max_deg;
     s->mles.resize(n_mles);

@@ -97,7 +97,8 @@ typedef struct dp_sc_product {
 
 /* IOPProverState::prover_init_parallel (sumcheck/src/prover.rs:588-612).  Input MLEs are BORROWED and
  * never modified (the reference clones on the first fold, prover.rs:659-670); they must stay alive
- * until dp_sc_destroy.  All MLEs of one product must have equal length (virtual_poly.rs:148-160). */
+ * until dp_sc_destroy.  All MLEs of one product must have equal length (virtual_poly.rs:148-160).
+ * max_degree must lie between the highest product degree and 5; above 5 it is DP_ERR_UNSUPPORTED (prover.rs:710). */
 int dp_sc_create(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *products, uint32_t n_products,
                  uint32_t max_num_variables, uint32_t max_degree, dp_sc **out);
 /* prove_round_and_update_state_parallel (prover.rs:625-741): `challenge` is NULL in round 0 and the
