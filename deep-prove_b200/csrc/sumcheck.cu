@@ -34,31 +34,6 @@ template <bool CG> __device__ __forceinline__ gle ldx_e(const gle *p) {
 template <bool CG> __device__ __forceinline__ ulonglong2 ldx_b2(const u64 *p) { return CG ? __ldcg(reinterpret_cast<const ulonglong2 *>(p)) : ld_b2(p); }
 template <bool CG> __device__ __forceinline__ u64 ldx_b(const u64 *p) { return CG ? __ldcg(p) : *p; }
 
-template <bool CG = false>
-__device__ __forceinline__ void sc_load_pair(const ScOp &op, u64 i, gle r, gle &lo, gle &hi) {
-    switch (op.mode) {
-    case OPM_B: {
-        ulonglong2 v = ldx_b2<CG>((const u64 *)op.src + 2 * i);
-        lo = e_from_base(v.x); hi = e_from_base(v.y);
-    } break;
-    case OPM_E: {
-        const gle *s = (const gle *)op.src + 2 * i;
-        lo = ldx_e<CG>(s); hi = ldx_e<CG>(s + 1);
-    } break;
-    case OPM_BF: {
-        const u64 *s = (const u64 *)op.src + 4 * i;
-        ulonglong2 v0 = ldx_b2<CG>(s), v1 = ldx_b2<CG>(s + 2);
-        lo = fold_b(v0.x, v0.y, r); hi = fold_b(v1.x, v1.y, r);
-        if (op.dst) { st_e(op.dst + 2 * i, lo); st_e(op.dst + 2 * i + 1, hi); }
-    } break;
-    default: {
-        const gle *s = (const gle *)op.src + 4 * i;
-        gle f0 = ldx_e<CG>(s), f1 = ldx_e<CG>(s + 1), f2 = ldx_e<CG>(s + 2), f3 = ldx_e<CG>(s + 3);
-        lo = fold_e(f0, f1, r); hi = fold_e(f2, f3, r);
-        if (op.dst) { st_e(op.dst + 2 * i, lo); st_e(op.dst + 2 * i + 1, hi); }
-    } break;
-    }
-}
 // length-1 operands (sumcheck_macro/src/lib.rs:236-241): value at every evaluation point
 template <bool CG = false>
 __device__ __forceinline__ gle sc_load_const(const ScOp &op, gle r) {
@@ -201,6 +176,30 @@ __device__ __forceinline__ void sc_body_split(const ScProd &pd, gle r, gle acc[S
     for (int tt = 0; tt <= D; tt++) if (tt == (int)t) acc[tt] = p;
 }
 
+// Degree dispatch of the bodies: DSEL = 1..5 is the degree of every product; DSEL = 0 takes the product's own degree
+template <int DSEL, bool CG>
+__device__ __forceinline__ void sc_body_dsel(const ScProd &pd, gle r, gle acc[SC_NACC], const u64 tid, const u64 stride) {
+    if constexpr (DSEL != 0) sc_body<DSEL, CG>(pd, r, acc, tid, stride);
+    else switch (pd.d) {
+    case 1: sc_body<1, CG>(pd, r, acc, tid, stride); break;
+    case 2: sc_body<2, CG>(pd, r, acc, tid, stride); break;
+    case 3: sc_body<3, CG>(pd, r, acc, tid, stride); break;
+    case 4: sc_body<4, CG>(pd, r, acc, tid, stride); break;
+    default: sc_body<5, CG>(pd, r, acc, tid, stride); break;
+    }
+}
+template <int DSEL, bool CG>
+__device__ __forceinline__ void sc_body_split_dsel(const ScProd &pd, gle r, gle acc[SC_NACC], const u64 L, const u32 tpl) {
+    if constexpr (DSEL != 0) sc_body_split<DSEL, CG>(pd, r, acc, L, tpl);
+    else switch (pd.d) {
+    case 1: sc_body_split<1, CG>(pd, r, acc, L, tpl); break;
+    case 2: sc_body_split<2, CG>(pd, r, acc, L, tpl); break;
+    case 3: sc_body_split<3, CG>(pd, r, acc, L, tpl); break;
+    case 4: sc_body_split<4, CG>(pd, r, acc, L, tpl); break;
+    default: sc_body_split<5, CG>(pd, r, acc, L, tpl); break;
+    }
+}
+
 // completion signal: `out` and `flag` live in mapped pinned host memory, so the round message reaches the host
 // with the kernel's own stores -- no D2H copy node, and the host spins on the flag instead of a stream sync.
 // Called by ONE thread after a block barrier that follows the message stores of its block mates: its system-scope fence
@@ -305,14 +304,7 @@ k_sc_round(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc
 #pragma unroll
     for (int t = 0; t < SC_NACC; t++) acc[t] = e_zero();
     const u64 gtid = (u64)blockIdx.x * blockDim.x + threadIdx.x, gstride = (u64)gridDim.x * blockDim.x;
-    if (DSEL != 0) sc_body<DSEL == 0 ? 1 : DSEL>(pd, r, acc, gtid, gstride);
-    else switch (pd.d) {
-    case 1: sc_body<1>(pd, r, acc, gtid, gstride); break;
-    case 2: sc_body<2>(pd, r, acc, gtid, gstride); break;
-    case 3: sc_body<3>(pd, r, acc, gtid, gstride); break;
-    case 4: sc_body<4>(pd, r, acc, gtid, gstride); break;
-    default: sc_body<5>(pd, r, acc, gtid, gstride); break;
-    }
+    sc_body_dsel<DSEL, false>(pd, r, acc, gtid, gstride);
     sc_epilogue<SC_THREADS>(acc, DSEL != 0 ? DSEL + 1 : (int)pd.d + 1, partials, counters, out, seq, flag, done);
 }
 
@@ -443,16 +435,50 @@ k_sc_lean(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc0
 // <= 2048 threads + two cluster barriers (~0.2 us each) + two PCIe hops + the host sponge -- no launch, no cross-block ticket
 // stage, no cold instruction cache.  The folded tables ping-pong in HBM/L2 (the cluster barrier orders the stores; readers use
 // L1-bypassing loads).  The per-round bookkeeping the host does for k_sc_round (operand order, fold destinations, ping-pong
-// buffers) is replayed identically by every CTA in shared memory.  The kernel cannot hang: the poll gives up after
+// buffers) runs in every CTA's shared memory through the same functions (sc_desc, sc_commit_fold).  The kernel cannot hang: the poll gives up after
 // SC_RES_TIMEOUT cycles or when the host posts the abort value, and the other CTAs only ever wait on the cluster barrier.
 // Opt-in per handle (dp_sc_set_resident_tail): the caller promises not to wait on other work in the same stream between rounds.
 static constexpr u32 SC_RES_MAXM = 96, SC_RES_MAXP = 48, SC_RES_MAXCTA = 8;
 static constexpr u64 SC_RES_WORK = 2048;                     // resident once sum over products of (pairs this round) <= this (larger rounds are faster in the multi-block kernels; 2048 measured best of 1024 / 2048 / 4096 on H100)
 static constexpr long long SC_RES_TIMEOUT = 6000000000LL;   // ~3 s at 1.9 GHz
 static constexpr u64 SC_TAIL_ABORT = ~0ULL, SC_TAIL_FAILED = ~0ULL - 1;
-struct TMle { const void *cur; gle *work; u64 len, len0; u32 is_ext, where; };
+static constexpr u32 SC_NO_WRITER = ~0u;
+
+// Round state of one MLE, kept by the host for the per-round kernels and by every CTA of the resident kernel
+struct ScMle {
+    const void *cur; gle *work;   // work: [len0/2 + len0/4] E: ping (offset 0) / pong (offset len0/2)
+    u64 len, len0;
+    u32 is_ext, where;            // where: 0 = caller's input, 1 = ping, 2 = pong (3 = owned by the resident kernel)
+};
+__host__ __device__ inline gle *sc_fold_dst(const ScMle &m) { return m.where == 1 ? m.work + (m.len0 >> 1) : m.work; }
+__host__ __device__ inline void sc_commit_fold(ScMle &m, gle *dst) { m.cur = dst; m.where = dst == m.work ? 1 : 2; m.len >>= 1; m.is_ext = 1; }
+
+// Descriptor of product p this round.  fold[i] / dst[i]: MLE i halves this round into dst[i]; writer[i]: the product that stores
+// the folded table (the first one referencing MLE i; its first operand on MLE i does the store).  The macro sorts Ext operands first
+// (sumcheck_macro/src/lib.rs:87-140); multiplication commutes, so only operand 0 must be an Ext one when the product is mixed (the
+// bodies multiply INTO it).
+__host__ __device__ inline void sc_desc(ScProd &pd, u32 p, const u32 *idx, u32 n_idx, const ScMle *mles, const unsigned char *fold,
+                                        gle *const *dst, const u32 *writer) {
+    u32 order[5], c = 0;
+    for (u32 j = 0; j < n_idx; j++) if (mles[idx[j]].is_ext || fold[idx[j]]) order[c++] = j;
+    for (u32 j = 0; j < n_idx; j++) if (!(mles[idx[j]].is_ext || fold[idx[j]])) order[c++] = j;
+    bool allbase = true; u64 newlen = 0;
+    for (u32 jj = 0; jj < n_idx; jj++) {
+        const u32 mi = idx[order[jj]]; const ScMle &m = mles[mi]; ScOp &op = pd.op[jj];
+        op.src = m.cur; op.dst = nullptr;
+        if (fold[mi]) {
+            op.mode = m.is_ext ? OPM_EF : OPM_BF;
+            bool first = writer[mi] == p;
+            for (u32 q = 0; q < jj; q++) if (idx[order[q]] == mi) first = false;
+            if (first) op.dst = dst[mi];
+            newlen = m.len >> 1; allbase = false;
+        } else { op.mode = m.is_ext ? OPM_E : OPM_B; newlen = m.len; if (m.is_ext) allbase = false; }
+    }
+    pd.d = n_idx; pd.allbase = allbase; pd.konst = newlen == 1; pd.npairs = newlen >> 1;
+}
+
 struct TProd { u32 n_idx; u32 idx[5]; };
-struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; TMle m[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; };
+struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; ScMle m[SC_RES_MAXM]; u32 writer[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; };
 
 __device__ __forceinline__ u32 cl_rank() { u32 r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ u32 cl_size() { u32 r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
@@ -465,22 +491,20 @@ template <int DSEL>
 __global__ void __launch_bounds__(SC_THREADS)
 k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pairs /* mapped */, volatile u64 *flag /* mapped */,
          volatile u64 *chal /* mapped: [seq, c0, c1] */, u64 seq0, gle *xpart /* device: warp partials */, u64 *xctl /* device: [status, c0, c1] */) {
-    __shared__ TMle sm[SC_RES_MAXM];
+    __shared__ ScMle sm[SC_RES_MAXM];
     __shared__ TProd sp[SC_RES_MAXP];
     __shared__ ScProd spd[SC_RES_MAXP];
     __shared__ gle *sdst[SC_RES_MAXM];
-    __shared__ unsigned char sfold[SC_RES_MAXM], swriter[SC_RES_MAXM];
+    __shared__ u32 swriter[SC_RES_MAXM];
+    __shared__ unsigned char sfold[SC_RES_MAXM];
     const u32 nm = cfg->n_mles, np = cfg->n_products, nr = cfg->n_rounds;
     const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = SC_THREADS / 32;
     const u32 rank = cl_rank(), ncta = cl_size();
     const u32 W = ncta * nwarps, gw = rank * nwarps + warp;              // warps of the cluster, this warp's index
     // pairs of a product are split over G warps (G a power of two, np * G <= W); with more products than warps a warp takes several
     u32 G = 1; while (np * (G << 1) <= W) G <<= 1;
-    for (u32 i = threadIdx.x; i < nm; i += blockDim.x) { sm[i] = cfg->m[i]; swriter[i] = 0xff; }
+    for (u32 i = threadIdx.x; i < nm; i += blockDim.x) { sm[i] = cfg->m[i]; swriter[i] = cfg->writer[i]; }
     for (u32 i = threadIdx.x; i < np; i += blockDim.x) sp[i] = cfg->p[i];
-    __syncthreads();
-    // the product that writes an MLE's folded table is the first one referencing it (the host's `written` rule); static
-    if (threadIdx.x == 0) for (u32 p = 0; p < np; p++) for (u32 j = 0; j < sp[p].n_idx; j++) { u32 mi = sp[p].idx[j]; if (swriter[mi] == 0xff) swriter[mi] = (unsigned char)p; }
     __syncthreads();
     gle r = r0;
     // The descriptors of a round depend on the fold bookkeeping only, never on the challenge VALUE: they are rebuilt right after a
@@ -490,27 +514,10 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
         for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
             bool f = fold && sm[i].len > 1;
             sfold[i] = f;
-            sdst[i] = f ? ((sm[i].where == 1) ? sm[i].work + (sm[i].len0 >> 1) : sm[i].work) : nullptr;
+            sdst[i] = f ? sc_fold_dst(sm[i]) : nullptr;
         }
         __syncthreads();
-        for (u32 p = threadIdx.x; p < np; p += blockDim.x) {   // the descriptor the host builds for k_sc_round, one thread per product
-            const TProd &pr = sp[p]; ScProd &pd = spd[p];
-            u32 order[5], c = 0;
-            for (u32 j = 0; j < pr.n_idx; j++) { u32 mi = pr.idx[j]; if (sm[mi].is_ext || sfold[mi]) order[c++] = j; }
-            for (u32 j = 0; j < pr.n_idx; j++) { u32 mi = pr.idx[j]; if (!(sm[mi].is_ext || sfold[mi])) order[c++] = j; }
-            bool allbase = true, wrote[5] = {false, false, false, false, false}; u64 newlen = 0;
-            for (u32 jj = 0; jj < pr.n_idx; jj++) {
-                u32 mi = pr.idx[order[jj]]; const TMle &m = sm[mi]; ScOp &op = pd.op[jj];
-                op.src = m.cur; op.dst = nullptr;
-                if (sfold[mi]) {
-                    op.mode = m.is_ext ? OPM_EF : OPM_BF;
-                    bool dup = false; for (u32 q = 0; q < jj; q++) if (wrote[q] && pr.idx[order[q]] == mi) dup = true;
-                    if (swriter[mi] == p && !dup) { op.dst = sdst[mi]; wrote[jj] = true; }
-                    newlen = m.len >> 1; allbase = false;
-                } else { op.mode = m.is_ext ? OPM_E : OPM_B; newlen = m.len; if (m.is_ext) allbase = false; }
-            }
-            pd.d = pr.n_idx; pd.allbase = allbase; pd.konst = newlen == 1; pd.npairs = newlen >> 1;
-        }
+        for (u32 p = threadIdx.x; p < np; p += blockDim.x) sc_desc(spd[p], p, sp[p].idx, sp[p].n_idx, sm, sfold, sdst, swriter);
         __syncthreads();
     };
     build_descs(cfg->first_has_challenge != 0);
@@ -542,24 +549,8 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
             const u64 first = (u64)s * 32 + lane, stride = (u64)G * 32;
             const u32 tpl = pd.d <= 3 ? 2 : 3;
             const bool split = !pd.konst && !pd.allbase && (pd.npairs << tpl) <= stride;     // uniform over the warps of this product
-            if (split) {
-                if (DSEL != 0) sc_body_split<DSEL == 0 ? 1 : DSEL, true>(pd, r, acc, first, tpl);
-                else switch (pd.d) {
-                case 1: sc_body_split<1, true>(pd, r, acc, first, tpl); break;
-                case 2: sc_body_split<2, true>(pd, r, acc, first, tpl); break;
-                case 3: sc_body_split<3, true>(pd, r, acc, first, tpl); break;
-                case 4: sc_body_split<4, true>(pd, r, acc, first, tpl); break;
-                default: sc_body_split<5, true>(pd, r, acc, first, tpl); break;
-                }
-            } else
-            if (DSEL != 0) sc_body<DSEL == 0 ? 1 : DSEL, true>(pd, r, acc, first, stride);
-            else switch (pd.d) {
-            case 1: sc_body<1, true>(pd, r, acc, first, stride); break;
-            case 2: sc_body<2, true>(pd, r, acc, first, stride); break;
-            case 3: sc_body<3, true>(pd, r, acc, first, stride); break;
-            case 4: sc_body<4, true>(pd, r, acc, first, stride); break;
-            default: sc_body<5, true>(pd, r, acc, first, stride); break;
-            }
+            if (split) sc_body_split_dsel<DSEL, true>(pd, r, acc, first, tpl);
+            else sc_body_dsel<DSEL, true>(pd, r, acc, first, stride);
             const int nacc = DSEL != 0 ? DSEL + 1 : (int)pd.d + 1;
 #pragma unroll
             for (int t = 0; t < SC_NACC; t++) if (t < nacc) {     // lazy 96-bit warp sums, one reduction per limb (see sc_epilogue)
@@ -591,15 +582,12 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
                 if (lane == 0) st_e(out + (u64)p * SC_NACC + t, e_make(ws_reduce(v0), ws_reduce(v1)));
             }
         }
-        for (u32 i = threadIdx.x; i < nm; i += blockDim.x) if (sfold[i]) {     // fold bookkeeping (every CTA keeps its own copy)
-            TMle &m = sm[i];
-            m.cur = sdst[i]; m.where = (sdst[i] == m.work) ? 1 : 2; m.len >>= 1; m.is_ext = 1;
-        }
+        for (u32 i = threadIdx.x; i < nm; i += blockDim.x) if (sfold[i]) sc_commit_fold(sm[i], sdst[i]);   // every CTA keeps its own copy
         __syncthreads();
         if (rank == 0) {
             if (k == nr - 1) {   // last round: hand the (<= 2)-entry tables over with the message (k_sc_gather's job)
                 for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
-                    const TMle &m = sm[i]; gle a, b;
+                    const ScMle &m = sm[i]; gle a, b;
                     if (m.is_ext) { a = ldx_e<true>((const gle *)m.cur); b = m.len > 1 ? ldx_e<true>((const gle *)m.cur + 1) : a; }
                     else { a = e_from_base(ldx_b<true>((const u64 *)m.cur)); b = m.len > 1 ? e_from_base(ldx_b<true>((const u64 *)m.cur + 1)) : a; }
                     st_e(pairs + 2 * i, a); st_e(pairs + 2 * i + 1, b);
@@ -614,17 +602,6 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
 }
 
 struct ScFin { const void *src; u32 mode; u32 len; };
-__global__ void k_sc_final(const ScFin *__restrict__ f, u32 n, gle r, gle *__restrict__ out) {
-    u32 m = blockIdx.x * blockDim.x + threadIdx.x;
-    if (m >= n) return;
-    ScFin d = f[m];
-    gle v;
-    if (d.len == 1) v = d.mode == OPM_E ? ld_e((const gle *)d.src) : e_from_base(*(const u64 *)d.src);
-    else if (d.mode == OPM_E) { const gle *s = (const gle *)d.src; v = fold_e(ld_e(s), ld_e(s + 1), r); }
-    else { ulonglong2 q = ld_b2((const u64 *)d.src); v = fold_b(q.x, q.y, r); }
-    st_e(out + m, v);
-}
-
 // after the LAST round every MLE has <= 2 entries: copy them out with the round message so the closing fold
 // (prover.rs:544-568) needs no further device round trip
 __global__ void k_sc_gather(const ScFin *__restrict__ f, u32 n, gle *__restrict__ out /* 2 per MLE */) {
@@ -638,15 +615,11 @@ __global__ void k_sc_gather(const ScFin *__restrict__ f, u32 n, gle *__restrict_
 }
 
 // ---------------------------------------------------------------------------------------------------
-struct ScMle {
-    const void *cur = nullptr; u64 len = 0; bool is_ext = false;
-    gle *work = nullptr;  // [len0/2 + len0/4] E: ping (offset 0) / pong (offset len0/2)
-    u64 len0 = 0; int where = 0;  // 0 = caller's input, 1 = ping, 2 = pong
-};
 struct dp_sc {
     u32 n_mles = 0, n_products = 0, max_nv = 0, max_deg = 0, round = 0;
     bool finished = false;
     std::vector<ScMle> mles;
+    std::vector<u32> writer;                              // per MLE: the product that stores its folded tables (SC_NO_WRITER: none)
     std::vector<dp_sc_product> products;
     ScProd *d_descs = nullptr, *h_descs = nullptr;
     gle *d_partials = nullptr, *d_out = nullptr, *h_out = nullptr;
@@ -752,20 +725,16 @@ static u64 sc_round_work(const dp_sc *s, bool fold) {
 }
 static bool sc_tail_eligible(const dp_sc *s, bool fold) {
     if (!s->tail_enabled || s->n_mles > SC_RES_MAXM || s->n_products > SC_RES_MAXP || s->max_nv - s->round < 2) return false;
-    std::vector<char> used(s->n_mles, 0);
-    for (auto &pr : s->products) for (u32 j = 0; j < pr.n_idx; j++) used[pr.idx[j]] = 1;
-    for (u32 i = 0; i < s->n_mles; i++) if (!used[i] && s->mles[i].len > 1) return false;
+    for (u32 i = 0; i < s->n_mles; i++) if (s->writer[i] == SC_NO_WRITER && s->mles[i].len > 1) return false;
     return sc_round_work(s, fold) <= SC_RES_WORK;
 }
-template <int DSEL>
-static cudaError_t sc_res_launch(u32 ncta, cudaStream_t st, const ScTail *cfg, gle r, gle *out, gle *pairs, u64 *flag, u64 *chal, u64 seq, gle *xpart, u64 *xctl) {
-    cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(ncta); lc.blockDim = dim3(SC_THREADS); lc.dynamicSmemBytes = 0; lc.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    lc.attrs = at; lc.numAttrs = 1;
-    return cudaLaunchKernelEx(&lc, k_sc_res<DSEL>, cfg, r, out, pairs, (volatile u64 *)flag, (volatile u64 *)chal, seq, xpart, xctl);
-}
+// the kernels by DSEL (0: mixed degrees, 1..5: every product has this degree) and the lean ones by [MODE][D - 2]
+static decltype(&k_sc_res<0>) const k_sc_res_dsel[6] = {k_sc_res<0>, k_sc_res<1>, k_sc_res<2>, k_sc_res<3>, k_sc_res<4>, k_sc_res<5>};
+static decltype(&k_sc_round<0>) const k_sc_round_dsel[6] = {k_sc_round<0>, k_sc_round<1>, k_sc_round<2>, k_sc_round<3>, k_sc_round<4>, k_sc_round<5>};
+static decltype(&k_sc_round<0>) const k_sc_lean_md[4][2] = {{k_sc_lean<2, OPM_B>, k_sc_lean<3, OPM_B>}, {k_sc_lean<2, OPM_E>, k_sc_lean<3, OPM_E>},
+                                                              {k_sc_lean<2, OPM_BF>, k_sc_lean<3, OPM_BF>}, {k_sc_lean<2, OPM_EF>, k_sc_lean<3, OPM_EF>}};
+static constexpr int SC_LEAN_BLOCK[4] = {ScLeanShape<OPM_B>::BLOCK, ScLeanShape<OPM_E>::BLOCK, ScLeanShape<OPM_BF>::BLOCK, ScLeanShape<OPM_EF>::BLOCK};
+
 // one round served by the resident kernel (started here on its first round)
 static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
     cudaStream_t st = dp_ctx().stream;
@@ -779,7 +748,7 @@ static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
         for (u32 i = 0; i < s->n_mles; i++) {
             ScMle &m = s->mles[i];
             if (m.len > 1 && !m.work) { if ((e = dp_dev_alloc((void **)&m.work, sizeof(gle) * ((m.len0 >> 1) + (m.len0 >> 2) + 1)))) return e; }
-            t.m[i].cur = m.cur; t.m[i].work = m.work; t.m[i].len = m.len; t.m[i].len0 = m.len0; t.m[i].is_ext = m.is_ext; t.m[i].where = (u32)m.where;
+            t.m[i] = m; t.writer[i] = s->writer[i];
         }
         for (u32 p = 0; p < s->n_products; p++) { t.p[p].n_idx = s->products[p].n_idx; for (u32 j = 0; j < 5; j++) t.p[p].idx[j] = s->products[p].idx[j]; }
         s->h_chal[0] = 0;
@@ -791,16 +760,14 @@ static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
         if (!s->d_xctl && (e = dp_dev_alloc((void **)&s->d_xctl, 64))) return e;
         u32 dsel = s->products[0].n_idx;
         for (auto &pr : s->products) if (pr.n_idx != dsel) dsel = 0;
+        cudaLaunchConfig_t lc{};
+        lc.gridDim = dim3(ncta); lc.blockDim = dim3(SC_THREADS); lc.dynamicSmemBytes = 0; lc.stream = st;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        lc.attrs = at; lc.numAttrs = 1;
         DpProfScope prof("k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)", 0);
-        cudaError_t ce;
-        switch (dsel) {
-        case 1: ce = sc_res_launch<1>(ncta, st, s->h_tail, r, s->h_out, s->h_pairs, s->h_flag, s->h_chal, s->seq, s->d_xpart, s->d_xctl); break;
-        case 2: ce = sc_res_launch<2>(ncta, st, s->h_tail, r, s->h_out, s->h_pairs, s->h_flag, s->h_chal, s->seq, s->d_xpart, s->d_xctl); break;
-        case 3: ce = sc_res_launch<3>(ncta, st, s->h_tail, r, s->h_out, s->h_pairs, s->h_flag, s->h_chal, s->seq, s->d_xpart, s->d_xctl); break;
-        case 4: ce = sc_res_launch<4>(ncta, st, s->h_tail, r, s->h_out, s->h_pairs, s->h_flag, s->h_chal, s->seq, s->d_xpart, s->d_xctl); break;
-        case 5: ce = sc_res_launch<5>(ncta, st, s->h_tail, r, s->h_out, s->h_pairs, s->h_flag, s->h_chal, s->seq, s->d_xpart, s->d_xctl); break;
-        default: ce = sc_res_launch<0>(ncta, st, s->h_tail, r, s->h_out, s->h_pairs, s->h_flag, s->h_chal, s->seq, s->d_xpart, s->d_xctl); break;
-        }
+        const cudaError_t ce = cudaLaunchKernelEx(&lc, k_sc_res_dsel[dsel], (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs, (volatile u64 *)s->h_flag,
+                                                  (volatile u64 *)s->h_chal, s->seq, s->d_xpart, s->d_xctl);
         DP_LAUNCHED();
         DP_CUDA(ce);
         DP_CUDA(cudaGetLastError());
@@ -851,6 +818,8 @@ int dp_sc_create(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *prod
         m.cur = mles[i]->data; m.len = m.len0 = mles[i]->len; m.is_ext = mles[i]->is_ext; m.where = 0;
         max_pairs = std::max<u64>(max_pairs, m.len >> 1);
     }
+    s->writer.assign(n_mles, SC_NO_WRITER);
+    for (u32 p = n_products; p-- > 0;) for (u32 j = 0; j < products[p].n_idx; j++) s->writer[products[p].idx[j]] = p;
     s->products.assign(products, products + n_products);
     for (auto &pr : s->products) { pr.coef[0] = gl_canon(pr.coef[0]); pr.coef[1] = gl_canon(pr.coef[1]); }
     s->gx = (int)std::min<u64>((max_pairs + 127) / 128 + 1, (u64)dp_ctx().sm_count * 16);   // upper bound of any round's grid (partials buffer): lean folding rounds use 128-thread blocks, one pair per thread
@@ -867,7 +836,7 @@ int dp_sc_create(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *prod
         *s->h_flag = 0;
         if ((e = dp_dev_alloc((void **)&s->d_fin, sizeof(ScFin) * n_mles + sizeof(gle) * 2 * n_mles))) return e;
         if ((e = dp_pinned_alloc((void **)&s->h_descs, sizeof(ScProd) * n_products))) return e;
-        if ((e = dp_pinned_alloc((void **)&s->h_out, sizeof(gle) * std::max<size_t>(SC_NACC * n_products, n_mles)))) return e;
+        if ((e = dp_pinned_alloc((void **)&s->h_out, sizeof(gle) * SC_NACC * n_products))) return e;
         if ((e = dp_pinned_alloc((void **)&s->h_fin, sizeof(ScFin) * n_mles))) return e;
         if ((e = dp_pinned_alloc((void **)&s->h_pairs, sizeof(gle) * 2 * n_mles))) return e;
         return DP_OK;
@@ -896,50 +865,24 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
     if (s->tail_active || sc_tail_eligible(s, fold)) return sc_tail_round(s, r, fold, out_evals);
     // plan this round's folds: every MLE with >= 1 variable halves (prover.rs:659-684)
     std::vector<gle *> dst(s->n_mles, nullptr);
-    std::vector<char> folds(s->n_mles, 0), written(s->n_mles, 0);
+    std::vector<unsigned char> folds(s->n_mles, 0);
+    u64 bytes = 0, round_pairs = 1;                       // bytes: operand reads + folded-table writes, for the profile
     if (fold) {
         for (u32 i = 0; i < s->n_mles; i++) {
             ScMle &m = s->mles[i];
             if (m.len <= 1) continue;
             if (!m.work) { if (int e = dp_dev_alloc((void **)&m.work, sizeof(gle) * ((m.len0 >> 1) + (m.len0 >> 2) + 1))) return e; }
             folds[i] = 1;
-            dst[i] = (m.where == 1) ? m.work + (m.len0 >> 1) : m.work;
+            dst[i] = sc_fold_dst(m);
+            if (s->writer[i] != SC_NO_WRITER) bytes += (m.len >> 1) * 16;
         }
     }
-    u64 bytes = 0, round_pairs = 1;
     for (u32 p = 0; p < s->n_products; p++) {
         const dp_sc_product &pr = s->products[p];
         ScProd &d = s->h_descs[p];
         memset(&d, 0, sizeof d);
-        d.d = pr.n_idx;
-        // the macro sorts Ext operands first (sumcheck_macro/src/lib.rs:87-140); multiplication commutes,
-        // so only operand 0 must be an Ext one when the product is mixed (the body multiplies INTO it)
-        u32 order[5]; u32 k = 0;
-        for (u32 j = 0; j < pr.n_idx; j++) { const ScMle &m = s->mles[pr.idx[j]]; if (m.is_ext || folds[pr.idx[j]]) order[k++] = j; }
-        for (u32 j = 0; j < pr.n_idx; j++) { const ScMle &m = s->mles[pr.idx[j]]; if (!(m.is_ext || folds[pr.idx[j]])) order[k++] = j; }
-        bool allbase = true;
-        u64 newlen = 0;
-        for (u32 jj = 0; jj < pr.n_idx; jj++) {
-            u32 mi = pr.idx[order[jj]];
-            const ScMle &m = s->mles[mi];
-            ScOp &op = d.op[jj];
-            op.src = m.cur;
-            if (folds[mi]) {
-                op.mode = m.is_ext ? OPM_EF : OPM_BF;
-                if (!written[mi]) { op.dst = dst[mi]; written[mi] = 1; bytes += (m.len >> 1) * 16; }
-                bytes += m.len * (m.is_ext ? 16 : 8);
-                newlen = m.len >> 1;
-                allbase = false;
-            } else {
-                op.mode = m.is_ext ? OPM_E : OPM_B;
-                bytes += m.len * (m.is_ext ? 16 : 8);
-                newlen = m.len;
-                if (m.is_ext) allbase = false;
-            }
-        }
-        d.allbase = allbase ? 1 : 0;
-        d.konst = newlen == 1 ? 1 : 0;
-        d.npairs = newlen >> 1;
+        sc_desc(d, p, pr.idx, pr.n_idx, s->mles.data(), folds.data(), dst.data(), s->writer.data());
+        for (u32 j = 0; j < pr.n_idx; j++) { const ScMle &m = s->mles[pr.idx[j]]; bytes += m.len * (m.is_ext ? 16 : 8); }
         round_pairs = std::max<u64>(round_pairs, d.npairs);
     }
     // uniform rounds take the lean kernels: every operand of every product in the same mode, one degree in {2, 3}, no constants
@@ -967,7 +910,7 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
                                  : std::min(s->gx, dp_grid_for(round_pairs <= 256 ? round_pairs : (round_pairs + 1) / 2, SC_THREADS, 4));
     cudaStream_t st = dp_ctx().stream;
     // MLEs no product references still have to be folded (cannot happen through add_mle_list, kept for safety)
-    for (u32 i = 0; i < s->n_mles; i++) if (folds[i] && !written[i]) {
+    for (u32 i = 0; i < s->n_mles; i++) if (folds[i] && s->writer[i] == SC_NO_WRITER) {
         ScMle &m = s->mles[i];
         if (int e = dpk_fold_low(m.cur, m.is_ext, m.len, r, dst[i])) return e;
     }
@@ -979,34 +922,15 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
         const ScProd *descs_arg = s->h_descs;                 // mapped pinned memory: no copy node on the latency path
         if (s->n_products == 1) descs_arg = nullptr;          // descriptor travels in the kernel parameters
         else if ((u64)gx * s->n_products > 32) { DP_CUDA(cudaMemcpyAsync(s->d_descs, s->h_descs, sizeof(ScProd) * s->n_products, cudaMemcpyHostToDevice, st)); descs_arg = s->d_descs; }
-#define SC_ARGS descs_arg, s->h_descs[0], r, s->d_partials, s->d_counters, s->h_out, s->seq, s->h_flag, s->d_done
-#define SC_LEAN(D, M) k_sc_lean<D, M><<<grid, ScLeanShape<M>::BLOCK, 0, st>>>(SC_ARGS)
-        if (lean_mode >= 0) {
-            switch (lean_mode * 4 + (int)dsel) {
-            case OPM_B * 4 + 2: SC_LEAN(2, OPM_B); break;   case OPM_B * 4 + 3: SC_LEAN(3, OPM_B); break;
-            case OPM_E * 4 + 2: SC_LEAN(2, OPM_E); break;   case OPM_E * 4 + 3: SC_LEAN(3, OPM_E); break;
-            case OPM_BF * 4 + 2: SC_LEAN(2, OPM_BF); break; case OPM_BF * 4 + 3: SC_LEAN(3, OPM_BF); break;
-            case OPM_EF * 4 + 2: SC_LEAN(2, OPM_EF); break; default: SC_LEAN(3, OPM_EF); break;
-            }
-        } else
-        switch (dsel) {   // one small kernel per uniform degree keeps the instruction footprint low
-        case 1: k_sc_round<1><<<grid, SC_THREADS, 0, st>>>(SC_ARGS); break;
-        case 2: k_sc_round<2><<<grid, SC_THREADS, 0, st>>>(SC_ARGS); break;
-        case 3: k_sc_round<3><<<grid, SC_THREADS, 0, st>>>(SC_ARGS); break;
-        case 4: k_sc_round<4><<<grid, SC_THREADS, 0, st>>>(SC_ARGS); break;
-        case 5: k_sc_round<5><<<grid, SC_THREADS, 0, st>>>(SC_ARGS); break;
-        default: k_sc_round<0><<<grid, SC_THREADS, 0, st>>>(SC_ARGS); break;
-        }
-#undef SC_LEAN
-#undef SC_ARGS
+        // one small kernel per uniform degree keeps the instruction footprint low
+        const auto kern = lean_mode >= 0 ? k_sc_lean_md[lean_mode][dsel - 2] : k_sc_round_dsel[dsel];
+        const int block = lean_mode >= 0 ? SC_LEAN_BLOCK[lean_mode] : SC_THREADS;
+        kern<<<grid, block, 0, st>>>(descs_arg, s->h_descs[0], r, s->d_partials, s->d_counters, s->h_out, s->seq, s->h_flag, s->d_done);
         DP_LAUNCHED();
     }
     DP_CUDA(cudaGetLastError());
     // commit the folds to the bookkeeping while the GPU works
-    for (u32 i = 0; i < s->n_mles; i++) if (folds[i]) {
-        ScMle &m = s->mles[i];
-        m.cur = dst[i]; m.where = (dst[i] == m.work) ? 1 : 2; m.len >>= 1; m.is_ext = true;
-    }
+    for (u32 i = 0; i < s->n_mles; i++) if (folds[i]) sc_commit_fold(s->mles[i], dst[i]);
     s->round += 1;
     if (s->round == s->max_nv) {   // last round: bring the (<= 2)-entry tables back together with the message
         bool ok = true;
@@ -1035,30 +959,14 @@ int dp_sc_finish(dp_sc *s, const uint64_t *last_challenge, uint64_t *out_final) 
     DP_CHECK(!s->finished && s->round == s->max_nv, DP_ERR_STATE, "dp_sc_finish: rounds not complete");
     gle r = e_make(gl_canon(last_challenge[0]), gl_canon(last_challenge[1]));
     s->challenges.push_back(r);
-    if (s->have_pairs) {   // O(#MLEs) host glue on the pairs fetched with the last message
-        for (u32 i = 0; i < s->n_mles; i++) {
-            gle a = s->h_pairs[2 * i], b = s->h_pairs[2 * i + 1];
-            gle v = s->mles[i].len > 1 ? e_add(a, e_mul(e_sub(b, a), r)) : a;
-            out_final[2 * i] = v.c0; out_final[2 * i + 1] = v.c1;
-        }
-        s->finished = true;
-        return DP_OK;
+    // the last round fetched the pairs unless an MLE still had more than 2 entries; get_mle_final_evaluations asserts
+    // len == 1 after the last fix (prover.rs:479-483)
+    DP_CHECK(s->have_pairs, DP_ERR_STATE, "mle.evaluations.len() != 1, must be called after prove_round_and_update_state");
+    for (u32 i = 0; i < s->n_mles; i++) {   // O(#MLEs) host glue on the pairs fetched with the last message
+        gle a = s->h_pairs[2 * i], b = s->h_pairs[2 * i + 1];
+        gle v = s->mles[i].len > 1 ? e_add(a, e_mul(e_sub(b, a), r)) : a;
+        out_final[2 * i] = v.c0; out_final[2 * i + 1] = v.c1;
     }
-    for (u32 i = 0; i < s->n_mles; i++) {
-        const ScMle &m = s->mles[i];
-        // get_mle_final_evaluations asserts len == 1 after the last fix (prover.rs:479-483)
-        DP_CHECK(m.len <= 2, DP_ERR_STATE, "mle.evaluations.len() != 1, must be called after prove_round_and_update_state");
-        s->h_fin[i].src = m.cur; s->h_fin[i].mode = m.is_ext ? OPM_E : OPM_B; s->h_fin[i].len = (u32)m.len;
-    }
-    cudaStream_t st = dp_ctx().stream;
-    gle *d_vals = (gle *)((char *)s->d_fin + sizeof(ScFin) * s->n_mles);
-    // d_fin region: [ScFin x n][gle x n]; ScFin is 16 bytes so the gle part stays 16-byte aligned
-    DP_CUDA(cudaMemcpyAsync(s->d_fin, s->h_fin, sizeof(ScFin) * s->n_mles, cudaMemcpyHostToDevice, st));
-    k_sc_final<<<(s->n_mles + 127) / 128, 128, 0, st>>>(s->d_fin, s->n_mles, r, d_vals); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
-    DP_CUDA(cudaMemcpyAsync(s->h_out, d_vals, sizeof(gle) * s->n_mles, cudaMemcpyDeviceToHost, st));
-    DP_CUDA(dp_stream_sync(st));
-    for (u32 i = 0; i < s->n_mles; i++) { out_final[2 * i] = s->h_out[i].c0; out_final[2 * i + 1] = s->h_out[i].c1; }
     s->finished = true;
     return DP_OK;
 }

@@ -47,7 +47,31 @@ static std::vector<uint32_t> first_use_remap(const dp_sc_product *products, uint
     for (uint32_t p = 0; p < n_products; p++) for (uint32_t j = 0; j < products[p].n_idx; j++) { uint32_t i = products[p].idx[j]; if (i < n_mles && remap[i] == UINT32_MAX) remap[i] = next++; }
     return remap;
 }
-static void write_finals(const ExtVec &fin, const std::vector<uint32_t> &remap, uint64_t *out_final) {
+// The caller's products over views of its device MLEs (no copies); with T > 1, over slice t of T (the t-th contiguous part of every MLE)
+static VirtualPolynomial make_poly(dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *products, uint32_t n_products, size_t max_nv,
+                                   uint32_t t = 0, uint32_t T = 1) {
+    VirtualPolynomial vp(max_nv);
+    std::vector<DeviceMle> views;
+    for (uint32_t i = 0; i < n_mles; i++) {
+        uint64_t len; int ext; check(dp_mle_info(mles[i], &len, &ext, nullptr));
+        uint64_t sl = len / T;
+        views.push_back(DeviceMle::wrap_device((char *)dp_mle_device_ptr(mles[i]) + (size_t)t * sl * (ext ? 16 : 8), sl, ext));
+    }
+    for (uint32_t p = 0; p < n_products; p++) {
+        std::vector<DeviceMle> l;
+        for (uint32_t j = 0; j < products[p].n_idx; j++) l.push_back(views.at(products[p].idx[j]));
+        vp.add_mle_list(l, Ext(products[p].coef[0], products[p].coef[1]));
+    }
+    return vp;
+}
+// out_point: nv x E; out_msgs: nv x (max_deg+1) x E; out_final: n_mles x E in the caller's `mles` order
+static void write_proof(const std::pair<IOPProof, IOPProverState> &res, const dp_sc_product *products, uint32_t n_products, uint32_t n_mles,
+                        uint64_t *out_point, uint64_t *out_msgs, uint64_t *out_final) {
+    for (size_t i = 0; i < res.first.point.size(); i++) { out_point[2 * i] = res.first.point[i].c0; out_point[2 * i + 1] = res.first.point[i].c1; }
+    size_t k = 0;
+    for (auto &m : res.first.proofs) for (auto &e : m.evaluations) { out_msgs[2 * k] = e.c0; out_msgs[2 * k + 1] = e.c1; k++; }
+    const ExtVec &fin = res.second.get_mle_final_evaluations();
+    const std::vector<uint32_t> remap = first_use_remap(products, n_products, n_mles);
     for (size_t i = 0; i < remap.size(); i++) {
         Ext v = (remap[i] != UINT32_MAX && remap[i] < fin.size()) ? fin[remap[i]] : Ext::zero();
         out_final[2 * i] = v.c0; out_final[2 * i + 1] = v.c1;
@@ -60,29 +84,13 @@ int dph_sumcheck_prove_parallel(dp_mle *const *mles, uint32_t n_mles, const dp_s
                                 uint32_t max_nv, const char *label, void *transcript, uint64_t *out_point, uint64_t *out_msgs,
                                 uint64_t *out_final, uint32_t *out_max_deg) {
     DPH_TRY
-    VirtualPolynomial vp(max_nv);
-    std::vector<DeviceMle> views;
-    for (uint32_t i = 0; i < n_mles; i++) {
-        uint64_t len; int ext; check(dp_mle_info(mles[i], &len, &ext, nullptr));
-        views.push_back(DeviceMle::wrap_device(dp_mle_device_ptr(mles[i]), len, ext));
-    }
-    // register in caller order so final evaluations line up with `mles`
-    for (uint32_t p = 0; p < n_products; p++) {
-        std::vector<DeviceMle> l;
-        for (uint32_t j = 0; j < products[p].n_idx; j++) l.push_back(views.at(products[p].idx[j]));
-        vp.add_mle_list(l, Ext(products[p].coef[0], products[p].coef[1]));
-    }
-    std::vector<uint32_t> remap = first_use_remap(products, n_products, n_mles);
+    VirtualPolynomial vp = make_poly(mles, n_mles, products, n_products, max_nv);
     DynTranscript local(label ? label : "");
     DynTranscript &t = transcript ? *(DynTranscript *)transcript : local;
     auto res = IOPProverState::prove_parallel(std::move(vp), t);
     size_t deg = res.first.proofs.empty() ? 0 : res.first.proofs[0].evaluations.size() - 1;
     *out_max_deg = (uint32_t)deg;
-    for (size_t i = 0; i < res.first.point.size(); i++) { out_point[2 * i] = res.first.point[i].c0; out_point[2 * i + 1] = res.first.point[i].c1; }
-    size_t k = 0;
-    for (auto &m : res.first.proofs) for (auto &e : m.evaluations) { out_msgs[2 * k] = e.c0; out_msgs[2 * k + 1] = e.c1; k++; }
-    const ExtVec &fin = res.second.get_mle_final_evaluations();
-    write_finals(fin, remap, out_final);
+    write_proof(res, products, n_products, n_mles, out_point, out_msgs, out_final);
     return 0;
     DPH_CATCH
 }
@@ -293,13 +301,7 @@ extern "C" int dph_sumcheck_prove_sharded(uint32_t world, uint32_t rank, dp_mle 
                                           uint64_t *out_point, uint64_t *out_msgs, uint64_t *out_final) {
     DPH_TRY
     uint32_t logG = 0; while ((1u << logG) < world) logG++;
-    VirtualPolynomial vp(nv_total - logG);
-    std::vector<DeviceMle> views;
-    for (uint32_t i = 0; i < n_mles; i++) {
-        uint64_t len; int ext; check(dp_mle_info(mles[i], &len, &ext, nullptr));
-        views.push_back(DeviceMle::wrap_device(dp_mle_device_ptr(mles[i]), len, ext));
-    }
-    for (uint32_t p = 0; p < n_products; p++) { std::vector<DeviceMle> l; for (uint32_t j = 0; j < products[p].n_idx; j++) l.push_back(views.at(products[p].idx[j])); vp.add_mle_list(l, Ext(products[p].coef[0], products[p].coef[1])); }
+    VirtualPolynomial vp = make_poly(mles, n_mles, products, n_products, nv_total - logG);
     DynTranscript tr(label);
     std::pair<IOPProof, IOPProverState> res;
     if (shm_region) {
@@ -309,11 +311,7 @@ extern "C" int dph_sumcheck_prove_sharded(uint32_t world, uint32_t rank, dp_mle 
         if (shm_seq) *shm_seq = ex.seq;
     }
     else { if (!cb && world > 1) throw Error(DP_ERR_INVALID, "prove_sharded: no exchange given"); CallbackExchange ex(cb, user, world, rank); res = IOPProverState::prove_sharded(std::move(vp), nv_total, ex, tr); }
-    for (size_t i = 0; i < res.first.point.size(); i++) { out_point[2 * i] = res.first.point[i].c0; out_point[2 * i + 1] = res.first.point[i].c1; }
-    size_t k = 0;
-    for (auto &m : res.first.proofs) for (auto &e : m.evaluations) { out_msgs[2 * k] = e.c0; out_msgs[2 * k + 1] = e.c1; k++; }
-    const ExtVec &fin = res.second.get_mle_final_evaluations();
-    write_finals(fin, first_use_remap(products, n_products, n_mles), out_final);
+    write_proof(res, products, n_products, n_mles, out_point, out_msgs, out_final);
     return 0;
     DPH_CATCH
 }
@@ -359,24 +357,10 @@ extern "C" int dph_sumcheck_prove_batch_polys(uint32_t T, dp_mle *const *mles, u
     DPH_TRY
     uint32_t logT = 0; while ((1u << logT) < T) logT++;
     std::vector<VirtualPolynomial> polys;
-    for (uint32_t t = 0; t < T; t++) {
-        VirtualPolynomial vp(max_nv - logT);
-        std::vector<DeviceMle> views;
-        for (uint32_t i = 0; i < n_mles; i++) {
-            uint64_t len; int ext; check(dp_mle_info(mles[i], &len, &ext, nullptr));
-            uint64_t sl = len / T;
-            views.push_back(DeviceMle::wrap_device((char *)dp_mle_device_ptr(mles[i]) + (size_t)t * sl * (ext ? 16 : 8), sl, ext));
-        }
-        for (uint32_t p = 0; p < n_products; p++) { std::vector<DeviceMle> l; for (uint32_t j = 0; j < products[p].n_idx; j++) l.push_back(views.at(products[p].idx[j])); vp.add_mle_list(l, Ext(products[p].coef[0], products[p].coef[1])); }
-        polys.push_back(std::move(vp));
-    }
+    for (uint32_t t = 0; t < T; t++) polys.push_back(make_poly(mles, n_mles, products, n_products, max_nv - logT, t, T));
     DynTranscript tr(label);
     auto res = IOPProverState::prove_batch_polys(T, std::move(polys), tr);
-    for (size_t i = 0; i < res.first.point.size(); i++) { out_point[2 * i] = res.first.point[i].c0; out_point[2 * i + 1] = res.first.point[i].c1; }
-    size_t k = 0;
-    for (auto &m : res.first.proofs) for (auto &e : m.evaluations) { out_msgs[2 * k] = e.c0; out_msgs[2 * k + 1] = e.c1; k++; }
-    const ExtVec &fin = res.second.get_mle_final_evaluations();
-    write_finals(fin, first_use_remap(products, n_products, n_mles), out_final);
+    write_proof(res, products, n_products, n_mles, out_point, out_msgs, out_final);
     return 0;
     DPH_CATCH
 }

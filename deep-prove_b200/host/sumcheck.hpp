@@ -170,18 +170,11 @@ class IOPProverState {
         check(dp_sc_create(hs.data(), (uint32_t)hs.size(), poly.products.data(), (uint32_t)poly.products.size(), (uint32_t)nv, (uint32_t)deg, &st.sc_));
         check(dp_sc_set_resident_tail(st.sc_, 1));   // this loop only runs the transcript between rounds: small rounds stay resident on the device
         std::vector<u64> buf(2 * (deg + 1));
-        Ext challenge; bool have = false;
-        for (size_t i = 0; i < nv; i++) {
-            u64 c[2] = {challenge.c0, challenge.c1};
-            check(dp_sc_round(st.sc_, have ? c : nullptr, buf.data()));
-            IOPProverMessage msg;
-            for (size_t t = 0; t <= deg; t++) msg.evaluations.push_back(Ext(buf[2 * t], buf[2 * t + 1]));
-            transcript.append_field_element_exts(msg.evaluations);
-            proof.proofs.push_back(std::move(msg));
-            challenge = transcript.get_and_append_challenge("Internal round"); have = true;
-            st.challenges.push_back(challenge);
-        }
-        u64 c[2] = {challenge.c0, challenge.c1};
+        run_rounds(nv, deg, transcript, proof, st, [&](const u64 *c, ExtVec &ev) {
+            check(dp_sc_round(st.sc_, c, buf.data()));
+            for (size_t t = 0; t <= deg; t++) ev[t] = Ext(buf[2 * t], buf[2 * t + 1]);
+        });
+        u64 c[2] = {st.challenges.back().c0, st.challenges.back().c1};
         std::vector<u64> fin(2 * hs.size());
         check(dp_sc_finish(st.sc_, c, fin.data()));
         for (size_t i = 0; i < hs.size(); i++) st.finals_.push_back(Ext(fin[2 * i], fin[2 * i + 1]));
@@ -209,19 +202,12 @@ class IOPProverState {
             check(dp_sc_create(mh[t].data(), (uint32_t)mh[t].size(), polys[t].products.data(), (uint32_t)polys[t].products.size(), (uint32_t)nv, (uint32_t)deg, &hs[t].h));
         }
         std::vector<u64> buf(2 * (deg + 1));
-        Ext challenge; bool have = false;
-        for (size_t i = 0; i < nv; i++) {
-            IOPProverMessage msg; msg.evaluations.assign(deg + 1, Ext::zero());
-            u64 c[2] = {challenge.c0, challenge.c1};
-            for (auto &h : hs) { check(dp_sc_round(h.h, have ? c : nullptr, buf.data())); for (size_t k = 0; k <= deg; k++) msg.evaluations[k] += Ext(buf[2 * k], buf[2 * k + 1]); }
-            transcript.append_field_element_exts(msg.evaluations);
-            proof.proofs.push_back(std::move(msg));
-            challenge = transcript.get_and_append_challenge("Internal round"); have = true;
-            st.challenges.push_back(challenge);
-        }
+        run_rounds(nv, deg, transcript, proof, st, [&](const u64 *c, ExtVec &ev) {
+            for (auto &h : hs) { check(dp_sc_round(h.h, c, buf.data())); for (size_t k = 0; k <= deg; k++) ev[k] += Ext(buf[2 * k], buf[2 * k + 1]); }
+        });
         size_t n_mles = mh[0].size();
         std::vector<ExtVec> residual(n_mles);                 // merge_sumcheck_polys (util.rs:215-243)
-        u64 c[2] = {challenge.c0, challenge.c1};
+        u64 c[2] = {st.challenges.back().c0, st.challenges.back().c1};
         for (auto &h : hs) { std::vector<u64> fin(2 * n_mles); check(dp_sc_finish(h.h, c, fin.data())); for (size_t i = 0; i < n_mles; i++) residual[i].push_back(Ext(fin[2 * i], fin[2 * i + 1])); }
         if (logT == 0) { for (size_t i = 0; i < n_mles; i++) st.finals_.push_back(residual[i][0]); proof.point = st.challenges; return {std::move(proof), std::move(st)}; }
         finish_merged(residual, polys[0].products, deg, logT, transcript, proof, st);
@@ -247,20 +233,13 @@ class IOPProverState {
         check(dp_sc_create(mh.data(), (uint32_t)mh.size(), poly.products.data(), (uint32_t)poly.products.size(), (uint32_t)nv, (uint32_t)deg, &hs.h));
         size_t W = 2 * (deg + 1);
         std::vector<u64> buf(W), all(W * G);
-        Ext challenge; bool have = false;
-        for (size_t i = 0; i < nv; i++) {
-            u64 c[2] = {challenge.c0, challenge.c1};
-            check(dp_sc_round(hs.h, have ? c : nullptr, buf.data()));
+        run_rounds(nv, deg, transcript, proof, st, [&](const u64 *c, ExtVec &ev) {
+            check(dp_sc_round(hs.h, c, buf.data()));
             ex.allgather(buf.data(), W, all.data());
-            IOPProverMessage msg; msg.evaluations.assign(deg + 1, Ext::zero());
-            for (size_t g = 0; g < G; g++) for (size_t k = 0; k <= deg; k++) msg.evaluations[k] += Ext(all[g * W + 2 * k], all[g * W + 2 * k + 1]);
-            transcript.append_field_element_exts(msg.evaluations);
-            proof.proofs.push_back(std::move(msg));
-            challenge = transcript.get_and_append_challenge("Internal round"); have = true;
-            st.challenges.push_back(challenge);
-        }
+            for (size_t g = 0; g < G; g++) for (size_t k = 0; k <= deg; k++) ev[k] += Ext(all[g * W + 2 * k], all[g * W + 2 * k + 1]);
+        });
         size_t n_mles = mh.size();
-        u64 c[2] = {challenge.c0, challenge.c1};
+        u64 c[2] = {st.challenges.back().c0, st.challenges.back().c1};
         std::vector<u64> fin(2 * n_mles), fall(2 * n_mles * G);
         check(dp_sc_finish(hs.h, c, fin.data()));
         if (G == 1) { for (size_t i = 0; i < n_mles; i++) st.finals_.push_back(Ext(fin[2 * i], fin[2 * i + 1])); proof.point = st.challenges; return {std::move(proof), std::move(st)}; }
@@ -271,13 +250,26 @@ class IOPProverState {
         return {std::move(proof), std::move(st)};
     }
   private:
+    // The rounds of one sumcheck: round(c, evals) fills the (deg + 1) zeroed evaluations of the next message from the previous
+    // round's challenge c ([c0, c1]; null in round 0).  Each message goes to the transcript, which draws the next challenge.
+    template <class T, class F>
+    static void run_rounds(size_t nv, size_t deg, T &transcript, IOPProof &proof, IOPProverState &st, F &&round) {
+        for (size_t i = 0; i < nv; i++) {
+            u64 c[2] = {0, 0};
+            if (i > 0) { c[0] = st.challenges.back().c0; c[1] = st.challenges.back().c1; }
+            IOPProverMessage msg; msg.evaluations.assign(deg + 1, Ext::zero());
+            round(i > 0 ? c : nullptr, msg.evaluations);
+            transcript.append_field_element_exts(msg.evaluations);
+            proof.proofs.push_back(std::move(msg));
+            st.challenges.push_back(transcript.get_and_append_challenge("Internal round"));
+        }
+    }
     // stage 2 of the devirgo split: the last log T rounds over the T residual values of every MLE
     template <class T>
     static void finish_merged(const std::vector<ExtVec> &residual, const std::vector<dp_sc_product> &products, size_t deg, size_t logT, T &transcript, IOPProof &proof, IOPProverState &st) {
         size_t n_mles = residual.size();
         struct H { dp_sc *h = nullptr; ~H() { if (h) dp_sc_destroy(h); } };
         std::vector<u64> buf(2 * (deg + 1));
-        Ext challenge; bool have = false;
         VirtualPolynomial merged(logT);
         std::vector<DeviceMle> mm; for (auto &r : residual) mm.push_back(DeviceMle::from_evaluations_ext_vec(r));
         for (auto &pr : products) { std::vector<DeviceMle> l; for (uint32_t j = 0; j < pr.n_idx; j++) l.push_back(mm[pr.idx[j]]); merged.add_mle_list(l, Ext(pr.coef[0], pr.coef[1])); }
@@ -287,16 +279,11 @@ class IOPProverState {
         dp_sc *s2 = nullptr;
         check(dp_sc_create(h2.data(), (uint32_t)h2.size(), merged.products.data(), (uint32_t)merged.products.size(), (uint32_t)logT, (uint32_t)deg, &s2));
         H g2; g2.h = s2;
-        for (size_t i = 0; i < logT; i++) {
-            u64 cc[2] = {challenge.c0, challenge.c1};
-            check(dp_sc_round(s2, have ? cc : nullptr, buf.data()));
-            IOPProverMessage msg; for (size_t k = 0; k <= deg; k++) msg.evaluations.push_back(Ext(buf[2 * k], buf[2 * k + 1]));
-            transcript.append_field_element_exts(msg.evaluations);
-            proof.proofs.push_back(std::move(msg));
-            challenge = transcript.get_and_append_challenge("Internal round"); have = true;
-            st.challenges.push_back(challenge);
-        }
-        u64 cc[2] = {challenge.c0, challenge.c1};
+        run_rounds(logT, deg, transcript, proof, st, [&](const u64 *c, ExtVec &ev) {
+            check(dp_sc_round(s2, c, buf.data()));
+            for (size_t k = 0; k <= deg; k++) ev[k] = Ext(buf[2 * k], buf[2 * k + 1]);
+        });
+        u64 cc[2] = {st.challenges.back().c0, st.challenges.back().c1};
         std::vector<u64> fin(2 * h2.size()); check(dp_sc_finish(s2, cc, fin.data()));
         ExtVec f2; for (size_t i = 0; i < h2.size(); i++) f2.push_back(Ext(fin[2 * i], fin[2 * i + 1]));
         for (size_t i = 0; i < n_mles; i++) { Ext v; for (size_t k = 0; k < h2.size(); k++) if (h2[k] == mm[i].handle()) v = f2[k]; st.finals_.push_back(v); }

@@ -187,6 +187,13 @@ def test_sumcheck_protocol_errors(gpu):
         sc.round(c)
     assert e.value.code == gpu.DP_ERR_STATE and "Prover is not active" in str(e.value)
     sc.finish(c)
+    # an MLE no product references may have more variables than max_nv: after the last round it still has more than one entry
+    big = gpu.Mle.upload(O.splitmix_f(3, 32), False)
+    sc = gpu.Sumcheck([a, big], [((1, 0), [0])], 3, 1)
+    sc.round(None); sc.round(c); sc.round(c)
+    with pytest.raises(gpu.DpError) as e:
+        sc.finish(c)
+    assert e.value.code == gpu.DP_ERR_STATE and "mle.evaluations.len() != 1, must be called after prove_round_and_update_state" in str(e.value)
 
 
 @pytest.mark.parametrize("nv,shape,T", [(6, [["b", "e"]], 2), (9, [["e", "e", "e"], ["b", "e"]], 4), (12, [["b", "b", "b"]], 8)])

@@ -23,15 +23,15 @@ P = O.P
 # ---- constants of sumcheck.cu the model depends on -----------------------------------------------------------------------------
 SC_THREADS = 256            # :25   threads per block of k_sc_round and k_sc_res
 WARP = 32
-LEAN_MIN_PAIRS = 2048       # :948  lean kernels only when the round has MORE pairs than this
-SC_RES_WORK = 2048          # :450  resident once the round's pair-items, summed over products, are <= this
-SC_RES_CTA_WORK = 512       # :788  ~pair-items per CTA of the resident cluster
-SC_RES_MAXCTA = 8           # :449
-SC_RES_MAXP = 48            # :449
-SC_RES_MAXM = 96            # :449
-COUNTER_POOL_BYTES = 256    # :862  tick counters (n_products + 1 u32) come from a pooled 256-byte block when they fit
+LEAN_MIN_PAIRS = 2048       # :892  lean kernels only when the round has MORE pairs than this
+SC_RES_WORK = 2048          # :442  resident once the round's pair-items, summed over products, are <= this
+SC_RES_CTA_WORK = 512       # :757  ~pair-items per CTA of the resident cluster
+SC_RES_MAXCTA = 8           # :441
+SC_RES_MAXP = 48            # :441
+SC_RES_MAXM = 96            # :441
+COUNTER_POOL_BYTES = 256    # :832  tick counters (n_products + 1 u32) come from a pooled 256-byte block when they fit
 H100_SMS = 132              # common.cuh:14 default; on the device the real count is read from torch
-# sumcheck.cu:732-733: the tail disables itself under tools that serialise launches
+# sumcheck.cu:705-706: the tail disables itself under tools that serialise launches
 INJECTION_VARS = ("CUDA_INJECTION64_PATH", "CUDA_INJECTION32_PATH", "NV_NSIGHT_INJECTION_TRANSPORT_TYPE",
                   "NV_NSIGHT_INJECTION_PORT_BASE", "NV_COMPUTE_PROFILER_PERFWORKS_DIR")
 
@@ -43,14 +43,14 @@ def _grid_for(work, threads, max_ctas_per_sm, sm_count):          # common.cuh:1
     return int(max(1, min((work + threads - 1) // threads, sm_count * max_ctas_per_sm)))
 
 
-def res_ncta(work):                                                 # :788
+def res_ncta(work):                                                 # :757
     n = 1
     while n < SC_RES_MAXCTA and n * SC_RES_CTA_WORK < work:
         n <<= 1
     return n
 
 
-def res_groups(n_products, ncta):                                   # :476-478  warps per product, a power of two
+def res_groups(n_products, ncta):                                   # :503-505  warps per product, a power of two
     W = ncta * (SC_THREADS // WARP)
     G = 1
     while n_products * (G << 1) <= W:
@@ -58,7 +58,7 @@ def res_groups(n_products, ncta):                                   # :476-478  
     return W, G
 
 
-def _dsel(products):                                                # :792-793, :945-946  one degree for all products, else 0
+def _dsel(products):                                                # :761-762, :889-890  one degree for all products, else 0
     d = len(products[0])
     return d if all(len(p) == d for p in products) else 0
 
@@ -70,14 +70,14 @@ def dispatch(mle_shapes, products, max_nv, tail, sm_count=H100_SMS):
     ext = [k == "e" for _, k in mle_shapes]
     n_m, n_p = len(mle_shapes), len(products)
     used = {i for p in products for i in p}
-    s_gx = min((max([1] + [ln >> 1 for ln in lens]) + 127) // 128 + 1, sm_count * 16)      # :847-855
+    s_gx = min((max([1] + [ln >> 1 for ln in lens]) + 127) // 128 + 1, sm_count * 16)      # :815-825
     res = None
     rounds = []
     for k in range(max_nv):
         fold = k > 0
-        folds = [fold and ln > 1 for ln in lens]                    # :899-906 (and :491 in the kernel)
+        folds = [fold and ln > 1 for ln in lens]                    # :870-879 (and :515 in the kernel)
         if res is None and tail:
-            # sc_tail_eligible (:753-759) with sc_round_work (:748-751): the length of each product's FIRST operand decides
+            # sc_tail_eligible (:726-730) with sc_round_work (:721-725): the length of each product's FIRST operand decides
             work = sum(max(((lens[p[0]] >> 1) if folds[p[0]] else lens[p[0]]) >> 1, 1) for p in products)
             eligible = (n_m <= SC_RES_MAXM and n_p <= SC_RES_MAXP and max_nv - k >= 2
                         and all(i in used or lens[i] <= 1 for i in range(n_m)) and work <= SC_RES_WORK)
@@ -85,7 +85,7 @@ def dispatch(mle_shapes, products, max_nv, tail, sm_count=H100_SMS):
                 ncta = res_ncta(work)
                 W, G = res_groups(n_p, ncta)
                 res = dict(dsel=_dsel(products), ncta=ncta, W=W, G=G, round0=(k == 0), start=k)
-        descs = []                                                  # the descriptors of :909-943 (the kernel's build_descs, :496-513)
+        descs = []                                                  # the descriptors of sc_desc (:460-478), built by dp_sc_round (:884) and the kernel (:520)
         for p in products:
             modes = [("EF" if ext[i] else "BF") if folds[i] else ("E" if ext[i] else "B") for i in p]
             newlen = (lens[p[0]] >> 1) if folds[p[0]] else lens[p[0]]
@@ -94,19 +94,19 @@ def dispatch(mle_shapes, products, max_nv, tail, sm_count=H100_SMS):
         if res is not None:
             prods = []
             for d in descs:
-                tpl = 2 if d["d"] <= 3 else 3                       # :543-544
+                tpl = 2 if d["d"] <= 3 else 3                       # :550-551
                 split = not d["konst"] and not d["allbase"] and (d["npairs"] << tpl) <= res["G"] * WARP
                 prods.append(dict(split=split, konst=d["konst"], square=d["square"]))
             rounds.append(dict(family="resident", first=(k == res["start"]), products=prods, **res))
         else:
             dsel = _dsel(products)
             round_pairs = max([1] + [d["npairs"] for d in descs])
-            lean = None                                             # :947-955
+            lean = None                                             # :891-899
             if dsel in (2, 3) and round_pairs > LEAN_MIN_PAIRS:
                 m0 = descs[0]["modes"][0]
                 if all(not d["konst"] and all(m == m0 for m in d["modes"]) for d in descs):
                     lean = m0
-            if lean == "B":                                         # :963-966
+            if lean == "B":                                         # :907-910
                 gx = min((round_pairs + 511) // 512, sm_count * 4)
             elif lean is not None:
                 gx = min((round_pairs + 127) // 128, s_gx)
@@ -114,8 +114,8 @@ def dispatch(mle_shapes, products, max_nv, tail, sm_count=H100_SMS):
                 gx = min(s_gx, _grid_for(round_pairs, SC_THREADS, 6, sm_count))
             else:
                 gx = min(s_gx, _grid_for(round_pairs if round_pairs <= 256 else (round_pairs + 1) // 2, SC_THREADS, 4, sm_count))
-            transport = "param" if n_p == 1 else ("device" if gx * n_p > 32 else "mapped")       # :978-980
-            counters = "pooled" if 4 * (n_p + 1) <= COUNTER_POOL_BYTES else "dedicated"       # :862-863
+            transport = "param" if n_p == 1 else ("device" if gx * n_p > 32 else "mapped")       # :922-924
+            counters = "pooled" if 4 * (n_p + 1) <= COUNTER_POOL_BYTES else "dedicated"       # :832-833
             r = dict(gx=gx, transport=transport, counters=counters, round_pairs=round_pairs)
             if lean is not None:
                 r.update(family="lean", D=dsel, mode=lean, profile=LEAN_PROFILE_NAME[lean],
@@ -125,7 +125,7 @@ def dispatch(mle_shapes, products, max_nv, tail, sm_count=H100_SMS):
                           for d in descs]
                 r.update(family="general", dsel=dsel, products=bodies, profile="k_sc_round(fold+msg)" if fold else "k_sc_round(msg)")
             rounds.append(r)
-        for i in range(n_m):                                        # commit the folds (:1005-1008, :594-597)
+        for i in range(n_m):                                        # commit the folds (sc_commit_fold, :454; :933 and :585)
             if folds[i]:
                 lens[i] >>= 1
                 ext[i] = True
