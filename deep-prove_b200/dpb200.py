@@ -515,6 +515,21 @@ class ZkmlContext:
                                            out, self._out.size, C.byref(n)))
         return (sec.value, self._out[: n.value].copy()) if want_proof else sec.value
 
+    def prove_concurrent_all(self, n_workers, n_proofs, stride, device=0, e2e=False, label=b"m2vec"):
+        """prove_concurrent, keeping every job's flat proof (dph_zkml_prove_concurrent_all).  Returns (seconds, proofs, workers):
+        proofs[j] is job j's flat proof (at most `stride` words), workers[j] the index of the worker thread that proved it."""
+        H = host()
+        H.dph_zkml_prove_concurrent_all.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_int, C.c_char_p, C.POINTER(C.c_double),
+                                                    C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+        out = np.zeros(int(n_proofs) * int(stride), dtype=np.uint64)
+        lens = np.zeros(int(n_proofs), dtype=np.uint64)
+        workers = np.zeros(int(n_proofs), dtype=np.uint32)
+        sec = C.c_double()
+        hcheck(H.dph_zkml_prove_concurrent_all(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
+                                               _ptr(out), int(stride), _ptr(lens), _ptr(workers)))
+        out = out.reshape(int(n_proofs), int(stride))
+        return sec.value, [out[j, : int(lens[j])] for j in range(int(n_proofs))], workers
+
     def free(self):
         if self.h:
             host().dph_zkml_context_free(self.h)

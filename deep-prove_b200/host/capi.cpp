@@ -215,6 +215,8 @@ struct ZkPool {
     std::vector<std::thread> th; std::mutex mu; std::condition_variable cv, done_cv;
     ZkHandle *h = nullptr; int device = 0; bool stop = false; uint64_t pending = 0, inflight = 0; std::string label, err; bool failed = false; bool e2e = false;
     uint64_t *out = nullptr, out_cap = 0, *out_len = nullptr;   // when set: the flat proof of the call's last job is copied here
+    // when set: every job's flat proof goes to all_out + job * all_stride, its length to all_lens[job], its worker to all_worker[job]
+    uint64_t *all_out = nullptr, all_stride = 0, *all_lens = nullptr; uint32_t *all_worker = nullptr; uint64_t next_job = 0;
     // Identical proofs started together stay in lockstep: all of them sit in the latency-bound layer sumchecks (GPU nearly idle)
     // and then all of them queue their GPU-filling opening kernels behind each other (CUPTI timeline).  So the
     // workers of one call start `stagger_s` apart (one proof duration spread over the workers; the duration is an average over the
@@ -224,8 +226,8 @@ struct ZkPool {
     void worker(uint32_t idx) {
         bool inited = false; uint64_t seen_gen = 0;
         for (;;) {
-            uint64_t gen; double delay = 0.0; bool keep = false;
-            { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || (pending > 0 && idx < active); }); if (stop) break; pending--; inflight++; keep = pending == 0 && out; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } }
+            uint64_t gen, job; double delay = 0.0; bool keep = false, all = false;
+            { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || (pending > 0 && idx < active); }); if (stop) break; pending--; inflight++; keep = pending == 0 && out; all = all_out != nullptr; job = next_job++; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } }
             try {
                 const bool first_ever = !inited;     // grows this thread's device arena: not a representative duration
                 if (!inited) { dp::check(dp_init(device)); inited = true; }
@@ -238,11 +240,16 @@ struct ZkPool {
                     dp::zkml::Proof p = prover.prove(h->trace_input);
                     flat = p.flatten(h->model.nodes.size());
                     if (flat.empty()) throw dp::Error(DP_ERR_STATE, "empty proof");
-                } else { dp::zkml::Proof p = prover.prove(h->trace); if (keep) flat = p.flatten(h->model.nodes.size()); }
+                } else { dp::zkml::Proof p = prover.prove(h->trace); if (keep || all) flat = p.flatten(h->model.nodes.size()); }
                 if (keep) {
                     std::lock_guard<std::mutex> lk(mu);
                     if (flat.size() > out_cap) throw dp::Error(DP_ERR_INVALID, "dph_zkml_prove_concurrent: output buffer too small");
                     memcpy(out, flat.data(), 8 * flat.size()); *out_len = flat.size();
+                }
+                if (all) {   // each job owns its slot: no lock
+                    all_lens[job] = flat.size(); if (all_worker) all_worker[job] = idx;
+                    if (flat.size() > all_stride) throw dp::Error(DP_ERR_INVALID, "dph_zkml_prove_concurrent_all: proof longer than the stride");
+                    memcpy(all_out + job * all_stride, flat.data(), 8 * flat.size());
                 }
                 const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
                 if (!first_ever) { std::lock_guard<std::mutex> lk(mu); n_timed++; avg_proof_s += (sec - avg_proof_s) / (double)std::min<uint64_t>(n_timed, 64); }
@@ -257,9 +264,10 @@ struct ZkPool {
 std::mutex g_pools_mu; std::map<void *, std::unique_ptr<ZkPool>> g_pools;
 }
 extern "C" void dph_zkml_pool_free(void *handle) { std::lock_guard<std::mutex> lk(g_pools_mu); g_pools.erase(handle); }
-// out (optional, cap words): receives the flat proof of the last job handed out, *out_len its length in words.
-extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
-                                         uint64_t *out, uint64_t cap, uint64_t *out_len) {
+namespace {
+struct AllOut { uint64_t *out; uint64_t stride; uint64_t *lens; uint32_t *worker; };
+int prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
+                     uint64_t *out, uint64_t cap, uint64_t *out_len, const AllOut &all) {
     DPH_TRY
     ZkHandle *h = (ZkHandle *)handle;
     if (!h->trace.valid()) throw dp::Error(DP_ERR_STATE, "dph_zkml_prove_concurrent: run inference first (mode 1)");
@@ -271,6 +279,7 @@ extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_wo
         std::lock_guard<std::mutex> lk(pool->mu);
         pool->label = label; pool->failed = false; pool->e2e = e2e != 0; pool->pending = n_proofs; pool->active = n_workers; pool->call_gen++;
         pool->out = out; pool->out_cap = cap; pool->out_len = out_len; if (out_len) *out_len = 0;
+        pool->all_out = all.out; pool->all_stride = all.stride; pool->all_lens = all.lens; pool->all_worker = all.worker; pool->next_job = 0;
         // stagger only when every worker gets several proofs (otherwise the ramps cost more than the overlap gains)
         pool->stagger_s = (n_workers > 1 && n_proofs >= 3 * n_workers && pool->n_timed > 0) ? pool->avg_proof_s / n_workers : 0.0;
     }
@@ -281,6 +290,22 @@ extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_wo
     if (pool->failed) { g_herr = pool->err; return 1; }
     return 0;
     DPH_CATCH
+}
+}
+// out (optional, cap words): receives the flat proof of the last job handed out, *out_len its length in words.
+extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
+                                         uint64_t *out, uint64_t cap, uint64_t *out_len) {
+    return prove_concurrent(handle, device, n_workers, n_proofs, e2e, label, out_seconds, out, cap, out_len, AllOut{nullptr, 0, nullptr, nullptr});
+}
+// The same call, but every job's flat proof is kept: job j's proof is written to out + j * stride (n_proofs x stride words),
+// its length in words to out_lens[j] and, when out_worker is given, the index of the worker thread that proved it to out_worker[j].
+// Jobs are numbered in the order workers take them.  Flattening every proof costs host time that dph_zkml_prove_concurrent does
+// not spend on the stored-trace path.
+extern "C" int dph_zkml_prove_concurrent_all(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
+                                             uint64_t *out, uint64_t stride, uint64_t *out_lens, uint32_t *out_worker) {
+    if (!out || !out_lens) { g_herr = "dph_zkml_prove_concurrent_all: out and out_lens are required"; return 1; }
+    for (uint32_t j = 0; j < n_proofs; j++) out_lens[j] = 0;
+    return prove_concurrent(handle, device, n_workers, n_proofs, e2e, label, out_seconds, nullptr, 0, nullptr, AllOut{out, stride, out_lens, out_worker});
 }
 
 // One proof sharded over `world` ranks: `mles` are THIS rank's slices (nv_total - log2(world) variables each).
