@@ -185,6 +185,37 @@ __device__ __forceinline__ u64 p2x8_compress(u64 xw, u64 yw, int lane8) {
     return gl_canon_weak(s);    // lane k holds state[k]; digest = [s3, s2, s1, s0]
 }
 
+// DuplexChallenger<F, Poseidon2, WIDTH = 8, RATE = 4> (host/transcript.hpp Sponge) on the 8 lanes of a group: lane k holds state
+// word k (canonical) and, for k < 4, input word k; nin / nout are uniform.  The output buffer is not stored: a duplex copies the
+// first four state words into it and nothing else changes the state before the next duplex, so out[k] == state[k] while nout > 0.
+// Every lane of the warp must call these together (the permutation shuffles over the full mask).
+// Exchange format with the host (Sponge::save / load): [state[0..7], in[0..3], nin, nout].
+static constexpr int P2S_WORDS = 14;
+struct P2Sponge { u64 st, in; u32 nin, nout; };
+__device__ __forceinline__ void p2s_load(P2Sponge &s, const u64 *w, int lane8) {
+    s.st = w[lane8]; s.in = lane8 < 4 ? w[8 + lane8] : 0; s.nin = (u32)w[12]; s.nout = (u32)w[13];
+}
+__device__ __forceinline__ void p2s_store(const P2Sponge &s, u64 *w, int lane8) {
+    w[lane8] = s.st;
+    if (lane8 < 4) w[8 + lane8] = s.in;
+    if (lane8 == 0) { w[12] = s.nin; w[13] = s.nout; }
+}
+__device__ __forceinline__ void p2s_duplex(P2Sponge &s, int lane8) {
+    if (lane8 < (int)s.nin) s.st = s.in;
+    s.nin = 0;
+    s.st = gl_canon_weak(p2x8_permute(s.st, lane8));
+    s.nout = 4;
+}
+__device__ __forceinline__ void p2s_observe(P2Sponge &s, u64 v, int lane8) {
+    s.nout = 0;
+    if (lane8 == (int)s.nin) s.in = v;
+    if (++s.nin == 4) p2s_duplex(s, lane8);
+}
+__device__ __forceinline__ u64 p2s_sample(P2Sponge &s, int lane8) {
+    if (s.nin || !s.nout) p2s_duplex(s, lane8);
+    return shfl8(s.st, (int)--s.nout);
+}
+
 // compress(x, y): absorb x -> permute -> overwrite rate with y -> permute -> [s3, s2, s1, s0]  (one copy of the permutation: see above)
 __device__ __forceinline__ void p2_compress(const u64 x[4], const u64 y[4], u64 out[4]) {
     u64 s[8] = {x[0], x[1], x[2], x[3], 0, 0, 0, 0};

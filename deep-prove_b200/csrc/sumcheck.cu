@@ -15,6 +15,7 @@
 // O(deg^2) glue (2^k multiplicity, coefficient, barycentric extrapolation -- prover.rs:713-724,
 // util.rs:101-136) runs on the host inside dp_sc_round, exactly where the reference has it.
 #include "common.cuh"
+#include "poseidon2.cuh"
 #include <mutex>
 #include <algorithm>
 
@@ -478,7 +479,12 @@ __host__ __device__ inline void sc_desc(ScProd &pd, u32 p, const u32 *idx, u32 n
 }
 
 struct TProd { u32 n_idx; u32 idx[5]; };
-struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; ScMle m[SC_RES_MAXM]; u32 writer[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; };
+// Fiat-Shamir in the resident kernel (dp_sc_run_tail_fs): what sc_glue and BasicTranscript need.  bary[d - 1][i][j]: weight of
+// point j when a degree-d product is extrapolated to point d + 1 + i (exact constants of sc_extrapolate).
+static constexpr u32 SC_MAX_ROUNDS = 40;
+struct ScTailFs { u32 max_deg, max_nv, round0, pad; u64 label[2]; u64 coef[SC_RES_MAXP][2]; u64 bary[4][4][5]; u64 sponge[P2S_WORDS]; };
+struct ScTailFsOut { gle msg[SC_MAX_ROUNDS][SC_NACC]; gle chal[SC_MAX_ROUNDS]; u64 sponge[P2S_WORDS]; };
+struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; ScMle m[SC_RES_MAXM]; u32 writer[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; ScTailFs fs; };
 
 __device__ __forceinline__ u32 cl_rank() { u32 r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ u32 cl_size() { u32 r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
@@ -487,17 +493,61 @@ __device__ __forceinline__ void cl_sync() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
+// Round k of the device-transcript tail, in CTA 0 once the product sums are in sprod and this round's folds are committed to sm:
+// sc_glue (one thread per product, on the lengths the host's bookkeeping has after the fold), the sum over products, then
+// BasicTranscript on warp 0 -- append_field_element_exts(message), get_and_append_challenge("Internal round") -- and the challenge
+// goes to xctl for the cluster.  Out of line: the round loop keeps its registers (sponge state in shared memory between rounds).
+__device__ __noinline__ void sc_res_fs_round(ScTailFs &f, gle (*sprod)[SC_NACC], const TProd *sp, const ScMle *sm, u32 np, u32 k, bool last,
+                                             ScTailFsOut *fsout, u64 *xctl) {
+    const u32 R = f.round0 + k + 1, max_deg = f.max_deg;
+    for (u32 p = threadIdx.x; p < np; p += blockDim.x) {
+        const u32 d = sp[p].n_idx; const u64 len = sm[sp[p].idx[0]].len;
+        u32 l2 = 1; while ((1ULL << l2) < len) l2++;
+        const int mult = (int)f.max_nv - (int)(l2 + R - 1);      // >= 0: dp_sc_create bounds every MLE's num_vars by max_nv
+        const gle coef = e_make(f.coef[p][0], f.coef[p][1]);
+        const u64 scale = gl_canon(1ULL << (mult > 0 ? mult : 0));
+        for (u32 t = 0; t <= d; t++) { gle v = sprod[p][t]; if (mult > 0) v = e_mul_base(v, scale); sprod[p][t] = e_mul_ni(v, coef); }
+        for (u32 i = 0; d + 1 + i <= max_deg; i++) {
+            gle v = e_zero();
+            for (u32 j = 0; j <= d; j++) v = e_add(v, e_mul_base(sprod[p][j], f.bary[d - 1][i][j]));
+            sprod[p][d + 1 + i] = v;
+        }
+    }
+    __syncthreads();
+    for (u32 t = threadIdx.x; t <= max_deg; t += blockDim.x) {
+        gle v = e_zero();
+        for (u32 p = 0; p < np; p++) v = e_add(v, sprod[p][t]);
+        sprod[0][t] = v;                                         // column t is read and written by this thread only
+        st_e(&fsout->msg[k][t], v);
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const int l8 = threadIdx.x & 7;
+        P2Sponge s; p2s_load(s, f.sponge, l8);
+        for (u32 t = 0; t <= max_deg; t++) { p2s_observe(s, sprod[0][t].c0, l8); p2s_observe(s, sprod[0][t].c1, l8); }
+        p2s_observe(s, f.label[0], l8); p2s_observe(s, f.label[1], l8);
+        const u64 c0 = p2s_sample(s, l8), c1 = p2s_sample(s, l8);
+        __syncwarp();
+        if (threadIdx.x < 8) { p2s_store(s, f.sponge, l8); if (last) p2s_store(s, fsout->sponge, l8); }
+        if (threadIdx.x == 0) { __stcg(xctl + 1, c0); __stcg(xctl + 2, c1); __stcg(xctl, 0ULL); st_e(&fsout->chal[k], e_make(c0, c1)); }
+    }
+}
+
 template <int DSEL>
 __global__ void __launch_bounds__(SC_THREADS)
 k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pairs /* mapped */, volatile u64 *flag /* mapped */,
-         volatile u64 *chal /* mapped: [seq, c0, c1] */, u64 seq0, gle *xpart /* device: warp partials */, u64 *xctl /* device: [status, c0, c1] */) {
+         volatile u64 *chal /* mapped: [seq, c0, c1] */, u64 seq0, gle *xpart /* device: warp partials */, u64 *xctl /* device: [status, c0, c1] */,
+         ScTailFsOut *fsout /* mapped; null: the host runs the transcript between rounds */) {
     __shared__ ScMle sm[SC_RES_MAXM];
     __shared__ TProd sp[SC_RES_MAXP];
     __shared__ ScProd spd[SC_RES_MAXP];
     __shared__ gle *sdst[SC_RES_MAXM];
     __shared__ u32 swriter[SC_RES_MAXM];
     __shared__ unsigned char sfold[SC_RES_MAXM];
+    __shared__ gle sprod[SC_RES_MAXP][SC_NACC];                       // device transcript: each product's sums
+    __shared__ ScTailFs sfs;
     const u32 nm = cfg->n_mles, np = cfg->n_products, nr = cfg->n_rounds;
+    const bool fs = fsout != nullptr;
     const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = SC_THREADS / 32;
     const u32 rank = cl_rank(), ncta = cl_size();
     const u32 W = ncta * nwarps, gw = rank * nwarps + warp;              // warps of the cluster, this warp's index
@@ -505,6 +555,8 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
     u32 G = 1; while (np * (G << 1) <= W) G <<= 1;
     for (u32 i = threadIdx.x; i < nm; i += blockDim.x) { sm[i] = cfg->m[i]; swriter[i] = cfg->writer[i]; }
     for (u32 i = threadIdx.x; i < np; i += blockDim.x) sp[i] = cfg->p[i];
+    if (fs && rank == 0)
+        for (u32 i = threadIdx.x; i < sizeof(ScTailFs) / 8; i += blockDim.x) ((u64 *)&sfs)[i] = ((const u64 *)&cfg->fs)[i];
     __syncthreads();
     gle r = r0;
     // The descriptors of a round depend on the fold bookkeeping only, never on the challenge VALUE: they are rebuilt right after a
@@ -523,8 +575,8 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
     build_descs(cfg->first_has_challenge != 0);
     for (u32 k = 0; k < nr; k++) {
         const u64 seq = seq0 + k;
-        if (k > 0) {   // wait for the host's challenge for this round
-            if (rank == 0 && threadIdx.x == 0) {
+        if (k > 0) {   // wait for the host's challenge for this round (device transcript: CTA 0 posted it to xctl last round)
+            if (rank == 0 && threadIdx.x == 0 && !fs) {
                 long long t0 = clock64(); u64 v, status = 0;
                 while ((v = chal[0]) != seq) {
                     if (v == SC_TAIL_ABORT) { status = 1; break; }
@@ -561,6 +613,7 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
         }
         cl_sync();                                             // warp partials and folded tables of every CTA are visible
         if (rank == 0) {                                       // the message first: it is what the host is waiting for
+            gle *const mout = fs ? &sprod[0][0] : out;
             // few partials per (product, point): one THREAD each (many products run side by side); many (a single product spread over
             // >= 32 warps): one WARP each, its lanes gather the partials with independent L2 loads -- faster for a single wide product,
             // while the warp form slows the 6-product LogUp shape
@@ -570,7 +623,7 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
                     if (t > spd[p].d) continue;
                     gle v = e_zero();
                     for (u32 s = 0; s < G; s++) { ulonglong2 q = __ldcg(reinterpret_cast<const ulonglong2 *>(xpart + ((u64)p * G + s) * SC_NACC + t)); v = e_add(v, e_make(q.x, q.y)); }
-                    st_e(out + (u64)p * SC_NACC + t, v);
+                    st_e(mout + (u64)p * SC_NACC + t, v);
                 }
             } else
             for (u32 x = warp; x < np * SC_NACC; x += nwarps) {
@@ -579,11 +632,12 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
                 wsum96 v0 = {0, 0}, v1 = {0, 0};
                 for (u32 s = lane; s < G; s += 32) { ulonglong2 q = __ldcg(reinterpret_cast<const ulonglong2 *>(xpart + ((u64)p * G + s) * SC_NACC + t)); ws_add(v0, q.x, 0); ws_add(v1, q.y, 0); }
                 ws_warp_reduce(v0); ws_warp_reduce(v1);
-                if (lane == 0) st_e(out + (u64)p * SC_NACC + t, e_make(ws_reduce(v0), ws_reduce(v1)));
+                if (lane == 0) st_e(mout + (u64)p * SC_NACC + t, e_make(ws_reduce(v0), ws_reduce(v1)));
             }
         }
         for (u32 i = threadIdx.x; i < nm; i += blockDim.x) if (sfold[i]) sc_commit_fold(sm[i], sdst[i]);   // every CTA keeps its own copy
         __syncthreads();
+        if (rank == 0 && fs) sc_res_fs_round(sfs, sprod, sp, sm, np, k, k == nr - 1, fsout, xctl);
         if (rank == 0) {
             if (k == nr - 1) {   // last round: hand the (<= 2)-entry tables over with the message (k_sc_gather's job)
                 for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
@@ -594,7 +648,7 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
                 }
                 __syncthreads();
             }
-            if (threadIdx.x == 0) { __threadfence_system(); *flag = seq; }
+            if (threadIdx.x == 0 && (!fs || k == nr - 1)) { __threadfence_system(); *flag = seq; }   // device transcript: once, at the end
         }
         if (k + 1 < nr) build_descs(true);                     // next round's descriptors while the host hashes
         // CTAs other than 0 run ahead to the next cluster barrier; xpart is not rewritten before it (the work phase follows it)
@@ -629,7 +683,7 @@ struct dp_sc {
     u64 seq = 0; u64 *h_flag = nullptr; u32 *d_done = nullptr;
     int gx = 1;
     bool tail_enabled = false, tail_active = false; u32 tail_last_round = 0;
-    ScTail *h_tail = nullptr; u64 *h_chal = nullptr;
+    ScTail *h_tail = nullptr; u64 *h_chal = nullptr; ScTailFsOut *h_fs = nullptr;
     gle *d_xpart = nullptr; u64 *d_xctl = nullptr;        // resident cluster kernel: warp partials, [status, c0, c1]
     std::vector<gle> challenges;
 };
@@ -638,16 +692,17 @@ static u32 ceil_log2_u64(u64 x) { u32 l = 0; while ((1ULL << l) < x) l++; return
 
 // barycentric extrapolation of a degree-(n-1) polynomial given at 0..n-1 to the point `at`
 // (sumcheck/src/util.rs:19-136; exact arithmetic, so plain Lagrange gives the same element)
+static u64 sc_bary_weight(u32 n, u64 at, u32 j) {
+    u64 num = 1, den = 1;
+    for (u32 i = 0; i < n; i++) if (i != j) {
+        num = gl_mul(num, gl_sub(gl_canon(at), (u64)i));
+        den = gl_mul(den, gl_sub((u64)j, (u64)i));
+    }
+    return gl_mul(num, gl_inv(den));
+}
 static gle sc_extrapolate(const gle *evals, u32 n, u64 at) {
     gle res = e_zero();
-    for (u32 j = 0; j < n; j++) {
-        u64 num = 1, den = 1;
-        for (u32 i = 0; i < n; i++) if (i != j) {
-            num = gl_mul(num, gl_sub(gl_canon(at), (u64)i));
-            den = gl_mul(den, gl_sub((u64)j, (u64)i));
-        }
-        res = e_add(res, e_mul_base(evals[j], gl_mul(num, gl_inv(den))));
-    }
+    for (u32 j = 0; j < n; j++) res = e_add(res, e_mul_base(evals[j], sc_bary_weight(n, at, j)));
     return res;
 }
 
@@ -658,7 +713,7 @@ static int sc_free_all(dp_sc *s) {
     dp_dev_free(s->d_xpart); dp_dev_free(s->d_xctl);
     dp_pinned_free(s->h_flag);
     dp_pinned_free(s->h_descs); dp_pinned_free(s->h_out); dp_pinned_free(s->h_fin); dp_pinned_free(s->h_pairs);
-    dp_pinned_free(s->h_tail); dp_pinned_free(s->h_chal);
+    dp_pinned_free(s->h_tail); dp_pinned_free(s->h_chal); dp_pinned_free(s->h_fs);
     return DP_OK;
 }
 
@@ -735,16 +790,18 @@ static decltype(&k_sc_round<0>) const k_sc_lean_md[4][2] = {{k_sc_lean<2, OPM_B>
                                                               {k_sc_lean<2, OPM_BF>, k_sc_lean<3, OPM_BF>}, {k_sc_lean<2, OPM_EF>, k_sc_lean<3, OPM_EF>}};
 static constexpr int SC_LEAN_BLOCK[4] = {ScLeanShape<OPM_B>::BLOCK, ScLeanShape<OPM_E>::BLOCK, ScLeanShape<OPM_BF>::BLOCK, ScLeanShape<OPM_EF>::BLOCK};
 
-// one round served by the resident kernel (started here on its first round)
-static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
+// start the resident kernel for all remaining rounds; the first one's message is tagged s->seq.  fs: the kernel runs the transcript
+// from this sponge state and writes messages, challenges and the final state to s->h_fs (null: the host posts every challenge).
+static int sc_tail_launch(dp_sc *s, gle r, bool fold, const ScTailFs *fs) {
     cudaStream_t st = dp_ctx().stream;
-    s->seq++;
-    if (!s->tail_active) {
+    {
         int e = 0;
         if (!s->h_tail && (e = dp_pinned_alloc((void **)&s->h_tail, sizeof(ScTail)))) return e;
         if (!s->h_chal && (e = dp_pinned_alloc((void **)&s->h_chal, 64))) return e;
+        if (fs && !s->h_fs && (e = dp_pinned_alloc((void **)&s->h_fs, sizeof(ScTailFsOut)))) return e;
         ScTail &t = *s->h_tail;
         t.n_mles = s->n_mles; t.n_products = s->n_products; t.n_rounds = s->max_nv - s->round; t.first_has_challenge = fold ? 1 : 0;
+        if (fs) t.fs = *fs;
         for (u32 i = 0; i < s->n_mles; i++) {
             ScMle &m = s->mles[i];
             if (m.len > 1 && !m.work) { if ((e = dp_dev_alloc((void **)&m.work, sizeof(gle) * ((m.len0 >> 1) + (m.len0 >> 2) + 1)))) return e; }
@@ -765,13 +822,24 @@ static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         lc.attrs = at; lc.numAttrs = 1;
-        DpProfScope prof("k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)", 0);
+        DpProfScope prof(fs ? "k_sc_res(resident cluster rounds with the device transcript)"
+                            : "k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)", 0);
         const cudaError_t ce = cudaLaunchKernelEx(&lc, k_sc_res_dsel[dsel], (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs, (volatile u64 *)s->h_flag,
-                                                  (volatile u64 *)s->h_chal, s->seq, s->d_xpart, s->d_xctl);
+                                                  (volatile u64 *)s->h_chal, s->seq, s->d_xpart, s->d_xctl, fs ? s->h_fs : (ScTailFsOut *)nullptr);
         DP_LAUNCHED();
         DP_CUDA(ce);
         DP_CUDA(cudaGetLastError());
         s->tail_active = true;
+    }
+    return DP_OK;
+}
+
+// one round served by the resident kernel (started here on its first round)
+static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
+    cudaStream_t st = dp_ctx().stream;
+    s->seq++;
+    if (!s->tail_active) {
+        if (int e = sc_tail_launch(s, r, fold, nullptr)) return e;
     } else {   // post the challenge: value first, then the sequence number the kernel polls
         s->h_chal[1] = r.c0; s->h_chal[2] = r.c1;
         __atomic_store_n(&s->h_chal[0], s->seq, __ATOMIC_RELEASE);
@@ -986,6 +1054,73 @@ int dp_sc_set_resident_tail(dp_sc *s, int enable) {
     DP_REQUIRE_CTX();
     DP_CHECK(s && !s->tail_active, DP_ERR_STATE, "dp_sc_set_resident_tail: null handle or tail already running");
     s->tail_enabled = enable != 0 && sc_tail_supported();
+    return DP_OK;
+}
+
+// The device transcript pays where a proving thread would otherwise sleep through every round trip: in blocking wait mode, many
+// proofs in flight.  In spin mode the host's round trip is a few microseconds, less than the 3 dependent permutations the kernel
+// runs on one warp per round (DESIGN.md section 5.2), so a lone proof keeps the host transcript.
+int dp_sc_tail_fs_next(dp_sc *s, int *out) {
+    DP_REQUIRE_CTX();
+    DP_CHECK(s && out, DP_ERR_INVALID, "dp_sc_tail_fs_next: null argument");
+    *out = !s->finished && s->round < s->max_nv && !s->tail_active && dp_wait_mode() == DP_WAIT_BLOCK && sc_tail_eligible(s, s->round > 0);
+    return DP_OK;
+}
+
+int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
+                      uint64_t *sponge_out) {
+    DP_REQUIRE_CTX();
+    DP_CHECK(s && sponge_in && msgs_out && challenges_out && sponge_out, DP_ERR_INVALID, "dp_sc_run_tail_fs: null argument");
+    DP_CHECK(!s->finished && s->round < s->max_nv && !s->tail_active, DP_ERR_STATE, "Prover is not active");
+    const bool fold = s->round > 0;
+    DP_CHECK(fold == (prev_challenge != nullptr), DP_ERR_STATE, fold ? "verifier message is empty" : "first round should be prover first.");
+    DP_CHECK(sponge_in[12] < 4 && sponge_in[13] <= 4, DP_ERR_INVALID, "dp_sc_run_tail_fs: sponge state out of range");
+    DP_CHECK(sc_tail_eligible(s, fold), DP_ERR_STATE, "dp_sc_run_tail_fs: the next round does not start the resident tail");
+    {   // the Poseidon2 constants of this module's copy of the permutation: the transcript's, never those of dp_poseidon2_init
+        static std::once_flag once; static cudaError_t ce = cudaSuccess;
+        std::call_once(once, [] {
+            cudaStream_t st = dp_ctx().stream;
+            if ((ce = cudaMemcpyToSymbolAsync(c_p2_ext, &DP_P2_EXT_RC[0][0][0], sizeof(u64) * 64, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess &&
+                (ce = cudaMemcpyToSymbolAsync(c_p2_int, DP_P2_INT_RC, sizeof(u64) * 22, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess &&
+                (ce = cudaMemcpyToSymbolAsync(c_p2_diag, DP_P2_DIAG, sizeof(u64) * 8, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess)
+                ce = dp_stream_sync(st);
+        });
+        DP_CUDA(ce);
+    }
+    gle r = e_zero();
+    if (fold) {
+        r = e_make(gl_canon(prev_challenge[0]), gl_canon(prev_challenge[1]));
+        s->challenges.push_back(r);
+        if (s->challenges.size() == 1)
+            for (auto &m : s->mles) DP_CHECK(m.len > 1, DP_ERR_INVALID, "calling sumcheck on constant");  // prover.rs:667-669
+    }
+    ScTailFs fs{};
+    fs.max_deg = s->max_deg; fs.max_nv = s->max_nv; fs.round0 = s->round;
+    static const char label[] = "Internal round";                 // BasicTranscript::append_message: 8-byte little-endian words
+    memcpy(fs.label, label, sizeof label - 1);
+    for (u32 p = 0; p < s->n_products; p++) { fs.coef[p][0] = s->products[p].coef[0]; fs.coef[p][1] = s->products[p].coef[1]; }
+    for (u32 d = 1; d < s->max_deg; d++)
+        for (u32 i = 0; d + 1 + i <= s->max_deg; i++)
+            for (u32 j = 0; j <= d; j++) fs.bary[d - 1][i][j] = sc_bary_weight(d + 1, d + 1 + i, j);
+    for (int w = 0; w < P2S_WORDS; w++) fs.sponge[w] = w < 12 ? gl_canon(sponge_in[w]) : sponge_in[w];
+    const u32 nr = s->max_nv - s->round;
+    s->seq++;
+    if (int e = sc_tail_launch(s, r, fold, &fs)) return e;
+    s->seq += nr - 1;                                              // the kernel raises the flag once, with the last round's tag
+    for (u32 k = 0; k < nr; k++)
+        if (k > 0 || fold) for (auto &m : s->mles) if (m.len > 1) { m.len >>= 1; m.is_ext = true; m.cur = nullptr; m.where = 3; }
+    s->round = s->max_nv;
+    const bool ok = dp_wait_flag(s->h_flag, s->seq, true, SC_TAIL_FAILED, 8.0) == s->seq;
+    if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(dp_ctx().stream); DP_CHECK(false, DP_ERR_CUDA, "dp_sc_run_tail_fs: the resident kernel did not finish"); }
+    s->have_pairs = true;
+    const ScTailFsOut &o = *s->h_fs;
+    const u32 w = s->max_deg + 1;
+    for (u32 k = 0; k < nr; k++) {
+        for (u32 t = 0; t < w; t++) { msgs_out[2 * (k * w + t)] = o.msg[k][t].c0; msgs_out[2 * (k * w + t) + 1] = o.msg[k][t].c1; }
+        challenges_out[2 * k] = o.chal[k].c0; challenges_out[2 * k + 1] = o.chal[k].c1;
+        if (k + 1 < nr) s->challenges.push_back(o.chal[k]);     // the last one is dp_sc_finish's
+    }
+    for (int i = 0; i < P2S_WORDS; i++) sponge_out[i] = o.sponge[i];
     return DP_OK;
 }
 

@@ -21,7 +21,7 @@ ABI_SYMBOLS = [
     "dp_mle_upload", "dp_mle_wrap_device", "dp_mle_clone", "dp_mle_download", "dp_mle_info", "dp_mle_device_ptr",
     "dp_mle_free", "dp_mle_fix_high", "dp_mle_fix_high_new", "dp_mle_fix_low", "dp_mle_evaluate", "dp_mle_evaluate_many", "dp_eq_build",
     "dp_sc_create", "dp_sc_round", "dp_sc_finish", "dp_sc_destroy", "dp_sc_current_mle", "dp_sc_set_resident_tail",
-    "dp_poseidon2_init", "dp_set_merkle_hasher", "dp_get_merkle_hasher", "dp_pcs_commit", "dp_pcs_commit_many", "dp_pcs_batch_commit", "dp_pcs_comm_num_polys", "dp_pcs_comm_part", "dp_pcs_comm_info", "dp_pcs_comm_codeword", "dp_pcs_comm_bh_evals", "dp_pcs_comm_free",
+    "dp_sc_tail_fs_next", "dp_sc_run_tail_fs", "dp_poseidon2_init", "dp_set_merkle_hasher", "dp_get_merkle_hasher", "dp_pcs_commit", "dp_pcs_commit_many", "dp_pcs_batch_commit", "dp_pcs_comm_num_polys", "dp_pcs_comm_part", "dp_pcs_comm_info", "dp_pcs_comm_codeword", "dp_pcs_comm_bh_evals", "dp_pcs_comm_free",
     "dp_pcs_open_begin", "dp_pcs_open_round", "dp_pcs_open_final_message", "dp_pcs_open_query_words", "dp_pcs_open_query",
     "dp_pcs_open_free", "dp_pcs_commit_shard", "dp_pcs_comm_shard_info", "dp_pcs_comm_set_shard_roots", "dp_pcs_open_set_shard_roots",
     "dp_logup_build", "dp_logup_num_vars", "dp_logup_outputs", "dp_logup_layer_mles", "dp_logup_free", "dp_mle_linear_combination",
@@ -76,6 +76,8 @@ def lib():
         _lib.dp_sc_round.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.dp_sc_finish.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.dp_sc_destroy.argtypes = [C.c_void_p]
+        _lib.dp_sc_tail_fs_next.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
+        _lib.dp_sc_run_tail_fs.argtypes = [C.c_void_p] + [C.c_void_p] * 5
     return _lib
 
 

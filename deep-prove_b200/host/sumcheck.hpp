@@ -173,7 +173,7 @@ class IOPProverState {
         run_rounds(nv, deg, transcript, proof, st, [&](const u64 *c, ExtVec &ev) {
             check(dp_sc_round(st.sc_, c, buf.data()));
             for (size_t t = 0; t <= deg; t++) ev[t] = Ext(buf[2 * t], buf[2 * t + 1]);
-        });
+        }, st.sc_);
         u64 c[2] = {st.challenges.back().c0, st.challenges.back().c1};
         std::vector<u64> fin(2 * hs.size());
         check(dp_sc_finish(st.sc_, c, fin.data()));
@@ -252,11 +252,29 @@ class IOPProverState {
   private:
     // The rounds of one sumcheck: round(c, evals) fills the (deg + 1) zeroed evaluations of the next message from the previous
     // round's challenge c ([c0, c1]; null in round 0).  Each message goes to the transcript, which draws the next challenge.
+    // sc: the single device handle behind `round`, if there is one; when the library says its resident tail runs the transcript
+    // on the device from the next round on (dp_sc_tail_fs_next) and the transcript's state can go there, the remaining rounds
+    // are one dp_sc_run_tail_fs call.
     template <class T, class F>
-    static void run_rounds(size_t nv, size_t deg, T &transcript, IOPProof &proof, IOPProverState &st, F &&round) {
+    static void run_rounds(size_t nv, size_t deg, T &transcript, IOPProof &proof, IOPProverState &st, F &&round, dp_sc *sc = nullptr) {
         for (size_t i = 0; i < nv; i++) {
             u64 c[2] = {0, 0};
             if (i > 0) { c[0] = st.challenges.back().c0; c[1] = st.challenges.back().c1; }
+            int dev = 0; u64 sp[Sponge::WORDS];
+            if (sc) check(dp_sc_tail_fs_next(sc, &dev));
+            if (dev && transcript.save_sponge(sp)) {
+                const size_t n = nv - i, w = 2 * (deg + 1);
+                std::vector<u64> msgs(n * w), ch(2 * n);
+                check(dp_sc_run_tail_fs(sc, i > 0 ? c : nullptr, sp, msgs.data(), ch.data(), sp));
+                transcript.load_sponge(sp);
+                for (size_t k = 0; k < n; k++) {
+                    IOPProverMessage msg;
+                    for (size_t t = 0; t <= deg; t++) msg.evaluations.push_back(Ext(msgs[k * w + 2 * t], msgs[k * w + 2 * t + 1]));
+                    proof.proofs.push_back(std::move(msg));
+                    st.challenges.push_back(Ext(ch[2 * k], ch[2 * k + 1]));
+                }
+                return;
+            }
             IOPProverMessage msg; msg.evaluations.assign(deg + 1, Ext::zero());
             round(i > 0 ? c : nullptr, msg.evaluations);
             transcript.append_field_element_exts(msg.evaluations);

@@ -82,7 +82,7 @@ class Poseidon2 {
 // DuplexChallenger<F, Poseidon2, WIDTH = 8, RATE = 4>
 class Sponge {
   public:
-    Sponge() { memset(st_, 0, sizeof st_); }
+    Sponge() { memset(st_, 0, sizeof st_); memset(in_, 0, sizeof in_); memset(out_, 0, sizeof out_); }
     void observe(u64 v) {
         nout_ = 0;
         in_[nin_++] = v;
@@ -92,6 +92,11 @@ class Sponge {
         if (nin_ || !nout_) duplex();
         return out_[--nout_];
     }
+    // the whole state as 14 words [st[0..7], in[0..3], nin, nout] (dp_sc_run_tail_fs continues it on the device).  out is not
+    // part of it: a duplex copies st[0..3] into it and nothing else changes st before the next duplex.
+    static constexpr int WORDS = 14;
+    void save(u64 w[WORDS]) const { memcpy(w, st_, 64); memcpy(w + 8, in_, 32); w[12] = (u64)nin_; w[13] = (u64)nout_; }
+    void load(const u64 w[WORDS]) { memcpy(st_, w, 64); memcpy(in_, w + 8, 32); nin_ = (int)w[12]; nout_ = (int)w[13]; memcpy(out_, st_, 32); }
   private:
     void duplex() {
         for (int i = 0; i < nin_; i++) st_[i] = in_[i];
@@ -118,6 +123,9 @@ class BasicTranscript {
     void append_field_element_exts(const ExtVec &v) { for (auto &e : v) append_field_element_ext(e); }
     Ext read_challenge() { u64 a = sp_.sample(); u64 b = sp_.sample(); return Ext(a, b); }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
+    // the sponge state for dp_sc_run_tail_fs: true, this transcript can continue on the device
+    bool save_sponge(u64 w[Sponge::WORDS]) const { sp_.save(w); return true; }
+    void load_sponge(const u64 w[Sponge::WORDS]) { sp_.load(w); }
   private:
     Sponge sp_;
 };
@@ -150,6 +158,8 @@ class BlakeTranscript {
         }
     }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
+    bool save_sponge(u64 *) const { return false; }                 // BLAKE3: no device counterpart, the host runs every round
+    void load_sponge(const u64 *) { throw std::logic_error("BlakeTranscript has no sponge state"); }
   private:
     static size_t le(u64 c, uint8_t b[8]) { size_t n = 0; for (int k = 0; k < 8; k++) { b[k] = (uint8_t)(c >> (8 * k)); if (b[k]) n = k + 1; } return n ? n : 1; }
     dpb3::Hasher h_;
@@ -169,6 +179,8 @@ class DynTranscript {
     void append_field_element_exts(const ExtVec &v) { for (auto &e : v) append_field_element_ext(e); }
     Ext read_challenge() { return blake_ ? k_.read_challenge() : b_.read_challenge(); }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
+    bool save_sponge(u64 *w) const { return blake_ ? k_.save_sponge(w) : b_.save_sponge(w); }
+    void load_sponge(const u64 *w) { blake_ ? k_.load_sponge(w) : b_.load_sponge(w); }
   private:
     bool blake_; BasicTranscript b_; BlakeTranscript k_;
 };

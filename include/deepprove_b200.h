@@ -115,6 +115,19 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals);
  * kernel launches (Nsight Compute, compute-sanitizer): a one-time probe checks that a running kernel can see a word the
  * host posts after the launch call returned. */
 int dp_sc_set_resident_tail(dp_sc *s, int enable);
+/* *out = 1 when the library runs the next round and all later ones with the transcript on the device (dp_sc_run_tail_fs): the
+ * next round starts the resident tail and the wait mode is blocking (dp_set_wait_mode(1)).  In spin mode a host round trip is
+ * cheaper than the kernel's own Poseidon2 chain, so callers keep calling dp_sc_round there. */
+int dp_sc_tail_fs_next(dp_sc *s, int *out);
+/* Every remaining round in the resident tail, with BasicTranscript's Fiat-Shamir run by the kernel: each round message is absorbed
+ * (append_field_element_exts), then the label "Internal round", and the challenge (c0, c1) is sampled.  prev_challenge: the
+ * challenge of the previous round (NULL in round 0).  sponge_in / sponge_out: the Poseidon2 duplex state before and after, 14
+ * words [state[0..7], input[0..3], n_input, n_output] (may be the same buffer).  With n = max_num_variables - rounds done:
+ * msgs_out receives n x (max_degree+1) x [c0,c1] (what dp_sc_round returns), challenges_out n x [c0,c1]; the last challenge goes
+ * to dp_sc_finish.  DP_ERR_STATE unless the next round would start the resident tail (dp_sc_set_resident_tail enabled, small
+ * enough rounds). */
+int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
+                      uint64_t *sponge_out);
 /* Tail of prove_parallel (prover.rs:544-568) + get_mle_final_evaluations (:474-490): fixes the last
  * challenge and writes n_mles x [c0,c1]. */
 int dp_sc_finish(dp_sc *s, const uint64_t *last_challenge, uint64_t *out_final_evals);
