@@ -84,8 +84,9 @@ int dp_logup_build(dp_mle *const *columns, uint32_t n_columns, const dp_mle *mul
                    const uint64_t column_separation_challenge[2], dp_logup **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(columns && n_columns >= 1 && n_columns <= 16 && out && constant_challenge && column_separation_challenge, DP_ERR_INVALID, "dp_logup_build: bad argument");
+    for (u32 k = 0; k < n_columns; k++) DP_CHECK(columns[k], DP_ERR_INVALID, "dp_logup_build: null column");
     u64 len = columns[0]->len;
-    for (u32 k = 0; k < n_columns; k++) DP_CHECK(columns[k] && !columns[k]->is_ext && columns[k]->len == len, DP_ERR_INVALID, "All sets of evaluations should be the same length");   // structs.rs:168-176
+    for (u32 k = 0; k < n_columns; k++) DP_CHECK(!columns[k]->is_ext && columns[k]->len == len, DP_ERR_INVALID, "All sets of evaluations should be the same length");   // structs.rs:168-176
     DP_CHECK(len >= 4, DP_ERR_INVALID, "dp_logup_build: need at least 4 evaluations");
     if (multiplicities) DP_CHECK(!multiplicities->is_ext && multiplicities->len == len, DP_ERR_INVALID, "Multiplicities length was not equal to column evaluations length");
     DpCtx &c = dp_ctx();
@@ -95,7 +96,7 @@ int dp_logup_build(dp_mle *const *columns, uint32_t n_columns, const dp_mle *mul
     // one allocation: layer k has 2^(nv-k) entries, k = 0..nv-1; (num, den) each
     u64 total = 0;
     for (u32 k = 0; k < L->nv; k++) total += 2 * (len >> k);
-    if (int e = dp_dev_alloc((void **)&L->block, sizeof(gle) * total)) return e;
+    if (int e = dp_dev_alloc((void **)&L->block, sizeof(gle) * total)) { delete L; return e; }
     gle *p = L->block;
     for (u32 k = 0; k < L->nv; k++) { L->num.push_back(p); p += len >> k; L->den.push_back(p); p += len >> k; }
     ColsArg ca; memset(&ca, 0, sizeof ca); ca.n = n_columns;
@@ -184,10 +185,11 @@ int dp_logup_free(dp_logup *L) {
 int dp_mle_linear_combination(dp_mle *const *mles, const uint64_t *coefs, uint32_t n, dp_mle **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(mles && coefs && out && n >= 1 && n <= 16, DP_ERR_INVALID, "dp_mle_linear_combination: bad argument");
+    for (u32 k = 0; k < n; k++) DP_CHECK(mles[k], DP_ERR_INVALID, "dp_mle_linear_combination: null operand");
     LinArg a; memset(&a, 0, sizeof a); a.n = n;
     u64 len = mles[0]->len;
     for (u32 k = 0; k < n; k++) {
-        DP_CHECK(mles[k] && mles[k]->is_ext && mles[k]->len == len, DP_ERR_INVALID, "dp_mle_linear_combination: operands must be Ext MLEs of equal length");
+        DP_CHECK(mles[k]->is_ext && mles[k]->len == len, DP_ERR_INVALID, "dp_mle_linear_combination: operands must be Ext MLEs of equal length");
         a.m[k] = (const gle *)mles[k]->data; a.coef[k] = e_make(gl_canon(coefs[2 * k]), gl_canon(coefs[2 * k + 1]));
     }
     dp_mle *r = new dp_mle(); r->len = len; r->is_ext = true; r->owned = true;

@@ -113,15 +113,26 @@ static int wit_new_base(u64 len, dp_mle **out) {
     if (int e = dp_dev_alloc(&m->data, m->bytes())) { delete m; return e; }
     *out = m; return DP_OK;
 }
+// n fresh columns of `len`, or none: on a failed allocation the ones already made are freed
+static int wit_new_cols(u64 len, u32 n, dp_mle **cols) {
+    for (u32 k = 0; k < n; k++) {
+        if (int e = wit_new_base(len, &cols[k])) {
+            for (u32 q = 0; q < k; q++) { dp_mle_free(cols[q]); cols[q] = nullptr; }
+            return e;
+        }
+    }
+    return DP_OK;
+}
 
 extern "C" {
 
 int dp_wit_begin(uint32_t n_tables, const uint32_t *kinds, const uint32_t *sizes, dp_wit **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(out && kinds && sizes && n_tables >= 1 && n_tables <= 8, DP_ERR_INVALID, "dp_wit_begin: 1..8 tables");
+    for (u32 t = 0; t < n_tables; t++)
+        DP_CHECK(kinds[t] == 0 || kinds[t] == 2 || (kinds[t] == 3 && sizes[t] >= 1 && sizes[t] <= 24), DP_ERR_INVALID, "dp_wit_begin: unknown table type");
     dp_wit *w = new dp_wit(); w->n_tables = n_tables;
     for (u32 t = 0; t < n_tables; t++) {
-        DP_CHECK(kinds[t] == 0 || kinds[t] == 2 || (kinds[t] == 3 && sizes[t] >= 1 && sizes[t] <= 24), DP_ERR_INVALID, "dp_wit_begin: unknown table type");
         w->kind[t] = kinds[t]; w->size[t] = sizes[t]; w->off[t + 1] = w->off[t] + (1ULL << wit_vars(kinds[t], sizes[t]));
     }
     int e;
@@ -171,9 +182,11 @@ int dp_wit_requant(dp_wit *w, const dp_mle *x, uint32_t shift, int64_t fixed_poi
     DP_CHECK(w && x && cols && !x->is_ext, DP_ERR_INVALID, "dp_wit_requant: bad argument");
     DP_CHECK(shift >= 1 && shift <= 62 && shift % W_BIT_LEN == 0 && shift / W_BIT_LEN <= 8 && n_cols == 2 + shift / W_BIT_LEN, DP_ERR_INVALID, "dp_wit_requant: shift must be a multiple of BIT_LEN (<= 64 bits) and n_cols = 2 + shift / BIT_LEN");
     if (int e = wit_table(w, clamp_table, 3, "dp_wit_requant")) return e;
+    // 1 << intermediate_bit_size bounds |x|; the reference asserts intermediate_bit_size + fp_scale <= 63 (requant.rs:423-427)
+    DP_CHECK(intermediate_bit_size <= 62, DP_ERR_INVALID, "dp_wit_requant: intermediate_bit_size must be at most 62");
     if (int e = wit_table(w, range_table, 2, "dp_wit_requant")) return e;
     RqCols c; c.n_chunks = shift / W_BIT_LEN;
-    for (u32 k = 0; k < n_cols; k++) { if (int e = wit_new_base(x->len, &cols[k])) return e; }
+    if (int e = wit_new_cols(x->len, n_cols, cols)) return e;
     c.cin = (u64 *)cols[0]->data; c.cout = (u64 *)cols[1]->data;
     for (u32 j = 0; j < c.n_chunks; j++) c.chunk[j] = (u64 *)cols[2 + j]->data;
     DpProfScope prof("k_wit_requant", x->bytes() * (1 + n_cols));
@@ -203,7 +216,7 @@ int dp_wit_pool(dp_wit *w, const dp_mle *x, uint32_t C, uint32_t H, uint32_t Wd,
     const u64 n = (u64)C * (H / 2) * (Wd / 2);
     DP_CHECK((n & (n - 1)) == 0, DP_ERR_INVALID, "dp_wit_pool: output length must be a power of two");
     PoolCols p;
-    for (u32 k = 0; k < 5; k++) { if (int e = wit_new_base(n, &cols[k])) return e; }
+    if (int e = wit_new_cols(n, 5, cols)) return e;
     for (u32 k = 0; k < 4; k++) p.diff[k] = (u64 *)cols[k]->data;
     p.out = (u64 *)cols[4]->data;
     DpProfScope prof("k_wit_pool", x->bytes() + 5 * n * 8);

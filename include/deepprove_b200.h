@@ -254,7 +254,9 @@ int dp_wit_dense(const dp_mle *weights /* [nrows][ncols] */, const dp_mle *bias,
 /* MatMul::op (layers/matrix_mul.rs:230-311): left [R][K] x right ([K][C], or [C][K] when `transposed`: Config::TransposeB) + bias[C] on every
  * row (bias may be NULL) -> [R][C] */
 int dp_wit_matmul(const dp_mle *left, const dp_mle *right, const dp_mle *bias, uint32_t R, uint32_t K, uint32_t C, int transposed, dp_mle **out);
-/* cols[0] clamping input, cols[1] clamping output (= the node's output tensor), cols[2 ..] the shift / BIT_LEN byte chunks */
+/* cols[0] clamping input, cols[1] clamping output (= the node's output tensor), cols[2 ..] the shift / BIT_LEN byte chunks.
+ * Inputs with |x| > 2^intermediate_bit_size set error bit 1; intermediate_bit_size must be at most 62 (the reference requires
+ * intermediate_bit_size + fp_scale <= 63, requant.rs:423-427), larger values are refused with DP_ERR_INVALID. */
 int dp_wit_requant(dp_wit *w, const dp_mle *x, uint32_t shift, int64_t fixed_point_multiplier, uint32_t intermediate_bit_size,
                    uint32_t clamp_table, uint32_t range_table, dp_mle **cols, uint32_t n_cols);
 int dp_wit_relu(dp_wit *w, const dp_mle *x, uint32_t relu_table, dp_mle **out);

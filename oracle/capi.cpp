@@ -260,6 +260,23 @@ void dpo_synthetic_mlp(u32 n_layers, u32 width, u64 seed, int64_t *weights /* n_
     }
 }
 void dpo_synthetic_input(u32 width, u64 seed, int64_t *out) { auto v = synthetic_input(width, seed); memcpy(out, v.data(), 8 * v.size()); }
+// LogUpCircuit::new_lookup_circuit (mult == NULL) / new_table_circuit: every layer, bottom to top.  Layer k (k = 0 .. log2(len) - 1)
+// has len >> k fractions; `out` holds, layer after layer, its numerators and then its denominators ([c0, c1] each).  The numerators
+// of an initial lookup layer (all -1, never stored) are written as zeros.
+void dpo_logup_circuit(const u64 *const *cols, u32 n_cols, u64 len, const u64 *mult, const u64 c[2], const u64 gamma[2], u64 *out) {
+    std::vector<std::vector<u64>> cv(n_cols);
+    std::vector<const std::vector<u64> *> cp;
+    for (u32 k = 0; k < n_cols; k++) { cv[k].assign(cols[k], cols[k] + len); cp.push_back(&cv[k]); }
+    std::vector<u64> mv; if (mult) mv.assign(mult, mult + len);
+    LogUpCircuit C = logup_circuit(cp, mult ? &mv : nullptr, E(f_from_u64(c[0]), f_from_u64(c[1])), E(f_from_u64(gamma[0]), f_from_u64(gamma[1])));
+    size_t o = 0;
+    for (const LogUpLayer &l : C.layers) {
+        for (size_t i = 0; i < l.den.size(); i++) put_e(out, o + i, l.has_num ? l.num[i] : E());
+        o += l.den.size();
+        for (size_t i = 0; i < l.den.size(); i++) put_e(out, o + i, l.den[i]);
+        o += l.den.size();
+    }
+}
 }
 
 // prove_batch_polys: the caller passes the FULL MLEs; they are split into T contiguous slices here
