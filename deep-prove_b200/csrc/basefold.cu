@@ -24,6 +24,7 @@
 #include <algorithm>
 #include <atomic>
 #include <map>
+#include <memory>
 
 static constexpr u32 BF_RATE_LOG = 1;            // RSCodeDefaultSpec (rs.rs:192-214)
 static constexpr u32 BF_BASECODE_LOG = 7;
@@ -37,28 +38,52 @@ __global__ void k_pow_table(u64 base, u64 *t /* 3 x 2048 */) {
     u64 e = (u64)idx << (11 * part);
     t[k] = gl_pow(base, e);
 }
-struct BfGlobals { u64 *root_tab = nullptr; bool p2_ready = false; };
+static PowTab powtab_at(const u64 *t) { PowTab p; p.t0 = t; p.t1 = t + 2048; p.t2 = t + 4096; return p; }
+// a table that lives for the rest of the process, complete before it is returned: other host threads' streams may read it as soon
+// as the caller publishes the pointer
+static int pow_table_build(u64 base, const u64 **out) {
+    u64 *tab = nullptr;
+    DP_CUDA(cudaMalloc((void **)&tab, sizeof(u64) * 3 * 2048));
+    k_pow_table<<<24, 256, 0, dp_ctx().stream>>>(base, tab); DP_LAUNCHED();
+    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_stream_sync(dp_ctx().stream));
+    *out = tab;
+    return DP_OK;
+}
+struct BfGlobals { std::atomic<const u64 *> root_tab{nullptr}; std::atomic<bool> p2_ready{false}; };
 static BfGlobals g_bf;          // process-wide, read-only once built (shared by every host thread's context)
 static std::mutex g_bf_mu;
 static int bf_prepare() {
-    if (g_bf.p2_ready && g_bf.root_tab) return DP_OK;
+    if (g_bf.p2_ready.load() && g_bf.root_tab.load()) return DP_OK;
     std::lock_guard<std::mutex> lk(g_bf_mu);
-    if (!g_bf.p2_ready) {
+    if (!g_bf.p2_ready.load()) {
         DP_CUDA(p2_upload_constants((const u64 *)&DP_P2_EXT_RC[0][0][0], (const u64 *)DP_P2_INT_RC, (const u64 *)DP_P2_DIAG));
-        g_bf.p2_ready = true;
+        g_bf.p2_ready.store(true);
     }
-    if (!g_bf.root_tab) {
-        u64 *tab = nullptr;
-        DP_CUDA(cudaMalloc((void **)&tab, sizeof(u64) * 3 * 2048));
-        k_pow_table<<<24, 256, 0, dp_ctx().stream>>>(GL_ROOT32, tab); DP_LAUNCHED();
-        DP_CUDA(cudaGetLastError());
-        DP_CUDA(dp_stream_sync(dp_ctx().stream));   // complete before any other thread's stream reads it
-        g_bf.root_tab = tab;
+    if (!g_bf.root_tab.load()) {
+        const u64 *tab = nullptr;
+        if (int e = pow_table_build(GL_ROOT32, &tab)) return e;
+        g_bf.root_tab.store(tab);
     }
     return DP_OK;
 }
-static PowTab root_tab() { PowTab t; t.t0 = g_bf.root_tab; t.t1 = g_bf.root_tab + 2048; t.t2 = g_bf.root_tab + 4096; return t; }
+static PowTab root_tab() { return powtab_at(g_bf.root_tab.load()); }
 int dp_root_powtab(PowTab *out) { if (int e = bf_prepare()) return e; *out = root_tab(); return DP_OK; }
+// shift^j tables, one per coset shift (i.e. per full_log - nv), built on first use and kept
+static int shift_powtab(u64 shift, PowTab *out) {
+    static std::map<u64, const u64 *> tabs;
+    std::lock_guard<std::mutex> lk(g_bf_mu);
+    auto it = tabs.find(shift);
+    if (it == tabs.end()) {
+        const u64 *tab = nullptr;
+        if (int e = pow_table_build(shift, &tab)) return e;
+        it = tabs.emplace(shift, tab).first;
+    }
+    *out = powtab_at(it->second);
+    return DP_OK;
+}
+// coset shift of a 2^nv polynomial committed under full_log: 7^(2^(full_log - nv))  (rs.rs:481-488)
+static u64 coset_shift(u32 full_log, u32 nv) { u64 shift = 7; for (u32 i = 0; i < full_log - nv; i++) shift = gl_sqr(shift); return shift; }
 
 // ---- bit reversal (out of place) ----
 template <typename T>
@@ -208,27 +233,37 @@ template <bool EXT> __device__ __forceinline__ void leaf_pair_digest(const void 
     if (EXT) { const gle *l = (const gle *)leaves + 2 * pair; gle a = ld_e(l), b = ld_e(l + 1); d[0] = a.c0; d[1] = a.c1; d[2] = b.c0; d[3] = b.c1; }
     else { ulonglong2 v = ld_b2((const u64 *)leaves + 2 * pair); d[0] = v.x; d[1] = v.y; d[2] = 0; d[3] = 0; }
 }
+// the two children of hash i on the first level of a single-polynomial tree: leaf pairs 2i and 2i + 1
+template <bool EXT> __device__ __forceinline__ void mk_leaf_children(const void *leaves, u64 i, u64 x[4], u64 y[4]) {
+    leaf_pair_digest<EXT>(leaves, 2 * i, x); leaf_pair_digest<EXT>(leaves, 2 * i + 1, y);
+}
+// the two children of a hash on a higher level: the 8 digest words at `in`
+__device__ __forceinline__ void mk_node_children(const u64 *in, u64 x[4], u64 y[4]) {
+    ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(in), b = *reinterpret_cast<const ulonglong2 *>(in + 2);
+    ulonglong2 c = *reinterpret_cast<const ulonglong2 *>(in + 4), d = *reinterpret_cast<const ulonglong2 *>(in + 6);
+    x[0] = a.x; x[1] = a.y; x[2] = b.x; x[3] = b.y; y[0] = c.x; y[1] = c.y; y[2] = d.x; y[3] = d.y;
+}
+__device__ __forceinline__ void mk_store(u64 *out, u64 i, const u64 d[4]) {
+    *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(d[0], d[1]);
+    *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(d[2], d[3]);
+}
 template <bool EXT>
 __global__ void k_merkle_l1(const void *__restrict__ leaves, u64 n_out, u64 *__restrict__ out) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
     for (; i < n_out; i += stride) {
         u64 x[4], y[4], o[4];
-        leaf_pair_digest<EXT>(leaves, 2 * i, x); leaf_pair_digest<EXT>(leaves, 2 * i + 1, y);
+        mk_leaf_children<EXT>(leaves, i, x, y);
         p2_compress(x, y, o);
-        *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(o[0], o[1]);
-        *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(o[2], o[3]);
+        mk_store(out, i, o);
     }
 }
 __global__ void k_merkle_up(const u64 *__restrict__ in, u64 n_out, u64 *__restrict__ out) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
     for (; i < n_out; i += stride) {
         u64 x[4], y[4], o[4];
-        ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(in + 8 * i), b = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + 2);
-        ulonglong2 c = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + 4), d = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + 6);
-        x[0] = a.x; x[1] = a.y; x[2] = b.x; x[3] = b.y; y[0] = c.x; y[1] = c.y; y[2] = d.x; y[3] = d.y;
+        mk_node_children(in + 8 * i, x, y);
         p2_compress(x, y, o);
-        *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(o[0], o[1]);
-        *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(o[2], o[3]);
+        mk_store(out, i, o);
     }
 }
 template <bool EXT, bool FROM_LEAVES>
@@ -236,16 +271,10 @@ __global__ void __launch_bounds__(64) k_merkle_mid(const void *__restrict__ src,
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_out) return;
     u64 x[4], y[4], o[4];
-    if (FROM_LEAVES) { leaf_pair_digest<EXT>(src, 2 * i, x); leaf_pair_digest<EXT>(src, 2 * i + 1, y); }
-    else {
-        const u64 *in = (const u64 *)src;
-        ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(in + 8 * i), b = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + 2);
-        ulonglong2 c = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + 4), d = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + 6);
-        x[0] = a.x; x[1] = a.y; x[2] = b.x; x[3] = b.y; y[0] = c.x; y[1] = c.y; y[2] = d.x; y[3] = d.y;
-    }
+    if (FROM_LEAVES) mk_leaf_children<EXT>(src, i, x, y);
+    else mk_node_children((const u64 *)src + 8 * i, x, y);
     p2_compress_lat(x, y, o);
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(o[0], o[1]);
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(o[2], o[3]);
+    mk_store(out, i, o);
 }
 // 8 lanes per hash (poseidon2.cuh): word w of the leaf-pair digest `pair`
 template <bool EXT> __device__ __forceinline__ u64 leaf_pair_word(const void *leaves, u64 pair, int w) {
@@ -286,16 +315,15 @@ __global__ void __launch_bounds__(256) k_merkle_small(const void *src, u32 first
             if (threadIdx.x < cnt) {
                 const u64 i = base + threadIdx.x;
                 u64 x[4], y[4], o[4];
-                if (k == 0 && FROM_LEAVES) { leaf_pair_digest<EXT>(src, 2 * i, x); leaf_pair_digest<EXT>(src, 2 * i + 1, y); }
-                else {
+                if (k == 0 && FROM_LEAVES) mk_leaf_children<EXT>(src, i, x, y);
+                else {   // the 8 words inline: through mk_node_children this kernel's instruction order changes
                     const u64 *in = prev + 8 * i;
                     ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(in), b = *reinterpret_cast<const ulonglong2 *>(in + 2);
                     ulonglong2 c = *reinterpret_cast<const ulonglong2 *>(in + 4), d = *reinterpret_cast<const ulonglong2 *>(in + 6);
                     x[0] = a.x; x[1] = a.y; x[2] = b.x; x[3] = b.y; y[0] = c.x; y[1] = c.y; y[2] = d.x; y[3] = d.y;
                 }
                 p2_compress_lat(x, y, o);
-                *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(o[0], o[1]);
-                *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(o[2], o[3]);
+                mk_store(out, i, o);
             }
         } else for (u32 b = 0; b < cnt; b += 32) {         // 8 lanes per hash, 32 hashes per pass
             if (b + (grp & ~3u) >= cnt) continue;          // warp-uniform (a warp holds 4 lane groups): idle warps skip the permutations
@@ -334,13 +362,19 @@ __global__ void __launch_bounds__(256) k_merkle_small(const void *src, u32 first
     if (threadIdx.x == 0) mk_publish_root(rt, levels + 4 * lo.off[lg - 1]);
 }
 // process-wide pool of zeroed ticket counters (each k_merkle_small launch takes the next one and leaves it zero again)
-static u32 *g_mk_tickets = nullptr; static std::atomic<u32> g_mk_next{0}; static constexpr u32 MK_TICKETS = 4096;
+static std::atomic<u32 *> g_mk_tickets{nullptr}; static std::atomic<u32> g_mk_next{0}; static constexpr u32 MK_TICKETS = 4096;
 static int mk_ticket(u32 **out) {
-    if (!g_mk_tickets) {
+    u32 *tickets = g_mk_tickets.load();
+    if (!tickets) {
         std::lock_guard<std::mutex> lk(g_bf_mu);
-        if (!g_mk_tickets) { u32 *p = nullptr; DP_CUDA(cudaMalloc((void **)&p, sizeof(u32) * MK_TICKETS)); DP_CUDA(cudaMemset(p, 0, sizeof(u32) * MK_TICKETS)); g_mk_tickets = p; }
+        tickets = g_mk_tickets.load();
+        if (!tickets) {
+            DP_CUDA(cudaMalloc((void **)&tickets, sizeof(u32) * MK_TICKETS));
+            DP_CUDA(cudaMemset(tickets, 0, sizeof(u32) * MK_TICKETS));
+            g_mk_tickets.store(tickets);
+        }
     }
-    *out = g_mk_tickets + (g_mk_next.fetch_add(1, std::memory_order_relaxed) % MK_TICKETS);
+    *out = tickets + (g_mk_next.fetch_add(1, std::memory_order_relaxed) % MK_TICKETS);
     return DP_OK;
 }
 
@@ -357,8 +391,7 @@ __global__ void k_merkle_batch_l0(BatchPtrs bp, u32 m, u64 n_out, u64 *__restric
     auto gb = [&](int k) -> u64 { return EXT ? ((const u64 *)bp.p[k >> 1])[2 * (2 * i + 1) + (k & 1)] : ((const u64 *)bp.p[k])[2 * i + 1]; };
     p2_hash_or_noop(ga, n, x); p2_hash_or_noop(gb, n, y);
     p2_compress(x, y, o);
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(o[0], o[1]);
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(o[2], o[3]);
+    mk_store(out, i, o);
 }
 template <bool EXT> __global__ void k_leafpair_root(const void *leaves, u64 *out) { u64 d[4]; leaf_pair_digest<EXT>(leaves, 0, d); for (int i = 0; i < 4; i++) out[i] = d[i]; }
 
@@ -377,7 +410,7 @@ template <bool EXT> __global__ void k_b3_leaves(const void *__restrict__ leaves,
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_out) return;
     u64 d[4]; b3_leaf_pair<EXT>(leaves, i, d);
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(d[0], d[1]); *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(d[2], d[3]);
+    mk_store(out, i, d);
 }
 __global__ void k_b3_up(const u64 *__restrict__ in, u64 n_out, u64 *__restrict__ out) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -386,7 +419,7 @@ __global__ void k_b3_up(const u64 *__restrict__ in, u64 n_out, u64 *__restrict__
 #pragma unroll
     for (int k = 0; k < 8; k += 2) { ulonglong2 v = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + k); w[k] = v.x; w[k + 1] = v.y; }
     u64 d[4]; b3::hash_words(w, 8, d);
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(d[0], d[1]); *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(d[2], d[3]);
+    mk_store(out, i, d);
 }
 // every remaining level (<= 1024 hashes at the first one) in one single-block launch
 __global__ void __launch_bounds__(1024) k_b3_tail(const u64 *__restrict__ in0, u32 first_level, u32 lg, u64 nl_first, u64 *levels, LvlOff lo) {
@@ -427,7 +460,6 @@ struct DevTree {
     u64 *levels = nullptr;            // level l (1-based) at offset lvl_off[l] (in digests)
     std::vector<u64> lvl_off;         // lvl_off[l] for l = 1..lg-1
     u64 *root_dev = nullptr;          // 4 limbs
-    bool own_leaves = false;
     const u64 *level0 = nullptr;      // batch trees only: stored digests of the leaf pairs (single-polynomial trees recompute them)
     bool own_levels = true;           // false for the per-polynomial views of a batch commitment
     bool own_level0 = false;          // BLAKE3 trees of one polynomial store their leaf-pair digests (Poseidon2 recomputes them: zero-padded copies)
@@ -445,19 +477,19 @@ static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64
     u64 total = 0;
     for (u32 l = 1; l < t.lg; l++) { t.lvl_off[l] = total; total += n >> (l + 1); }
     if (int e = dp_dev_alloc((void **)&t.levels, sizeof(u64) * 4 * (total + 1))) return e;
+    LvlOff lo_all; memset(&lo_all, 0, sizeof lo_all);
+    for (u32 k = 1; k < t.lg && k < 36; k++) lo_all.off[k] = t.lvl_off[k];
     if (blake_on()) {
         const u64 *l0 = lvl0;
         if (!l0) {
             u64 *own = nullptr; if (int e = dp_dev_alloc((void **)&own, sizeof(u64) * 4 * (n >> 1))) return e;
             DpProfScope prof("k_b3_leaves(blake3)", n * (ext ? 16 : 8) + (n >> 1) * 32);
             const unsigned g = (unsigned)(((n >> 1) + 255) / 256);
-            if (ext) k_b3_leaves<true><<<g, 256, 0, c.stream>>>(leaves, n >> 1, own); else k_b3_leaves<false><<<g, 256, 0, c.stream>>>(leaves, n >> 1, own);
-            DP_LAUNCHED();
+            const auto kern = ext ? k_b3_leaves<true> : k_b3_leaves<false>;
+            kern<<<g, 256, 0, c.stream>>>(leaves, n >> 1, own); DP_LAUNCHED();
             t.level0 = l0 = own; t.own_level0 = true;
         }
         if (t.lg == 1) { t.root_dev = const_cast<u64 *>(l0); DP_CUDA(cudaGetLastError()); return DP_OK; }
-        LvlOff lo_all; memset(&lo_all, 0, sizeof lo_all);
-        for (u32 k = 1; k < t.lg && k < 36; k++) lo_all.off[k] = t.lvl_off[k];
         for (u32 l = 1; l < t.lg; l++) {
             const u64 nl = n >> (l + 1);
             const u64 *in = l == 1 ? l0 : t.levels + 4 * t.lvl_off[l - 1];
@@ -471,27 +503,25 @@ static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64
     }
     if (t.lg == 1 && lvl0) { t.root_dev = const_cast<u64 *>(lvl0); }
     else if (t.lg == 1) {
-        if (ext) k_leafpair_root<true><<<1, 1, 0, c.stream>>>(leaves, t.levels); else k_leafpair_root<false><<<1, 1, 0, c.stream>>>(leaves, t.levels);
-        DP_LAUNCHED(); t.root_dev = t.levels;
+        const auto kern = ext ? k_leafpair_root<true> : k_leafpair_root<false>;
+        kern<<<1, 1, 0, c.stream>>>(leaves, t.levels); DP_LAUNCHED();
+        t.root_dev = t.levels;
     } else {
-        u32 l = 1;
-        LvlOff lo_all; memset(&lo_all, 0, sizeof lo_all);
-        for (u32 k = 1; k < t.lg && k < 36; k++) lo_all.off[k] = t.lvl_off[k];
-        for (; l < t.lg; l++) {
+        for (u32 l = 1; l < t.lg; l++) {
             const u64 nl = n >> (l + 1);
             const bool from_leaves = (l == 1 && !lvl0);
             const u64 in_bytes = from_leaves ? nl * (ext ? 64 : 32) : nl * 64;
+            const void *src = l == 1 ? (lvl0 ? (const void *)lvl0 : leaves) : (const void *)(t.levels + 4 * t.lvl_off[l - 1]);
+            u64 *out = t.levels + 4 * t.lvl_off[l];
             if (nl <= MK_SMALL && t.lg < 36) {   // this and every remaining level in one launch
                 DpProfScope prof("k_merkle_small(poseidon2 compress, all remaining levels)", in_bytes + (2 * nl - 1) * 32 * 2, 2 * (2 * nl - 1));
                 const bool many = dp_wait_mode() == DP_WAIT_BLOCK;     // the throughput configuration (many proofs in flight)
                 const u32 sub_max = many ? MK_SUB : 32, tph_min = many ? 64 : 0xFFFFFFFFu;
                 const unsigned g = (unsigned)((nl + sub_max - 1) / sub_max);
                 u32 *ticket = nullptr; if (int e = mk_ticket(&ticket)) return e;
-                const void *src = l == 1 ? (lvl0 ? (const void *)lvl0 : leaves) : (const void *)(t.levels + 4 * t.lvl_off[l - 1]);
                 RootOut ro = rt ? *rt : RootOut{nullptr, nullptr, 0};
-                if (from_leaves) { if (ext) k_merkle_small<true, true><<<g, 256, 0, c.stream>>>(src, l, t.lg, nl, t.levels, lo_all, ticket, ro, sub_max, tph_min); else k_merkle_small<false, true><<<g, 256, 0, c.stream>>>(src, l, t.lg, nl, t.levels, lo_all, ticket, ro, sub_max, tph_min); }
-                else k_merkle_small<false, false><<<g, 256, 0, c.stream>>>(src, l, t.lg, nl, t.levels, lo_all, ticket, ro, sub_max, tph_min);
-                DP_LAUNCHED();
+                const auto kern = from_leaves ? (ext ? k_merkle_small<true, true> : k_merkle_small<false, true>) : k_merkle_small<false, false>;
+                kern<<<g, 256, 0, c.stream>>>(src, l, t.lg, nl, t.levels, lo_all, ticket, ro, sub_max, tph_min); DP_LAUNCHED();
                 if (rt && rt_done) *rt_done = true;
                 break;
             }
@@ -501,20 +531,16 @@ static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64
                 // for the 8-lanes-per-hash kernel used before), but it now holds 1/8 of the thread slots and issues ~1/5 of the
                 // instructions, so the mid levels of many proofs' trees overlap instead of queueing behind each other.
                 DpProfScope prof("k_merkle_mid(poseidon2 compress, thread per hash)", in_bytes + nl * 32, 2 * nl);
-                const unsigned g = (unsigned)((nl + 63) / 64);
-                if (from_leaves) { if (ext) k_merkle_mid<true, true><<<g, 64, 0, c.stream>>>(leaves, nl, t.levels); else k_merkle_mid<false, true><<<g, 64, 0, c.stream>>>(leaves, nl, t.levels); }
-                else k_merkle_mid<false, false><<<g, 64, 0, c.stream>>>(l == 1 ? (const void *)lvl0 : (const void *)(t.levels + 4 * t.lvl_off[l - 1]), nl, t.levels + 4 * t.lvl_off[l]);
-                DP_LAUNCHED();
+                const auto kern = from_leaves ? (ext ? k_merkle_mid<true, true> : k_merkle_mid<false, true>) : k_merkle_mid<false, false>;
+                kern<<<(unsigned)((nl + 63) / 64), 64, 0, c.stream>>>(src, nl, out); DP_LAUNCHED();
                 continue;
             }
             DpProfScope prof("k_merkle(poseidon2 compress)", in_bytes + nl * 32, 2 * nl);
             const unsigned mgrid = (unsigned)std::min<u64>((nl + 127) / 128, 1u << 22);
-            if (from_leaves) {
-                // one hash per thread, many SHORT blocks (no persistent grid-stride blocks): with 16 proofs in flight the block
-                // scheduler can interleave other streams' latency-critical single-block kernels every few microseconds
-                if (ext) k_merkle_l1<true><<<mgrid, 128, 0, c.stream>>>(leaves, nl, t.levels);
-                else k_merkle_l1<false><<<mgrid, 128, 0, c.stream>>>(leaves, nl, t.levels);
-            } else k_merkle_up<<<mgrid, 128, 0, c.stream>>>(l == 1 ? lvl0 : t.levels + 4 * t.lvl_off[l - 1], nl, t.levels + 4 * t.lvl_off[l]);
+            // one hash per thread, many SHORT blocks (no persistent grid-stride blocks): with 16 proofs in flight the block
+            // scheduler can interleave other streams' latency-critical single-block kernels every few microseconds
+            if (from_leaves) { const auto kern = ext ? k_merkle_l1<true> : k_merkle_l1<false>; kern<<<mgrid, 128, 0, c.stream>>>(src, nl, out); }
+            else k_merkle_up<<<mgrid, 128, 0, c.stream>>>((const u64 *)src, nl, out);
             DP_LAUNCHED();
         }
         t.root_dev = t.levels + 4 * t.lvl_off[t.lg - 1];
@@ -522,7 +548,9 @@ static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64
     DP_CUDA(cudaGetLastError());
     return DP_OK;
 }
-static void tree_free(DevTree &t) { if (t.own_levels) dp_dev_free(t.levels); t.levels = nullptr; if (t.own_level0) { dp_dev_free(const_cast<u64 *>(t.level0)); t.level0 = nullptr; t.own_level0 = false; } if (t.own_leaves) dp_dev_free(const_cast<void *>(t.leaves)); t.leaves = nullptr; }
+static void tree_free(DevTree &t) { if (t.own_levels) dp_dev_free(t.levels); t.levels = nullptr; if (t.own_level0) { dp_dev_free(const_cast<u64 *>(t.level0)); t.level0 = nullptr; t.own_level0 = false; } t.leaves = nullptr; }
+// the same tree, owning nothing (the per-polynomial views of a batch commitment)
+static DevTree tree_view(const DevTree &t) { DevTree v = t; v.own_levels = false; v.own_level0 = false; return v; }
 
 // ---- K10 FRI fold (commit_phase.rs:511-526, rs.rs:377-410, arithmetic.rs:120-132) ----
 // out[i] = y0 + (r - x0) * (y1 - y0) * w,  x0 = w_{2^(level+1)}^{rev(i, level)} * gamma_lvl,  w = -1/(2 x0)
@@ -683,6 +711,56 @@ static void msg_to_coeffs(const uint64_t *ev /* p(0),p(1),p(2) */, uint64_t *out
     out[0] = p0.c0; out[1] = p0.c1; out[2] = c1.c0; out[3] = c1.c1; out[4] = c2.c0; out[5] = c2.c1;
 }
 
+// Owning handles for objects under construction: an error return releases whatever has been built so far.
+template <auto Free> struct FreeWith { template <typename P> void operator()(P *p) const { Free(p); } };
+using CommPtr = std::unique_ptr<dp_pcs_comm, FreeWith<dp_pcs_comm_free>>;
+using OpenPtr = std::unique_ptr<dp_pcs_open, FreeWith<dp_pcs_open_free>>;
+using MlePtr = std::unique_ptr<dp_mle, FreeWith<dp_mle_free>>;
+using DevPtr = std::unique_ptr<void, FreeWith<dp_dev_free>>;
+
+// Encode of a 2^nv polynomial whose whole codeword fits in one block's shared memory: one launch
+template <typename T>
+static int encode_small(const void *evals, void *bh_evals, void *codeword, u32 nv, u64 shift) {
+    const u64 m = 1ULL << nv;
+    const size_t smem = sizeof(T) << (nv + BF_RATE_LOG);
+    DpProfScope p("k_encode_small(bitrev+moebius+expand+ntt)", sizeof(T) * m * 2 + smem);
+    if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_encode_small<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_encode_small<T><<<1, 512, smem, dp_ctx().stream>>>((const T *)evals, (T *)bh_evals, (T *)codeword, nv, shift, root_tab()); DP_LAUNCHED();
+    DP_CUDA(cudaGetLastError());
+    return DP_OK;
+}
+
+// Tiled encode of a 2^nv polynomial: bit reversal, Moebius levels (K7), then zero-pad + coset scale + the DIF levels (K8).
+// logG = 0: bh_evals and codeword are whole; k_expand does the first DIF level, tiled passes do levels [1, n_log).
+// logG > 0: they are rank `rank`'s slices (2^(nv - logG) evaluations, 2^(n_log - logG) codeword entries); k_shard_expand does the
+// first logG levels for this slice, tiled passes do levels [0, n_log - logG) on it.
+template <typename T>
+static int encode_tiled(const void *evals, void *bh_evals, void *codeword, u32 nv, u64 shift, u32 logG, u32 rank) {
+    DpCtx &c = dp_ctx();
+    const size_t esz = sizeof(T);
+    const u32 n_log = nv + BF_RATE_LOG;
+    const u64 m = 1ULL << nv, Ml = m >> logG, S = (1ULL << n_log) >> logG;
+    T *bh = (T *)bh_evals, *cw = (T *)codeword, *coef = nullptr;
+    if (int e = dp_dev_alloc((void **)&coef, esz * m)) return e;
+    DevPtr coef_owner(coef);
+    PowTab st; if (int e = shift_powtab(shift, &st)) return e;
+    const int g = dp_grid_for(m, 256, 8);
+    { DpProfScope p("k_bitrev", esz * m * 2); k_bitrev<T><<<g, 256, 0, c.stream>>>((const T *)evals, logG ? coef : bh, nv); DP_LAUNCHED(); }
+    if (!logG) DP_CUDA(cudaMemcpyAsync(coef, bh, esz * m, cudaMemcpyDeviceToDevice, c.stream));
+    else if (cudaMemcpyAsync(bh, coef + Ml * rank, esz * Ml, cudaMemcpyDeviceToDevice, c.stream) != cudaSuccess)
+        return dp_fail(DP_ERR_CUDA, "dp_pcs_commit_shard: copy of the evaluation slice failed");
+    if (int e = run_levels<T, 0>(coef, nv, 0, nv)) return e;
+    if (!logG) { DpProfScope p("k_expand", esz * m * 3); k_expand<T><<<g, 256, 0, c.stream>>>(coef, cw, nv, st, root_tab()); DP_LAUNCHED(); }
+    else {
+        u32 rev_rank = 0; for (u32 b = 0; b < logG; b++) if (rank >> b & 1) rev_rank |= 1u << (logG - 1 - b);
+        DpProfScope p("k_shard_expand", esz * (m + S));
+        k_shard_expand<T><<<dp_grid_for(S, 256, 8), 256, 0, c.stream>>>(coef, cw, nv, logG, rev_rank, st, root_tab()); DP_LAUNCHED();
+    }
+    if (int e = run_levels<T, 1>(cw, n_log - logG, logG ? 0 : 1, n_log - logG)) return e;
+    DP_CUDA(cudaGetLastError());
+    return DP_OK;
+}
+
 extern "C" {
 
 int dp_set_merkle_hasher(int kind) {
@@ -701,7 +779,7 @@ int dp_poseidon2_init(const uint64_t *ext_rc /*2x4x8*/, const uint64_t *int_rc /
     for (int i = 0; i < 8; i++) d[i] = gl_canon(diag[i]);
     DP_CUDA(dp_stream_sync(dp_ctx().stream));
     DP_CUDA(p2_upload_constants(a, b, d));
-    g_bf.p2_ready = true;
+    g_bf.p2_ready.store(true);
     return DP_OK;
 }
 
@@ -713,7 +791,7 @@ static int commit_enqueue(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **o
     if (int e = bf_prepare()) return e;
     DpCtx &c = dp_ctx();
     if (!root_pinned && with_tree) return dp_fail(DP_ERR_INVALID, "commit_enqueue: no root buffer");
-    dp_pcs_comm *cm = new dp_pcs_comm();
+    CommPtr cm(new dp_pcs_comm());
     cm->num_vars = nv; cm->full_log = full_log; cm->is_base = !poly->is_ext;
     size_t esz = poly->is_ext ? 16 : 8;
     u64 m = poly->len;
@@ -723,65 +801,21 @@ static int commit_enqueue(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **o
         DP_CUDA(cudaMemcpyAsync(cm->bh_evals, poly->data, esz * m, cudaMemcpyDeviceToDevice, c.stream));
         cm->codeword = cm->bh_evals; cm->cw_len = m;
     } else {
-        u64 N = m << BF_RATE_LOG; u32 n_log = nv + BF_RATE_LOG;
-        cm->cw_len = N;
-        if (int e = dp_dev_alloc(&cm->codeword, esz * N)) return e;
-        // coset shift: shift = 7^(2^(full_log - lg m))  (rs.rs:481-488)
-        u64 shift = 7; for (u32 i = 0; i < full_log - nv; i++) shift = gl_sqr(shift);
-        if (esz * N <= 64 * 1024 && nv <= 15) {   // the whole codeword fits in one block's shared memory: one launch
-            size_t smem = esz * N;
-            DpProfScope p("k_encode_small(bitrev+moebius+expand+ntt)", esz * m * 2 + esz * N);
-            if (poly->is_ext) {
-                if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_encode_small<gle>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                k_encode_small<gle><<<1, 512, smem, c.stream>>>((const gle *)poly->data, (gle *)cm->bh_evals, (gle *)cm->codeword, nv, shift, root_tab());
-            } else {
-                if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_encode_small<u64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                k_encode_small<u64><<<1, 512, smem, c.stream>>>((const u64 *)poly->data, (u64 *)cm->bh_evals, (u64 *)cm->codeword, nv, shift, root_tab());
-            }
-            DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
-        } else {
-        void *coef = nullptr;
-        if (int e = dp_dev_alloc(&coef, esz * m)) return e;
-        // powers of the coset shift: one table per (full_log - nv), built once per process and kept (read-only afterwards)
-        const u64 *stab = nullptr;
-        {
-            static std::map<u64, const u64 *> shift_tabs;
-            std::lock_guard<std::mutex> lk(g_bf_mu);
-            auto it = shift_tabs.find(shift);
-            if (it == shift_tabs.end()) {
-                u64 *nt = nullptr;
-                DP_CUDA(cudaMalloc((void **)&nt, sizeof(u64) * 3 * 2048));
-                k_pow_table<<<24, 256, 0, c.stream>>>(shift, nt); DP_LAUNCHED();
-                DP_CUDA(dp_stream_sync(c.stream));       // other host threads' streams may read it as soon as the map holds it
-                it = shift_tabs.emplace(shift, nt).first;
-            }
-            stab = it->second;
-        }
-        PowTab st; st.t0 = stab; st.t1 = stab + 2048; st.t2 = stab + 4096;
-        int g = dp_grid_for(m, 256, 8);
-        if (poly->is_ext) {
-            { DpProfScope p("k_bitrev", esz * m * 2); k_bitrev<gle><<<g, 256, 0, c.stream>>>((const gle *)poly->data, (gle *)cm->bh_evals, nv); DP_LAUNCHED(); }
-            DP_CUDA(cudaMemcpyAsync(coef, cm->bh_evals, esz * m, cudaMemcpyDeviceToDevice, c.stream));
-            if (int e = run_levels<gle, 0>((gle *)coef, nv, 0, nv)) return e;                 // K7
-            { DpProfScope p("k_expand", esz * m * 3); k_expand<gle><<<g, 256, 0, c.stream>>>((const gle *)coef, (gle *)cm->codeword, nv, st, root_tab()); DP_LAUNCHED(); }
-            if (int e = run_levels<gle, 1>((gle *)cm->codeword, n_log, 1, n_log)) return e;  // K8
-        } else {
-            { DpProfScope p("k_bitrev", esz * m * 2); k_bitrev<u64><<<g, 256, 0, c.stream>>>((const u64 *)poly->data, (u64 *)cm->bh_evals, nv); DP_LAUNCHED(); }
-            DP_CUDA(cudaMemcpyAsync(coef, cm->bh_evals, esz * m, cudaMemcpyDeviceToDevice, c.stream));
-            if (int e = run_levels<u64, 0>((u64 *)coef, nv, 0, nv)) return e;
-            { DpProfScope p("k_expand", esz * m * 3); k_expand<u64><<<g, 256, 0, c.stream>>>((const u64 *)coef, (u64 *)cm->codeword, nv, st, root_tab()); DP_LAUNCHED(); }
-            if (int e = run_levels<u64, 1>((u64 *)cm->codeword, n_log, 1, n_log)) return e;
-        }
-        DP_CUDA(cudaGetLastError());
-        dp_dev_free(coef);
-        }
+        cm->cw_len = m << BF_RATE_LOG;
+        if (int e = dp_dev_alloc(&cm->codeword, esz * cm->cw_len)) return e;
+        const u64 shift = coset_shift(full_log, nv);
+        int rc;
+        if (esz * cm->cw_len <= 64 * 1024 && nv <= 15)   // the whole codeword fits in one block's shared memory
+            rc = poly->is_ext ? encode_small<gle>(poly->data, cm->bh_evals, cm->codeword, nv, shift) : encode_small<u64>(poly->data, cm->bh_evals, cm->codeword, nv, shift);
+        else rc = poly->is_ext ? encode_tiled<gle>(poly->data, cm->bh_evals, cm->codeword, nv, shift, 0, 0) : encode_tiled<u64>(poly->data, cm->bh_evals, cm->codeword, nv, shift, 0, 0);
+        if (rc) return rc;
     }
     if (with_tree) {
         RootOut ro{root_pinned, nullptr, 0}; bool published = false;
         if (int e = tree_build(cm->tree, cm->codeword, poly->is_ext, cm->cw_len, nullptr, &ro, &published)) return e;   // K9
         if (!published) DP_CUDA(cudaMemcpyAsync(root_pinned, cm->tree.root_dev, 32, cudaMemcpyDeviceToHost, c.stream));
     }
-    *out = cm;
+    *out = cm.release();
     return DP_OK;
 }
 
@@ -797,21 +831,6 @@ int dp_pcs_commit(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **out) {
 }
 
 
-// shift^j tables per (full_log - nv): shared with commit_enqueue
-static int shift_powtab(u64 shift, PowTab *out) {
-    static std::map<u64, const u64 *> tabs;
-    std::lock_guard<std::mutex> lk(g_bf_mu);
-    auto it = tabs.find(shift);
-    if (it == tabs.end()) {
-        u64 *nt = nullptr;
-        DP_CUDA(cudaMalloc((void **)&nt, sizeof(u64) * 3 * 2048));
-        k_pow_table<<<24, 256, 0, dp_ctx().stream>>>(shift, nt); DP_LAUNCHED();
-        DP_CUDA(cudaStreamSynchronize(dp_ctx().stream));
-        it = tabs.emplace(shift, nt).first;
-    }
-    out->t0 = it->second; out->t1 = it->second + 2048; out->t2 = it->second + 4096;
-    return DP_OK;
-}
 // the replicated tree over the world's subtree roots: level "0" = the G roots, then log G levels of compress
 static int top_tree_build(DevTree &top, u64 **top_lvl0, const uint64_t *roots, u32 logG, u64 out_root[4]) {
     DpCtx &c = dp_ctx();
@@ -843,39 +862,19 @@ int dp_pcs_commit_shard(const dp_mle *poly, uint32_t full_log, uint32_t rank, ui
     DP_CHECK(logG <= 6 && nv >= BF_BASECODE_LOG + 4 && nv > logG + 11, DP_ERR_INVALID, "dp_pcs_commit_shard: polynomial too small to shard over this many ranks");
     if (int e = bf_prepare()) return e;
     DpCtx &c = dp_ctx();
-    dp_pcs_comm *cm = new dp_pcs_comm();
+    CommPtr cm(new dp_pcs_comm());
     cm->num_vars = nv; cm->full_log = full_log; cm->is_base = !poly->is_ext; cm->shard_rank = rank; cm->shard_log = logG;
     const size_t esz = poly->is_ext ? 16 : 8;
-    const u64 m = poly->len, N = m << BF_RATE_LOG, S = N >> logG, Ml = m >> logG; const u32 n_log = nv + BF_RATE_LOG;
-    cm->cw_len = S;
-    void *coef = nullptr;
-    auto fail = [&](int e) { dp_dev_free(coef); dp_pcs_comm_free(cm); return e; };
-    if (int e = dp_dev_alloc(&cm->bh_evals, esz * Ml)) return fail(e);
-    if (int e = dp_dev_alloc(&cm->codeword, esz * S)) return fail(e);
-    if (int e = dp_dev_alloc(&coef, esz * m)) return fail(e);
-    u64 shift = 7; for (u32 i = 0; i < full_log - nv; i++) shift = gl_sqr(shift);
-    PowTab st; if (int e = shift_powtab(shift, &st)) return fail(e);
-    const int g = dp_grid_for(m, 256, 8), gs = dp_grid_for(S, 256, 8);
-    u32 rev_rank = 0; for (u32 b = 0; b < logG; b++) if (rank >> b & 1) rev_rank |= 1u << (logG - 1 - b);
-    if (poly->is_ext) {
-        { DpProfScope p("k_bitrev", esz * m * 2); k_bitrev<gle><<<g, 256, 0, c.stream>>>((const gle *)poly->data, (gle *)coef, nv); DP_LAUNCHED(); }
-        if (cudaMemcpyAsync(cm->bh_evals, (const char *)coef + esz * Ml * rank, esz * Ml, cudaMemcpyDeviceToDevice, c.stream) != cudaSuccess) return fail(dp_fail(DP_ERR_CUDA, "dp_pcs_commit_shard: copy of the evaluation slice failed"));
-        if (int e = run_levels<gle, 0>((gle *)coef, nv, 0, nv)) return fail(e);
-        { DpProfScope p("k_shard_expand", esz * (m + S)); k_shard_expand<gle><<<gs, 256, 0, c.stream>>>((const gle *)coef, (gle *)cm->codeword, nv, logG, rev_rank, st, root_tab()); DP_LAUNCHED(); }
-        if (int e = run_levels<gle, 1>((gle *)cm->codeword, n_log - logG, 0, n_log - logG)) return fail(e);
-    } else {
-        { DpProfScope p("k_bitrev", esz * m * 2); k_bitrev<u64><<<g, 256, 0, c.stream>>>((const u64 *)poly->data, (u64 *)coef, nv); DP_LAUNCHED(); }
-        if (cudaMemcpyAsync(cm->bh_evals, (const char *)coef + esz * Ml * rank, esz * Ml, cudaMemcpyDeviceToDevice, c.stream) != cudaSuccess) return fail(dp_fail(DP_ERR_CUDA, "dp_pcs_commit_shard: copy of the evaluation slice failed"));
-        if (int e = run_levels<u64, 0>((u64 *)coef, nv, 0, nv)) return fail(e);
-        { DpProfScope p("k_shard_expand", esz * (m + S)); k_shard_expand<u64><<<gs, 256, 0, c.stream>>>((const u64 *)coef, (u64 *)cm->codeword, nv, logG, rev_rank, st, root_tab()); DP_LAUNCHED(); }
-        if (int e = run_levels<u64, 1>((u64 *)cm->codeword, n_log - logG, 0, n_log - logG)) return fail(e);
-    }
-    DP_CUDA(cudaGetLastError());
-    if (int e = tree_build(cm->tree, cm->codeword, poly->is_ext, S)) return fail(e);
-    if (int e = dp_d2h(cm->local_root, cm->tree.root_dev, 32, c.stream)) return fail(e);
-    dp_dev_free(coef); coef = nullptr;
+    cm->cw_len = (poly->len << BF_RATE_LOG) >> logG;
+    if (int e = dp_dev_alloc(&cm->bh_evals, esz * (poly->len >> logG))) return e;
+    if (int e = dp_dev_alloc(&cm->codeword, esz * cm->cw_len)) return e;
+    const u64 shift = coset_shift(full_log, nv);
+    if (int e = poly->is_ext ? encode_tiled<gle>(poly->data, cm->bh_evals, cm->codeword, nv, shift, logG, rank)
+                             : encode_tiled<u64>(poly->data, cm->bh_evals, cm->codeword, nv, shift, logG, rank)) return e;
+    if (int e = tree_build(cm->tree, cm->codeword, poly->is_ext, cm->cw_len)) return e;
+    if (int e = dp_d2h(cm->local_root, cm->tree.root_dev, 32, c.stream)) return e;
     memcpy(cm->root, cm->local_root, 32);
-    *out = cm;
+    *out = cm.release();
     return DP_OK;
 }
 // `roots`: world x 4 words, rank-major (the all-gathered subtree roots).  Builds the replicated top of the tree; afterwards
@@ -908,50 +907,41 @@ int dp_pcs_batch_commit(const dp_mle *const *polys, uint32_t n, uint32_t full_lo
                                          "cannot batch commit to polynomials with different number of variables");   // :379-386
     if (int e = bf_prepare()) return e;
     DpCtx &c = dp_ctx();
-    dp_pcs_comm *b = new dp_pcs_comm();
+    CommPtr b(new dp_pcs_comm());
     b->num_vars = polys[0]->num_vars(); b->full_log = full_log; b->is_base = !polys[0]->is_ext;
     if (n == 1) {   // merkelize with one value vector is the plain tree (merkle_tree.rs:274-285): the batch is a view of an ordinary commitment
         dp_pcs_comm *part = nullptr; u64 *pin1 = nullptr;
-        if (int e = dp_pinned_alloc((void **)&pin1, 32)) { dp_pcs_comm_free(b); return e; }
+        if (int e = dp_pinned_alloc((void **)&pin1, 32)) return e;
         int rc = commit_enqueue(polys[0], full_log, &part, pin1, true);
         if (rc == DP_OK) { dp_stream_sync(c.stream); memcpy(part->root, pin1, 32); memcpy(b->root, pin1, 32); }
         dp_pinned_free(pin1);
-        if (rc != DP_OK) { dp_pcs_comm_free(b); return rc; }
+        if (rc != DP_OK) return rc;
         b->parts.push_back(part); b->trivial = part->trivial; b->cw_len = part->cw_len;
-        b->tree = part->tree; b->tree.own_levels = false; b->tree.own_leaves = false;
-        *out = b;
+        b->tree = tree_view(part->tree);
+        *out = b.release();
         return DP_OK;
     }
     BatchPtrs bp; memset(&bp, 0, sizeof bp);
     for (u32 i = 0; i < n; i++) {
         dp_pcs_comm *part = nullptr;
-        if (int e = commit_enqueue(polys[i], full_log, &part, nullptr, false)) { dp_pcs_comm_free(b); return e; }
+        if (int e = commit_enqueue(polys[i], full_log, &part, nullptr, false)) return e;
         b->parts.push_back(part); bp.p[i] = part->codeword;
     }
     b->trivial = b->parts[0]->trivial; b->cw_len = b->parts[0]->cw_len;
     u64 N = b->cw_len, n0 = N >> 1;
-    if (int e = dp_dev_alloc((void **)&b->level0, 32 * n0)) { dp_pcs_comm_free(b); return e; }
+    if (int e = dp_dev_alloc((void **)&b->level0, 32 * n0)) return e;
     {
         DpProfScope prof("k_merkle_batch_l0(poseidon2 sponge + compress)", (u64)n * N * (b->is_base ? 8 : 16) + 32 * n0);
-        unsigned g = (unsigned)((n0 + 127) / 128);
-        if (blake_on()) {
-            DP_CHECK((b->is_base ? n : 2 * n) <= 128, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: BLAKE3 batch leaves are limited to one 1024-byte chunk (128 base / 64 extension polynomials)");
-            if (b->is_base) k_b3_batch_l0<false><<<g, 128, 0, c.stream>>>(bp, n, n0, b->level0); else k_b3_batch_l0<true><<<g, 128, 0, c.stream>>>(bp, n, n0, b->level0);
-        }
-        else if (b->is_base) k_merkle_batch_l0<false><<<g, 128, 0, c.stream>>>(bp, n, n0, b->level0); else k_merkle_batch_l0<true><<<g, 128, 0, c.stream>>>(bp, n, n0, b->level0);
-        DP_LAUNCHED();
+        const bool blake = blake_on();
+        if (blake) DP_CHECK((b->is_base ? n : 2 * n) <= 128, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: BLAKE3 batch leaves are limited to one 1024-byte chunk (128 base / 64 extension polynomials)");
+        const auto kern = blake ? (b->is_base ? k_b3_batch_l0<false> : k_b3_batch_l0<true>) : (b->is_base ? k_merkle_batch_l0<false> : k_merkle_batch_l0<true>);
+        kern<<<(unsigned)((n0 + 127) / 128), 128, 0, c.stream>>>(bp, n, n0, b->level0); DP_LAUNCHED();
     }
-    if (int e = tree_build(b->tree, b->parts[0]->codeword, !b->is_base, N, b->level0)) { dp_pcs_comm_free(b); return e; }
-    for (auto *part : b->parts) {   // per-polynomial views: own leaves, the batch tree's digests
-        DevTree &t = part->tree; t = b->tree; t.leaves = part->codeword; t.own_levels = false; t.own_leaves = false;
-    }
-    u64 *pin = nullptr;
-    if (int e = dp_pinned_alloc((void **)&pin, 32)) { dp_pcs_comm_free(b); return e; }
-    DP_CUDA(cudaMemcpyAsync(pin, b->tree.root_dev, 32, cudaMemcpyDeviceToHost, c.stream));
-    DP_CUDA(dp_stream_sync(c.stream));
-    memcpy(b->root, pin, 32); for (auto *part : b->parts) memcpy(part->root, pin, 32);
-    dp_pinned_free(pin);
-    *out = b;
+    if (int e = tree_build(b->tree, b->parts[0]->codeword, !b->is_base, N, b->level0)) return e;
+    for (auto *part : b->parts) { part->tree = tree_view(b->tree); part->tree.leaves = part->codeword; }   // own leaves, the batch tree's digests
+    if (int e = dp_d2h(b->root, b->tree.root_dev, 32, c.stream)) return e;
+    for (auto *part : b->parts) memcpy(part->root, b->root, 32);
+    *out = b.release();
     return DP_OK;
 }
 // number of polynomials under a commitment (1 for dp_pcs_commit) and the i-th per-polynomial view of a batch commitment
@@ -966,12 +956,13 @@ int dp_pcs_comm_part(const dp_pcs_comm *cm, uint32_t i, const dp_pcs_comm **out)
 // Independent commitments (the reference commits witness columns from rayon workers: activation.rs:293,
 // requant.rs:298/315, lookup/context.rs:677) are enqueued round-robin on a pool of streams so their
 // latency chains (tree depth x Poseidon2 latency) overlap; one synchronisation at the end.
-static thread_local std::vector<cudaStream_t> g_pool; static thread_local std::vector<cudaEvent_t> g_pool_ev; static thread_local cudaEvent_t g_main_ev = nullptr;
-// stream sets are recycled across (short-lived) host threads: creating streams/events is slow and synchronising
-struct StreamSet { std::vector<cudaStream_t> s; std::vector<cudaEvent_t> e; cudaEvent_t main_ev; };
+// A host thread's streams for independent commits, recycled across (short-lived) host threads: creating streams and events is slow
+// and synchronising.  The thread's set goes back to g_free_sets when the thread exits.
+struct StreamSet { std::vector<cudaStream_t> s; std::vector<cudaEvent_t> e; cudaEvent_t main_ev = nullptr; };
 static std::vector<StreamSet> g_free_sets; static std::mutex g_sets_mu;
-struct StreamSetReturn { ~StreamSetReturn() { if (!g_pool.empty()) { std::lock_guard<std::mutex> lk(g_sets_mu); g_free_sets.push_back({g_pool, g_pool_ev, g_main_ev}); } } };
-static thread_local StreamSetReturn g_set_return;
+static thread_local struct ThreadStreamSet : StreamSet {
+    ~ThreadStreamSet() { if (!s.empty()) { std::lock_guard<std::mutex> lk(g_sets_mu); g_free_sets.push_back(std::move(*this)); } }
+} t_streams;
 int dp_pcs_commit_many(const dp_mle *const *polys, uint32_t n, uint32_t full_log, dp_pcs_comm **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(polys && out && n > 0, DP_ERR_INVALID, "dp_pcs_commit_many: null argument");
@@ -982,27 +973,27 @@ int dp_pcs_commit_many(const dp_mle *const *polys, uint32_t n, uint32_t full_log
     // latency chain each), with many proofs in flight 4 are enough and keep the number of live streams near the 32 hardware queues
     static const u32 SMAX = 8;
     const u32 S = dp_wait_mode() == DP_WAIT_BLOCK ? 4u : 8u;
-    (void)g_set_return;
-    if (g_pool.empty()) {
+    StreamSet &ss = t_streams;
+    if (ss.s.empty()) {
         std::lock_guard<std::mutex> lk(g_sets_mu);
-        if (!g_free_sets.empty()) { g_pool = g_free_sets.back().s; g_pool_ev = g_free_sets.back().e; g_main_ev = g_free_sets.back().main_ev; g_free_sets.pop_back(); }
+        if (!g_free_sets.empty()) { ss = std::move(g_free_sets.back()); g_free_sets.pop_back(); }
     }
-    if (g_pool.empty()) {
-        g_pool.resize(SMAX); g_pool_ev.resize(SMAX);
-        for (u32 s = 0; s < SMAX; s++) { DP_CUDA(cudaStreamCreateWithFlags(&g_pool[s], cudaStreamNonBlocking)); DP_CUDA(cudaEventCreateWithFlags(&g_pool_ev[s], cudaEventDisableTiming)); }
-        DP_CUDA(cudaEventCreateWithFlags(&g_main_ev, cudaEventDisableTiming));
+    if (ss.s.empty()) {
+        ss.s.resize(SMAX); ss.e.resize(SMAX);
+        for (u32 s = 0; s < SMAX; s++) { DP_CUDA(cudaStreamCreateWithFlags(&ss.s[s], cudaStreamNonBlocking)); DP_CUDA(cudaEventCreateWithFlags(&ss.e[s], cudaEventDisableTiming)); }
+        DP_CUDA(cudaEventCreateWithFlags(&ss.main_ev, cudaEventDisableTiming));
     }
     u64 *pin = nullptr;
     if (int e = dp_pinned_alloc((void **)&pin, 32 * (size_t)n)) return e;
     cudaStream_t main = c.stream;
-    DP_CUDA(cudaEventRecord(g_main_ev, main));
+    DP_CUDA(cudaEventRecord(ss.main_ev, main));
     u32 used = n < S ? n : S;
-    for (u32 s = 0; s < used; s++) DP_CUDA(cudaStreamWaitEvent(g_pool[s], g_main_ev, 0));
+    for (u32 s = 0; s < used; s++) DP_CUDA(cudaStreamWaitEvent(ss.s[s], ss.main_ev, 0));
     int rc = DP_OK;
     dp_arena_defer(true);    // temporaries released by one commit must not be handed to another stream's commit
-    for (u32 i = 0; i < n && rc == DP_OK; i++) { c.stream = g_pool[i % S]; rc = commit_enqueue(polys[i], full_log, &out[i], pin + 4 * i); }
+    for (u32 i = 0; i < n && rc == DP_OK; i++) { c.stream = ss.s[i % S]; rc = commit_enqueue(polys[i], full_log, &out[i], pin + 4 * i); }
     c.stream = main;
-    for (u32 s = 0; s < used; s++) { cudaEventRecord(g_pool_ev[s], g_pool[s]); cudaStreamWaitEvent(main, g_pool_ev[s], 0); }
+    for (u32 s = 0; s < used; s++) { cudaEventRecord(ss.e[s], ss.s[s]); cudaStreamWaitEvent(main, ss.e[s], 0); }
     cudaError_t se = dp_stream_sync(main);
     dp_arena_defer(false);
     if (se != cudaSuccess) return dp_fail(DP_ERR_CUDA, std::string("dp_pcs_commit_many: ") + cudaGetErrorString(se));
@@ -1040,6 +1031,16 @@ int dp_pcs_comm_free(dp_pcs_comm *cm) {
     return DP_OK;
 }
 
+// oracle0 of the opening of one commitment (or of this rank's slice of it): its codeword, in the extension field
+static int open_oracle_from_codeword(dp_pcs_open *o, const dp_pcs_comm *cm) {
+    DpCtx &c = dp_ctx();
+    o->n0 = cm->cw_len;
+    if (int e = dp_dev_alloc((void **)&o->oracle0, sizeof(gle) * o->n0)) return e;
+    if (cm->is_base) { k_lift<<<dp_grid_for(o->n0, 256, 8), 256, 0, c.stream>>>((const u64 *)cm->codeword, o->oracle0, o->n0); DP_LAUNCHED(); }
+    else DP_CUDA(cudaMemcpyAsync(o->oracle0, cm->codeword, sizeof(gle) * o->n0, cudaMemcpyDeviceToDevice, c.stream));
+    return DP_OK;
+}
+
 // commit_phase / batch_commit_phase up to and including the first sumcheck message
 int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, uint32_t n_comms, const uint64_t *point, uint32_t num_vars,
                       dp_pcs_open **out, uint64_t first_msg[6]) {
@@ -1047,97 +1048,79 @@ int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, u
     DP_CHECK(comms && n_comms >= 1 && point && out && first_msg, DP_ERR_INVALID, "dp_pcs_open_begin: null argument");
     if (int e = bf_prepare()) return e;
     DpCtx &c = dp_ctx();
-    dp_pcs_open *o = new dp_pcs_open();
-    o->num_vars = num_vars; o->batch = coeffs != nullptr; o->full_log = comms[0]->full_log;
+    const dp_pcs_comm *cm = comms[0];
+    const u32 full_log = cm ? cm->full_log : 0;
     for (u32 i = 0; i < n_comms; i++) {
         DP_CHECK(comms[i] && !comms[i]->trivial, DP_ERR_INVALID, "dp_pcs_open_begin: trivial commitment (open it on the host)");   // basefold.rs:481-483, 562-565
-        DP_CHECK(comms[i]->num_vars <= num_vars && comms[i]->full_log == o->full_log, DP_ERR_INVALID, "dp_pcs_open_begin: commitment larger than the opening");
-        o->comms.push_back(comms[i]);
-        if (coeffs) o->coeffs.push_back(e_make(gl_canon(coeffs[2 * i]), gl_canon(coeffs[2 * i + 1])));
+        DP_CHECK(comms[i]->num_vars <= num_vars && comms[i]->full_log == full_log, DP_ERR_INVALID, "dp_pcs_open_begin: commitment larger than the opening");
     }
     DP_CHECK(num_vars > BF_BASECODE_LOG, DP_ERR_INVALID, "minimum number of variables must be greater than basecode_msg_size_log");
     for (u32 i = 0; i < n_comms; i++) DP_CHECK(comms[i]->shard_log == 0 || (n_comms == 1 && !coeffs), DP_ERR_UNSUPPORTED, "dp_pcs_open_begin: a sharded commitment is opened alone");
-    if (comms[0]->shard_log) {
+    if (cm->shard_log) DP_CHECK(cm->num_vars == num_vars && cm->top_lvl0, DP_ERR_STATE, "dp_pcs_open_begin: sharded commitment needs num_vars variables and its shard roots set");
+    else if (!coeffs) DP_CHECK(n_comms == 1 && cm->num_vars == num_vars, DP_ERR_INVALID, "dp_pcs_open_begin: single open needs one commitment of num_vars variables");
+
+    OpenPtr o(new dp_pcs_open());
+    o->num_vars = num_vars; o->batch = coeffs != nullptr; o->full_log = full_log;
+    o->num_rounds = num_vars - BF_BASECODE_LOG;
+    o->comms.assign(comms, comms + n_comms);
+    if (coeffs) for (u32 i = 0; i < n_comms; i++) o->coeffs.push_back(e_make(gl_canon(coeffs[2 * i]), gl_canon(coeffs[2 * i + 1])));
+    // eq = bitrev(build_eq_x_r_vec(point)) == build_eq_x_r_vec(reversed point)  (commit_phase.rs:61-64)
+    std::vector<uint64_t> rp(2 * num_vars);
+    for (u32 i = 0; i < num_vars; i++) { rp[2 * i] = point[2 * (num_vars - 1 - i)]; rp[2 * i + 1] = point[2 * (num_vars - 1 - i) + 1]; }
+    u32 sc_vars = num_vars;
+    if (cm->shard_log) {
         // Sharded opening: everything below works on this rank's contiguous slices; the messages it returns are PARTIAL sums (the
         // coefficient form is linear in the evaluations), the roots SUBTREE roots -- the caller all-gathers and adds / combines them.
-        const dp_pcs_comm *cm = comms[0];
-        DP_CHECK(cm->num_vars == num_vars && cm->top_lvl0, DP_ERR_STATE, "dp_pcs_open_begin: sharded commitment needs num_vars variables and its shard roots set");
         const u32 logG = cm->shard_log, nvl = num_vars - logG;
+        const u64 Ml = 1ULL << nvl;
         o->shard_rank = cm->shard_rank; o->shard_log = logG;
-        o->num_rounds = num_vars - BF_BASECODE_LOG;
-        const u64 Nl = cm->cw_len, Ml = 1ULL << nvl;
-        o->n0 = Nl;
-        if (int e = dp_dev_alloc((void **)&o->oracle0, sizeof(gle) * Nl)) return e;
-        if (cm->is_base) { k_lift<<<dp_grid_for(Nl, 256, 8), 256, 0, c.stream>>>((const u64 *)cm->codeword, o->oracle0, Nl); DP_LAUNCHED(); }
-        else DP_CUDA(cudaMemcpyAsync(o->oracle0, cm->codeword, sizeof(gle) * Nl, cudaMemcpyDeviceToDevice, c.stream));
-        dp_mle *ev = new dp_mle(); ev->len = Ml; ev->owned = false; ev->data = cm->bh_evals; ev->is_ext = !cm->is_base;
-        o->evals = ev;
+        if (int e = open_oracle_from_codeword(o.get(), cm)) return e;
+        o->evals = new dp_mle(); o->evals->len = Ml; o->evals->owned = false; o->evals->data = cm->bh_evals; o->evals->is_ext = !cm->is_base;
         // eq slice: the table over the low nvl variables of the reversed point, times the eq factor of this rank's top bits
-        std::vector<uint64_t> rp(2 * num_vars);
-        for (u32 i = 0; i < num_vars; i++) { rp[2 * i] = point[2 * (num_vars - 1 - i)]; rp[2 * i + 1] = point[2 * (num_vars - 1 - i) + 1]; }
         dp_mle *eq_low = nullptr;
         if (int e = dp_eq_build(rp.data(), nvl, &eq_low)) return e;
+        MlePtr eq_low_owner(eq_low);
         gle scal = e_one();
         for (u32 j = 0; j < logG; j++) {
             gle x = e_make(gl_canon(rp[2 * (nvl + j)]), gl_canon(rp[2 * (nvl + j) + 1]));
             scal = e_mul(scal, ((cm->shard_rank >> j) & 1) ? x : e_sub(e_one(), x));
         }
-        dp_mle *eq = new dp_mle(); eq->len = Ml; eq->is_ext = true; eq->owned = true;
-        if (int e = dp_dev_alloc(&eq->data, sizeof(gle) * Ml)) return e;
-        if (int e = lincomb_bcast((gle *)eq->data, nullptr, {LcTerm{eq_low->data, scal, true, 0}}, Ml)) return e;
-        dp_mle_free(eq_low);
-        o->eq = eq;
-        dp_mle *ms[2] = {o->eq, o->evals};
-        dp_sc_product pr; memset(&pr, 0, sizeof pr); pr.coef[0] = 1; pr.n_idx = 2; pr.idx[0] = 0; pr.idx[1] = 1;
-        if (int e = dp_sc_create(ms, 2, &pr, 1, nvl, 2, &o->sc)) return e;
-        uint64_t ev3[6];
-        if (int e = dp_sc_round(o->sc, nullptr, ev3)) return e;
-        msg_to_coeffs(ev3, first_msg);
-        *out = o;
-        return DP_OK;
-    }
-    if (!o->batch) DP_CHECK(n_comms == 1 && comms[0]->num_vars == num_vars, DP_ERR_INVALID, "dp_pcs_open_begin: single open needs one commitment of num_vars variables");
-    o->num_rounds = num_vars - BF_BASECODE_LOG;
-    u64 N = 1ULL << (num_vars + BF_RATE_LOG), M = 1ULL << num_vars;
-    o->n0 = N;
-    if (int e = dp_dev_alloc((void **)&o->oracle0, sizeof(gle) * N)) return e;
-    dp_mle *ev = new dp_mle(); ev->len = M; ev->owned = false;
-    if (!o->batch) {
-        const dp_pcs_comm *cm = comms[0];
-        if (cm->is_base) { k_lift<<<dp_grid_for(N, 256, 8), 256, 0, c.stream>>>((const u64 *)cm->codeword, o->oracle0, N); DP_LAUNCHED(); }
-        else DP_CUDA(cudaMemcpyAsync(o->oracle0, cm->codeword, sizeof(gle) * N, cudaMemcpyDeviceToDevice, c.stream));
-        ev->data = cm->bh_evals; ev->is_ext = !cm->is_base;     // running_evals = bh_evals (commit_phase.rs:50)
+        o->eq = new dp_mle(); o->eq->len = Ml; o->eq->is_ext = true; o->eq->owned = true;
+        if (int e = dp_dev_alloc(&o->eq->data, sizeof(gle) * Ml)) return e;
+        if (int e = lincomb_bcast((gle *)o->eq->data, nullptr, {LcTerm{eq_low->data, scal, true, 0}}, Ml)) return e;
+        sc_vars = nvl;
     } else {
-        // running_oracle = sum of coeff * codeword over the full-size commitments (commit_phase.rs:205-223)
-        {
+        const u64 N = 1ULL << (num_vars + BF_RATE_LOG), M = 1ULL << num_vars;
+        o->evals = new dp_mle(); o->evals->len = M; o->evals->owned = false;
+        if (!o->batch) {
+            if (int e = open_oracle_from_codeword(o.get(), cm)) return e;
+            o->evals->data = cm->bh_evals; o->evals->is_ext = !cm->is_base;     // running_evals = bh_evals (commit_phase.rs:50)
+        } else {
+            // running_oracle = sum of coeff * codeword over the full-size commitments (commit_phase.rs:205-223)
+            o->n0 = N;
+            if (int e = dp_dev_alloc((void **)&o->oracle0, sizeof(gle) * N)) return e;
             std::vector<LcTerm> terms;
             for (u32 i = 0; i < n_comms; i++) if (comms[i]->cw_len == N) terms.push_back({comms[i]->codeword, o->coeffs[i], !comms[i]->is_base, 0});
             if (int e = lincomb_bcast(o->oracle0, nullptr, terms, N)) return e;
-        }
-        // sum_of_all_evals_for_sumcheck: smaller polynomials are broadcast over chunks (commit_phase.rs:225-236)
-        if (int e = dp_dev_alloc((void **)&o->scratch_sum_evals, sizeof(gle) * M)) return e;
-        {
-            std::vector<LcTerm> terms;
+            // sum_of_all_evals_for_sumcheck: smaller polynomials are broadcast over chunks (commit_phase.rs:225-236)
+            if (int e = dp_dev_alloc((void **)&o->scratch_sum_evals, sizeof(gle) * M)) return e;
+            terms.clear();
             for (u32 i = 0; i < n_comms; i++) terms.push_back({comms[i]->bh_evals, o->coeffs[i], !comms[i]->is_base, num_vars - comms[i]->num_vars});
             if (int e = lincomb_bcast(o->scratch_sum_evals, nullptr, terms, M)) return e;
+            o->evals->data = o->scratch_sum_evals; o->evals->is_ext = true;
         }
-        ev->data = o->scratch_sum_evals; ev->is_ext = true;
+        DP_CUDA(cudaGetLastError());
+        if (int e = dp_eq_build(rp.data(), num_vars, &o->eq)) return e;
     }
-    DP_CUDA(cudaGetLastError());
-    o->evals = ev;
-    // eq = bitrev(build_eq_x_r_vec(point)) == build_eq_x_r_vec(reversed point)  (commit_phase.rs:61-64)
-    std::vector<uint64_t> rp(2 * num_vars);
-    for (u32 i = 0; i < num_vars; i++) { rp[2 * i] = point[2 * (num_vars - 1 - i)]; rp[2 * i + 1] = point[2 * (num_vars - 1 - i) + 1]; }
-    if (int e = dp_eq_build(rp.data(), num_vars, &o->eq)) return e;
     // the Basefold-internal sumcheck (basefold/sumcheck.rs) is a degree-2 LSB-first sumcheck of eq * evals on
     // the bit-reversed tables; its coefficient-form message is recovered from p(0), p(1), p(2)
     dp_mle *ms[2] = {o->eq, o->evals};
     dp_sc_product pr; memset(&pr, 0, sizeof pr); pr.coef[0] = 1; pr.n_idx = 2; pr.idx[0] = 0; pr.idx[1] = 1;
-    if (int e = dp_sc_create(ms, 2, &pr, 1, num_vars, 2, &o->sc)) return e;
+    if (int e = dp_sc_create(ms, 2, &pr, 1, sc_vars, 2, &o->sc)) return e;
     uint64_t ev3[6];
     if (int e = dp_sc_round(o->sc, nullptr, ev3)) return e;
     msg_to_coeffs(ev3, first_msg);
-    *out = o;
+    *out = o.release();
     return DP_OK;
 }
 

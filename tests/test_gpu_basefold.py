@@ -1,7 +1,11 @@
 """GPU parity tests (-m gpu): Basefold commit / open / batch_open through the C ABI + host mirror against
 the oracle -- bit-exact roots, codewords, round messages, final message and every query opening."""
+import ctypes as C
+
 import numpy as np
 import pytest
+
+import dpb200
 import oracle_py as O
 from test_oracle_basefold import parse_flat
 
@@ -120,3 +124,132 @@ def test_batch_open_with_shared_points(gpu):
     exp, _, _ = O.pcs_batch_open_evals(polys, 11, points, eval_poly, eval_point)
     got = gpu.pcs_batch_open_evals([gpu.Mle.upload(a, e) for a, e in polys], 11, points, eval_poly, eval_point)
     assert got.shape == exp.shape and (got == exp).all()
+
+
+# ---- refusals of the Basefold C ABI ------------------------------------------------------------------------------------------------
+def _abi(gpu):
+    L = gpu._pcs_setup()
+    L.dp_pcs_commit_shard.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
+    L.dp_pcs_batch_commit.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
+    return L
+
+
+def _commit(gpu, nv, full_log):
+    return gpu.Commitment(gpu.Mle.upload(rnd_poly(600 + nv, nv, False), False), full_log)
+
+
+def _open_begin(gpu, handles, num_vars, batch=False):
+    """dp_pcs_open_begin over raw commitment handles -> return code (an opening that starts is freed again)"""
+    L = _abi(gpu)
+    hs = (C.c_void_p * len(handles))(*handles)
+    pt = gpu._u64(O.splitmix_e(610, num_vars)).reshape(-1)
+    coeffs = np.ones(2 * len(handles), dtype=np.uint64) if batch else None
+    o, msg = C.c_void_p(), np.zeros(6, dtype=np.uint64)
+    rc = L.dp_pcs_open_begin(hs, None if coeffs is None else coeffs.ctypes.data, len(handles), pt.ctypes.data, num_vars, C.byref(o), msg.ctypes.data)
+    if rc == 0:
+        L.dp_pcs_open_free(o)
+    return rc
+
+
+def _open_trivial(gpu):
+    c = _commit(gpu, 5, 8)
+    return _open_begin(gpu, [c.h.value], 5)
+
+
+def _open_larger(gpu):
+    c = _commit(gpu, 10, 10)
+    return _open_begin(gpu, [c.h.value], 9)
+
+
+def _open_few_vars(gpu):
+    # every non-trivial commitment has more than 7 variables, so the size check above comes first and its message wins
+    c = _commit(gpu, 8, 8)
+    return _open_begin(gpu, [c.h.value], 7)
+
+
+def _open_single_wrong_vars(gpu):
+    c = _commit(gpu, 9, 10)
+    return _open_begin(gpu, [c.h.value], 10)
+
+
+def _sharded(gpu, nv=13):
+    L = _abi(gpu)
+    m, h = gpu.Mle.upload(rnd_poly(620, nv, False), False), C.c_void_p()
+    gpu.check(L.dp_pcs_commit_shard(m.h, nv, 0, 2, C.byref(h)))
+    return h
+
+
+def _open_sharded_in_batch(gpu):
+    h = _sharded(gpu)
+    try:
+        return _open_begin(gpu, [h.value], 13, batch=True)
+    finally:
+        _abi(gpu).dp_pcs_comm_free(h)
+
+
+def _open_sharded_without_roots(gpu):
+    h = _sharded(gpu)
+    try:
+        return _open_begin(gpu, [h.value], 13)
+    finally:
+        _abi(gpu).dp_pcs_comm_free(h)
+
+
+def _shard(gpu, nv, rank, world, hasher=0):
+    L = _abi(gpu)
+    m, h = gpu.Mle.upload(rnd_poly(630, nv, False), False), C.c_void_p()
+    gpu.set_hasher(hasher)
+    try:
+        rc = L.dp_pcs_commit_shard(m.h, nv, rank, world, C.byref(h))
+    finally:
+        gpu.set_hasher(0)
+    if rc == 0:
+        L.dp_pcs_comm_free(h)
+    return rc
+
+
+def _batch(gpu, nvs):
+    L = _abi(gpu)
+    mles = [gpu.Mle.upload(rnd_poly(640 + i, nv, False), False) for i, nv in enumerate(nvs)]
+    hs = (C.c_void_p * max(1, len(mles)))(*[m.h for m in mles])
+    h = C.c_void_p()
+    rc = L.dp_pcs_batch_commit(hs, len(mles), 10, C.byref(h))
+    if rc == 0:
+        L.dp_pcs_comm_free(h)
+    return rc
+
+
+E = dpb200
+REFUSALS = {   # case -> (call, return code, dp_last_error text)
+    "open trivial commitment": (_open_trivial, E.DP_ERR_INVALID, "dp_pcs_open_begin: trivial commitment (open it on the host)"),
+    "open commitment larger than the opening": (_open_larger, E.DP_ERR_INVALID, "dp_pcs_open_begin: commitment larger than the opening"),
+    "open num_vars <= 7": (_open_few_vars, E.DP_ERR_INVALID, "dp_pcs_open_begin: commitment larger than the opening"),
+    "single open with the wrong num_vars": (_open_single_wrong_vars, E.DP_ERR_INVALID,
+                                            "dp_pcs_open_begin: single open needs one commitment of num_vars variables"),
+    "sharded commitment in a batch": (_open_sharded_in_batch, E.DP_ERR_UNSUPPORTED, "dp_pcs_open_begin: a sharded commitment is opened alone"),
+    "sharded commitment without its shard roots": (_open_sharded_without_roots, E.DP_ERR_STATE,
+                                                   "dp_pcs_open_begin: sharded commitment needs num_vars variables and its shard roots set"),
+    "shard over a world that is not a power of two": (lambda g: _shard(g, 13, 0, 3), E.DP_ERR_INVALID,
+                                                      "dp_pcs_commit_shard: world must be a power of two >= 2 and rank < world"),
+    "shard with rank >= world": (lambda g: _shard(g, 13, 2, 2), E.DP_ERR_INVALID,
+                                 "dp_pcs_commit_shard: world must be a power of two >= 2 and rank < world"),
+    "shard a polynomial that is too small": (lambda g: _shard(g, 12, 0, 2), E.DP_ERR_INVALID,
+                                             "dp_pcs_commit_shard: polynomial too small to shard over this many ranks"),
+    "shard under BLAKE3": (lambda g: _shard(g, 13, 0, 2, hasher=1), E.DP_ERR_UNSUPPORTED, "dp_pcs_commit_shard: Poseidon2 trees only"),
+    "batch commit of 0 polynomials": (lambda g: _batch(g, []), E.DP_ERR_INVALID, "cannot batch commit to zero polynomials"),
+    "batch commit of 65 polynomials": (lambda g: _batch(g, [8] * 65), E.DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: at most 64 polynomials per batch"),
+    "batch commit of mixed sizes": (lambda g: _batch(g, [9, 10]), E.DP_ERR_INVALID,
+                                    "cannot batch commit to polynomials with different number of variables"),
+}
+
+
+@pytest.mark.parametrize("case", list(REFUSALS))
+def test_abi_refusal(gpu, case):
+    """each refusal returns its code and message, and the context it happened in still commits and opens like the oracle"""
+    call, code, text = REFUSALS[case]
+    assert call(gpu) == code
+    assert gpu.lib().dp_last_error().decode() == text
+    ev, pt = rnd_poly(650, 9, False), O.splitmix_e(651, 9)
+    root, got = gpu.pcs_open(gpu.Mle.upload(ev, False), 10, pt)
+    assert (root == O.pcs_commit(ev, False, 10, want_codeword=False)[0]).all()
+    assert (got == O.pcs_open(ev, False, 10, pt)).all()

@@ -2,7 +2,7 @@
 (dp_set_wait_mode(1)) -- against the oracle.
 
 Several device paths exist only in that configuration:
-  * the Merkle builder changes shape with the wait mode (deep-prove_b200/csrc/basefold.cu tree_build, :438-524): in block mode
+  * the Merkle builder changes shape with the wait mode (deep-prove_b200/csrc/basefold.cu tree_build, :470-550): in block mode
     k_merkle_small takes 256-hash subtrees, hashes every level of >= 64 hashes one thread per hash (p2_compress_lat) and folds
     up to 8 subtree roots in the last block; in spin mode it takes 32-hash subtrees, always uses the 8-lane p2x8_compress and
     folds up to 64.  `tree_plan` below restates tree_build rule by rule; CASES is a matrix of commitments that, run through the
@@ -17,9 +17,9 @@ Several device paths exist only in that configuration:
   * the concurrent prover pool (host/capi.cpp): per-worker contexts, staggered starts from a pool's second call, the shared
     Merkle ticket ring.  dph_zkml_prove_concurrent_all returns every job's proof, and each must equal the oracle's.
 
-The ticket ring (basefold.cu:337-345, MK_TICKETS = 4096 counters handed out round robin) is safe only while fewer than 4096
+The ticket ring (basefold.cu:365-379, MK_TICKETS = 4096 counters handed out round robin) is safe only while fewer than 4096
 k_merkle_small launches lie between one launch's enqueue and its completion.  A proof commits about 38 witness trees per
-dp_pcs_commit_many call (basefold.cu:981) and its thread waits for the call to finish, so 48 proofs in flight hold at most
+dp_pcs_commit_many call (basefold.cu:972) and its thread waits for the call to finish, so 48 proofs in flight hold at most
 about 48 x 38 = 1.8 k launches: a margin of about 2x.  Nothing here tries to provoke a collision.
 """
 import ctypes as C
@@ -41,13 +41,13 @@ P = O.P
 SPIN, BLOCK = 0, 1
 
 # ---- constants of basefold.cu the model depends on -----------------------------------------------------------------------------
-MK_SMALL = 2048             # :264  k_merkle_small builds every remaining level once a level has <= this many hashes
-MK_SUB = 256                # :263  hashes of the first level per block in block mode
-SPIN_SUB = 32               # :487  ... and in spin mode
-TPH_MIN = 64                # :487  block mode: a block level with >= this many hashes runs one thread per hash
-MK_MID_MAX = 32768          # :498  k_merkle_mid up to this many hashes per level, k_merkle_l1 / k_merkle_up above
-B3_TAIL_MAX = 1024          # :464  BLAKE3: k_b3_tail takes every remaining level once a level has <= this many hashes
-LVL_MAX = 36                # :262  LvlOff holds 36 level offsets: the one-launch kernels need lg < 36
+MK_SMALL = 2048             # :293  k_merkle_small builds every remaining level once a level has <= this many hashes
+MK_SUB = 256                # :292  hashes of the first level per block in block mode
+SPIN_SUB = 32               # :519  ... and in spin mode
+TPH_MIN = 64                # :519  block mode: a block level with >= this many hashes runs one thread per hash
+MK_MID_MAX = 32768          # :528  k_merkle_mid up to this many hashes per level, k_merkle_l1 / k_merkle_up above
+B3_TAIL_MAX = 1024          # :496  BLAKE3: k_b3_tail takes every remaining level once a level has <= this many hashes
+LVL_MAX = 36                # :291  LvlOff holds 36 level offsets: the one-launch kernels need lg < 36
 BF_BASECODE_LOG = 7         # nv <= 7: a trivial commitment, the tree is over the evaluations themselves
 BF_RATE_LOG = 1             # otherwise the tree is over the 2^(nv + 1) codeword entries
 
@@ -65,48 +65,48 @@ TREE_PROFILE_NAMES = {v for v in PROFILE_NAME.values() if v}
 
 
 def tree_plan(n_leaves, ext, batch_lvl0, hasher, wait_mode):
-    """tree_build (basefold.cu:438-524) for a tree over n_leaves leaves.  batch_lvl0: the leaf-pair digests are given (a batch
+    """tree_build (basefold.cu:470-550) for a tree over n_leaves leaves.  batch_lvl0: the leaf-pair digests are given (a batch
     commitment); hasher: "poseidon2" or "blake3".  Returns dict(lg, launches: Counter of kernel names, route: [(kernel, level,
     hashes, source)], small: None or the k_merkle_small launch as dict(first_level, hashes, source, ext, grid, sub,
     levels: [(hashes per block, "thread" | "8 lanes")], fold: [hashes per fold level]))."""
     lg = 0
-    while (1 << lg) < n_leaves:                                                    # :442
+    while (1 << lg) < n_leaves:                                                    # :474
         lg += 1
-    assert lg >= 1                                                                 # :443
+    assert lg >= 1                                                                 # :475
     launches, route, small = Counter(), [], None
-    if hasher == "blake3":                                                         # :448-471
-        if not batch_lvl0:                                                         # :450-457  level 0 is stored
+    if hasher == "blake3":                                                         # :482-503
+        if not batch_lvl0:                                                         # :484-491  level 0 is stored
             launches["k_b3_leaves"] += 1
-        for l in range(1, lg):                                                     # :461
+        for l in range(1, lg):                                                     # :493
             nl = n_leaves >> (l + 1)
-            if nl <= B3_TAIL_MAX and lg < LVL_MAX:                                 # :464
+            if nl <= B3_TAIL_MAX and lg < LVL_MAX:                                 # :496
                 launches["k_b3_tail"] += 1
                 route.append(("k_b3_tail", l, nl, None))
                 break
-            launches["k_b3_up"] += 1                                               # :465-466
+            launches["k_b3_up"] += 1                                               # :497-498
             route.append(("k_b3_up", l, nl, None))
         return dict(lg=lg, launches=launches, route=route, small=None)
-    if lg == 1:                                                                    # :472-475
+    if lg == 1:                                                                    # :504-508
         if not batch_lvl0:
             launches["k_leafpair_root"] += 1
             route.append(("k_leafpair_root", 0, 1, "leaves"))
         return dict(lg=lg, launches=launches, route=route, small=None)
-    for l in range(1, lg):                                                         # :480
+    for l in range(1, lg):                                                         # :510
         nl = n_leaves >> (l + 1)
-        source = ("batch level 0" if batch_lvl0 else "leaves") if l == 1 else "digests"     # :482, :490
-        if nl <= MK_SMALL and lg < LVL_MAX:                                        # :484
-            many = wait_mode == BLOCK                                              # :486-487
+        source = ("batch level 0" if batch_lvl0 else "leaves") if l == 1 else "digests"     # :512, :514
+        if nl <= MK_SMALL and lg < LVL_MAX:                                        # :516
+            many = wait_mode == BLOCK                                              # :518-519
             sub_max, tph_min = (MK_SUB, TPH_MIN) if many else (SPIN_SUB, None)
-            grid = (nl + sub_max - 1) // sub_max                                   # :488
-            sub = min(nl, sub_max)                                                 # kernel :279
+            grid = (nl + sub_max - 1) // sub_max                                   # :520
+            sub = min(nl, sub_max)                                                 # kernel :308
             levels, lv, k = [], l, 0
-            while (sub >> k) >= 1 and lv < lg:                                     # kernel :281-312
+            while (sub >> k) >= 1 and lv < lg:                                     # kernel :310-340
                 cnt = sub >> k
                 levels.append((cnt, "thread" if tph_min is not None and cnt >= tph_min else "8 lanes"))
                 k += 1
                 lv += 1
             fold = []
-            if grid > 1:                                                           # kernel :313, :321-333
+            if grid > 1:                                                           # kernel :341, :349-361
                 cnt = grid >> 1
                 while cnt >= 1 and lv < lg:
                     fold.append(cnt)
@@ -118,7 +118,7 @@ def tree_plan(n_leaves, ext, batch_lvl0, hasher, wait_mode):
             launches["k_merkle_small"] += 1
             route.append(("k_merkle_small", l, nl, source))
             break
-        kernel = "k_merkle_mid" if nl <= MK_MID_MAX else ("k_merkle_l1" if source == "leaves" else "k_merkle_up")   # :498, :512-517
+        kernel = "k_merkle_mid" if nl <= MK_MID_MAX else ("k_merkle_l1" if source == "leaves" else "k_merkle_up")   # :528, :542-543
         launches[kernel] += 1
         route.append((kernel, l, nl, source))
     return dict(lg=lg, launches=launches, route=route, small=small)
