@@ -574,11 +574,6 @@ __global__ void k_fri_fold(const gle *__restrict__ in, gle *__restrict__ out, u3
 // the whole running oracle per commitment -- 47 passes over a 16 MB table in a Dense-4M opening.  Each thread owns one output
 // element, walks the source table (kernel parameters, <= LC_MAX entries per launch) and accumulates the raw 128-bit products in
 // 192-bit sums that are reduced once (field addition is exact, so the order is free and the element is identical).
-struct bacc192 { u64 lo, hi; u32 top; };
-__device__ __forceinline__ void bacc_mac(bacc192 &a, u64 x, u64 y) {
-    u64 pl = x * y, ph = __umul64hi(x, y);
-    asm("{\n\tadd.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u32 %2, %2, 0;\n\t}" : "+l"(a.lo), "+l"(a.hi), "+r"(a.top) : "l"(pl), "l"(ph));
-}
 static constexpr u32 LC_MAX = 96;
 struct LcSrc { const void *p; u64 c0, c1; u32 ext, rep_log; };
 struct LcArgs { LcSrc s[LC_MAX]; u32 n; u32 pad; };
@@ -586,20 +581,20 @@ template <bool HAS_BASE>
 __global__ void __launch_bounds__(256) k_lincomb_bcast(gle *__restrict__ out, const gle *__restrict__ base, const __grid_constant__ LcArgs a, u64 n) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
     for (; i < n; i += stride) {
-        bacc192 s0 = {0, 0, 0}, s1 = {0, 0, 0};
+        gl_acc s0 = {0, 0, 0}, s1 = {0, 0, 0};
         for (u32 k = 0; k < a.n; k++) {
             const LcSrc &q = a.s[k];
             const u64 j = i >> q.rep_log;
             if (q.ext) {   // (c0 + c1 X)(x0 + x1 X) = c0 x0 + 7 c1 x1 + (c0 x1 + c1 x0) X
                 const gle x = ld_e((const gle *)q.p + j);
-                bacc_mac(s1, q.c0, x.c1); bacc_mac(s1, q.c1, x.c0);
-                bacc_mac(s0, q.c0, x.c0); bacc_mac(s0, gl_reduce128_weak(q.c1 * x.c1, __umul64hi(q.c1, x.c1)), 7ULL);
+                gl_acc_mac(s1, q.c0, x.c1); gl_acc_mac(s1, q.c1, x.c0);
+                gl_acc_mac(s0, q.c0, x.c0); gl_acc_mac(s0, gl_reduce128_weak(q.c1 * x.c1, __umul64hi(q.c1, x.c1)), 7ULL);
             } else {
                 const u64 x = ((const u64 *)q.p)[j];
-                bacc_mac(s0, q.c0, x); bacc_mac(s1, q.c1, x);
+                gl_acc_mac(s0, q.c0, x); gl_acc_mac(s1, q.c1, x);
             }
         }
-        gle v = e_make(gl_reduce160(s0.lo, s0.hi, s0.top), gl_reduce160(s1.lo, s1.hi, s1.top));
+        gle v = e_make(gl_acc_reduce(s0), gl_acc_reduce(s1));
         if (HAS_BASE) v = e_add(v, ld_e(base + i));
         st_e(out + i, v);
     }
@@ -711,12 +706,9 @@ static void msg_to_coeffs(const uint64_t *ev /* p(0),p(1),p(2) */, uint64_t *out
     out[0] = p0.c0; out[1] = p0.c1; out[2] = c1.c0; out[3] = c1.c1; out[4] = c2.c0; out[5] = c2.c1;
 }
 
-// Owning handles for objects under construction: an error return releases whatever has been built so far.
-template <auto Free> struct FreeWith { template <typename P> void operator()(P *p) const { Free(p); } };
+// Owning handles (common.cuh) for the commitments and openings under construction
 using CommPtr = std::unique_ptr<dp_pcs_comm, FreeWith<dp_pcs_comm_free>>;
 using OpenPtr = std::unique_ptr<dp_pcs_open, FreeWith<dp_pcs_open_free>>;
-using MlePtr = std::unique_ptr<dp_mle, FreeWith<dp_mle_free>>;
-using DevPtr = std::unique_ptr<void, FreeWith<dp_dev_free>>;
 
 // Encode of a 2^nv polynomial whose whole codeword fits in one block's shared memory: one launch
 template <typename T>
@@ -1013,13 +1005,13 @@ int dp_pcs_comm_info(const dp_pcs_comm *cm, uint32_t *num_vars, int *is_base, in
 int dp_pcs_comm_codeword(const dp_pcs_comm *cm, dp_mle **view) {
     DP_REQUIRE_CTX();
     DP_CHECK(cm && view, DP_ERR_INVALID, "dp_pcs_comm_codeword: null");
-    dp_mle *v = new dp_mle(); v->data = cm->codeword; v->len = cm->cw_len; v->is_ext = !cm->is_base; v->owned = false; *view = v;
+    *view = dp_mle_view(cm->codeword, cm->cw_len, !cm->is_base);
     return DP_OK;
 }
 int dp_pcs_comm_bh_evals(const dp_pcs_comm *cm, dp_mle **view) {
     DP_REQUIRE_CTX();
     DP_CHECK(cm && view, DP_ERR_INVALID, "dp_pcs_comm_bh_evals: null");
-    dp_mle *v = new dp_mle(); v->data = cm->bh_evals; v->len = 1ULL << cm->num_vars; v->is_ext = !cm->is_base; v->owned = false; *view = v;
+    *view = dp_mle_view(cm->bh_evals, 1ULL << cm->num_vars, !cm->is_base);
     return DP_OK;
 }
 int dp_pcs_comm_free(dp_pcs_comm *cm) {
@@ -1063,7 +1055,7 @@ int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, u
     o->num_vars = num_vars; o->batch = coeffs != nullptr; o->full_log = full_log;
     o->num_rounds = num_vars - BF_BASECODE_LOG;
     o->comms.assign(comms, comms + n_comms);
-    if (coeffs) for (u32 i = 0; i < n_comms; i++) o->coeffs.push_back(e_make(gl_canon(coeffs[2 * i]), gl_canon(coeffs[2 * i + 1])));
+    if (coeffs) for (u32 i = 0; i < n_comms; i++) o->coeffs.push_back(e_from_host(coeffs + 2 * i));
     // eq = bitrev(build_eq_x_r_vec(point)) == build_eq_x_r_vec(reversed point)  (commit_phase.rs:61-64)
     std::vector<uint64_t> rp(2 * num_vars);
     for (u32 i = 0; i < num_vars; i++) { rp[2 * i] = point[2 * (num_vars - 1 - i)]; rp[2 * i + 1] = point[2 * (num_vars - 1 - i) + 1]; }
@@ -1075,26 +1067,26 @@ int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, u
         const u64 Ml = 1ULL << nvl;
         o->shard_rank = cm->shard_rank; o->shard_log = logG;
         if (int e = open_oracle_from_codeword(o.get(), cm)) return e;
-        o->evals = new dp_mle(); o->evals->len = Ml; o->evals->owned = false; o->evals->data = cm->bh_evals; o->evals->is_ext = !cm->is_base;
+        o->evals = dp_mle_view(cm->bh_evals, Ml, !cm->is_base);
         // eq slice: the table over the low nvl variables of the reversed point, times the eq factor of this rank's top bits
         dp_mle *eq_low = nullptr;
         if (int e = dp_eq_build(rp.data(), nvl, &eq_low)) return e;
         MlePtr eq_low_owner(eq_low);
         gle scal = e_one();
         for (u32 j = 0; j < logG; j++) {
-            gle x = e_make(gl_canon(rp[2 * (nvl + j)]), gl_canon(rp[2 * (nvl + j) + 1]));
+            gle x = e_from_host(&rp[2 * (nvl + j)]);
             scal = e_mul(scal, ((cm->shard_rank >> j) & 1) ? x : e_sub(e_one(), x));
         }
-        o->eq = new dp_mle(); o->eq->len = Ml; o->eq->is_ext = true; o->eq->owned = true;
-        if (int e = dp_dev_alloc(&o->eq->data, sizeof(gle) * Ml)) return e;
+        MlePtr eq;
+        if (int e = dp_mle_alloc(Ml, true, eq)) return e;
+        o->eq = eq.release();
         if (int e = lincomb_bcast((gle *)o->eq->data, nullptr, {LcTerm{eq_low->data, scal, true, 0}}, Ml)) return e;
         sc_vars = nvl;
     } else {
         const u64 N = 1ULL << (num_vars + BF_RATE_LOG), M = 1ULL << num_vars;
-        o->evals = new dp_mle(); o->evals->len = M; o->evals->owned = false;
         if (!o->batch) {
             if (int e = open_oracle_from_codeword(o.get(), cm)) return e;
-            o->evals->data = cm->bh_evals; o->evals->is_ext = !cm->is_base;     // running_evals = bh_evals (commit_phase.rs:50)
+            o->evals = dp_mle_view(cm->bh_evals, M, !cm->is_base);     // running_evals = bh_evals (commit_phase.rs:50)
         } else {
             // running_oracle = sum of coeff * codeword over the full-size commitments (commit_phase.rs:205-223)
             o->n0 = N;
@@ -1107,7 +1099,7 @@ int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, u
             terms.clear();
             for (u32 i = 0; i < n_comms; i++) terms.push_back({comms[i]->bh_evals, o->coeffs[i], !comms[i]->is_base, num_vars - comms[i]->num_vars});
             if (int e = lincomb_bcast(o->scratch_sum_evals, nullptr, terms, M)) return e;
-            o->evals->data = o->scratch_sum_evals; o->evals->is_ext = true;
+            o->evals = dp_mle_view(o->scratch_sum_evals, M, true);
         }
         DP_CUDA(cudaGetLastError());
         if (int e = dp_eq_build(rp.data(), num_vars, &o->eq)) return e;
@@ -1131,7 +1123,7 @@ int dp_pcs_open_round(dp_pcs_open *o, const uint64_t challenge[2], uint64_t next
     DP_CHECK(o && challenge && is_last, DP_ERR_INVALID, "dp_pcs_open_round: null argument");
     DP_CHECK(o->round < o->num_rounds, DP_ERR_STATE, "dp_pcs_open_round: commit phase already finished");
     DpCtx &c = dp_ctx();
-    gle r = e_make(gl_canon(challenge[0]), gl_canon(challenge[1]));
+    gle r = e_from_host(challenge);
     u32 i = o->round;
     if (i > 0 && o->batch) {
         // merge the commitments whose codeword size matches the running oracle (commit_phase.rs:271-282); the

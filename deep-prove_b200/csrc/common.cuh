@@ -1,7 +1,8 @@
-// Library-internal context: one process per GPU, one stream, stream-ordered memory pool.
+// Library-internal context: one per host thread, with its own stream and device arena.
 #pragma once
 #include "gl.cuh"
 #include "../../include/deepprove_b200.h"
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -14,14 +15,11 @@ struct DpCtx {
     int sm_count = 132;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    cudaMemPool_t pool = nullptr;       // this thread's stream-ordered pool (no cross-stream reuse dependencies)
     std::recursive_mutex mu;
-    unsigned long long launches = 0;
     u64 *sync_flag = nullptr; u64 sync_seq = 0;   // dp_stream_sync: this thread's pinned completion word
     std::vector<void *> zero_blocks;               // 256-byte device blocks known to hold zeros (dp_zero_block_get/put)
 };
 DpCtx &dp_ctx();
-void dp_set_error(const std::string &s);
 int dp_fail(int code, const std::string &s);
 
 #define DP_CUDA(x)                                                                                          \
@@ -81,7 +79,7 @@ struct DpD2H {
 int dp_zero_block_get(void **p);
 void dp_zero_block_put(void *p);
 
-// stream-ordered allocation helpers
+// device blocks from this thread's arena
 int dp_dev_alloc(void **p, size_t bytes);
 int dp_dev_free(void *p);
 void dp_arena_defer(bool on);   // hold releases back while several streams are in flight (dp_pcs_commit_many)
@@ -98,6 +96,27 @@ struct dp_mle {
     size_t bytes() const { return (size_t)len * (is_ext ? 16 : 8); }
 };
 
+// Owning handles for objects under construction: an error return releases whatever has been built so far.
+template <auto Free> struct FreeWith { template <typename P> void operator()(P *p) const { Free(p); } };
+using MlePtr = std::unique_ptr<dp_mle, FreeWith<dp_mle_free>>;
+using DevPtr = std::unique_ptr<void, FreeWith<dp_dev_free>>;
+using PinnedPtr = std::unique_ptr<void, FreeWith<dp_pinned_free>>;
+
+// A table of `len` elements that the MLE owns, allocated in the arena (contents undefined)
+static inline int dp_mle_alloc(u64 len, bool ext, MlePtr &out) {
+    MlePtr m(new dp_mle());
+    m->len = len; m->is_ext = ext;
+    if (int e = dp_dev_alloc(&m->data, m->bytes())) return e;
+    out = std::move(m);
+    return DP_OK;
+}
+// A view of `len` elements at `data`, which stay the owner's
+static inline dp_mle *dp_mle_view(void *data, u64 len, bool ext) {
+    dp_mle *v = new dp_mle();
+    v->data = data; v->len = len; v->is_ext = ext; v->owned = false;
+    return v;
+}
+
 static inline int dp_grid_for(u64 work_items, int threads, int max_ctas_per_sm) {
     u64 g = (work_items + threads - 1) / threads;
     u64 cap = (u64)dp_ctx().sm_count * max_ctas_per_sm;
@@ -107,6 +126,4 @@ static inline int dp_grid_for(u64 work_items, int threads, int max_ctas_per_sm) 
 }
 
 // ---- kernel launchers shared between translation units (mle.cu) ----
-int dpk_eq_build(const gle *point_host, u32 nv, gle *out_dev);                       // K5
-int dpk_fix_high(const void *src, bool src_ext, u64 len, const gle *point_host, u32 k, gle *out_dev);  // K3
 int dpk_fold_low(const void *src, bool src_ext, u64 len, gle r, gle *out_dev);      // K2 (stand-alone)

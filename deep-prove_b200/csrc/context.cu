@@ -1,17 +1,16 @@
-// Context, error reporting and memory-pool plumbing of libdeepprove_b200.so.
+// Context, error reporting, device arena and pinned-memory plumbing of libdeepprove_b200.so.
 #include "common.cuh"
 #include <cstdlib>
 #include <atomic>
 #include <mutex>
 
 static thread_local std::string g_err;
-// One context PER HOST THREAD (own stream, pinned cache, launch counter): independent proofs run concurrently
+// One context PER HOST THREAD (own stream, device arena, pinned cache): independent proofs run concurrently
 // from several host threads on one GPU and share only read-only device data (model, tables, twiddles).
 static thread_local DpCtx g_ctx;
 DpCtx &dp_ctx() { return g_ctx; }
 static std::atomic<unsigned long long> g_total_launches{0};
 void dp_count_launch() { g_total_launches.fetch_add(1, std::memory_order_relaxed); }
-void dp_set_error(const std::string &s) { g_err = s; }
 int dp_fail(int code, const std::string &s) { g_err = s; return code; }
 
 // ---- per-thread device arena -------------------------------------------------------------------------
@@ -30,7 +29,6 @@ struct DpArena {
     // blocks of THIS arena released by other host threads (e.g. a handle created on one proving thread and destroyed on
     // another): parked here under the registry lock and folded back into the free lists by the owner's next allocation
     std::vector<void *> returned; std::atomic<unsigned> n_returned{0};
-    unsigned long long foreign_frees = 0;
     ~DpArena();
 };
 // process-wide slab registry: which arena owns an address (only consulted on the rare foreign free and on teardown)
@@ -82,7 +80,6 @@ int dp_dev_free(void *p) {
     if (it == a.cls.end()) {
         // owned by another thread's arena: hand it back to its owner.  The owner's stream knows nothing about the work this
         // thread queued on the block, so that work is drained first (foreign frees are rare: cross-thread handle teardown).
-        a.foreign_frees++;
         if (g_ctx.ready && g_ctx.stream) cudaStreamSynchronize(g_ctx.stream);
         std::lock_guard<std::mutex> lk(g_slab_mu);
         for (auto &r : g_slab_reg) if ((char *)p >= r.base && (char *)p < r.base + r.cap) { r.owner->returned.push_back(p); r.owner->n_returned.fetch_add(1, std::memory_order_release); break; }
@@ -394,9 +391,6 @@ int dp_init(int device) {
     DP_CUDA(cudaGetDeviceProperties(&prop, device));
     g_ctx.sm_count = prop.multiProcessorCount;
     if (!g_ctx.stream) { DP_CUDA(cudaStreamCreateWithFlags(&g_ctx.stream, cudaStreamNonBlocking)); g_ctx.own_stream = true; }
-    // keep freed blocks in the pool: sumcheck rounds allocate/free ping-pong buffers constantly.  Each host thread
-    // gets its OWN pool so that reuse never creates a dependency on another thread's stream.
-    (void)device;
     g_ctx.device = device;
     g_ctx.ready = true;
     return DP_OK;

@@ -7,12 +7,7 @@
 #include "common.cuh"
 #include "powtab.cuh"
 #include "../../include/deepprove_b200.h"
-
-static inline int new_mle(u64 len, bool ext, dp_mle **out) {
-    dp_mle *m = new dp_mle(); m->len = len; m->is_ext = ext; m->owned = true;
-    if (int e = dp_dev_alloc(&m->data, m->bytes())) { delete m; return e; }
-    *out = m; return DP_OK;
-}
+#include <algorithm>
 
 // ---- fft(v, flag) on rows (tensor.rs:261-323): natural order in/out, w = get_root_of_unity(log n) (inverse when flag) ----
 __global__ void __launch_bounds__(256) k_fft_rows(gle *data, u32 lg, int inverse, PowTab tab) {
@@ -67,12 +62,12 @@ extern "C" int dp_pad_rows(const dp_mle *src, uint64_t rows, uint32_t n_real, ui
     DP_CHECK(src->len == rows * n_real * n_real, DP_ERR_INVALID, "dp_pad_rows: source length != rows * n_real^2");
     u64 total = rows * out_len;
     DP_CHECK(total && (total & (total - 1)) == 0, DP_ERR_INVALID, "dp_pad_rows: rows * out_len must be a power of two");
-    dp_mle *m; if (int e = new_mle(total, true, &m)) return e;
+    MlePtr m; if (int e = dp_mle_alloc(total, true, m)) return e;
     int g = dp_grid_for(total, 256, 8);
     if (src->is_ext) k_pad_rows<true><<<g, 256, 0, dp_ctx().stream>>>(src->data, rows, n_real, n, out_len, (gle *)m->data);
     else k_pad_rows<false><<<g, 256, 0, dp_ctx().stream>>>(src->data, rows, n_real, n, out_len, (gle *)m->data);
     DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
-    *out = m; return DP_OK;
+    *out = m.release(); return DP_OK;
 }
 
 // ---- fft_conv accumulation (tensor.rs:489-509): out[i][k] = sum_j x_fft[j][k] * w_fft[i][j][k] ----
@@ -89,11 +84,11 @@ extern "C" int dp_conv_prod(const dp_mle *x_fft, const dp_mle *w_fft, uint32_t k
     DP_REQUIRE_CTX();
     DP_CHECK(x_fft && w_fft && out && x_fft->is_ext && w_fft->is_ext, DP_ERR_INVALID, "dp_conv_prod: need Ext operands");
     DP_CHECK(x_fft->len == (u64)kx * row_len && w_fft->len == (u64)kw * kx * row_len, DP_ERR_INVALID, "dp_conv_prod: operand shapes do not match [kx, n] / [kw, kx, n]");
-    dp_mle *m; if (int e = new_mle((u64)kw * row_len, true, &m)) return e;
+    MlePtr m; if (int e = dp_mle_alloc((u64)kw * row_len, true, m)) return e;
     DpProfScope prof("k_conv_prod", (w_fft->bytes() + x_fft->bytes() + m->bytes()));
     k_conv_prod<<<dp_grid_for((u64)kw * row_len, 128, 8), 128, 0, dp_ctx().stream>>>((const gle *)x_fft->data, (const gle *)w_fft->data, kw, kx, row_len, (gle *)m->data); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    *out = m; return DP_OK;
+    *out = m.release(); return DP_OK;
 }
 
 // ---- index_u + to_element + add_bias: out[i][t] = to_element(rows[i][n_x^2 - 1 - t]) + bias[i] ----
@@ -112,14 +107,14 @@ extern "C" int dp_conv_output_elements(const dp_mle *out_rows, uint32_t kw, uint
     DP_CHECK(out_rows && out_rows->is_ext && bias && out_host && out_rows->len == 2 * nx2 * kw, DP_ERR_INVALID, "dp_conv_output_elements: need [kw, 2 n_x^2] Ext rows");
     long long *d = nullptr, *db = nullptr;
     if (int e = dp_dev_alloc((void **)&d, 8 * nx2 * kw)) return e;
-    if (int e = dp_dev_alloc((void **)&db, 8 * (size_t)kw)) { dp_dev_free(d); return e; }
+    DevPtr d_owner(d);
+    if (int e = dp_dev_alloc((void **)&db, 8 * (size_t)kw)) return e;
+    DevPtr db_owner(db);
     cudaStream_t st = dp_ctx().stream;
     DP_CUDA(cudaMemcpyAsync(db, bias, 8 * (size_t)kw, cudaMemcpyHostToDevice, st));
     k_conv_out_elems<<<dp_grid_for(nx2 * kw, 256, 8), 256, 0, st>>>((const gle *)out_rows->data, kw, (u32)nx2, db, d); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    const int rc = dp_d2h(out_host, d, 8 * nx2 * kw, st);
-    dp_dev_free(d); dp_dev_free(db);
-    return rc;
+    return dp_d2h(out_host, d, 8 * nx2 * kw, st);
 }
 
 // ---- phi_g_init (iop/prover.rs:231-289): the FFT / iFFT matrix row W(rx, .) and its per-level prefixes, one launch ----
@@ -156,15 +151,18 @@ extern "C" int dp_phi_g_init(const uint64_t *rx, uint32_t n, const uint64_t *sca
     DP_CHECK(rx && scale && w_red && mid && n >= 2 && n <= 14, DP_ERR_INVALID, "dp_phi_g_init: need 2 <= n <= 14");
     PowTab tab; if (int e = dp_root_powtab(&tab)) return e;
     PhiArgs a; memset(&a, 0, sizeof a);
-    for (u32 i = 0; i < n; i++) a.rx[i] = e_make(gl_canon(rx[2 * i]), gl_canon(rx[2 * i + 1]));
-    a.scale = e_make(gl_canon(scale[0]), gl_canon(scale[1]));
-    dp_mle *w; if (int e = new_mle(1ULL << n, true, &w)) return e;
+    for (u32 i = 0; i < n; i++) a.rx[i] = e_from_host(rx + 2 * i);
+    a.scale = e_from_host(scale);
+    std::fill(mid, mid + n - 1, nullptr);   // a failed call leaves no dangling entries
+    MlePtr w; if (int e = dp_mle_alloc(1ULL << n, true, w)) return e;
     cudaStream_t st = dp_ctx().stream;
     DP_CUDA(cudaMemsetAsync(w->data, 0, w->bytes(), st));                // the reference's vec![E::ZERO; ..]: the FFT case leaves the top half zero
-    for (u32 i = 0; i + 1 < n; i++) { if (int e = new_mle(2ULL << i, true, &mid[i])) return e; a.mid[i] = (gle *)mid[i]->data; }
+    std::vector<MlePtr> own(n - 1);
+    for (u32 i = 0; i + 1 < n; i++) { if (int e = dp_mle_alloc(2ULL << i, true, own[i])) return e; a.mid[i] = (gle *)own[i]->data; }
     k_phi_g_init<<<1, 1024, 0, st>>>((gle *)w->data, a, n, is_fft, tab); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    *w_red = w; return DP_OK;
+    for (u32 i = 0; i + 1 < n; i++) mid[i] = own[i].release();
+    *w_red = w.release(); return DP_OK;
 }
 
 // ---- one level of delegate_matrix_evaluation (prover.rs:182-195): phi[i] = A + B * omega^(i << shift), omega of order 2^n_total ----
@@ -179,11 +177,11 @@ extern "C" int dp_phi_level(uint32_t len_log, uint32_t n_total, uint32_t shift, 
     DP_REQUIRE_CTX();
     DP_CHECK(A && B && out && n_total >= 1 && n_total <= 32 && len_log + shift <= n_total, DP_ERR_INVALID, "dp_phi_level: bad arguments");
     PowTab tab; if (int e = dp_root_powtab(&tab)) return e;
-    dp_mle *m; if (int e = new_mle(1ULL << len_log, true, &m)) return e;
+    MlePtr m; if (int e = dp_mle_alloc(1ULL << len_log, true, m)) return e;
     u32 len = 1u << len_log;
-    k_phi_level<<<(len + 255) / 256, 256, 0, dp_ctx().stream>>>((gle *)m->data, len, n_total, shift, e_make(gl_canon(A[0]), gl_canon(A[1])), e_make(gl_canon(B[0]), gl_canon(B[1])), inverse, tab); DP_LAUNCHED();
+    k_phi_level<<<(len + 255) / 256, 256, 0, dp_ctx().stream>>>((gle *)m->data, len, n_total, shift, e_from_host(A), e_from_host(B), inverse, tab); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    *out = m; return DP_OK;
+    *out = m.release(); return DP_OK;
 }
 
 // ---- out = src repeated `times` times (beta_acc = vec![beta2; kx].concat(), convolution.rs:870) ----
@@ -194,8 +192,8 @@ __global__ void k_repeat(const gle *src, u64 len, u64 total, gle *out) {
 extern "C" int dp_mle_repeat(const dp_mle *src, uint32_t times, dp_mle **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(src && out && src->is_ext && times && (times & (times - 1)) == 0, DP_ERR_INVALID, "dp_mle_repeat: need an Ext MLE and a power-of-two count");
-    dp_mle *m; if (int e = new_mle(src->len * times, true, &m)) return e;
+    MlePtr m; if (int e = dp_mle_alloc(src->len * times, true, m)) return e;
     k_repeat<<<dp_grid_for(m->len, 256, 8), 256, 0, dp_ctx().stream>>>((const gle *)src->data, src->len, m->len, (gle *)m->data); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    *out = m; return DP_OK;
+    *out = m.release(); return DP_OK;
 }

@@ -101,6 +101,7 @@ struct __align__(16) gle {  // one E element
     u64 c0, c1;
 };
 GL_HD gle e_make(u64 a, u64 b) { gle r; r.c0 = a; r.c1 = b; return r; }
+GL_HD gle e_from_host(const uint64_t *p) { return e_make(gl_canon(p[0]), gl_canon(p[1])); }   // an element as the C ABI passes it: {c0, c1}, any u64
 GL_HD gle e_zero() { return e_make(0, 0); }
 GL_HD gle e_one() { return e_make(1, 0); }
 GL_HD gle e_from_base(u64 a) { return e_make(a, 0); }
@@ -109,9 +110,6 @@ GL_HD gle e_sub(gle a, gle b) { return e_make(gl_sub(a.c0, b.c0), gl_sub(a.c1, b
 GL_HD gle e_neg(gle a) { return e_make(gl_neg(a.c0), gl_neg(a.c1)); }
 GL_HD gle e_dbl(gle a) { return e_add(a, a); }
 GL_HD bool e_eq(gle a, gle b) { return a.c0 == b.c0 && a.c1 == b.c1; }
-// (a0 + a1 X)(b0 + b1 X) = (a0 b0 + 7 a1 b1) + (a0 b1 + a1 b0) X.
-// The two limbs are each ONE reduction of a <=131-bit sum of raw 128-bit products (fewer reductions
-// than 4 reduced multiplies; same canonical result because the arithmetic is exact).
 #ifdef __CUDA_ARCH__
 // top*2^128 + hi*2^64 + lo with top < 2^31.  2^128 = (2^32-1)^2 = -2^32 (mod p)  =>  subtract top << 32.
 __device__ __forceinline__ u64 gl_reduce160(u64 lo, u64 hi, u32 top) {
@@ -120,29 +118,38 @@ __device__ __forceinline__ u64 gl_reduce160(u64 lo, u64 hi, u32 top) {
     asm("{\n\tsub.cc.u64 %0, %2, %3;\n\tsubc.u32 %1, 0, 0;\n\t}" : "=l"(d), "=r"(m) : "l"(r), "l"(x));
     return gl_canon_weak(d - (u64)m);                          // borrow: - EPS; r < x < 2^63 here, so no second borrow
 }
-// (h:l) += a*b as a 160-bit accumulator (l, h, t)
-__device__ __forceinline__ void gl_mac160(u64 &l, u64 &h, u32 &t, u64 a, u64 b) {
-    u64 pl = a * b, ph = __umul64hi(a, b);
-    asm("{\n\tadd.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u32 %2, %2, 0;\n\t}" : "+l"(l), "+l"(h), "+r"(t) : "l"(pl), "l"(ph));
-}
-__device__ __forceinline__ gle e_mul(gle a, gle b) {
-    // c1 = a0 b1 + a1 b0 : one reduction of the 129-bit sum
-    u64 l = a.c0 * b.c1, h = __umul64hi(a.c0, b.c1); u32 t = 0;
-    gl_mac160(l, h, t, a.c1, b.c0);
-    u64 c1 = gl_reduce160(l, h, t);
-    // c0 = a0 b0 + 7 (a1 b1) : reduce a1 b1 to 64 bits (weak), times 7 is a 67-bit addend
-    u64 w = gl_reduce128_weak(a.c1 * b.c1, __umul64hi(a.c1, b.c1));
-    l = a.c0 * b.c0; h = __umul64hi(a.c0, b.c0); t = 0;
-    gl_mac160(l, h, t, w, 7ULL);
-    u64 c0 = gl_reduce160(l, h, t);
-    return e_make(c0, c1);
-}
 #else
 GL_HD u64 gl_reduce160(u64 lo, u64 hi, u64 top) {  // top*2^128 + hi*2^64 + lo, top < 2^32
     // 2^128 = (2^32-1)^2 mod p = 2^64 - 2^33 + 1 = -2^32 (mod p)  => top*2^128 = -(top << 32)
     u64 r = gl_reduce128(lo, hi);
     return gl_sub(r, gl_canon(top << 32));
 }
+#endif
+// Lazy sum of raw 128-bit products, lo + hi 2^64 + top 2^128: one reduction for the whole sum instead of one per term.
+// top < #terms must stay below 2^31 (gl_reduce160).
+struct gl_acc { u64 lo, hi; u32 top; };
+__device__ __forceinline__ void gl_acc_mac(gl_acc &a, u64 x, u64 y) {   // a += x * y
+    u64 pl = x * y, ph = __umul64hi(x, y);
+    asm("{\n\tadd.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u32 %2, %2, 0;\n\t}" : "+l"(a.lo), "+l"(a.hi), "+r"(a.top) : "l"(pl), "l"(ph));
+}
+__device__ __forceinline__ u64 gl_acc_reduce(const gl_acc &a) { return gl_reduce160(a.lo, a.hi, a.top); }
+// (a0 + a1 X)(b0 + b1 X) = (a0 b0 + 7 a1 b1) + (a0 b1 + a1 b0) X.
+// The two limbs are each ONE reduction of a <=131-bit sum of raw 128-bit products (fewer reductions
+// than 4 reduced multiplies; same canonical result because the arithmetic is exact).
+#ifdef __CUDA_ARCH__
+__device__ __forceinline__ gle e_mul(gle a, gle b) {
+    // c1 = a0 b1 + a1 b0 : one reduction of the 129-bit sum
+    gl_acc s = {a.c0 * b.c1, __umul64hi(a.c0, b.c1), 0};
+    gl_acc_mac(s, a.c1, b.c0);
+    u64 c1 = gl_acc_reduce(s);
+    // c0 = a0 b0 + 7 (a1 b1) : reduce a1 b1 to 64 bits (weak), times 7 is a 67-bit addend
+    u64 w = gl_reduce128_weak(a.c1 * b.c1, __umul64hi(a.c1, b.c1));
+    s = {a.c0 * b.c0, __umul64hi(a.c0, b.c0), 0};
+    gl_acc_mac(s, w, 7ULL);
+    u64 c0 = gl_acc_reduce(s);
+    return e_make(c0, c1);
+}
+#else
 GL_HD gle e_mul(gle a, gle b) {
     u64 l0, h0, l1, h1;
     // c1 = a0 b1 + a1 b0  (129 bits)

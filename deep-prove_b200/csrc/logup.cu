@@ -90,20 +90,20 @@ int dp_logup_build(dp_mle *const *columns, uint32_t n_columns, const dp_mle *mul
     DP_CHECK(len >= 4, DP_ERR_INVALID, "dp_logup_build: need at least 4 evaluations");
     if (multiplicities) DP_CHECK(!multiplicities->is_ext && multiplicities->len == len, DP_ERR_INVALID, "Multiplicities length was not equal to column evaluations length");
     DpCtx &c = dp_ctx();
-    dp_logup *L = new dp_logup();
+    std::unique_ptr<dp_logup, FreeWith<dp_logup_free>> L(new dp_logup());
     L->table = multiplicities != nullptr;
     L->nv = 0; while ((1ULL << L->nv) < len) L->nv++;
     // one allocation: layer k has 2^(nv-k) entries, k = 0..nv-1; (num, den) each
     u64 total = 0;
     for (u32 k = 0; k < L->nv; k++) total += 2 * (len >> k);
-    if (int e = dp_dev_alloc((void **)&L->block, sizeof(gle) * total)) { delete L; return e; }
+    if (int e = dp_dev_alloc((void **)&L->block, sizeof(gle) * total)) return e;
     gle *p = L->block;
     for (u32 k = 0; k < L->nv; k++) { L->num.push_back(p); p += len >> k; L->den.push_back(p); p += len >> k; }
     ColsArg ca; memset(&ca, 0, sizeof ca); ca.n = n_columns;
-    gle sep = e_make(gl_canon(column_separation_challenge[0]), gl_canon(column_separation_challenge[1]));
+    gle sep = e_from_host(column_separation_challenge);
     gle pw = e_one();
     for (u32 k = 0; k < n_columns; k++) { ca.col[k] = (const u64 *)columns[k]->data; ca.pw[k] = pw; pw = e_mul(pw, sep); }
-    gle cc = e_make(gl_canon(constant_challenge[0]), gl_canon(constant_challenge[1]));
+    gle cc = e_from_host(constant_challenge);
     int g = dp_grid_for(len, 256, 8);
     { DpProfScope prof("k_logup_den", len * (8 * n_columns + 16)); k_logup_den<<<g, 256, 0, c.stream>>>(ca, cc, len, L->den[0]); DP_LAUNCHED(); }
     if (L->table) { k_lift_b2e<<<g, 256, 0, c.stream>>>((const u64 *)multiplicities->data, L->num[0], len); DP_LAUNCHED(); }
@@ -126,7 +126,7 @@ int dp_logup_build(dp_mle *const *columns, uint32_t n_columns, const dp_mle *mul
     }
     DP_CUDA(cudaGetLastError());
     if (!L->table) L->num[0] = nullptr;
-    *out = L;
+    *out = L.release();
     return DP_OK;
 }
 
@@ -161,10 +161,9 @@ int dp_logup_layer_mles(const dp_logup *L, uint32_t layer_vars, dp_mle **out_vie
     DP_CHECK(layer_vars + 1 <= L->nv, DP_ERR_INVALID, "One of the circuits was not the same size as the others");   // prover.rs:103-105
     u32 k = L->nv - 1 - layer_vars;          // layer index: 2^(layer_vars+1) entries
     u64 half = 1ULL << layer_vars;
-    auto view = [&](gle *p) { dp_mle *v = new dp_mle(); v->data = p; v->len = half; v->is_ext = true; v->owned = false; return v; };
     u32 n = 0;
-    if (L->num[k]) { out_views[n++] = view(L->num[k]); out_views[n++] = view(L->num[k] + half); }
-    out_views[n++] = view(L->den[k]); out_views[n++] = view(L->den[k] + half);
+    if (L->num[k]) { out_views[n++] = dp_mle_view(L->num[k], half, true); out_views[n++] = dp_mle_view(L->num[k] + half, half, true); }
+    out_views[n++] = dp_mle_view(L->den[k], half, true); out_views[n++] = dp_mle_view(L->den[k] + half, half, true);
     *n_views = n;
     return DP_OK;
 }
@@ -190,13 +189,13 @@ int dp_mle_linear_combination(dp_mle *const *mles, const uint64_t *coefs, uint32
     u64 len = mles[0]->len;
     for (u32 k = 0; k < n; k++) {
         DP_CHECK(mles[k]->is_ext && mles[k]->len == len, DP_ERR_INVALID, "dp_mle_linear_combination: operands must be Ext MLEs of equal length");
-        a.m[k] = (const gle *)mles[k]->data; a.coef[k] = e_make(gl_canon(coefs[2 * k]), gl_canon(coefs[2 * k + 1]));
+        a.m[k] = (const gle *)mles[k]->data; a.coef[k] = e_from_host(coefs + 2 * k);
     }
-    dp_mle *r = new dp_mle(); r->len = len; r->is_ext = true; r->owned = true;
-    if (int e = dp_dev_alloc(&r->data, r->bytes())) { delete r; return e; }
+    MlePtr r;
+    if (int e = dp_mle_alloc(len, true, r)) return e;
     k_lincomb<<<dp_grid_for(len, 256, 8), 256, 0, dp_ctx().stream>>>(a, len, (gle *)r->data); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    *out = r;
+    *out = r.release();
     return DP_OK;
 }
 

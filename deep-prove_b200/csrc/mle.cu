@@ -1,24 +1,12 @@
 // multilinear_extensions on device: upload/canonicalise, eq table (K5), MSB fold (K3), LSB fold (K2),
 // evaluate (K4).  Reference: multilinear_extensions/src/mle.rs:454-712, virtual_poly.rs:346-453,
 // zkml/src/commit/mod.rs:10-28.  All kernels are HBM-streaming integer kernels: 16-byte vector loads,
-// coalesced along the fastest index, lazy (192-bit) accumulation so a dot product costs one modular
+// coalesced along the fastest index, lazy (160-bit) accumulation so a dot product costs one modular
 // reduction per output instead of one per term.
 #include "common.cuh"
 #include <algorithm>
 
 struct PointArg { gle r[32]; };
-
-// 192-bit accumulator of raw 128-bit products
-struct Acc192 { u64 lo, hi, top; };
-__device__ __forceinline__ void acc_init(Acc192 &a) { a.lo = a.hi = a.top = 0; }
-__device__ __forceinline__ void acc_mac(Acc192 &a, u64 x, u64 y) {
-    u64 pl = x * y, ph = __umul64hi(x, y);
-    a.lo += pl; u64 c = a.lo < pl;
-    a.hi += ph; u64 c2 = a.hi < ph;
-    a.hi += c; c2 += (a.hi < c);
-    a.top += c2;
-}
-__device__ __forceinline__ u64 acc_reduce(const Acc192 &a) { return gl_reduce160(a.lo, a.hi, a.top); /* top < #terms < 2^32 */ }
 
 __global__ void k_canonicalize(u64 *v, u64 n) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
@@ -44,7 +32,7 @@ __global__ void k_eq_expand(const gle *__restrict__ lo, const gle *__restrict__ 
     for (; i < n; i += stride) st_e(out + i, e_mul(ld_e(hi + (i >> L)), ld_e(lo + (i & mask))));
 }
 
-int dpk_eq_build(const gle *point, u32 nv, gle *out) {
+static int dpk_eq_build(const gle *point, u32 nv, gle *out) {
     DpCtx &c = dp_ctx();
     DP_CHECK(nv <= 32, DP_ERR_INVALID, "eq_build: num_vars > 32");
     PointArg pa; memset(&pa, 0, sizeof pa);
@@ -59,7 +47,9 @@ int dpk_eq_build(const gle *point, u32 nv, gle *out) {
     u32 H = nv - L;
     gle *lo = nullptr, *hi = nullptr;
     if (int e = dp_dev_alloc((void **)&lo, sizeof(gle) << L)) return e;
+    DevPtr lo_owner(lo);
     if (int e = dp_dev_alloc((void **)&hi, sizeof(gle) << H)) return e;
+    DevPtr hi_owner(hi);
     k_eq_small<<<((1u << L) + 127) / 128, 128, 0, c.stream>>>(pa, 0, L, lo); DP_LAUNCHED();
     if (H <= 14) { k_eq_small<<<((1u << H) + 127) / 128, 128, 0, c.stream>>>(pa, L, H, hi); DP_LAUNCHED(); }
     else {  // recurse once for very large tables
@@ -70,7 +60,6 @@ int dpk_eq_build(const gle *point, u32 nv, gle *out) {
     u64 n = 1ULL << nv;
     k_eq_expand<<<dp_grid_for(n, 256, 8), 256, 0, c.stream>>>(lo, hi, L, n, out); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    dp_dev_free(lo); dp_dev_free(hi);
     return DP_OK;
 }
 
@@ -112,22 +101,22 @@ __global__ void k_fixhigh_cols(const void *__restrict__ src, const gle *__restri
     u64 j0 = (u64)blockIdx.y * rows_per_y, j1 = j0 + rows_per_y; if (j1 > J) j1 = J;
     if (EXT) {
         const gle *f = (const gle *)src;
-        Acc192 s00, s11, s01; acc_init(s00); acc_init(s11); acc_init(s01);
+        gl_acc s00 = {0, 0, 0}, s11 = {0, 0, 0}, s01 = {0, 0, 0};
 #pragma unroll 4
         for (u64 j = j0; j < j1; j++) {
             gle a = ld_e(w + j), b = ld_e(f + j * S + i);
-            acc_mac(s00, a.c0, b.c0); acc_mac(s11, a.c1, b.c1); acc_mac(s01, a.c0, b.c1); acc_mac(s01, a.c1, b.c0);
+            gl_acc_mac(s00, a.c0, b.c0); gl_acc_mac(s11, a.c1, b.c1); gl_acc_mac(s01, a.c0, b.c1); gl_acc_mac(s01, a.c1, b.c0);
         }
-        st_e(part + (u64)blockIdx.y * S + i, e_make(gl_add(acc_reduce(s00), gl_mul7(acc_reduce(s11))), acc_reduce(s01)));
+        st_e(part + (u64)blockIdx.y * S + i, e_make(gl_add(gl_acc_reduce(s00), gl_mul7(gl_acc_reduce(s11))), gl_acc_reduce(s01)));
     } else {
         const u64 *f = (const u64 *)src;
-        Acc192 s0, s1; acc_init(s0); acc_init(s1);
+        gl_acc s0 = {0, 0, 0}, s1 = {0, 0, 0};
 #pragma unroll 4
         for (u64 j = j0; j < j1; j++) {
             gle a = ld_e(w + j); u64 b = f[j * S + i];
-            acc_mac(s0, a.c0, b); acc_mac(s1, a.c1, b);
+            gl_acc_mac(s0, a.c0, b); gl_acc_mac(s1, a.c1, b);
         }
-        st_e(part + (u64)blockIdx.y * S + i, e_make(acc_reduce(s0), acc_reduce(s1)));
+        st_e(part + (u64)blockIdx.y * S + i, e_make(gl_acc_reduce(s0), gl_acc_reduce(s1)));
     }
 }
 __global__ void k_sum_parts(const gle *__restrict__ part, u64 S, u32 ny, gle *__restrict__ out) {
@@ -136,6 +125,18 @@ __global__ void k_sum_parts(const gle *__restrict__ part, u64 S, u32 ny, gle *__
     gle a = e_zero();
     for (u32 y = 0; y < ny; y++) a = e_add(a, ld_e(part + (u64)y * S + i));
     st_e(out + i, a);
+}
+// the sum of every thread's `acc` (blockDim.x a multiple of 32), stored to *dst by thread 0
+__device__ __forceinline__ void block_sum_store(gle acc, gle *dst) {
+    __shared__ gle sm[32];
+    for (int d = 16; d > 0; d >>= 1) acc = e_add(acc, shfl_down_e(acc, d));
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        acc = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : e_zero();
+        for (int d = 16; d > 0; d >>= 1) acc = e_add(acc, shfl_down_e(acc, d));
+        if (threadIdx.x == 0) st_e(dst, acc);
+    }
 }
 // few outputs (S < 32): one block per output, threads stride over the J rows, block reduction
 template <bool EXT>
@@ -147,15 +148,7 @@ __global__ void k_fixhigh_dot(const void *__restrict__ src, const gle *__restric
         if (EXT) acc = e_add(acc, e_mul(a, ld_e((const gle *)src + j * S + i)));
         else acc = e_add(acc, e_mul_base(a, ((const u64 *)src)[j * S + i]));
     }
-    __shared__ gle sm[32];
-    for (int d = 16; d > 0; d >>= 1) acc = e_add(acc, shfl_down_e(acc, d));
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        acc = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : e_zero();
-        for (int d = 16; d > 0; d >>= 1) acc = e_add(acc, shfl_down_e(acc, d));
-        if (threadIdx.x == 0) st_e(out + i, acc);
-    }
+    block_sum_store(acc, out + i);
 }
 
 // several MLEs of equal size evaluated at ONE point: the eq table is built once, one launch, one copy back
@@ -168,22 +161,15 @@ __global__ void k_eval_many(EvalArg a, const gle *__restrict__ w, u64 J, gle *__
         if (a.ext[y]) acc = e_add(acc, e_mul(wj, ld_e((const gle *)a.src[y] + j)));
         else acc = e_add(acc, e_mul_base(wj, ((const u64 *)a.src[y])[j]));
     }
-    __shared__ gle sm[32];
-    for (int d = 16; d > 0; d >>= 1) acc = e_add(acc, shfl_down_e(acc, d));
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        acc = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : e_zero();
-        for (int d = 16; d > 0; d >>= 1) acc = e_add(acc, shfl_down_e(acc, d));
-        if (threadIdx.x == 0) st_e(out + y, acc);
-    }
+    block_sum_store(acc, out + y);
 }
 
-int dpk_fix_high(const void *src, bool src_ext, u64 len, const gle *point, u32 k, gle *out) {
+static int dpk_fix_high(const void *src, bool src_ext, u64 len, const gle *point, u32 k, gle *out) {
     DpCtx &c = dp_ctx();
     u64 J = 1ULL << k, S = len >> k;
     gle *w = nullptr;
     if (int e = dp_dev_alloc((void **)&w, sizeof(gle) * J)) return e;
+    DevPtr w_owner(w);
     if (int e = dpk_eq_build(point, k, w)) return e;
     DpProfScope prof(S < 32 ? "k_fixhigh_dot" : "k_fixhigh_cols", len * (src_ext ? 16 : 8) + S * 16);
     if (S < 32) {
@@ -199,41 +185,46 @@ int dpk_fix_high(const void *src, bool src_ext, u64 len, const gle *point, u32 k
         if (ny > 1024) ny = 1024;
         u64 rows = (J + ny - 1) / ny; ny = (J + rows - 1) / rows;
         gle *part = out;
-        if (ny > 1) { if (int e = dp_dev_alloc((void **)&part, sizeof(gle) * S * ny)) return e; }
+        DevPtr part_owner;
+        if (ny > 1) { if (int e = dp_dev_alloc((void **)&part, sizeof(gle) * S * ny)) return e; part_owner.reset(part); }
         dim3 grid((unsigned)gx, (unsigned)ny);
         if (src_ext) k_fixhigh_cols<true><<<grid, T, 0, c.stream>>>(src, w, S, J, rows, part);
         else k_fixhigh_cols<false><<<grid, T, 0, c.stream>>>(src, w, S, J, rows, part);
         DP_LAUNCHED();
-        if (ny > 1) {
-            k_sum_parts<<<(unsigned)((S + 255) / 256), 256, 0, c.stream>>>(part, S, (u32)ny, out); DP_LAUNCHED();
-            dp_dev_free(part);
-        }
+        if (ny > 1) { k_sum_parts<<<(unsigned)((S + 255) / 256), 256, 0, c.stream>>>(part, S, (u32)ny, out); DP_LAUNCHED(); }
     }
     DP_CUDA(cudaGetLastError());
-    dp_dev_free(w);
+    return DP_OK;
+}
+
+static void point_from_host(const uint64_t *point, u32 k, gle *out) {
+    for (u32 i = 0; i < k; i++) out[i] = e_from_host(point + 2 * i);
+}
+
+// fix_high_variables (mle.rs:529-603): `m` with its top k >= 1 variables fixed at `point`, as a new Ext MLE
+static int fix_high(const dp_mle *m, const uint64_t *point, u32 k, MlePtr &out) {
+    gle pt[32]; point_from_host(point, k, pt);
+    MlePtr r;
+    if (int e = dp_mle_alloc(m->len >> k, true, r)) return e;
+    if (int e = dpk_fix_high(m->data, m->is_ext, m->len, pt, k, (gle *)r->data)) return e;
+    out = std::move(r);
     return DP_OK;
 }
 
 // =====================================================================================================
 extern "C" {
 
-static int point_from_host(const uint64_t *point, u32 k, gle *out) {
-    for (u32 i = 0; i < k; i++) out[i] = e_make(gl_canon(point[2 * i]), gl_canon(point[2 * i + 1]));
-    return DP_OK;
-}
-
 int dp_mle_upload(const uint64_t *evals, uint64_t len, int is_ext, dp_mle **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(out && evals, DP_ERR_INVALID, "dp_mle_upload: null argument");
     DP_CHECK(len > 0 && (len & (len - 1)) == 0, DP_ERR_INVALID, "dp_mle_upload: len must be a power of two");
-    dp_mle *m = new dp_mle();
-    m->len = len; m->is_ext = is_ext != 0; m->owned = true;
-    if (int e = dp_dev_alloc(&m->data, m->bytes())) { delete m; return e; }
+    MlePtr m;
+    if (int e = dp_mle_alloc(len, is_ext != 0, m)) return e;
     DP_CUDA(cudaMemcpyAsync(m->data, evals, m->bytes(), cudaMemcpyHostToDevice, dp_ctx().stream));
     u64 n = len * (is_ext ? 2 : 1);
     k_canonicalize<<<dp_grid_for(n, 256, 8), 256, 0, dp_ctx().stream>>>((u64 *)m->data, n); DP_LAUNCHED();
     DP_CUDA(cudaGetLastError());
-    *out = m;
+    *out = m.release();
     return DP_OK;
 }
 
@@ -242,20 +233,17 @@ int dp_mle_wrap_device(void *dev_ptr, uint64_t len, int is_ext, dp_mle **out) {
     DP_CHECK(out && dev_ptr, DP_ERR_INVALID, "dp_mle_wrap_device: null argument");
     DP_CHECK(len > 0 && (len & (len - 1)) == 0, DP_ERR_INVALID, "dp_mle_wrap_device: len must be a power of two");
     DP_CHECK(((uintptr_t)dev_ptr & 15) == 0, DP_ERR_INVALID, "dp_mle_wrap_device: pointer must be 16-byte aligned");
-    dp_mle *m = new dp_mle();
-    m->data = dev_ptr; m->len = len; m->is_ext = is_ext != 0; m->owned = false;
-    *out = m;
+    *out = dp_mle_view(dev_ptr, len, is_ext != 0);
     return DP_OK;
 }
 
 int dp_mle_clone(const dp_mle *src, dp_mle **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(src && out, DP_ERR_INVALID, "dp_mle_clone: null argument");
-    dp_mle *m = new dp_mle(*src);
-    m->owned = true; m->data = nullptr;
-    if (int e = dp_dev_alloc(&m->data, m->bytes())) { delete m; return e; }
+    MlePtr m;
+    if (int e = dp_mle_alloc(src->len, src->is_ext, m)) return e;
     DP_CUDA(cudaMemcpyAsync(m->data, src->data, m->bytes(), cudaMemcpyDeviceToDevice, dp_ctx().stream));
-    *out = m;
+    *out = m.release();
     return DP_OK;
 }
 
@@ -287,13 +275,9 @@ int dp_mle_fix_high(dp_mle *m, const uint64_t *point, uint32_t k) {
     DP_CHECK(m && (point || k == 0), DP_ERR_INVALID, "dp_mle_fix_high: null argument");
     DP_CHECK(k <= m->num_vars(), DP_ERR_INVALID, "invalid size of partial point");  // mle.rs:564-567
     if (k == 0) return DP_OK;  // reference leaves a Base MLE untouched when the point is empty
-    gle pt[32]; point_from_host(point, k, pt);
-    gle *out = nullptr;
-    u64 S = m->len >> k;
-    if (int e = dp_dev_alloc((void **)&out, sizeof(gle) * S)) return e;
-    if (int e = dpk_fix_high(m->data, m->is_ext, m->len, pt, k, out)) return e;
-    if (m->owned) dp_dev_free(m->data);
-    m->data = out; m->len = S; m->is_ext = true; m->owned = true;
+    MlePtr r;
+    if (int e = fix_high(m, point, k, r)) return e;
+    std::swap(*m, *r);         // m takes the folded table; its old one leaves with r
     return DP_OK;
 }
 
@@ -303,11 +287,9 @@ int dp_mle_fix_high_new(const dp_mle *m, const uint64_t *point, uint32_t k, dp_m
     DP_CHECK(m && outp && (point || k == 0), DP_ERR_INVALID, "dp_mle_fix_high_new: null argument");
     DP_CHECK(k <= m->num_vars(), DP_ERR_INVALID, "invalid size of partial point");
     if (k == 0) return dp_mle_clone(m, outp);
-    gle pt[32]; point_from_host(point, k, pt);
-    dp_mle *r = new dp_mle(); r->len = m->len >> k; r->is_ext = true; r->owned = true;
-    if (int e = dp_dev_alloc(&r->data, r->bytes())) { delete r; return e; }
-    if (int e = dpk_fix_high(m->data, m->is_ext, m->len, pt, k, (gle *)r->data)) return e;
-    *outp = r;
+    MlePtr r;
+    if (int e = fix_high(m, point, k, r)) return e;
+    *outp = r.release();
     return DP_OK;
 }
 
@@ -317,17 +299,14 @@ int dp_mle_fix_low(const dp_mle *m, const uint64_t *point, uint32_t k, dp_mle **
     DP_CHECK(k <= m->num_vars(), DP_ERR_INVALID, "invalid size of partial point");  // mle.rs:457-460
     if (k == 0) return dp_mle_clone(m, outp);
     gle pt[32]; point_from_host(point, k, pt);
-    const void *cur = m->data; bool cur_ext = m->is_ext; u64 len = m->len; gle *owned_cur = nullptr;
+    MlePtr cur(dp_mle_view(m->data, m->len, m->is_ext));    // each fold reads the previous table and frees it once done
     for (u32 i = 0; i < k; i++) {
-        gle *nxt = nullptr;
-        if (int e = dp_dev_alloc((void **)&nxt, sizeof(gle) * (len >> 1))) return e;
-        if (int e = dpk_fold_low(cur, cur_ext, len, pt[i], nxt)) return e;
-        if (owned_cur) dp_dev_free(owned_cur);
-        owned_cur = nxt; cur = nxt; cur_ext = true; len >>= 1;
+        MlePtr nxt;
+        if (int e = dp_mle_alloc(cur->len >> 1, true, nxt)) return e;
+        if (int e = dpk_fold_low(cur->data, cur->is_ext, cur->len, pt[i], (gle *)nxt->data)) return e;
+        cur = std::move(nxt);
     }
-    dp_mle *r = new dp_mle();
-    r->data = owned_cur; r->len = len; r->is_ext = true; r->owned = true;
-    *outp = r;
+    *outp = cur.release();
     return DP_OK;
 }
 
@@ -337,6 +316,7 @@ int dp_mle_evaluate(const dp_mle *m, const uint64_t *point, uint32_t num_vars, u
     DP_CHECK(num_vars == m->num_vars(), DP_ERR_INVALID, "MLE size does not match the point");  // mle.rs:609-613
     gle *res = nullptr;
     if (int e = dp_dev_alloc((void **)&res, sizeof(gle))) return e;
+    DevPtr res_owner(res);
     if (num_vars == 0) {
         if (m->is_ext) DP_CUDA(cudaMemcpyAsync(res, m->data, 16, cudaMemcpyDeviceToDevice, dp_ctx().stream));
         else { DP_CUDA(cudaMemsetAsync(res, 0, 16, dp_ctx().stream)); DP_CUDA(cudaMemcpyAsync(res, m->data, 8, cudaMemcpyDeviceToDevice, dp_ctx().stream)); }
@@ -350,14 +330,12 @@ int dp_mle_evaluate(const dp_mle *m, const uint64_t *point, uint32_t num_vars, u
         } else {
             gle *mid = nullptr;
             if (int e = dp_dev_alloc((void **)&mid, sizeof(gle) << LOW)) return e;
+            DevPtr mid_owner(mid);
             if (int e = dpk_fix_high(m->data, m->is_ext, m->len, pt + LOW, num_vars - LOW, mid)) return e;
             if (int e = dpk_fix_high(mid, true, 1ULL << LOW, pt, LOW, res)) return e;
-            dp_dev_free(mid);
         }
     }
-    const int rc = dp_d2h(out, res, 16, dp_ctx().stream);
-    dp_dev_free(res);
-    return rc;
+    return dp_d2h(out, res, 16, dp_ctx().stream);
 }
 
 // evaluate (mle.rs:607-623) for n MLEs with the same num_vars at the same point (e.g. the LogUp output claims,
@@ -374,8 +352,11 @@ int dp_mle_evaluate_many(const dp_mle *const *mles, uint32_t n, const uint64_t *
     u64 J = 1ULL << num_vars;
     gle *w = nullptr, *res = nullptr, *hres = nullptr;
     if (int e = dp_dev_alloc((void **)&w, sizeof(gle) * J)) return e;
+    DevPtr w_owner(w);
     if (int e = dp_dev_alloc((void **)&res, sizeof(gle) * n)) return e;
+    DevPtr res_owner(res);
     if (int e = dp_pinned_alloc((void **)&hres, sizeof(gle) * n)) return e;
+    PinnedPtr hres_owner(hres);
     if (int e = dpk_eq_build(pt, num_vars, w)) return e;
     for (u32 base = 0; base < n; base += 16) {
         EvalArg a; memset(&a, 0, sizeof a);
@@ -387,7 +368,6 @@ int dp_mle_evaluate_many(const dp_mle *const *mles, uint32_t n, const uint64_t *
     DP_CUDA(cudaMemcpyAsync(hres, res, sizeof(gle) * n, cudaMemcpyDeviceToHost, dp_ctx().stream));
     DP_CUDA(dp_stream_sync(dp_ctx().stream));
     for (u32 i = 0; i < n; i++) { out[2 * i] = hres[i].c0; out[2 * i + 1] = hres[i].c1; }
-    dp_dev_free(w); dp_dev_free(res); dp_pinned_free(hres);
     return DP_OK;
 }
 
@@ -396,11 +376,10 @@ int dp_eq_build(const uint64_t *point, uint32_t num_vars, dp_mle **outp) {
     DP_CHECK(outp && (point || num_vars == 0), DP_ERR_INVALID, "dp_eq_build: null argument");
     DP_CHECK(num_vars <= 32, DP_ERR_INVALID, "dp_eq_build: num_vars > 32");
     gle pt[32]; point_from_host(point, num_vars, pt);
-    dp_mle *r = new dp_mle();
-    r->len = 1ULL << num_vars; r->is_ext = true; r->owned = true;
-    if (int e = dp_dev_alloc(&r->data, r->bytes())) { delete r; return e; }
+    MlePtr r;
+    if (int e = dp_mle_alloc(1ULL << num_vars, true, r)) return e;
     if (int e = dpk_eq_build(pt, num_vars, (gle *)r->data)) return e;
-    *outp = r;
+    *outp = r.release();
     return DP_OK;
 }
 

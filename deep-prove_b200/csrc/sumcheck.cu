@@ -314,20 +314,14 @@ k_sc_round(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc
 // folding Base->Ext: its second round; all folding Ext->Ext: every later round; all Ext: the first round of an Ext polynomial)
 // and every product has the same degree D in {2, 3}.  The mode and the degree are compile-time, so the body is a straight line
 // of loads and multiply chains (no per-operand switch, 64-118 registers instead of 122 for everything), the products of the
-// last multiplication are accumulated UNREDUCED in 192-bit (Base) / 2 x 160-bit (Ext) sums and reduced once per thread and
+// last multiplication are accumulated UNREDUCED in 160-bit (Base) / 2 x 160-bit (Ext) sums and reduced once per thread and
 // evaluation point, and the block shape follows the measurements in tools/kbench.cu: Base rounds 256 threads x 2 pairs in
 // flight (HBM-bound: 1.9 TB/s at nu = 20), folding rounds 128 threads x 1 pair (issue-bound: 122 instructions per E x E).
-struct acc192 { u64 lo, hi; u32 top; };                     // lo + hi 2^64 + top 2^128
-__device__ __forceinline__ void acc_mac(acc192 &a, u64 x, u64 y) {
-    u64 pl = x * y, ph = __umul64hi(x, y);
-    asm("{\n\tadd.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u32 %2, %2, 0;\n\t}" : "+l"(a.lo), "+l"(a.hi), "+r"(a.top) : "l"(pl), "l"(ph));
-}
-__device__ __forceinline__ u64 acc_reduce(const acc192 &a) { return gl_reduce160(a.lo, a.hi, a.top); }
-struct eacc { acc192 c0, c1; };
+struct eacc { gl_acc c0, c1; };
 __device__ __forceinline__ void eacc_mac(eacc &a, gle x, gle y) {   // a += x * y   (c1 = x0 y1 + x1 y0; c0 = x0 y0 + 7 w, w = weak(x1 y1))
-    acc_mac(a.c1, x.c0, y.c1); acc_mac(a.c1, x.c1, y.c0);
+    gl_acc_mac(a.c1, x.c0, y.c1); gl_acc_mac(a.c1, x.c1, y.c0);
     u64 w = gl_reduce128_weak(x.c1 * y.c1, __umul64hi(x.c1, y.c1));
-    acc_mac(a.c0, x.c0, y.c0); acc_mac(a.c0, w, 7ULL);
+    gl_acc_mac(a.c0, x.c0, y.c0); gl_acc_mac(a.c0, w, 7ULL);
 }
 template <int MODE> struct ScLeanShape { static constexpr int BLOCK = MODE == OPM_B ? 256 : 128, MINB = 4, PPT = MODE == OPM_B ? 2 : 1; };
 
@@ -348,7 +342,7 @@ k_sc_lean(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc0
 #pragma unroll
     for (int t = 0; t < SC_NACC; t++) acc[t] = e_zero();
     if (MODE == OPM_B) {
-        acc192 a[D + 1];
+        gl_acc a[D + 1];
 #pragma unroll
         for (int t = 0; t <= D; t++) { a[t].lo = 0; a[t].hi = 0; a[t].top = 0; }
         const u64 *src[D];
@@ -373,7 +367,7 @@ k_sc_lean(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc0
                     u64 q = c[0];
 #pragma unroll
                     for (int j = 1; j < D - 1; j++) q = gl_mul_weak(q, c[j]);
-                    acc_mac(a[t], q, c[D - 1]);
+                    gl_acc_mac(a[t], q, c[D - 1]);
                     if (t < D) {
 #pragma unroll
                         for (int j = 0; j < D; j++) c[j] = gl_add(c[j], s[j]);
@@ -382,7 +376,7 @@ k_sc_lean(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc0
             }
         }
 #pragma unroll
-        for (int t = 0; t <= D; t++) acc[t] = e_from_base(acc_reduce(a[t]));
+        for (int t = 0; t <= D; t++) acc[t] = e_from_base(gl_acc_reduce(a[t]));
     } else {
         eacc a[D + 1];
 #pragma unroll
@@ -421,7 +415,7 @@ k_sc_lean(const ScProd *__restrict__ descs, const __grid_constant__ ScProd desc0
             }
         }
 #pragma unroll
-        for (int t = 0; t <= D; t++) acc[t] = e_make(acc_reduce(a[t].c0), acc_reduce(a[t].c1));
+        for (int t = 0; t <= D; t++) acc[t] = e_make(gl_acc_reduce(a[t].c0), gl_acc_reduce(a[t].c1));
     }
     sc_epilogue<BLOCK>(acc, D + 1, partials, counters, out, seq, flag, done);
 }
@@ -924,7 +918,7 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
         DP_CHECK(challenge == nullptr, DP_ERR_STATE, "first round should be prover first.");  // prover.rs:655
     } else {
         DP_CHECK(challenge != nullptr, DP_ERR_STATE, "verifier message is empty");  // prover.rs:657
-        r = e_make(gl_canon(challenge[0]), gl_canon(challenge[1]));
+        r = e_from_host(challenge);
         s->challenges.push_back(r);
         fold = true;
         if (s->challenges.size() == 1)
@@ -1025,7 +1019,7 @@ int dp_sc_finish(dp_sc *s, const uint64_t *last_challenge, uint64_t *out_final) 
     DP_REQUIRE_CTX();
     DP_CHECK(s && last_challenge && out_final, DP_ERR_INVALID, "dp_sc_finish: null argument");
     DP_CHECK(!s->finished && s->round == s->max_nv, DP_ERR_STATE, "dp_sc_finish: rounds not complete");
-    gle r = e_make(gl_canon(last_challenge[0]), gl_canon(last_challenge[1]));
+    gle r = e_from_host(last_challenge);
     s->challenges.push_back(r);
     // the last round fetched the pairs unless an MLE still had more than 2 entries; get_mle_final_evaluations asserts
     // len == 1 after the last fix (prover.rs:479-483)
@@ -1089,7 +1083,7 @@ int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *
     }
     gle r = e_zero();
     if (fold) {
-        r = e_make(gl_canon(prev_challenge[0]), gl_canon(prev_challenge[1]));
+        r = e_from_host(prev_challenge);
         s->challenges.push_back(r);
         if (s->challenges.size() == 1)
             for (auto &m : s->mles) DP_CHECK(m.len > 1, DP_ERR_INVALID, "calling sumcheck on constant");  // prover.rs:667-669
@@ -1129,9 +1123,7 @@ int dp_sc_current_mle(dp_sc *s, uint32_t idx, dp_mle **out) {
     DP_CHECK(s && out && idx < s->n_mles, DP_ERR_INVALID, "dp_sc_current_mle: bad argument");
     const ScMle &m = s->mles[idx];
     DP_CHECK(!s->tail_active, DP_ERR_STATE, "dp_sc_current_mle: tables are owned by the resident tail kernel");
-    dp_mle *v = new dp_mle();
-    v->data = const_cast<void *>(m.cur); v->len = m.len; v->is_ext = m.is_ext; v->owned = false;
-    *out = v;
+    *out = dp_mle_view(const_cast<void *>(m.cur), m.len, m.is_ext);
     return DP_OK;
 }
 

@@ -10,6 +10,7 @@
 // histograms into the multiplicity polynomials.  Per proof only the model input crosses PCIe.
 // Values outside a table (a broken model/trace) raise an error flag that dp_wit_finish reports -- the reference panics there.
 #include "common.cuh"
+#include <algorithm>
 
 static constexpr long long WQMIN = -127, WQMAX = 127;     // quantization/mod.rs:28-29
 static constexpr u32 W_BIT_LEN = 8;
@@ -108,21 +109,15 @@ __global__ void k_wit_mult(const u32 *__restrict__ counts, MultOut o) {
     o.m[t][i - o.off[t]] = (u64)counts[i];
 }
 
-static int wit_new_base(u64 len, dp_mle **out) {
-    dp_mle *m = new dp_mle(); m->len = len; m->is_ext = false; m->owned = true;
-    if (int e = dp_dev_alloc(&m->data, m->bytes())) { delete m; return e; }
-    *out = m; return DP_OK;
-}
-// n fresh columns of `len`, or none: on a failed allocation the ones already made are freed
-static int wit_new_cols(u64 len, u32 n, dp_mle **cols) {
-    for (u32 k = 0; k < n; k++) {
-        if (int e = wit_new_base(len, &cols[k])) {
-            for (u32 q = 0; q < k; q++) { dp_mle_free(cols[q]); cols[q] = nullptr; }
-            return e;
-        }
-    }
+// n fresh Base columns of `len`, or none.  They stay in `own` until the call succeeds; the caller's array is cleared
+// first, so a failed call leaves it all nullptr.
+static int wit_new_cols(u64 len, u32 n, std::vector<MlePtr> &own, dp_mle **cols) {
+    std::fill(cols, cols + n, nullptr);
+    own.resize(n);
+    for (u32 k = 0; k < n; k++) if (int e = dp_mle_alloc(len, false, own[k])) return e;
     return DP_OK;
 }
+static void wit_hand_over(std::vector<MlePtr> &own, dp_mle **cols) { for (size_t k = 0; k < own.size(); k++) cols[k] = own[k].release(); }
 
 extern "C" {
 
@@ -131,15 +126,15 @@ int dp_wit_begin(uint32_t n_tables, const uint32_t *kinds, const uint32_t *sizes
     DP_CHECK(out && kinds && sizes && n_tables >= 1 && n_tables <= 8, DP_ERR_INVALID, "dp_wit_begin: 1..8 tables");
     for (u32 t = 0; t < n_tables; t++)
         DP_CHECK(kinds[t] == 0 || kinds[t] == 2 || (kinds[t] == 3 && sizes[t] >= 1 && sizes[t] <= 24), DP_ERR_INVALID, "dp_wit_begin: unknown table type");
-    dp_wit *w = new dp_wit(); w->n_tables = n_tables;
+    std::unique_ptr<dp_wit, FreeWith<dp_wit_free>> w(new dp_wit());
+    w->n_tables = n_tables;
     for (u32 t = 0; t < n_tables; t++) {
         w->kind[t] = kinds[t]; w->size[t] = sizes[t]; w->off[t + 1] = w->off[t] + (1ULL << wit_vars(kinds[t], sizes[t]));
     }
-    int e;
-    if ((e = dp_dev_alloc((void **)&w->counts, sizeof(u32) * (w->off[n_tables] + 4)))) { delete w; return e; }
-    if ((e = dp_pinned_alloc((void **)&w->err_pinned, 64))) { dp_dev_free(w->counts); delete w; return e; }
+    if (int e = dp_dev_alloc((void **)&w->counts, sizeof(u32) * (w->off[n_tables] + 4))) return e;
+    if (int e = dp_pinned_alloc((void **)&w->err_pinned, 64)) return e;
     DP_CUDA(cudaMemsetAsync(w->counts, 0, sizeof(u32) * (w->off[n_tables] + 4), dp_ctx().stream));
-    *out = w;
+    *out = w.release();
     return DP_OK;
 }
 
@@ -148,12 +143,12 @@ int dp_wit_dense(const dp_mle *weights, const dp_mle *bias, const dp_mle *x, uin
     DP_CHECK(weights && bias && x && out, DP_ERR_INVALID, "dp_wit_dense: null argument");
     DP_CHECK(!weights->is_ext && !bias->is_ext && !x->is_ext, DP_ERR_INVALID, "dp_wit_dense: tensors are Base");
     DP_CHECK(weights->len == (u64)nrows * ncols && bias->len == nrows && x->len == ncols, DP_ERR_INVALID, "dp_wit_dense: shape mismatch");
-    dp_mle *o; if (int e = wit_new_base(nrows, &o)) return e;
+    MlePtr o; if (int e = dp_mle_alloc(nrows, false, o)) return e;
     DpProfScope prof("k_wit_dense", weights->bytes() + x->bytes() + 16ull * nrows);
     if (ncols >= 2) k_wit_dense<<<(nrows * 32 + 255) / 256, 256, 0, dp_ctx().stream>>>((const u64 *)weights->data, (const u64 *)bias->data, (const u64 *)x->data, nrows, ncols, (u64 *)o->data);
     else k_wit_dense_small<<<(nrows + 255) / 256, 256, 0, dp_ctx().stream>>>((const u64 *)weights->data, (const u64 *)bias->data, (const u64 *)x->data, nrows, ncols, (u64 *)o->data);
     DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
-    *out = o;
+    *out = o.release();
     return DP_OK;
 }
 
@@ -162,11 +157,11 @@ int dp_wit_matmul(const dp_mle *left, const dp_mle *right, const dp_mle *bias, u
     DP_CHECK(left && right && out, DP_ERR_INVALID, "dp_wit_matmul: null argument");
     DP_CHECK(!left->is_ext && !right->is_ext && (!bias || !bias->is_ext), DP_ERR_INVALID, "dp_wit_matmul: tensors are Base");
     DP_CHECK(left->len == (u64)R * K && right->len == (u64)K * C && (!bias || bias->len == C), DP_ERR_INVALID, "Incompatible shape found for input matrix");   // matrix_mul.rs:277-283
-    dp_mle *o; if (int e = wit_new_base((u64)R * C, &o)) return e;
+    MlePtr o; if (int e = dp_mle_alloc((u64)R * C, false, o)) return e;
     DpProfScope prof("k_wit_matmul", left->bytes() + right->bytes() + 8ull * R * C);
     k_wit_matmul<<<(unsigned)(((u64)R * C + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)left->data, (const u64 *)right->data, bias ? (const u64 *)bias->data : nullptr, R, K, C, transposed, (u64 *)o->data);
     DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
-    *out = o;
+    *out = o.release();
     return DP_OK;
 }
 
@@ -186,13 +181,15 @@ int dp_wit_requant(dp_wit *w, const dp_mle *x, uint32_t shift, int64_t fixed_poi
     DP_CHECK(intermediate_bit_size <= 62, DP_ERR_INVALID, "dp_wit_requant: intermediate_bit_size must be at most 62");
     if (int e = wit_table(w, range_table, 2, "dp_wit_requant")) return e;
     RqCols c; c.n_chunks = shift / W_BIT_LEN;
-    if (int e = wit_new_cols(x->len, n_cols, cols)) return e;
-    c.cin = (u64 *)cols[0]->data; c.cout = (u64 *)cols[1]->data;
-    for (u32 j = 0; j < c.n_chunks; j++) c.chunk[j] = (u64 *)cols[2 + j]->data;
+    std::vector<MlePtr> own;
+    if (int e = wit_new_cols(x->len, n_cols, own, cols)) return e;
+    c.cin = (u64 *)own[0]->data; c.cout = (u64 *)own[1]->data;
+    for (u32 j = 0; j < c.n_chunks; j++) c.chunk[j] = (u64 *)own[2 + j]->data;
     DpProfScope prof("k_wit_requant", x->bytes() * (1 + n_cols));
     k_wit_requant<<<(unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)x->data, x->len, shift, (long long)fixed_point_multiplier, 1LL << intermediate_bit_size, c,
                                                                                w->counts + w->off[clamp_table], w->size[clamp_table], w->counts + w->off[range_table], w->counts + w->off[w->n_tables]);
     DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    wit_hand_over(own, cols);
     return DP_OK;
 }
 
@@ -200,11 +197,11 @@ int dp_wit_relu(dp_wit *w, const dp_mle *x, uint32_t relu_table, dp_mle **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(w && x && out && !x->is_ext, DP_ERR_INVALID, "dp_wit_relu: bad argument");
     if (int e = wit_table(w, relu_table, 0, "dp_wit_relu")) return e;
-    dp_mle *o; if (int e = wit_new_base(x->len, &o)) return e;
+    MlePtr o; if (int e = dp_mle_alloc(x->len, false, o)) return e;
     DpProfScope prof("k_wit_relu", x->bytes() * 2);
     k_wit_relu<<<(unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)x->data, x->len, (u64 *)o->data, w->counts + w->off[relu_table], w->counts + w->off[w->n_tables]);
     DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
-    *out = o;
+    *out = o.release();
     return DP_OK;
 }
 
@@ -216,12 +213,14 @@ int dp_wit_pool(dp_wit *w, const dp_mle *x, uint32_t C, uint32_t H, uint32_t Wd,
     const u64 n = (u64)C * (H / 2) * (Wd / 2);
     DP_CHECK((n & (n - 1)) == 0, DP_ERR_INVALID, "dp_wit_pool: output length must be a power of two");
     PoolCols p;
-    if (int e = wit_new_cols(n, 5, cols)) return e;
-    for (u32 k = 0; k < 4; k++) p.diff[k] = (u64 *)cols[k]->data;
-    p.out = (u64 *)cols[4]->data;
+    std::vector<MlePtr> own;
+    if (int e = wit_new_cols(n, 5, own, cols)) return e;
+    for (u32 k = 0; k < 4; k++) p.diff[k] = (u64 *)own[k]->data;
+    p.out = (u64 *)own[4]->data;
     DpProfScope prof("k_wit_pool", x->bytes() + 5 * n * 8);
     k_wit_pool<<<(unsigned)((n + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)x->data, C, H, Wd, p, w->counts + w->off[range_table], w->counts + w->off[w->n_tables]);
     DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    wit_hand_over(own, cols);
     return DP_OK;
 }
 
@@ -230,12 +229,15 @@ int dp_wit_finish(dp_wit *w, dp_mle **mults, uint32_t *error_bits) {
     DP_REQUIRE_CTX();
     DP_CHECK(w && mults && error_bits, DP_ERR_INVALID, "dp_wit_finish: null argument");
     MultOut o; o.n = w->n_tables;
-    for (u32 t = 0; t < w->n_tables; t++) { if (int e = wit_new_base(w->off[t + 1] - w->off[t], &mults[t])) return e; o.m[t] = (u64 *)mults[t]->data; }
+    std::fill(mults, mults + w->n_tables, nullptr);
+    std::vector<MlePtr> own(w->n_tables);
+    for (u32 t = 0; t < w->n_tables; t++) { if (int e = dp_mle_alloc(w->off[t + 1] - w->off[t], false, own[t])) return e; o.m[t] = (u64 *)own[t]->data; }
     for (u32 t = 0; t <= w->n_tables; t++) o.off[t] = w->off[t];
     cudaStream_t st = dp_ctx().stream;
     k_wit_mult<<<(unsigned)((w->off[w->n_tables] + 255) / 256), 256, 0, st>>>(w->counts, o); DP_LAUNCHED();
     DP_CUDA(cudaMemcpyAsync(w->err_pinned, w->counts + w->off[w->n_tables], 4, cudaMemcpyDeviceToHost, st));
     DP_CUDA(dp_stream_sync(st));
+    wit_hand_over(own, mults);
     *error_bits = *w->err_pinned;
     return DP_OK;
 }

@@ -518,7 +518,7 @@ def test_linear_combination_refusals(gpu):
 @pytest.mark.parametrize("nv", [0, 1, 10, 16, 17])
 @pytest.mark.parametrize("n", [1, 16, 17, 33])
 def test_evaluate_many(gpu, n, nv, values):
-    """n MLEs at one point: batches of 16 per launch (mle.cu:380-385), one by one for num_vars 0 and > 16 (:369-371); Base and
+    """n MLEs at one point: batches of 16 per launch (mle.cu:361-366), one by one for num_vars 0 and > 16 (:347-349); Base and
     Ext mixed; value-edge tables and points"""
     s = _seed("evalmany%d_%d_%s" % (n, nv, values))
     mles = []

@@ -1,5 +1,7 @@
 """GPU parity tests (-m gpu): the CUDA path, called through the C ABI, against the oracle on the same
 seeded inputs -- bit-exact (integer arithmetic).  Covers K1-K5 of SURVEY.md section 2."""
+import ctypes as C
+
 import numpy as np
 import pytest
 import oracle_py as O
@@ -67,6 +69,78 @@ def test_mle_argument_errors(gpu):
     assert "MLE size does not match the point" in str(e.value)
     with pytest.raises(gpu.DpError):
         gpu.Mle.upload(np.arange(6, dtype=np.uint64), False)
+
+
+def _pts(n):
+    return np.ascontiguousarray(O.splitmix_e(3 + n, n).reshape(-1))
+
+
+def _mle8(gpu):
+    return gpu.Mle.upload(np.arange(8, dtype=np.uint64), False)
+
+
+def _out():
+    return C.byref(C.c_void_p())
+
+
+def _upload(gpu, n):
+    v = np.arange(n, dtype=np.uint64)
+    return gpu.lib().dp_mle_upload(v.ctypes.data_as(C.c_void_p), n, 0, _out())
+
+
+def _wrap(gpu, offset, n):
+    m = _mle8(gpu)
+    return gpu.lib().dp_mle_wrap_device(C.c_void_p(gpu.lib().dp_mle_device_ptr(m.h) + offset), n, 0, _out())
+
+
+def _fix_high(gpu):
+    m, p = _mle8(gpu), _pts(4)
+    return gpu.lib().dp_mle_fix_high(m.h, p.ctypes.data_as(C.c_void_p), 4)
+
+
+def _fix_high_new(gpu):
+    m, p = _mle8(gpu), _pts(4)
+    return gpu.lib().dp_mle_fix_high_new(m.h, p.ctypes.data_as(C.c_void_p), C.c_uint32(4), _out())
+
+
+def _fix_low(gpu):
+    m, p = _mle8(gpu), _pts(4)
+    return gpu.lib().dp_mle_fix_low(m.h, p.ctypes.data_as(C.c_void_p), 4, _out())
+
+
+def _evaluate(gpu):
+    m, p, out = _mle8(gpu), _pts(2), np.zeros(2, dtype=np.uint64)
+    return gpu.lib().dp_mle_evaluate(m.h, p.ctypes.data_as(C.c_void_p), 2, out.ctypes.data_as(C.c_void_p))
+
+
+def _eq_build(gpu, nv):
+    p = _pts(nv)
+    return gpu.lib().dp_eq_build(p.ctypes.data_as(C.c_void_p), nv, _out())
+
+
+MLE_REFUSALS = {   # case -> (call, dp_last_error text); every one returns DP_ERR_INVALID
+    "upload of 6 values": (lambda g: _upload(g, 6), "dp_mle_upload: len must be a power of two"),
+    "wrap a misaligned pointer": (lambda g: _wrap(g, 8, 4), "dp_mle_wrap_device: pointer must be 16-byte aligned"),
+    "wrap 6 values": (lambda g: _wrap(g, 0, 6), "dp_mle_wrap_device: len must be a power of two"),
+    "fix_high k > num_vars": (_fix_high, "invalid size of partial point"),
+    "fix_high_new k > num_vars": (_fix_high_new, "invalid size of partial point"),
+    "fix_low k > num_vars": (_fix_low, "invalid size of partial point"),
+    "evaluate with the wrong num_vars": (_evaluate, "MLE size does not match the point"),
+    "eq table of 33 variables": (lambda g: _eq_build(g, 33), "dp_eq_build: num_vars > 32"),
+}
+
+
+@pytest.mark.parametrize("case", list(MLE_REFUSALS))
+def test_mle_abi_refusal(gpu, case):
+    """each refusal returns DP_ERR_INVALID and its message, and the context it happened in still folds and evaluates like the oracle"""
+    call, text = MLE_REFUSALS[case]
+    assert call(gpu) == gpu.DP_ERR_INVALID
+    assert gpu.lib().dp_last_error().decode() == text
+    f, hi, pt = O.splitmix_e(660, 1 << 12), O.splitmix_e(661, 5), O.splitmix_e(662, 7)
+    m = gpu.Mle.upload(f, True).fix_high(hi)
+    folded = O.fix_high(f, True, hi)
+    assert (m.download() == folded).all()
+    assert (m.evaluate(pt) == O.evaluate(folded, True, pt)).all()
 
 
 SHAPES = [

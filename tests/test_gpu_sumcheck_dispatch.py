@@ -30,7 +30,7 @@ SC_RES_MAXCTA = 8           # :441
 SC_RES_MAXP = 48            # :441
 SC_RES_MAXM = 96            # :441
 COUNTER_POOL_BYTES = 256    # :832  tick counters (n_products + 1 u32) come from a pooled 256-byte block when they fit
-H100_SMS = 132              # common.cuh:14 default; on the device the real count is read from torch
+H100_SMS = 132              # common.cuh:15 default; on the device the real count is read from torch
 # sumcheck.cu:705-706: the tail disables itself under tools that serialise launches
 INJECTION_VARS = ("CUDA_INJECTION64_PATH", "CUDA_INJECTION32_PATH", "NV_NSIGHT_INJECTION_TRANSPORT_TYPE",
                   "NV_NSIGHT_INJECTION_PORT_BASE", "NV_COMPUTE_PROFILER_PERFWORKS_DIR")
@@ -39,7 +39,7 @@ LEAN_PROFILE_NAME = {"B": "k_sc_lean(msg, Base)", "E": "k_sc_lean(msg, Ext)", "B
                      "EF": "k_sc_lean(fold Ext + msg)"}
 
 
-def _grid_for(work, threads, max_ctas_per_sm, sm_count):          # common.cuh:101-106
+def _grid_for(work, threads, max_ctas_per_sm, sm_count):          # common.cuh:120-125
     return int(max(1, min((work + threads - 1) // threads, sm_count * max_ctas_per_sm)))
 
 

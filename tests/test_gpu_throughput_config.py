@@ -19,7 +19,7 @@ Several device paths exist only in that configuration:
 
 The ticket ring (basefold.cu:365-379, MK_TICKETS = 4096 counters handed out round robin) is safe only while fewer than 4096
 k_merkle_small launches lie between one launch's enqueue and its completion.  A proof commits about 38 witness trees per
-dp_pcs_commit_many call (basefold.cu:972) and its thread waits for the call to finish, so 48 proofs in flight hold at most
+dp_pcs_commit_many call (basefold.cu:964) and its thread waits for the call to finish, so 48 proofs in flight hold at most
 about 48 x 38 = 1.8 k launches: a margin of about 2x.  Nothing here tries to provoke a collision.
 """
 import ctypes as C

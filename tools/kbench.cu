@@ -157,18 +157,12 @@ __global__ void k_chain_x8(u64 *io, int len) {   // 8 lanes per hash: hash h = t
 // =====================================================================================================================
 // Sumcheck round candidates (degree 3, one product of three MLEs)
 // =====================================================================================================================
-// 192-bit lazy accumulator of raw 128-bit products: one reduction per thread per evaluation point instead of one per product
-struct acc192 { u64 lo, hi; u32 top; };
-__device__ __forceinline__ void acc_mac(acc192 &a, u64 x, u64 y) {
-    u64 pl = x * y, ph = __umul64hi(x, y);
-    asm("{\n\tadd.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u32 %2, %2, 0;\n\t}" : "+l"(a.lo), "+l"(a.hi), "+r"(a.top) : "l"(pl), "l"(ph));
-}
-__device__ __forceinline__ u64 acc_reduce(const acc192 &a) { return gl_reduce160(a.lo, a.hi, a.top); }
+// gl_acc (gl.cuh): one reduction per thread per evaluation point instead of one per product
 
 // all-Base first round: message only.  PPT pairs in flight per thread (3 * PPT independent 16-byte loads).
 template <int PPT, int BLOCK, int MINB>
 __global__ void __launch_bounds__(BLOCK, MINB) k_scb3(const u64 *__restrict__ f0, const u64 *__restrict__ f1, const u64 *__restrict__ f2, u64 npairs, u64 *__restrict__ partials) {
-    acc192 a[4];
+    gl_acc a[4];
 #pragma unroll
     for (int t = 0; t < 4; t++) { a[t].lo = 0; a[t].hi = 0; a[t].top = 0; }
     const u64 T = (u64)gridDim.x * BLOCK;
@@ -186,7 +180,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_scb3(const u64 *__restrict__ f0
             const u64 s0 = gl_sub(v[p][0].y, c0), s1 = gl_sub(v[p][1].y, c1), s2 = gl_sub(v[p][2].y, c2);
 #pragma unroll
             for (int t = 0; t < 4; t++) {
-                acc_mac(a[t], w_mul(c0, c1), c2);
+                gl_acc_mac(a[t], w_mul(c0, c1), c2);
                 if (t < 3) { c0 = gl_add(c0, s0); c1 = gl_add(c1, s1); c2 = gl_add(c2, s2); }
             }
         }
@@ -194,7 +188,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_scb3(const u64 *__restrict__ f0
     __shared__ u64 ws[BLOCK / 32][4];
 #pragma unroll
     for (int t = 0; t < 4; t++) {
-        u64 v = acc_reduce(a[t]);
+        u64 v = gl_acc_reduce(a[t]);
         for (int d = 16; d > 0; d >>= 1) v = gl_add(v, __shfl_down_sync(0xffffffffu, v, d));
         if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5][t] = v;
     }
@@ -263,7 +257,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_scb3_tma(const u64 *__restrict_
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    acc192 a[4];
+    gl_acc a[4];
 #pragma unroll
     for (int t = 0; t < 4; t++) { a[t].lo = 0; a[t].hi = 0; a[t].top = 0; }
     // tiles of this block: blockIdx.x, blockIdx.x + gridDim.x, ...
@@ -289,7 +283,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_scb3_tma(const u64 *__restrict_
             const u64 s0 = gl_sub(v0.y, c0), s1 = gl_sub(v1.y, c1), s2 = gl_sub(v2.y, c2);
 #pragma unroll
             for (int t = 0; t < 4; t++) {
-                acc_mac(a[t], w_mul(c0, c1), c2);
+                gl_acc_mac(a[t], w_mul(c0, c1), c2);
                 if (t < 3) { c0 = gl_add(c0, s0); c1 = gl_add(c1, s1); c2 = gl_add(c2, s2); }
             }
         }
@@ -300,7 +294,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_scb3_tma(const u64 *__restrict_
     __shared__ u64 ws[BLOCK / 32][4];
 #pragma unroll
     for (int t = 0; t < 4; t++) {
-        u64 v = acc_reduce(a[t]);
+        u64 v = gl_acc_reduce(a[t]);
         for (int d = 16; d > 0; d >>= 1) v = gl_add(v, __shfl_down_sync(0xffffffffu, v, d));
         if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5][t] = v;
     }
@@ -311,11 +305,11 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_scb3_tma(const u64 *__restrict_
 // ---- round 2 of a Base polynomial: fold by r (Base -> Ext), write the half-size Ext tables, message from the folded pairs ----
 __device__ __forceinline__ gle kfold_b(u64 a, u64 b, gle r) { return e_add(e_mul_base(r, gl_sub(b, a)), e_from_base(a)); }
 // Ext lazy accumulation: both limbs of a product as 160-bit sums (c1 = a0 b1 + a1 b0; c0 = a0 b0 + 7 w, w = weak(a1 b1))
-struct eacc { acc192 c0, c1; };
+struct eacc { gl_acc c0, c1; };
 __device__ __forceinline__ void eacc_mac(eacc &a, gle x, gle y) {
-    acc_mac(a.c1, x.c0, y.c1); acc_mac(a.c1, x.c1, y.c0);
+    gl_acc_mac(a.c1, x.c0, y.c1); gl_acc_mac(a.c1, x.c1, y.c0);
     u64 w = gl_reduce128_weak(x.c1 * y.c1, __umul64hi(x.c1, y.c1));
-    acc_mac(a.c0, x.c0, y.c0); acc_mac(a.c0, w, 7ULL);
+    gl_acc_mac(a.c0, x.c0, y.c0); gl_acc_mac(a.c0, w, 7ULL);
 }
 template <int PPT, int BLOCK, int MINB, bool LAZY>
 __global__ void __launch_bounds__(BLOCK, MINB) k_scf3(const u64 *__restrict__ f0, const u64 *__restrict__ f1, const u64 *__restrict__ f2, gle r,
@@ -355,7 +349,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_scf3(const u64 *__restrict__ f0
     __shared__ gle ws[BLOCK / 32][4];
 #pragma unroll
     for (int t = 0; t < 4; t++) {
-        gle v = LAZY ? e_make(acc_reduce(la[t].c0), acc_reduce(la[t].c1)) : ca[t];
+        gle v = LAZY ? e_make(gl_acc_reduce(la[t].c0), gl_acc_reduce(la[t].c1)) : ca[t];
         for (int d = 16; d > 0; d >>= 1) v = e_add(v, shfl_down_e(v, d));
         if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5][t] = v;
     }
@@ -395,7 +389,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_sce3(const gle *__restrict__ f0
     __shared__ gle ws[BLOCK / 32][4];
 #pragma unroll
     for (int t = 0; t < 4; t++) {
-        gle v = LAZY ? e_make(acc_reduce(la[t].c0), acc_reduce(la[t].c1)) : ca[t];
+        gle v = LAZY ? e_make(gl_acc_reduce(la[t].c0), gl_acc_reduce(la[t].c1)) : ca[t];
         for (int d = 16; d > 0; d >>= 1) v = e_add(v, shfl_down_e(v, d));
         if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5][t] = v;
     }
