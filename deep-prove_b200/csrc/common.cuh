@@ -96,6 +96,14 @@ struct dp_mle {
     size_t bytes() const { return (size_t)len * (is_ext ? 16 : 8); }
 };
 
+// LogUp-GKR circuit (logup.cu); its small layers are also proved by the resident sumcheck kernel (sumcheck.cu)
+struct dp_logup {
+    bool table = false; u32 nv = 0;            // layer 0 has 2^nv entries
+    std::vector<gle *> num, den;               // per layer; num[0] == nullptr for a lookup circuit
+    gle *block = nullptr;
+    u64 *h_out = nullptr;                      // mapped pinned: outputs + completion word written by k_logup_tail
+};
+
 // Owning handles for objects under construction: an error return releases whatever has been built so far.
 template <auto Free> struct FreeWith { template <typename P> void operator()(P *p) const { Free(p); } };
 using MlePtr = std::unique_ptr<dp_mle, FreeWith<dp_mle_free>>;

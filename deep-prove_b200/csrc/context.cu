@@ -11,6 +11,7 @@ static thread_local DpCtx g_ctx;
 DpCtx &dp_ctx() { return g_ctx; }
 static std::atomic<unsigned long long> g_total_launches{0};
 void dp_count_launch() { g_total_launches.fetch_add(1, std::memory_order_relaxed); }
+static std::atomic<unsigned long long> g_host_waits{0};
 int dp_fail(int code, const std::string &s) { g_err = s; return code; }
 
 // ---- per-thread device arena -------------------------------------------------------------------------
@@ -177,6 +178,7 @@ static void poller_main() {
     }
 }
 u64 dp_wait_flag(volatile u64 *flag, u64 want, bool has_fail, u64 fail, double timeout_s) {
+    g_host_waits.fetch_add(1, std::memory_order_relaxed);
     // a result that is already there (or lands within a microsecond) never pays for a sleep
     for (int k = 0; k < 64; k++) { const u64 v = *flag; if (v == want || (has_fail && v == fail)) return v; __builtin_ia32_pause(); }
     const auto t_start = std::chrono::steady_clock::now();
@@ -239,7 +241,7 @@ u64 dp_wait_flag(volatile u64 *flag, u64 want, bool has_fail, u64 fail, double t
 }
 __global__ void k_signal(u64 *flag, u64 seq) { __threadfence_system(); *(volatile u64 *)flag = seq; }
 cudaError_t dp_stream_sync(cudaStream_t st) {
-    if (dp_wait_mode() == DP_WAIT_SPIN) return cudaStreamSynchronize(st);
+    if (dp_wait_mode() == DP_WAIT_SPIN) { g_host_waits.fetch_add(1, std::memory_order_relaxed); return cudaStreamSynchronize(st); }
     DpCtx &c = g_ctx;
     if (!c.sync_flag) { void *p = nullptr; if (dp_pinned_alloc(&p, 64) != DP_OK) return cudaErrorMemoryAllocation; c.sync_flag = (u64 *)p; *c.sync_flag = 0; c.sync_seq = 0; }
     const u64 seq = ++c.sync_seq;
@@ -424,5 +426,6 @@ int dp_synchronize(void) {
 
 // launches of the calling thread's context + those folded in by threads that have shut down
 uint64_t dp_kernel_launches(void) { return g_total_launches.load(); }   // process-wide, all host threads
+uint64_t dp_host_waits(void) { return g_host_waits.load(); }             // process-wide, all host threads
 
 }  // extern "C"

@@ -70,13 +70,6 @@ __global__ void k_lincomb(LinArg a, u64 len, gle *__restrict__ out) {
     }
 }
 
-struct dp_logup {
-    bool table = false; u32 nv = 0;            // layer 0 has 2^nv entries
-    std::vector<gle *> num, den;               // per layer; num[0] == nullptr for a lookup circuit
-    gle *block = nullptr;
-    u64 *h_out = nullptr;                      // mapped pinned: outputs + completion word written by k_logup_tail
-};
-
 extern "C" {
 
 // LogUpCircuit::new_lookup_circuit (multiplicities == NULL) / new_table_circuit

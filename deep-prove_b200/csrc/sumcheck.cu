@@ -527,46 +527,42 @@ __device__ __noinline__ void sc_res_fs_round(ScTailFs &f, gle (*sprod)[SC_NACC],
     }
 }
 
-template <int DSEL>
-__global__ void __launch_bounds__(SC_THREADS)
-k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pairs /* mapped */, volatile u64 *flag /* mapped */,
-         volatile u64 *chal /* mapped: [seq, c0, c1] */, u64 seq0, gle *xpart /* device: warp partials */, u64 *xctl /* device: [status, c0, c1] */,
-         ScTailFsOut *fsout /* mapped; null: the host runs the transcript between rounds */) {
-    __shared__ ScMle sm[SC_RES_MAXM];
-    __shared__ TProd sp[SC_RES_MAXP];
-    __shared__ ScProd spd[SC_RES_MAXP];
-    __shared__ gle *sdst[SC_RES_MAXM];
-    __shared__ u32 swriter[SC_RES_MAXM];
-    __shared__ unsigned char sfold[SC_RES_MAXM];
-    __shared__ gle sprod[SC_RES_MAXP][SC_NACC];                       // device transcript: each product's sums
-    __shared__ ScTailFs sfs;
-    const u32 nm = cfg->n_mles, np = cfg->n_products, nr = cfg->n_rounds;
+// Shared-memory round state of the resident kernels (every CTA keeps its own copy of the bookkeeping)
+struct ScResSmem {
+    ScMle sm[SC_RES_MAXM]; TProd sp[SC_RES_MAXP]; ScProd spd[SC_RES_MAXP]; gle *sdst[SC_RES_MAXM]; u32 swriter[SC_RES_MAXM];
+    unsigned char sfold[SC_RES_MAXM];
+    gle sprod[SC_RES_MAXP][SC_NACC];                                   // device transcript: each product's sums
+    ScTailFs sfs;
+};
+
+// The rounds of one sumcheck on the cluster, from the bookkeeping in S (nm MLEs, np products, nr rounds; first_fold: round 0 folds
+// by r first).  Returns early when the host aborted the tail or a challenge never came.  After the last round the tables' pairs go to
+// `pairs` and the flag is raised -- unless CHAIN (one of several sumchecks in a launch, device transcript): then every CTA records
+// the challenges of rounds 0 .. nr - 2 in schal (shared) and the caller does what follows the last round.
+template <int DSEL, bool CHAIN>
+__device__ __forceinline__ void sc_res_rounds(ScResSmem &S, const u32 nm, const u32 np, const u32 nr, const bool first_fold, gle r,
+                                              gle *out, gle *pairs, volatile u64 *flag, volatile u64 *chal, u64 seq0, gle *xpart, u64 *xctl,
+                                              ScTailFsOut *fsout, gle *schal) {
     const bool fs = fsout != nullptr;
     const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = SC_THREADS / 32;
     const u32 rank = cl_rank(), ncta = cl_size();
     const u32 W = ncta * nwarps, gw = rank * nwarps + warp;              // warps of the cluster, this warp's index
     // pairs of a product are split over G warps (G a power of two, np * G <= W); with more products than warps a warp takes several
     u32 G = 1; while (np * (G << 1) <= W) G <<= 1;
-    for (u32 i = threadIdx.x; i < nm; i += blockDim.x) { sm[i] = cfg->m[i]; swriter[i] = cfg->writer[i]; }
-    for (u32 i = threadIdx.x; i < np; i += blockDim.x) sp[i] = cfg->p[i];
-    if (fs && rank == 0)
-        for (u32 i = threadIdx.x; i < sizeof(ScTailFs) / 8; i += blockDim.x) ((u64 *)&sfs)[i] = ((const u64 *)&cfg->fs)[i];
-    __syncthreads();
-    gle r = r0;
     // The descriptors of a round depend on the fold bookkeeping only, never on the challenge VALUE: they are rebuilt right after a
     // round's message has been signalled, i.e. in the shadow of the host's Fiat-Shamir, which keeps ~2.2 us per round off the path
     // from the challenge's arrival to the first load.
     auto build_descs = [&](const bool fold) {
         for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
-            bool f = fold && sm[i].len > 1;
-            sfold[i] = f;
-            sdst[i] = f ? sc_fold_dst(sm[i]) : nullptr;
+            bool f = fold && S.sm[i].len > 1;
+            S.sfold[i] = f;
+            S.sdst[i] = f ? sc_fold_dst(S.sm[i]) : nullptr;
         }
         __syncthreads();
-        for (u32 p = threadIdx.x; p < np; p += blockDim.x) sc_desc(spd[p], p, sp[p].idx, sp[p].n_idx, sm, sfold, sdst, swriter);
+        for (u32 p = threadIdx.x; p < np; p += blockDim.x) sc_desc(S.spd[p], p, S.sp[p].idx, S.sp[p].n_idx, S.sm, S.sfold, S.sdst, S.swriter);
         __syncthreads();
     };
-    build_descs(cfg->first_has_challenge != 0);
+    build_descs(first_fold);
     for (u32 k = 0; k < nr; k++) {
         const u64 seq = seq0 + k;
         if (k > 0) {   // wait for the host's challenge for this round (device transcript: CTA 0 posted it to xctl last round)
@@ -584,11 +580,12 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
             const u64 status = __ldcg(xctl);
             if (status) { if (rank == 0 && threadIdx.x == 0 && status == 2) { __threadfence_system(); *flag = SC_TAIL_FAILED; } return; }   // uniform over the cluster
             r = e_make(__ldcg(xctl + 1), __ldcg(xctl + 2));
+            if (CHAIN && threadIdx.x == 0) schal[k - 1] = r;
         }
         // work: slot (p, s) = sub-slice s of product p's pairs; warp gw owns slots gw, gw + W, ...
         for (u32 slot = gw; slot < np * G; slot += W) {
             const u32 p = slot / G, s = slot % G;
-            const ScProd &pd = spd[p];
+            const ScProd &pd = S.spd[p];
             gle acc[SC_NACC];
 #pragma unroll
             for (int t = 0; t < SC_NACC; t++) acc[t] = e_zero();
@@ -607,14 +604,14 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
         }
         cl_sync();                                             // warp partials and folded tables of every CTA are visible
         if (rank == 0) {                                       // the message first: it is what the host is waiting for
-            gle *const mout = fs ? &sprod[0][0] : out;
+            gle *const mout = fs ? &S.sprod[0][0] : out;
             // few partials per (product, point): one THREAD each (many products run side by side); many (a single product spread over
             // >= 32 warps): one WARP each, its lanes gather the partials with independent L2 loads -- faster for a single wide product,
             // while the warp form slows the 6-product LogUp shape
             if (G < 32) {
                 for (u32 x = threadIdx.x; x < np * SC_NACC; x += blockDim.x) {
                     const u32 p = x / SC_NACC, t = x % SC_NACC;
-                    if (t > spd[p].d) continue;
+                    if (t > S.spd[p].d) continue;
                     gle v = e_zero();
                     for (u32 s = 0; s < G; s++) { ulonglong2 q = __ldcg(reinterpret_cast<const ulonglong2 *>(xpart + ((u64)p * G + s) * SC_NACC + t)); v = e_add(v, e_make(q.x, q.y)); }
                     st_e(mout + (u64)p * SC_NACC + t, v);
@@ -622,20 +619,20 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
             } else
             for (u32 x = warp; x < np * SC_NACC; x += nwarps) {
                 const u32 p = x / SC_NACC, t = x % SC_NACC;
-                if (t > spd[p].d) continue;                    // warp-uniform
+                if (t > S.spd[p].d) continue;                  // warp-uniform
                 wsum96 v0 = {0, 0}, v1 = {0, 0};
                 for (u32 s = lane; s < G; s += 32) { ulonglong2 q = __ldcg(reinterpret_cast<const ulonglong2 *>(xpart + ((u64)p * G + s) * SC_NACC + t)); ws_add(v0, q.x, 0); ws_add(v1, q.y, 0); }
                 ws_warp_reduce(v0); ws_warp_reduce(v1);
                 if (lane == 0) st_e(mout + (u64)p * SC_NACC + t, e_make(ws_reduce(v0), ws_reduce(v1)));
             }
         }
-        for (u32 i = threadIdx.x; i < nm; i += blockDim.x) if (sfold[i]) sc_commit_fold(sm[i], sdst[i]);   // every CTA keeps its own copy
+        for (u32 i = threadIdx.x; i < nm; i += blockDim.x) if (S.sfold[i]) sc_commit_fold(S.sm[i], S.sdst[i]);   // every CTA keeps its own copy
         __syncthreads();
-        if (rank == 0 && fs) sc_res_fs_round(sfs, sprod, sp, sm, np, k, k == nr - 1, fsout, xctl);
-        if (rank == 0) {
+        if (rank == 0 && fs) sc_res_fs_round(S.sfs, S.sprod, S.sp, S.sm, np, k, k == nr - 1, fsout, xctl);
+        if (rank == 0 && !CHAIN) {
             if (k == nr - 1) {   // last round: hand the (<= 2)-entry tables over with the message (k_sc_gather's job)
                 for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
-                    const ScMle &m = sm[i]; gle a, b;
+                    const ScMle &m = S.sm[i]; gle a, b;
                     if (m.is_ext) { a = ldx_e<true>((const gle *)m.cur); b = m.len > 1 ? ldx_e<true>((const gle *)m.cur + 1) : a; }
                     else { a = e_from_base(ldx_b<true>((const u64 *)m.cur)); b = m.len > 1 ? e_from_base(ldx_b<true>((const u64 *)m.cur + 1)) : a; }
                     st_e(pairs + 2 * i, a); st_e(pairs + 2 * i + 1, b);
@@ -646,6 +643,170 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
         }
         if (k + 1 < nr) build_descs(true);                     // next round's descriptors while the host hashes
         // CTAs other than 0 run ahead to the next cluster barrier; xpart is not rewritten before it (the work phase follows it)
+    }
+}
+
+template <int DSEL>
+__global__ void __launch_bounds__(SC_THREADS)
+k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pairs /* mapped */, volatile u64 *flag /* mapped */,
+         volatile u64 *chal /* mapped: [seq, c0, c1] */, u64 seq0, gle *xpart /* device: warp partials */, u64 *xctl /* device: [status, c0, c1] */,
+         ScTailFsOut *fsout /* mapped; null: the host runs the transcript between rounds */) {
+    __shared__ ScResSmem S;
+    const u32 nm = cfg->n_mles, np = cfg->n_products, nr = cfg->n_rounds;
+    const u32 rank = cl_rank();
+    for (u32 i = threadIdx.x; i < nm; i += blockDim.x) { S.sm[i] = cfg->m[i]; S.swriter[i] = cfg->writer[i]; }
+    for (u32 i = threadIdx.x; i < np; i += blockDim.x) S.sp[i] = cfg->p[i];
+    if (fsout && rank == 0)
+        for (u32 i = threadIdx.x; i < sizeof(ScTailFs) / 8; i += blockDim.x) ((u64 *)&S.sfs)[i] = ((const u64 *)&cfg->fs)[i];
+    __syncthreads();
+    sc_res_rounds<DSEL, false>(S, nm, np, nr, cfg->first_has_challenge != 0, r0, out, pairs, flag, chal, seq0, xpart, xctl, fsout, nullptr);
+}
+
+// ---- the small layers of a LogUp-GKR batch, back to back in ONE resident launch (dp_logup_run_layers_fs) --------------------------
+// logup_gkr::prover::batch_prove (prover.rs:24-237) layer by layer, with BasicTranscript on the device: per layer CTA 0 absorbs the
+// claim, num_vars and the degree (prove_parallel), every CTA builds its slice of the layer's eq table from the point and the layer's
+// bookkeeping (the products of zkml.hpp's logup_batch_prove), the rounds run through sc_res_rounds, and CTA 0 folds the final
+// evaluations, squeezes logup_batching / logup_alpha / logup_lambda and forms the next claim and point.  The host sleeps once per call
+// instead of once per layer, and no eq table, sumcheck handle or launch is made per layer.
+static constexpr u32 LG_MAXC = 16, LG_MAXL = 12;
+struct LgCfg {
+    u32 n_circuits, first, n_layers, pad;
+    gle claim, alpha, lambda;
+    gle point[SC_MAX_ROUNDS + 1];                                  // layer `first`'s point (its last entry is the batching challenge)
+    const gle *num[LG_MAXL][LG_MAXC], *den[LG_MAXL][LG_MAXC];     // layer first + l of circuit c: [lo | hi]; num null: numerators all -1
+    gle *eq, *work; u64 work_stride;                               // device scratch: the eq table, each MLE's ping-pong tables
+    u64 round_label[2], label[3][2];                               // "Internal round"; "logup_batching", "logup_alpha", "logup_lambda"
+    u64 bary[4][4][5]; u64 sponge[P2S_WORDS];
+};
+struct LgLayerOut { ScTailFsOut fs; gle evals[SC_RES_MAXM]; };
+struct LgOut { LgLayerOut layer[LG_MAXL]; gle point[SC_MAX_ROUNDS + 1]; gle claim, alpha, lambda; u64 sponge[P2S_WORDS]; u64 flag; };
+
+// state of the layer loop in shared memory: kept out of registers across the rounds, which need all of theirs
+struct LgSmem { gle pt[SC_MAX_ROUNDS + 1], fe[SC_RES_MAXM], claim, alpha, lambda, batching; u32 v, nm, per, two; };
+
+// layer l's start: its transcript prefix and coefficients (CTA 0), eq table slice and bookkeeping (every CTA)
+__device__ __noinline__ void lg_layer_begin(const LgCfg *cfg, ScResSmem &S, LgSmem &L, const u32 l, const gle *xpoint) {
+    const u32 rank = cl_rank(), ncta = cl_size(), nc = cfg->n_circuits, np = 3 * nc;
+    const u32 v = cfg->first + l;
+    const u64 half = 1ULL << v;
+    const bool two = cfg->num[l][0] == nullptr;                    // the lookup circuit's first layer: views [den_lo, den_hi]
+    const u32 per = two ? 2 : 4, nm = 1 + per * nc;
+    for (u32 i = threadIdx.x; i < v; i += blockDim.x) L.pt[i] = l == 0 ? cfg->point[i] : ldx_e<true>(xpoint + i);
+    if (rank == 0) {
+        for (u32 p = threadIdx.x; p < np; p += blockDim.x) {       // coefficients: alpha^c x (1, 1, lambda), or (-1, -1, lambda)
+            gle cur = e_one();
+            for (u32 c = 0; c < p / 3; c++) cur = e_mul_ni(cur, L.alpha);
+            const gle cf = p % 3 == 2 ? e_mul_ni(cur, L.lambda) : two ? e_neg(cur) : cur;
+            S.sfs.coef[p][0] = cf.c0; S.sfs.coef[p][1] = cf.c1;
+        }
+        if (threadIdx.x < 32) {                                    // t.append_field_element_ext(claim); append_usize(nv); append_usize(deg)
+            const int l8 = threadIdx.x & 7;
+            P2Sponge sp; p2s_load(sp, S.sfs.sponge, l8);
+            p2s_observe(sp, L.claim.c0, l8); p2s_observe(sp, L.claim.c1, l8); p2s_observe(sp, v, l8); p2s_observe(sp, 3, l8);
+            __syncwarp();
+            if (threadIdx.x < 8) p2s_store(sp, S.sfs.sponge, l8);
+        }
+        if (threadIdx.x == 0) S.sfs.max_nv = v;
+    }
+    if (threadIdx.x == 0) { L.v = v; L.nm = nm; L.per = per; L.two = two; }
+    __syncthreads();
+    for (u64 x = (u64)rank * blockDim.x + threadIdx.x; x < half; x += (u64)ncta * blockDim.x) {   // build_eq_x_r(point)
+        gle p = e_one();
+        for (u32 b = 0; b < v; b++) p = e_mul_ni(p, ((x >> b) & 1) ? L.pt[b] : e_sub(e_one(), L.pt[b]));
+        __stcg(reinterpret_cast<ulonglong2 *>(cfg->eq + x), make_ulonglong2(p.c0, p.c1));
+    }
+    // MLE order of VirtualPolynomial::add_mle_list: eq, then per circuit its views in first use, [num_lo, den_hi, num_hi, den_lo]
+    // ([den_hi, den_lo] with two views); writer = the first product using the MLE
+    for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
+        ScMle m; m.len = m.len0 = half; m.is_ext = 1; m.where = 0; m.work = cfg->work + i * cfg->work_stride;
+        u32 w = 0;
+        if (i == 0) m.cur = cfg->eq;
+        else {
+            const u32 c = (i - 1) / per, j = (i - 1) % per;
+            const gle *nu = cfg->num[l][c], *de = cfg->den[l][c];
+            if (two) { m.cur = j == 0 ? de + half : de; w = 3 * c + j; }
+            else { m.cur = j == 0 ? nu : j == 1 ? de + half : j == 2 ? nu + half : de; w = 3 * c + (j < 2 ? 0 : 1); }
+        }
+        S.sm[i] = m; S.swriter[i] = w;
+    }
+    for (u32 p = threadIdx.x; p < np; p += blockDim.x) {
+        const u32 b = 1 + per * (p / 3), q = p % 3;
+        TProd t = {};
+        if (two) { t.n_idx = q == 2 ? 3 : 2; t.idx[0] = 0; t.idx[1] = q == 0 ? b : b + 1; t.idx[2] = b; }
+        else { t.n_idx = 3; t.idx[0] = 0; t.idx[1] = q == 0 ? b : q == 1 ? b + 2 : b + 3; t.idx[2] = q == 0 ? b + 1 : q == 1 ? b + 3 : b + 1; }
+        S.sp[p] = t;
+    }
+    __syncthreads();
+}
+
+// layer l's end in CTA 0: get_mle_final_evaluations, logup_batching / logup_alpha / logup_lambda, the next claim and point (zkml.hpp)
+__device__ __noinline__ void lg_layer_end(const LgCfg *cfg, LgOut *out, ScResSmem &S, LgSmem &L, const u32 l, const u64 *xctl, gle *xpoint) {
+    const u32 v = L.v, nm = L.nm, per = L.per, nc = cfg->n_circuits;
+    const bool two = L.two;
+    const gle rl = e_make(__ldcg(xctl + 1), __ldcg(xctl + 2));    // the last round's challenge
+    for (u32 i = 1 + threadIdx.x; i < nm; i += blockDim.x) {
+        const gle *t = (const gle *)S.sm[i].cur, a = ldx_e<true>(t), b = ldx_e<true>(t + 1);
+        const gle f = e_add(a, e_mul_ni(e_sub(b, a), rl));
+        L.fe[i] = f; st_e(&out->layer[l].evals[i - 1], f);
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const int l8 = threadIdx.x & 7;
+        P2Sponge sp; p2s_load(sp, S.sfs.sponge, l8);
+        gle ch[3];
+        for (int q = 0; q < 3; q++) {
+            p2s_observe(sp, cfg->label[q][0], l8); p2s_observe(sp, cfg->label[q][1], l8);
+            const u64 c0 = p2s_sample(sp, l8), c1 = p2s_sample(sp, l8);
+            ch[q] = e_make(c0, c1);
+        }
+        __syncwarp();
+        if (threadIdx.x < 8) p2s_store(sp, S.sfs.sponge, l8);
+        if (threadIdx.x == 0) {
+            const gle bt = ch[0], al = ch[1], lm = ch[2];
+            gle acc = e_zero(), a = e_one();
+            for (u32 c = 0; c < nc; c++) {
+                const gle *e = &L.fe[1 + per * c];
+                const gle term = two ? e_add(e_mul_ni(bt, e_sub(e[0], e[1])), e[1])
+                                     : e_add(e_add(e_mul_ni(bt, e_sub(e[2], e[0])), e[0]), e_mul_ni(lm, e_add(e_mul_ni(bt, e_sub(e[1], e[3])), e[3])));
+                acc = e_add(acc, e_mul_ni(a, term)); a = e_mul_ni(a, al);
+            }
+            L.claim = acc; L.batching = bt; L.alpha = al; L.lambda = lm;
+            L.pt[v - 1] = rl;                                      // rounds 0 .. v - 2 recorded theirs
+        }
+    }
+    __syncthreads();
+    const bool last = l + 1 == cfg->n_layers;
+    for (u32 i = threadIdx.x; i <= v; i += blockDim.x) {           // point = sumcheck challenges || batching
+        const gle x = i < v ? L.pt[i] : L.batching;
+        __stcg(reinterpret_cast<ulonglong2 *>(xpoint + i), make_ulonglong2(x.c0, x.c1));
+        if (last) st_e(&out->point[i], x);
+    }
+    if (last) {
+        for (u32 i = threadIdx.x; i < P2S_WORDS; i += blockDim.x) out->sponge[i] = S.sfs.sponge[i];
+        if (threadIdx.x == 0) { st_e(&out->claim, L.claim); st_e(&out->alpha, L.alpha); st_e(&out->lambda, L.lambda); }
+        __syncthreads();
+        if (threadIdx.x == 0) { __threadfence_system(); *(volatile u64 *)&out->flag = 1; }
+    }
+}
+
+__global__ void __launch_bounds__(SC_THREADS)
+k_logup_res(const LgCfg *__restrict__ cfg, LgOut *out /* mapped */, gle *xpart, u64 *xctl, gle *xpoint /* device */) {
+    __shared__ ScResSmem S;
+    __shared__ LgSmem L;
+    if (cl_rank() == 0) {
+        if (threadIdx.x == 0) {
+            L.alpha = cfg->alpha; L.lambda = cfg->lambda; L.claim = cfg->claim;
+            S.sfs.label[0] = cfg->round_label[0]; S.sfs.label[1] = cfg->round_label[1]; S.sfs.max_deg = 3; S.sfs.round0 = 0;
+        }
+        for (u32 i = threadIdx.x; i < P2S_WORDS; i += blockDim.x) S.sfs.sponge[i] = cfg->sponge[i];
+        for (u32 i = threadIdx.x; i < 4 * 4 * 5; i += blockDim.x) (&S.sfs.bary[0][0][0])[i] = (&cfg->bary[0][0][0])[i];
+    }
+    for (u32 l = 0; l < cfg->n_layers; l++) {
+        lg_layer_begin(cfg, S, L, l, xpoint);
+        cl_sync();                                                 // the eq table of every CTA is visible
+        sc_res_rounds<0, true>(S, L.nm, 3 * cfg->n_circuits, L.v, false, e_zero(), nullptr, nullptr, nullptr, nullptr, 0, xpart, xctl, &out->layer[l].fs, L.pt);
+        if (cl_rank() == 0) { __syncthreads(); lg_layer_end(cfg, out, S, L, l, xctl, xpoint); }
+        cl_sync();                                                 // the next point is visible; every read of this layer's tables is done
     }
 }
 
@@ -844,6 +1005,31 @@ static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
     if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(st); DP_CHECK(false, DP_ERR_CUDA, "dp_sc_round: resident kernel timed out waiting for a challenge (other work queued in the same stream?)"); }
     if (s->round == s->max_nv) s->have_pairs = true;   // written to mapped memory before the flag
     return sc_glue(s, out_evals);
+}
+
+// the Poseidon2 constants of this module's copy of the permutation: the transcript's, never those of dp_poseidon2_init
+static cudaError_t sc_fs_constants() {
+    static std::once_flag once; static cudaError_t ce = cudaSuccess;
+    std::call_once(once, [] {
+        cudaStream_t st = dp_ctx().stream;
+        if ((ce = cudaMemcpyToSymbolAsync(c_p2_ext, &DP_P2_EXT_RC[0][0][0], sizeof(u64) * 64, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess &&
+            (ce = cudaMemcpyToSymbolAsync(c_p2_int, DP_P2_INT_RC, sizeof(u64) * 22, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess &&
+            (ce = cudaMemcpyToSymbolAsync(c_p2_diag, DP_P2_DIAG, sizeof(u64) * 8, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess)
+            ce = dp_stream_sync(st);
+    });
+    return ce;
+}
+
+// How many layers from `first` on dp_logup_run_layers_fs takes: blocking waits, a launch that can run resident, at most LG_MAXC equal
+// circuits, and layers whose first round is resident-sized (the same SC_RES_WORK bound as the tail of a single sumcheck).
+static u32 lg_fs_layers(dp_logup *const *c, u32 n, u32 first) {
+    if (dp_wait_mode() != DP_WAIT_BLOCK || !c || n == 0 || n > LG_MAXC || first == 0) return 0;
+    for (u32 i = 0; i < n; i++) if (!c[i] || c[i]->nv != c[0]->nv) return 0;
+    static_assert(1 + 4 * LG_MAXC <= SC_RES_MAXM && 3 * LG_MAXC <= SC_RES_MAXP, "a batch of LG_MAXC circuits fits the resident kernel");
+    const u32 total = c[0]->nv - 1;
+    u32 k = 0;
+    while (first + k <= total && k < LG_MAXL && first + k < SC_MAX_ROUNDS && (u64)3 * n * (1ULL << (first + k - 1)) <= SC_RES_WORK) k++;
+    return k && sc_tail_supported() ? k : 0;
 }
 
 extern "C" {
@@ -1070,17 +1256,7 @@ int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *
     DP_CHECK(fold == (prev_challenge != nullptr), DP_ERR_STATE, fold ? "verifier message is empty" : "first round should be prover first.");
     DP_CHECK(sponge_in[12] < 4 && sponge_in[13] <= 4, DP_ERR_INVALID, "dp_sc_run_tail_fs: sponge state out of range");
     DP_CHECK(sc_tail_eligible(s, fold), DP_ERR_STATE, "dp_sc_run_tail_fs: the next round does not start the resident tail");
-    {   // the Poseidon2 constants of this module's copy of the permutation: the transcript's, never those of dp_poseidon2_init
-        static std::once_flag once; static cudaError_t ce = cudaSuccess;
-        std::call_once(once, [] {
-            cudaStream_t st = dp_ctx().stream;
-            if ((ce = cudaMemcpyToSymbolAsync(c_p2_ext, &DP_P2_EXT_RC[0][0][0], sizeof(u64) * 64, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess &&
-                (ce = cudaMemcpyToSymbolAsync(c_p2_int, DP_P2_INT_RC, sizeof(u64) * 22, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess &&
-                (ce = cudaMemcpyToSymbolAsync(c_p2_diag, DP_P2_DIAG, sizeof(u64) * 8, 0, cudaMemcpyHostToDevice, st)) == cudaSuccess)
-                ce = dp_stream_sync(st);
-        });
-        DP_CUDA(ce);
-    }
+    DP_CUDA(sc_fs_constants());
     gle r = e_zero();
     if (fold) {
         r = e_from_host(prev_challenge);
@@ -1115,6 +1291,85 @@ int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *
         if (k + 1 < nr) s->challenges.push_back(o.chal[k]);     // the last one is dp_sc_finish's
     }
     for (int i = 0; i < P2S_WORDS; i++) sponge_out[i] = o.sponge[i];
+    return DP_OK;
+}
+
+int dp_logup_layers_fs_next(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t *n_layers) {
+    DP_REQUIRE_CTX();
+    DP_CHECK(circuits && n_layers, DP_ERR_INVALID, "dp_logup_layers_fs_next: null argument");
+    *n_layers = lg_fs_layers(circuits, n_circuits, first_layer);
+    return DP_OK;
+}
+
+int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
+                           uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
+                           uint64_t *evals_out) {
+    DP_REQUIRE_CTX();
+    DP_CHECK(circuits && claim && point && alpha && lambda && sponge && msgs_out && challenges_out && evals_out, DP_ERR_INVALID,
+             "dp_logup_run_layers_fs: null argument");
+    DP_CHECK(first_layer >= 1 && last_layer >= first_layer && last_layer - first_layer < lg_fs_layers(circuits, n_circuits, first_layer), DP_ERR_STATE,
+             "dp_logup_run_layers_fs: these layers do not run resident (wait mode, circuit count or layer size)");
+    DP_CHECK(sponge[12] < 4 && sponge[13] <= 4, DP_ERR_INVALID, "dp_logup_run_layers_fs: sponge state out of range");
+    DP_CUDA(sc_fs_constants());
+    const u32 nl = last_layer - first_layer + 1, n = n_circuits, np = 3 * n, nm_max = 1 + 4 * n;
+    const u64 len_max = 1ULL << last_layer, stride = (len_max >> 1) + (len_max >> 2) + 1;
+    const u64 work = (u64)np * (len_max >> 1);
+    u32 ncta = 1; while (ncta < SC_RES_MAXCTA && (u64)ncta * 512 < work) ncta <<= 1;      // sized like sc_tail_launch, by the largest layer
+    const u32 slots = std::max<u32>(ncta * (SC_THREADS / 32), np);
+    LgCfg *cfg = nullptr; LgOut *out = nullptr; char *scratch = nullptr;
+    if (int e = dp_pinned_alloc((void **)&cfg, sizeof(LgCfg))) return e;
+    PinnedPtr cfg_owner(cfg);
+    if (int e = dp_pinned_alloc((void **)&out, sizeof(LgOut))) return e;
+    PinnedPtr out_owner(out);
+    const size_t off_point = 64, off_part = off_point + sizeof(gle) * (SC_MAX_ROUNDS + 1), off_eq = off_part + sizeof(gle) * SC_NACC * slots,
+                 off_work = off_eq + sizeof(gle) * len_max, bytes = off_work + sizeof(gle) * stride * nm_max;
+    if (int e = dp_dev_alloc((void **)&scratch, bytes)) return e;
+    DevPtr scratch_owner(scratch);
+    memset(cfg, 0, sizeof(LgCfg));
+    cfg->n_circuits = n; cfg->first = first_layer; cfg->n_layers = nl;
+    cfg->claim = e_from_host(claim); cfg->alpha = e_from_host(alpha); cfg->lambda = e_from_host(lambda);
+    for (u32 i = 0; i < first_layer; i++) cfg->point[i] = e_from_host(point + 2 * i);
+    for (u32 l = 0; l < nl; l++) {
+        const u32 k = circuits[0]->nv - 1 - (first_layer + l);    // circuit layer with 2^(v+1) entries (dp_logup_layer_mles)
+        for (u32 c = 0; c < n; c++) { cfg->num[l][c] = circuits[c]->num[k]; cfg->den[l][c] = circuits[c]->den[k]; }
+    }
+    cfg->eq = (gle *)(scratch + off_eq); cfg->work = (gle *)(scratch + off_work); cfg->work_stride = stride;
+    static const char lbl[4][16] = {"Internal round", "logup_batching", "logup_alpha", "logup_lambda"};   // BasicTranscript::append_message words
+    memcpy(cfg->round_label, lbl[0], 16);
+    for (int q = 0; q < 3; q++) memcpy(cfg->label[q], lbl[q + 1], 16);
+    for (u32 d = 1; d < 3; d++)
+        for (u32 i = 0; d + 1 + i <= 3; i++)
+            for (u32 j = 0; j <= d; j++) cfg->bary[d - 1][i][j] = sc_bary_weight(d + 1, d + 1 + i, j);
+    for (int w = 0; w < P2S_WORDS; w++) cfg->sponge[w] = w < 12 ? gl_canon(sponge[w]) : sponge[w];
+    out->flag = 0;
+    cudaStream_t st = dp_ctx().stream;
+    {
+        cudaLaunchConfig_t lc{};
+        lc.gridDim = dim3(ncta); lc.blockDim = dim3(SC_THREADS); lc.dynamicSmemBytes = 0; lc.stream = st;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        lc.attrs = at; lc.numAttrs = 1;
+        DpProfScope prof("k_logup_res(resident LogUp-GKR layers, device transcript)", 0);
+        const cudaError_t ce = cudaLaunchKernelEx(&lc, k_logup_res, (const LgCfg *)cfg, out, (gle *)(scratch + off_part), (u64 *)scratch,
+                                                  (gle *)(scratch + off_point));
+        DP_LAUNCHED();
+        DP_CUDA(ce);
+        DP_CUDA(cudaGetLastError());
+    }
+    if (dp_wait_flag(&out->flag, 1, false, 0, 8.0) != 1) { dp_stream_sync(st); DP_CHECK(out->flag == 1, DP_ERR_CUDA, "dp_logup_run_layers_fs: the resident kernel did not finish"); }
+    size_t om = 0, oc = 0, oe = 0;
+    for (u32 l = 0; l < nl; l++) {
+        const u32 v = first_layer + l, per = cfg->num[l][0] ? 4 : 2;
+        const LgLayerOut &o = out->layer[l];
+        for (u32 k = 0; k < v; k++) {
+            for (u32 t = 0; t < 4; t++) { msgs_out[om++] = o.fs.msg[k][t].c0; msgs_out[om++] = o.fs.msg[k][t].c1; }
+            challenges_out[oc++] = o.fs.chal[k].c0; challenges_out[oc++] = o.fs.chal[k].c1;
+        }
+        for (u32 i = 0; i < per * n; i++) { evals_out[oe++] = o.evals[i].c0; evals_out[oe++] = o.evals[i].c1; }
+    }
+    for (u32 i = 0; i <= last_layer; i++) { point[2 * i] = out->point[i].c0; point[2 * i + 1] = out->point[i].c1; }
+    claim[0] = out->claim.c0; claim[1] = out->claim.c1; alpha[0] = out->alpha.c0; alpha[1] = out->alpha.c1; lambda[0] = out->lambda.c0; lambda[1] = out->lambda.c1;
+    for (int i = 0; i < P2S_WORDS; i++) sponge[i] = out->sponge[i];
     return DP_OK;
 }
 

@@ -492,3 +492,32 @@ extern "C" int dph_pcs_batch_open_evals(dp_mle *const *polys, uint32_t n, uint32
     return 0;
     DPH_CATCH
 }
+
+// logup_gkr::prover::batch_prove (zkml.hpp logup_batch_prove) over device columns with DynTranscript::new(label): `table` (then mult is
+// the multiplicities column) or lookup instances of columns_per_instance columns.  out: the proof as [n_proofs, then per proof its
+// rounds, (deg+1) x E per round and its point], [n_evals per layer, evals], the final point and claims, then one challenge drawn from
+// the transcript afterwards (its state); *out_len words.
+extern "C" int dph_logup_prove(dp_mle *const *cols, uint32_t n_cols, dp_mle *mult, uint32_t columns_per_instance, const uint64_t cc[2], const uint64_t sc[2],
+                    const char *label, uint64_t *out, uint64_t cap, uint64_t *out_len) {
+    DPH_TRY
+    zkml::LogUpInput in;
+    in.table = mult != nullptr;
+    auto view = [](dp_mle *m) { u64 len; int ext; check(dp_mle_info(m, &len, &ext, nullptr)); return DeviceMle::wrap_device(dp_mle_device_ptr(m), len, ext != 0); };
+    for (uint32_t i = 0; i < n_cols; i++) in.column_evals.push_back(view(cols[i]));
+    if (mult) in.multiplicities = view(mult);
+    in.constant_challenge = Ext(cc[0], cc[1]); in.column_separation_challenge = Ext(sc[0], sc[1]); in.columns_per_instance = columns_per_instance;
+    DynTranscript t(label ? label : "");
+    zkml::LogUpProof pr = zkml::logup_batch_prove(in, t);
+    std::vector<u64> w;
+    auto put = [&](const Ext &e) { w.push_back(e.c0); w.push_back(e.c1); };
+    w.push_back(pr.sumcheck_proofs.size());
+    for (auto &p : pr.sumcheck_proofs) { w.push_back(p.proofs.size()); for (auto &m : p.proofs) { w.push_back(m.evaluations.size()); for (auto &e : m.evaluations) put(e); } for (auto &e : p.point) put(e); }
+    for (auto &ev : pr.round_evaluations) { w.push_back(ev.size()); for (auto &e : ev) put(e); }
+    for (auto &c : pr.output_claims) { for (auto &e : c.point) put(e); put(c.eval); }
+    put(t.get_and_append_challenge("after"));
+    if (w.size() > cap) throw Error(DP_ERR_INVALID, "dph_logup_prove: output buffer too small");
+    std::copy(w.begin(), w.end(), out); *out_len = w.size();
+    return 0;
+    DPH_CATCH
+}
+

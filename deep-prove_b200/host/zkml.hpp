@@ -102,7 +102,39 @@ LogUpProof logup_batch_prove(const LogUpInput &in, T &t) {
     Ext claim = Ext::zero(), ac = Ext::one();
     for (auto &e : pr.circuit_outputs) { claim += ac * (batching * (e[1] - e[0]) + e[0] + lambda * (batching * (e[3] - e[2]) + e[2])); ac *= alpha; }
     ExtVec point = {batching};
-    for (size_t v = 1; v <= total_layers; v++) {
+    size_t v = 1;
+    // the leading small layers in one resident launch that runs the transcript on the device, when the library takes them (blocking
+    // waits) and the transcript's state can go there (BasicTranscript)
+    std::vector<dp_logup *> hs; for (auto &c : circuits) hs.push_back(c->h);
+    uint32_t n_dev = 0; u64 sp[Sponge::WORDS];
+    check(dp_logup_layers_fs_next(hs.data(), (uint32_t)hs.size(), 1, &n_dev));
+    if (n_dev > 0 && t.save_sponge(sp)) {
+        const size_t last = n_dev, n_rounds = last * (last + 1) / 2;
+        auto views = [&](size_t layer) -> size_t { return !in.table && layer == total_layers ? 2 : 4; };   // dp_logup_layer_mles
+        size_t n_evals = 0; for (size_t l = 1; l <= last; l++) n_evals += views(l) * circuits.size();
+        std::vector<u64> pt(2 * (last + 1)), msgs(2 * 4 * n_rounds), ch(2 * n_rounds), ev(2 * n_evals);
+        pt[0] = batching.c0; pt[1] = batching.c1;
+        u64 cl[2] = {claim.c0, claim.c1}, al[2] = {alpha.c0, alpha.c1}, lm[2] = {lambda.c0, lambda.c1};
+        check(dp_logup_run_layers_fs(hs.data(), (uint32_t)hs.size(), 1, (uint32_t)last, cl, pt.data(), al, lm, sp, msgs.data(), ch.data(), ev.data()));
+        t.load_sponge(sp);
+        size_t om = 0, oc = 0, oe = 0;
+        for (size_t l = 1; l <= last; l++) {
+            IOPProof p;
+            for (size_t k = 0; k < l; k++) {
+                IOPProverMessage m;
+                for (size_t q = 0; q < 4; q++, om += 2) m.evaluations.push_back(Ext(msgs[om], msgs[om + 1]));
+                p.proofs.push_back(std::move(m));
+                p.point.push_back(Ext(ch[oc], ch[oc + 1])); oc += 2;
+            }
+            pr.sumcheck_proofs.push_back(std::move(p));
+            ExtVec evals; for (size_t i = 0; i < views(l) * circuits.size(); i++, oe += 2) evals.push_back(Ext(ev[oe], ev[oe + 1]));
+            pr.round_evaluations.push_back(std::move(evals));
+        }
+        point.clear(); for (size_t i = 0; i <= last; i++) point.push_back(Ext(pt[2 * i], pt[2 * i + 1]));
+        claim = Ext(cl[0], cl[1]); alpha = Ext(al[0], al[1]); lambda = Ext(lm[0], lm[1]);
+        v = last + 1;
+    }
+    for (; v <= total_layers; v++) {
         t.append_field_element_ext(claim);
         DeviceMle eq = DeviceMle::build_eq_x_r(point);           // compute_betas_eval(&sumcheck_point)
         VirtualPolynomial vp(v);

@@ -46,6 +46,7 @@ const char *dp_version(void);
 int dp_set_stream(void *cuda_stream);    /* run on a caller-owned cudaStream_t (e.g. torch's current stream) */
 int dp_synchronize(void);
 uint64_t dp_kernel_launches(void);       /* number of kernels this library launched so far */
+uint64_t dp_host_waits(void);            /* number of times a host thread of this library waited for the device so far */
 /* How a host thread waits for the device at the end of a round (process-wide).  0 (default) = spin on the completion word:
  * lowest latency, one busy core per proof in flight.  1 = sleep on a futex that ONE poller thread of the library signals:
  * ~5 us more per wait, but waiting proofs cost no CPU, so many more proofs than cores can be in flight per GPU (the
@@ -148,6 +149,22 @@ int dp_logup_outputs(const dp_logup *l, uint64_t out[8]);                    /* 
  * [num_low, num_high, den_low, den_high] (or [den_low, den_high] for the initial lookup layer). */
 int dp_logup_layer_mles(const dp_logup *l, uint32_t layer_vars, dp_mle **out_views, uint32_t *n_views);
 int dp_logup_free(dp_logup *l);
+/* *n_layers = how many layers, from the layer whose halves have first_layer variables upwards, dp_logup_run_layers_fs proves for this
+ * batch of circuits (0: none, the caller proves each layer with the sumcheck entry points).  Nonzero only in the blocking wait mode
+ * (dp_set_wait_mode(1)), for at most 16 circuits of one size and layers whose first sumcheck round is small enough to run resident. */
+int dp_logup_layers_fs_next(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t *n_layers);
+/* Layers first_layer..last_layer of logup_gkr::prover::batch_prove (prover.rs:62-170) in one resident launch with BasicTranscript's
+ * Fiat-Shamir on the device.  Per layer v: append the claim, append_usize(v), append_usize(3), prove_parallel on the layer's
+ * VirtualPolynomial (eq(point) times each circuit's views, coefficients alpha^c (1, 1, lambda), or (-1, -1, lambda) for the two-view
+ * first layer of a lookup circuit), take the final evaluations, draw logup_batching, logup_alpha and logup_lambda and form the next
+ * claim and point.  In/out: claim [c0,c1]; point (in: first_layer elements, the last one the batching challenge; out: last_layer + 1);
+ * alpha, lambda [c0,c1]; sponge, the 14-word Poseidon2 duplex state of dp_sc_run_tail_fs.  Out, layer after layer: msgs_out
+ * v x 4 x [c0,c1] (the round messages), challenges_out v x [c0,c1] (the sumcheck point), evals_out n_views x n_circuits x [c0,c1]
+ * (the final evaluations without eq's, in add_mle_list order: [num_lo, den_hi, num_hi, den_lo] per circuit, [den_hi, den_lo] with
+ * two views).  DP_ERR_STATE unless dp_logup_layers_fs_next(first_layer) covers last_layer. */
+int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
+                           uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
+                           uint64_t *evals_out);
 /* out = sum_k coefs[k] * mles[k] over Ext MLEs of equal length (same_poly.rs:91-110 final_beta). */
 int dp_mle_linear_combination(dp_mle *const *mles, const uint64_t *coefs, uint32_t n, dp_mle **out);
 
