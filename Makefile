@@ -10,11 +10,11 @@ PKG       := deep-prove_b200
 CSRC      := $(PKG)/csrc
 CU_SRCS   := $(wildcard $(CSRC)/*.cu)
 CU_OBJS   := $(patsubst $(CSRC)/%.cu,build/%.o,$(CU_SRCS))
-CU_HDRS   := $(wildcard $(CSRC)/*.cuh) include/deepprove_b200.h include/dp_poseidon2_constants.h
+CU_HDRS   := $(wildcard $(CSRC)/*.cuh) include/deepprove_b200.h include/dp_poseidon2_constants.h include/dp_blake3.h
 HOST_SRCS := $(wildcard $(PKG)/host/*.cpp)
-HOST_HDRS := $(wildcard $(PKG)/host/*.hpp) include/deepprove_b200.h
+HOST_HDRS := $(wildcard $(PKG)/host/*.hpp) include/deepprove_b200.h include/dp_blake3.h
 ORC_SRCS  := $(wildcard oracle/*.cpp)
-ORC_HDRS  := $(wildcard oracle/*.hpp) include/dp_poseidon2_constants.h
+ORC_HDRS  := $(wildcard oracle/*.hpp) include/dp_poseidon2_constants.h include/dp_blake3.h
 
 all: product host oracle tools
 

@@ -16,6 +16,8 @@
 // util.rs:101-136) runs on the host inside dp_sc_round, exactly where the reference has it.
 #include "common.cuh"
 #include "poseidon2.cuh"
+#include "blake3.cuh"
+#include "../../include/dp_blake3.h"
 #include <mutex>
 #include <algorithm>
 
@@ -473,11 +475,15 @@ __host__ __device__ inline void sc_desc(ScProd &pd, u32 p, const u32 *idx, u32 n
 }
 
 struct TProd { u32 n_idx; u32 idx[5]; };
-// Fiat-Shamir in the resident kernel (dp_sc_run_tail_fs): what sc_glue and BasicTranscript need.  bary[d - 1][i][j]: weight of
+// Fiat-Shamir in the resident kernel (dp_sc_run_tail_fs[_blake]): what sc_glue and the transcript need.  bary[d - 1][i][j]: weight of
 // point j when a degree-d product is extrapolated to point d + 1 + i (exact constants of sc_extrapolate).
 static constexpr u32 SC_MAX_ROUNDS = 40;
-struct ScTailFs { u32 max_deg, max_nv, round0, pad; u64 label[2]; u64 coef[SC_RES_MAXP][2]; u64 bary[4][4][5]; u64 sponge[P2S_WORDS]; };
-struct ScTailFsOut { gle msg[SC_MAX_ROUNDS][SC_NACC]; gle chal[SC_MAX_ROUNDS]; u64 sponge[P2S_WORDS]; };
+// sponge: the transcript's state, the larger of the two images (TrP2: P2S_WORDS, TrB3: DP_B3T_WORDS)
+static constexpr int SC_FS_WORDS = DP_B3T_WORDS;
+static_assert(P2S_WORDS <= SC_FS_WORDS && DP_B3T_WORDS == (int)dpb3::IMAGE_WORDS && DP_B3T_STACK == (int)dpb3::IMAGE_STACK &&
+              DP_B3T_STACK == (int)b3::T_STACK_MAX, "one BLAKE3 state image");
+struct ScTailFs { u32 max_deg, max_nv, round0, pad; u64 label[2]; u64 coef[SC_RES_MAXP][2]; u64 bary[4][4][5]; u64 sponge[SC_FS_WORDS]; };
+struct ScTailFsOut { gle msg[SC_MAX_ROUNDS][SC_NACC]; gle chal[SC_MAX_ROUNDS]; u64 sponge[SC_FS_WORDS]; };
 struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; ScMle m[SC_RES_MAXM]; u32 writer[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; ScTailFs fs; };
 
 __device__ __forceinline__ u32 cl_rank() { u32 r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
@@ -487,10 +493,38 @@ __device__ __forceinline__ void cl_sync() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
+// The transcript of the resident kernels, a compile-time policy.  CTA 0's threads for which runs() holds build one and call its
+// members together; the state image lives in shared memory between calls and the challenges are valid in thread 0.
+// TrP2: BasicTranscript, the Poseidon2 duplex sponge on the 8-lane groups of warp 0 (poseidon2.cuh P2Sponge).
+struct TrP2 {
+    static constexpr int WORDS = P2S_WORDS;
+    __device__ static bool runs() { return threadIdx.x < 32; }
+    P2Sponge s; int l8;
+    __device__ explicit TrP2(const u64 *w) : l8(threadIdx.x & 7) { p2s_load(s, w, l8); }
+    __device__ void ext(gle e) { p2s_observe(s, e.c0, l8); p2s_observe(s, e.c1, l8); }                 // append_field_element_ext
+    __device__ void usize(u64 v) { p2s_observe(s, v, l8); }                                             // append_usize
+    __device__ void label(const u64 (&w)[2]) { p2s_observe(s, w[0], l8); p2s_observe(s, w[1], l8); }   // append_message, 9..16 bytes
+    __device__ gle challenge() { const u64 c0 = p2s_sample(s, l8), c1 = p2s_sample(s, l8); return e_make(c0, c1); }
+    __device__ void store(u64 *w, u64 *also /* or null */) { __syncwarp(); if (threadIdx.x < 8) { p2s_store(s, w, l8); if (also) p2s_store(s, also, l8); } }
+};
+// TrB3: BlakeTranscript, the incremental BLAKE3 hasher of blake3.cuh on thread 0, working on the image in place.
+struct TrB3 {
+    static constexpr int WORDS = DP_B3T_WORDS;
+    __device__ static bool runs() { return threadIdx.x == 0; }
+    u64 *w;
+    __device__ explicit TrB3(u64 *img) : w(img) {}
+    __device__ void ext(gle e) { b3::t_append_ext(w, e.c0, e.c1); }
+    __device__ void usize(u64 v) { b3::t_append_fe(w, v); }
+    __device__ void label(const u64 (&l)[2]) { b3::t_append_fe(w, l[0]); b3::t_append_fe(w, l[1]); }   // one field element per 8 bytes
+    __device__ gle challenge() { u64 a, b; b3::t_challenge(w, a, b); return e_make(a, b); }
+    __device__ void store(u64 *dst, u64 *also) { for (int i = 0; i < WORDS; i++) { if (dst != w) dst[i] = w[i]; if (also) also[i] = w[i]; } }
+};
+
 // Round k of the device-transcript tail, in CTA 0 once the product sums are in sprod and this round's folds are committed to sm:
-// sc_glue (one thread per product, on the lengths the host's bookkeeping has after the fold), the sum over products, then
-// BasicTranscript on warp 0 -- append_field_element_exts(message), get_and_append_challenge("Internal round") -- and the challenge
-// goes to xctl for the cluster.  Out of line: the round loop keeps its registers (sponge state in shared memory between rounds).
+// sc_glue (one thread per product, on the lengths the host's bookkeeping has after the fold), the sum over products, then the
+// transcript TR -- append_field_element_exts(message), get_and_append_challenge("Internal round") -- and the challenge goes to xctl
+// for the cluster.  Out of line: the round loop keeps its registers (transcript state in shared memory between rounds).
+template <class TR>
 __device__ __noinline__ void sc_res_fs_round(ScTailFs &f, gle (*sprod)[SC_NACC], const TProd *sp, const ScMle *sm, u32 np, u32 k, bool last,
                                              ScTailFsOut *fsout, u64 *xctl) {
     const u32 R = f.round0 + k + 1, max_deg = f.max_deg;
@@ -515,15 +549,13 @@ __device__ __noinline__ void sc_res_fs_round(ScTailFs &f, gle (*sprod)[SC_NACC],
         st_e(&fsout->msg[k][t], v);
     }
     __syncthreads();
-    if (threadIdx.x < 32) {
-        const int l8 = threadIdx.x & 7;
-        P2Sponge s; p2s_load(s, f.sponge, l8);
-        for (u32 t = 0; t <= max_deg; t++) { p2s_observe(s, sprod[0][t].c0, l8); p2s_observe(s, sprod[0][t].c1, l8); }
-        p2s_observe(s, f.label[0], l8); p2s_observe(s, f.label[1], l8);
-        const u64 c0 = p2s_sample(s, l8), c1 = p2s_sample(s, l8);
-        __syncwarp();
-        if (threadIdx.x < 8) { p2s_store(s, f.sponge, l8); if (last) p2s_store(s, fsout->sponge, l8); }
-        if (threadIdx.x == 0) { __stcg(xctl + 1, c0); __stcg(xctl + 2, c1); __stcg(xctl, 0ULL); st_e(&fsout->chal[k], e_make(c0, c1)); }
+    if (TR::runs()) {
+        TR t(f.sponge);
+        for (u32 i = 0; i <= max_deg; i++) t.ext(sprod[0][i]);
+        t.label(f.label);
+        const gle c = t.challenge();
+        t.store(f.sponge, last ? fsout->sponge : nullptr);
+        if (threadIdx.x == 0) { __stcg(xctl + 1, c.c0); __stcg(xctl + 2, c.c1); __stcg(xctl, 0ULL); st_e(&fsout->chal[k], c); }
     }
 }
 
@@ -539,7 +571,7 @@ struct ScResSmem {
 // by r first).  Returns early when the host aborted the tail or a challenge never came.  After the last round the tables' pairs go to
 // `pairs` and the flag is raised -- unless CHAIN (one of several sumchecks in a launch, device transcript): then every CTA records
 // the challenges of rounds 0 .. nr - 2 in schal (shared) and the caller does what follows the last round.
-template <int DSEL, bool CHAIN>
+template <int DSEL, bool CHAIN, class TR>
 __device__ __forceinline__ void sc_res_rounds(ScResSmem &S, const u32 nm, const u32 np, const u32 nr, const bool first_fold, gle r,
                                               gle *out, gle *pairs, volatile u64 *flag, volatile u64 *chal, u64 seq0, gle *xpart, u64 *xctl,
                                               ScTailFsOut *fsout, gle *schal) {
@@ -628,7 +660,7 @@ __device__ __forceinline__ void sc_res_rounds(ScResSmem &S, const u32 nm, const 
         }
         for (u32 i = threadIdx.x; i < nm; i += blockDim.x) if (S.sfold[i]) sc_commit_fold(S.sm[i], S.sdst[i]);   // every CTA keeps its own copy
         __syncthreads();
-        if (rank == 0 && fs) sc_res_fs_round(S.sfs, S.sprod, S.sp, S.sm, np, k, k == nr - 1, fsout, xctl);
+        if (rank == 0 && fs) sc_res_fs_round<TR>(S.sfs, S.sprod, S.sp, S.sm, np, k, k == nr - 1, fsout, xctl);
         if (rank == 0 && !CHAIN) {
             if (k == nr - 1) {   // last round: hand the (<= 2)-entry tables over with the message (k_sc_gather's job)
                 for (u32 i = threadIdx.x; i < nm; i += blockDim.x) {
@@ -646,7 +678,7 @@ __device__ __forceinline__ void sc_res_rounds(ScResSmem &S, const u32 nm, const 
     }
 }
 
-template <int DSEL>
+template <int DSEL, class TR>   // TR: the device transcript when fsout is not null (TrP2 serves the host-transcript launches too)
 __global__ void __launch_bounds__(SC_THREADS)
 k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pairs /* mapped */, volatile u64 *flag /* mapped */,
          volatile u64 *chal /* mapped: [seq, c0, c1] */, u64 seq0, gle *xpart /* device: warp partials */, u64 *xctl /* device: [status, c0, c1] */,
@@ -659,11 +691,11 @@ k_sc_res(const ScTail *__restrict__ cfg, gle r0, gle *out /* mapped */, gle *pai
     if (fsout && rank == 0)
         for (u32 i = threadIdx.x; i < sizeof(ScTailFs) / 8; i += blockDim.x) ((u64 *)&S.sfs)[i] = ((const u64 *)&cfg->fs)[i];
     __syncthreads();
-    sc_res_rounds<DSEL, false>(S, nm, np, nr, cfg->first_has_challenge != 0, r0, out, pairs, flag, chal, seq0, xpart, xctl, fsout, nullptr);
+    sc_res_rounds<DSEL, false, TR>(S, nm, np, nr, cfg->first_has_challenge != 0, r0, out, pairs, flag, chal, seq0, xpart, xctl, fsout, nullptr);
 }
 
 // ---- the small layers of a LogUp-GKR batch, back to back in ONE resident launch (dp_logup_run_layers_fs) --------------------------
-// logup_gkr::prover::batch_prove (prover.rs:24-237) layer by layer, with BasicTranscript on the device: per layer CTA 0 absorbs the
+// logup_gkr::prover::batch_prove (prover.rs:24-237) layer by layer, with the transcript TR on the device: per layer CTA 0 absorbs the
 // claim, num_vars and the degree (prove_parallel), every CTA builds its slice of the layer's eq table from the point and the layer's
 // bookkeeping (the products of zkml.hpp's logup_batch_prove), the rounds run through sc_res_rounds, and CTA 0 folds the final
 // evaluations, squeezes logup_batching / logup_alpha / logup_lambda and forms the next claim and point.  The host sleeps once per call
@@ -676,15 +708,16 @@ struct LgCfg {
     const gle *num[LG_MAXL][LG_MAXC], *den[LG_MAXL][LG_MAXC];     // layer first + l of circuit c: [lo | hi]; num null: numerators all -1
     gle *eq, *work; u64 work_stride;                               // device scratch: the eq table, each MLE's ping-pong tables
     u64 round_label[2], label[3][2];                               // "Internal round"; "logup_batching", "logup_alpha", "logup_lambda"
-    u64 bary[4][4][5]; u64 sponge[P2S_WORDS];
+    u64 bary[4][4][5]; u64 sponge[SC_FS_WORDS];
 };
 struct LgLayerOut { ScTailFsOut fs; gle evals[SC_RES_MAXM]; };
-struct LgOut { LgLayerOut layer[LG_MAXL]; gle point[SC_MAX_ROUNDS + 1]; gle claim, alpha, lambda; u64 sponge[P2S_WORDS]; u64 flag; };
+struct LgOut { LgLayerOut layer[LG_MAXL]; gle point[SC_MAX_ROUNDS + 1]; gle claim, alpha, lambda; u64 sponge[SC_FS_WORDS]; u64 flag; };
 
 // state of the layer loop in shared memory: kept out of registers across the rounds, which need all of theirs
 struct LgSmem { gle pt[SC_MAX_ROUNDS + 1], fe[SC_RES_MAXM], claim, alpha, lambda, batching; u32 v, nm, per, two; };
 
 // layer l's start: its transcript prefix and coefficients (CTA 0), eq table slice and bookkeeping (every CTA)
+template <class TR>
 __device__ __noinline__ void lg_layer_begin(const LgCfg *cfg, ScResSmem &S, LgSmem &L, const u32 l, const gle *xpoint) {
     const u32 rank = cl_rank(), ncta = cl_size(), nc = cfg->n_circuits, np = 3 * nc;
     const u32 v = cfg->first + l;
@@ -699,12 +732,10 @@ __device__ __noinline__ void lg_layer_begin(const LgCfg *cfg, ScResSmem &S, LgSm
             const gle cf = p % 3 == 2 ? e_mul_ni(cur, L.lambda) : two ? e_neg(cur) : cur;
             S.sfs.coef[p][0] = cf.c0; S.sfs.coef[p][1] = cf.c1;
         }
-        if (threadIdx.x < 32) {                                    // t.append_field_element_ext(claim); append_usize(nv); append_usize(deg)
-            const int l8 = threadIdx.x & 7;
-            P2Sponge sp; p2s_load(sp, S.sfs.sponge, l8);
-            p2s_observe(sp, L.claim.c0, l8); p2s_observe(sp, L.claim.c1, l8); p2s_observe(sp, v, l8); p2s_observe(sp, 3, l8);
-            __syncwarp();
-            if (threadIdx.x < 8) p2s_store(sp, S.sfs.sponge, l8);
+        if (TR::runs()) {                                          // t.append_field_element_ext(claim); append_usize(nv); append_usize(deg)
+            TR t(S.sfs.sponge);
+            t.ext(L.claim); t.usize(v); t.usize(3);
+            t.store(S.sfs.sponge, nullptr);
         }
         if (threadIdx.x == 0) S.sfs.max_nv = v;
     }
@@ -740,6 +771,7 @@ __device__ __noinline__ void lg_layer_begin(const LgCfg *cfg, ScResSmem &S, LgSm
 }
 
 // layer l's end in CTA 0: get_mle_final_evaluations, logup_batching / logup_alpha / logup_lambda, the next claim and point (zkml.hpp)
+template <class TR>
 __device__ __noinline__ void lg_layer_end(const LgCfg *cfg, LgOut *out, ScResSmem &S, LgSmem &L, const u32 l, const u64 *xctl, gle *xpoint) {
     const u32 v = L.v, nm = L.nm, per = L.per, nc = cfg->n_circuits;
     const bool two = L.two;
@@ -750,17 +782,11 @@ __device__ __noinline__ void lg_layer_end(const LgCfg *cfg, LgOut *out, ScResSme
         L.fe[i] = f; st_e(&out->layer[l].evals[i - 1], f);
     }
     __syncthreads();
-    if (threadIdx.x < 32) {
-        const int l8 = threadIdx.x & 7;
-        P2Sponge sp; p2s_load(sp, S.sfs.sponge, l8);
+    if (TR::runs()) {
+        TR t(S.sfs.sponge);
         gle ch[3];
-        for (int q = 0; q < 3; q++) {
-            p2s_observe(sp, cfg->label[q][0], l8); p2s_observe(sp, cfg->label[q][1], l8);
-            const u64 c0 = p2s_sample(sp, l8), c1 = p2s_sample(sp, l8);
-            ch[q] = e_make(c0, c1);
-        }
-        __syncwarp();
-        if (threadIdx.x < 8) p2s_store(sp, S.sfs.sponge, l8);
+        for (int q = 0; q < 3; q++) { t.label(cfg->label[q]); ch[q] = t.challenge(); }
+        t.store(S.sfs.sponge, nullptr);
         if (threadIdx.x == 0) {
             const gle bt = ch[0], al = ch[1], lm = ch[2];
             gle acc = e_zero(), a = e_one();
@@ -782,13 +808,14 @@ __device__ __noinline__ void lg_layer_end(const LgCfg *cfg, LgOut *out, ScResSme
         if (last) st_e(&out->point[i], x);
     }
     if (last) {
-        for (u32 i = threadIdx.x; i < P2S_WORDS; i += blockDim.x) out->sponge[i] = S.sfs.sponge[i];
+        for (u32 i = threadIdx.x; i < TR::WORDS; i += blockDim.x) out->sponge[i] = S.sfs.sponge[i];
         if (threadIdx.x == 0) { st_e(&out->claim, L.claim); st_e(&out->alpha, L.alpha); st_e(&out->lambda, L.lambda); }
         __syncthreads();
         if (threadIdx.x == 0) { __threadfence_system(); *(volatile u64 *)&out->flag = 1; }
     }
 }
 
+template <class TR>
 __global__ void __launch_bounds__(SC_THREADS)
 k_logup_res(const LgCfg *__restrict__ cfg, LgOut *out /* mapped */, gle *xpart, u64 *xctl, gle *xpoint /* device */) {
     __shared__ ScResSmem S;
@@ -798,14 +825,14 @@ k_logup_res(const LgCfg *__restrict__ cfg, LgOut *out /* mapped */, gle *xpart, 
             L.alpha = cfg->alpha; L.lambda = cfg->lambda; L.claim = cfg->claim;
             S.sfs.label[0] = cfg->round_label[0]; S.sfs.label[1] = cfg->round_label[1]; S.sfs.max_deg = 3; S.sfs.round0 = 0;
         }
-        for (u32 i = threadIdx.x; i < P2S_WORDS; i += blockDim.x) S.sfs.sponge[i] = cfg->sponge[i];
+        for (u32 i = threadIdx.x; i < TR::WORDS; i += blockDim.x) S.sfs.sponge[i] = cfg->sponge[i];
         for (u32 i = threadIdx.x; i < 4 * 4 * 5; i += blockDim.x) (&S.sfs.bary[0][0][0])[i] = (&cfg->bary[0][0][0])[i];
     }
     for (u32 l = 0; l < cfg->n_layers; l++) {
-        lg_layer_begin(cfg, S, L, l, xpoint);
+        lg_layer_begin<TR>(cfg, S, L, l, xpoint);
         cl_sync();                                                 // the eq table of every CTA is visible
-        sc_res_rounds<0, true>(S, L.nm, 3 * cfg->n_circuits, L.v, false, e_zero(), nullptr, nullptr, nullptr, nullptr, 0, xpart, xctl, &out->layer[l].fs, L.pt);
-        if (cl_rank() == 0) { __syncthreads(); lg_layer_end(cfg, out, S, L, l, xctl, xpoint); }
+        sc_res_rounds<0, true, TR>(S, L.nm, 3 * cfg->n_circuits, L.v, false, e_zero(), nullptr, nullptr, nullptr, nullptr, 0, xpart, xctl, &out->layer[l].fs, L.pt);
+        if (cl_rank() == 0) { __syncthreads(); lg_layer_end<TR>(cfg, out, S, L, l, xctl, xpoint); }
         cl_sync();                                                 // the next point is visible; every read of this layer's tables is done
     }
 }
@@ -939,15 +966,19 @@ static bool sc_tail_eligible(const dp_sc *s, bool fold) {
     return sc_round_work(s, fold) <= SC_RES_WORK;
 }
 // the kernels by DSEL (0: mixed degrees, 1..5: every product has this degree) and the lean ones by [MODE][D - 2]
-static decltype(&k_sc_res<0>) const k_sc_res_dsel[6] = {k_sc_res<0>, k_sc_res<1>, k_sc_res<2>, k_sc_res<3>, k_sc_res<4>, k_sc_res<5>};
+// [blake][DSEL]: k_sc_res with BasicTranscript (also every host-transcript launch) or BlakeTranscript on the device
+static decltype(&k_sc_res<0, TrP2>) const k_sc_res_dsel[2][6] = {
+    {k_sc_res<0, TrP2>, k_sc_res<1, TrP2>, k_sc_res<2, TrP2>, k_sc_res<3, TrP2>, k_sc_res<4, TrP2>, k_sc_res<5, TrP2>},
+    {k_sc_res<0, TrB3>, k_sc_res<1, TrB3>, k_sc_res<2, TrB3>, k_sc_res<3, TrB3>, k_sc_res<4, TrB3>, k_sc_res<5, TrB3>}};
 static decltype(&k_sc_round<0>) const k_sc_round_dsel[6] = {k_sc_round<0>, k_sc_round<1>, k_sc_round<2>, k_sc_round<3>, k_sc_round<4>, k_sc_round<5>};
 static decltype(&k_sc_round<0>) const k_sc_lean_md[4][2] = {{k_sc_lean<2, OPM_B>, k_sc_lean<3, OPM_B>}, {k_sc_lean<2, OPM_E>, k_sc_lean<3, OPM_E>},
                                                               {k_sc_lean<2, OPM_BF>, k_sc_lean<3, OPM_BF>}, {k_sc_lean<2, OPM_EF>, k_sc_lean<3, OPM_EF>}};
 static constexpr int SC_LEAN_BLOCK[4] = {ScLeanShape<OPM_B>::BLOCK, ScLeanShape<OPM_E>::BLOCK, ScLeanShape<OPM_BF>::BLOCK, ScLeanShape<OPM_EF>::BLOCK};
 
 // start the resident kernel for all remaining rounds; the first one's message is tagged s->seq.  fs: the kernel runs the transcript
-// from this sponge state and writes messages, challenges and the final state to s->h_fs (null: the host posts every challenge).
-static int sc_tail_launch(dp_sc *s, gle r, bool fold, const ScTailFs *fs) {
+// (BlakeTranscript when blake, else BasicTranscript) from this state and writes messages, challenges and the final state to s->h_fs
+// (null: the host posts every challenge).
+static int sc_tail_launch(dp_sc *s, gle r, bool fold, const ScTailFs *fs, bool blake = false) {
     cudaStream_t st = dp_ctx().stream;
     {
         int e = 0;
@@ -977,9 +1008,10 @@ static int sc_tail_launch(dp_sc *s, gle r, bool fold, const ScTailFs *fs) {
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         lc.attrs = at; lc.numAttrs = 1;
-        DpProfScope prof(fs ? "k_sc_res(resident cluster rounds with the device transcript)"
-                            : "k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)", 0);
-        const cudaError_t ce = cudaLaunchKernelEx(&lc, k_sc_res_dsel[dsel], (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs, (volatile u64 *)s->h_flag,
+        DpProfScope prof(!fs ? "k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)"
+                         : blake ? "k_sc_res(resident cluster rounds, BLAKE3 device transcript)"
+                                 : "k_sc_res(resident cluster rounds with the device transcript)", 0);
+        const cudaError_t ce = cudaLaunchKernelEx(&lc, k_sc_res_dsel[fs && blake][dsel], (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs, (volatile u64 *)s->h_flag,
                                                   (volatile u64 *)s->h_chal, s->seq, s->d_xpart, s->d_xctl, fs ? s->h_fs : (ScTailFsOut *)nullptr);
         DP_LAUNCHED();
         DP_CUDA(ce);
@@ -1238,8 +1270,9 @@ int dp_sc_set_resident_tail(dp_sc *s, int enable) {
 }
 
 // The device transcript pays where a proving thread would otherwise sleep through every round trip: in blocking wait mode, many
-// proofs in flight.  In spin mode the host's round trip is a few microseconds, less than the 3 dependent permutations the kernel
-// runs on one warp per round (DESIGN.md section 5.2), so a lone proof keeps the host transcript.
+// proofs in flight.  In spin mode the host's round trip is a few microseconds, less than the kernel's hash chain per round (3
+// dependent Poseidon2 permutations on one warp, or a few BLAKE3 compressions on one thread: DESIGN.md section 5.2), so a lone proof
+// keeps the host transcript with either hasher.
 int dp_sc_tail_fs_next(dp_sc *s, int *out) {
     DP_REQUIRE_CTX();
     DP_CHECK(s && out, DP_ERR_INVALID, "dp_sc_tail_fs_next: null argument");
@@ -1247,16 +1280,36 @@ int dp_sc_tail_fs_next(dp_sc *s, int *out) {
     return DP_OK;
 }
 
-int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
-                      uint64_t *sponge_out) {
-    DP_REQUIRE_CTX();
-    DP_CHECK(s && sponge_in && msgs_out && challenges_out && sponge_out, DP_ERR_INVALID, "dp_sc_run_tail_fs: null argument");
+}  // extern "C"
+
+// The transcript state an entry point takes: BasicTranscript's 14-word sponge (canonical words, counts in range), or a valid image of
+// BlakeTranscript's hasher (dpb3::image_ok), copied into the kernel's SC_FS_WORDS buffer.  False: out of range.
+static bool fs_state_in(const uint64_t *in, bool blake, u64 *dst) {
+    if (blake) { if (!dpb3::image_ok(in)) return false; for (int w = 0; w < DP_B3T_WORDS; w++) dst[w] = in[w]; return true; }
+    if (!(in[12] < 4 && in[13] <= 4)) return false;
+    for (int w = 0; w < P2S_WORDS; w++) dst[w] = w < 12 ? gl_canon(in[w]) : in[w];
+    return true;
+}
+// ... and the state the kernel returns, in dpb3::Hasher::save's form (the stack words past stack_len, which merges leave behind in
+// the kernel, are zero).  False: the BLAKE3 hasher needed more than DP_B3T_STACK stack entries (more than 2^17 chunks).
+static bool fs_state_out(const u64 *src, bool blake, uint64_t *out) {
+    if (blake && (src[b3::T_SLEN] & b3::T_OVERFLOW)) return false;
+    const int n = blake ? b3::T_STACK + 4 * (int)src[b3::T_SLEN] : P2S_WORDS;
+    for (int w = 0; w < (blake ? DP_B3T_WORDS : P2S_WORDS); w++) out[w] = w < n ? src[w] : 0;
+    return true;
+}
+
+static int sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
+                          uint64_t *sponge_out, bool blake) {
+    const char *const fn = blake ? "dp_sc_run_tail_fs_blake" : "dp_sc_run_tail_fs";
+    DP_CHECK(s && sponge_in && msgs_out && challenges_out && sponge_out, DP_ERR_INVALID, std::string(fn) + ": null argument");
     DP_CHECK(!s->finished && s->round < s->max_nv && !s->tail_active, DP_ERR_STATE, "Prover is not active");
     const bool fold = s->round > 0;
     DP_CHECK(fold == (prev_challenge != nullptr), DP_ERR_STATE, fold ? "verifier message is empty" : "first round should be prover first.");
-    DP_CHECK(sponge_in[12] < 4 && sponge_in[13] <= 4, DP_ERR_INVALID, "dp_sc_run_tail_fs: sponge state out of range");
-    DP_CHECK(sc_tail_eligible(s, fold), DP_ERR_STATE, "dp_sc_run_tail_fs: the next round does not start the resident tail");
-    DP_CUDA(sc_fs_constants());
+    ScTailFs fs{};
+    DP_CHECK(fs_state_in(sponge_in, blake, fs.sponge), DP_ERR_INVALID, std::string(fn) + (blake ? ": not a BLAKE3 hasher state" : ": sponge state out of range"));
+    DP_CHECK(sc_tail_eligible(s, fold), DP_ERR_STATE, std::string(fn) + ": the next round does not start the resident tail");
+    if (!blake) DP_CUDA(sc_fs_constants());
     gle r = e_zero();
     if (fold) {
         r = e_from_host(prev_challenge);
@@ -1264,24 +1317,22 @@ int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *
         if (s->challenges.size() == 1)
             for (auto &m : s->mles) DP_CHECK(m.len > 1, DP_ERR_INVALID, "calling sumcheck on constant");  // prover.rs:667-669
     }
-    ScTailFs fs{};
     fs.max_deg = s->max_deg; fs.max_nv = s->max_nv; fs.round0 = s->round;
-    static const char label[] = "Internal round";                 // BasicTranscript::append_message: 8-byte little-endian words
+    static const char label[] = "Internal round";                 // Transcript::append_message: 8-byte little-endian words
     memcpy(fs.label, label, sizeof label - 1);
     for (u32 p = 0; p < s->n_products; p++) { fs.coef[p][0] = s->products[p].coef[0]; fs.coef[p][1] = s->products[p].coef[1]; }
     for (u32 d = 1; d < s->max_deg; d++)
         for (u32 i = 0; d + 1 + i <= s->max_deg; i++)
             for (u32 j = 0; j <= d; j++) fs.bary[d - 1][i][j] = sc_bary_weight(d + 1, d + 1 + i, j);
-    for (int w = 0; w < P2S_WORDS; w++) fs.sponge[w] = w < 12 ? gl_canon(sponge_in[w]) : sponge_in[w];
     const u32 nr = s->max_nv - s->round;
     s->seq++;
-    if (int e = sc_tail_launch(s, r, fold, &fs)) return e;
+    if (int e = sc_tail_launch(s, r, fold, &fs, blake)) return e;
     s->seq += nr - 1;                                              // the kernel raises the flag once, with the last round's tag
     for (u32 k = 0; k < nr; k++)
         if (k > 0 || fold) for (auto &m : s->mles) if (m.len > 1) { m.len >>= 1; m.is_ext = true; m.cur = nullptr; m.where = 3; }
     s->round = s->max_nv;
     const bool ok = dp_wait_flag(s->h_flag, s->seq, true, SC_TAIL_FAILED, 8.0) == s->seq;
-    if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(dp_ctx().stream); DP_CHECK(false, DP_ERR_CUDA, "dp_sc_run_tail_fs: the resident kernel did not finish"); }
+    if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(dp_ctx().stream); DP_CHECK(false, DP_ERR_CUDA, std::string(fn) + ": the resident kernel did not finish"); }
     s->have_pairs = true;
     const ScTailFsOut &o = *s->h_fs;
     const u32 w = s->max_deg + 1;
@@ -1290,8 +1341,21 @@ int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *
         challenges_out[2 * k] = o.chal[k].c0; challenges_out[2 * k + 1] = o.chal[k].c1;
         if (k + 1 < nr) s->challenges.push_back(o.chal[k]);     // the last one is dp_sc_finish's
     }
-    for (int i = 0; i < P2S_WORDS; i++) sponge_out[i] = o.sponge[i];
+    DP_CHECK(fs_state_out(o.sponge, blake, sponge_out), DP_ERR_STATE, std::string(fn) + ": the transcript outgrew the BLAKE3 state image");
     return DP_OK;
+}
+
+extern "C" {
+
+int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
+                      uint64_t *sponge_out) {
+    DP_REQUIRE_CTX();
+    return sc_run_tail_fs(s, prev_challenge, sponge_in, msgs_out, challenges_out, sponge_out, false);
+}
+int dp_sc_run_tail_fs_blake(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *state_in, uint64_t *msgs_out, uint64_t *challenges_out,
+                            uint64_t *state_out) {
+    DP_REQUIRE_CTX();
+    return sc_run_tail_fs(s, prev_challenge, state_in, msgs_out, challenges_out, state_out, true);
 }
 
 int dp_logup_layers_fs_next(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t *n_layers) {
@@ -1301,16 +1365,19 @@ int dp_logup_layers_fs_next(dp_logup *const *circuits, uint32_t n_circuits, uint
     return DP_OK;
 }
 
-int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
-                           uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
-                           uint64_t *evals_out) {
-    DP_REQUIRE_CTX();
+}  // extern "C"
+
+static int lg_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
+                            uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
+                            uint64_t *evals_out, bool blake) {
+    const char *const fn = blake ? "dp_logup_run_layers_fs_blake" : "dp_logup_run_layers_fs";
     DP_CHECK(circuits && claim && point && alpha && lambda && sponge && msgs_out && challenges_out && evals_out, DP_ERR_INVALID,
-             "dp_logup_run_layers_fs: null argument");
+             std::string(fn) + ": null argument");
     DP_CHECK(first_layer >= 1 && last_layer >= first_layer && last_layer - first_layer < lg_fs_layers(circuits, n_circuits, first_layer), DP_ERR_STATE,
-             "dp_logup_run_layers_fs: these layers do not run resident (wait mode, circuit count or layer size)");
-    DP_CHECK(sponge[12] < 4 && sponge[13] <= 4, DP_ERR_INVALID, "dp_logup_run_layers_fs: sponge state out of range");
-    DP_CUDA(sc_fs_constants());
+             std::string(fn) + ": these layers do not run resident (wait mode, circuit count or layer size)");
+    u64 state[SC_FS_WORDS] = {};
+    DP_CHECK(fs_state_in(sponge, blake, state), DP_ERR_INVALID, std::string(fn) + (blake ? ": not a BLAKE3 hasher state" : ": sponge state out of range"));
+    if (!blake) DP_CUDA(sc_fs_constants());
     const u32 nl = last_layer - first_layer + 1, n = n_circuits, np = 3 * n, nm_max = 1 + 4 * n;
     const u64 len_max = 1ULL << last_layer, stride = (len_max >> 1) + (len_max >> 2) + 1;
     const u64 work = (u64)np * (len_max >> 1);
@@ -1340,7 +1407,7 @@ int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint3
     for (u32 d = 1; d < 3; d++)
         for (u32 i = 0; d + 1 + i <= 3; i++)
             for (u32 j = 0; j <= d; j++) cfg->bary[d - 1][i][j] = sc_bary_weight(d + 1, d + 1 + i, j);
-    for (int w = 0; w < P2S_WORDS; w++) cfg->sponge[w] = w < 12 ? gl_canon(sponge[w]) : sponge[w];
+    memcpy(cfg->sponge, state, sizeof state);
     out->flag = 0;
     cudaStream_t st = dp_ctx().stream;
     {
@@ -1349,14 +1416,14 @@ int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint3
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         lc.attrs = at; lc.numAttrs = 1;
-        DpProfScope prof("k_logup_res(resident LogUp-GKR layers, device transcript)", 0);
-        const cudaError_t ce = cudaLaunchKernelEx(&lc, k_logup_res, (const LgCfg *)cfg, out, (gle *)(scratch + off_part), (u64 *)scratch,
+        DpProfScope prof(blake ? "k_logup_res(resident LogUp-GKR layers, BLAKE3 transcript)" : "k_logup_res(resident LogUp-GKR layers, device transcript)", 0);
+        const cudaError_t ce = cudaLaunchKernelEx(&lc, blake ? k_logup_res<TrB3> : k_logup_res<TrP2>, (const LgCfg *)cfg, out, (gle *)(scratch + off_part), (u64 *)scratch,
                                                   (gle *)(scratch + off_point));
         DP_LAUNCHED();
         DP_CUDA(ce);
         DP_CUDA(cudaGetLastError());
     }
-    if (dp_wait_flag(&out->flag, 1, false, 0, 8.0) != 1) { dp_stream_sync(st); DP_CHECK(out->flag == 1, DP_ERR_CUDA, "dp_logup_run_layers_fs: the resident kernel did not finish"); }
+    if (dp_wait_flag(&out->flag, 1, false, 0, 8.0) != 1) { dp_stream_sync(st); DP_CHECK(out->flag == 1, DP_ERR_CUDA, std::string(fn) + ": the resident kernel did not finish"); }
     size_t om = 0, oc = 0, oe = 0;
     for (u32 l = 0; l < nl; l++) {
         const u32 v = first_layer + l, per = cfg->num[l][0] ? 4 : 2;
@@ -1369,8 +1436,23 @@ int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint3
     }
     for (u32 i = 0; i <= last_layer; i++) { point[2 * i] = out->point[i].c0; point[2 * i + 1] = out->point[i].c1; }
     claim[0] = out->claim.c0; claim[1] = out->claim.c1; alpha[0] = out->alpha.c0; alpha[1] = out->alpha.c1; lambda[0] = out->lambda.c0; lambda[1] = out->lambda.c1;
-    for (int i = 0; i < P2S_WORDS; i++) sponge[i] = out->sponge[i];
+    DP_CHECK(fs_state_out(out->sponge, blake, sponge), DP_ERR_STATE, std::string(fn) + ": the transcript outgrew the BLAKE3 state image");
     return DP_OK;
+}
+
+extern "C" {
+
+int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
+                           uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
+                           uint64_t *evals_out) {
+    DP_REQUIRE_CTX();
+    return lg_run_layers_fs(circuits, n_circuits, first_layer, last_layer, claim, point, alpha, lambda, sponge, msgs_out, challenges_out, evals_out, false);
+}
+int dp_logup_run_layers_fs_blake(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
+                                 uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *state, uint64_t *msgs_out, uint64_t *challenges_out,
+                                 uint64_t *evals_out) {
+    DP_REQUIRE_CTX();
+    return lg_run_layers_fs(circuits, n_circuits, first_layer, last_layer, claim, point, alpha, lambda, state, msgs_out, challenges_out, evals_out, true);
 }
 
 int dp_sc_current_mle(dp_sc *s, uint32_t idx, dp_mle **out) {

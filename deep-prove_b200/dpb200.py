@@ -21,10 +21,10 @@ ABI_SYMBOLS = [
     "dp_mle_upload", "dp_mle_wrap_device", "dp_mle_clone", "dp_mle_download", "dp_mle_info", "dp_mle_device_ptr",
     "dp_mle_free", "dp_mle_fix_high", "dp_mle_fix_high_new", "dp_mle_fix_low", "dp_mle_evaluate", "dp_mle_evaluate_many", "dp_eq_build",
     "dp_sc_create", "dp_sc_round", "dp_sc_finish", "dp_sc_destroy", "dp_sc_current_mle", "dp_sc_set_resident_tail",
-    "dp_sc_tail_fs_next", "dp_sc_run_tail_fs", "dp_poseidon2_init", "dp_set_merkle_hasher", "dp_get_merkle_hasher", "dp_pcs_commit", "dp_pcs_commit_many", "dp_pcs_batch_commit", "dp_pcs_comm_num_polys", "dp_pcs_comm_part", "dp_pcs_comm_info", "dp_pcs_comm_codeword", "dp_pcs_comm_bh_evals", "dp_pcs_comm_free",
+    "dp_sc_tail_fs_next", "dp_sc_run_tail_fs", "dp_sc_run_tail_fs_blake", "dp_poseidon2_init", "dp_set_merkle_hasher", "dp_get_merkle_hasher", "dp_pcs_commit", "dp_pcs_commit_many", "dp_pcs_batch_commit", "dp_pcs_comm_num_polys", "dp_pcs_comm_part", "dp_pcs_comm_info", "dp_pcs_comm_codeword", "dp_pcs_comm_bh_evals", "dp_pcs_comm_free",
     "dp_pcs_open_begin", "dp_pcs_open_round", "dp_pcs_open_final_message", "dp_pcs_open_query_words", "dp_pcs_open_query",
     "dp_pcs_open_free", "dp_pcs_commit_shard", "dp_pcs_comm_shard_info", "dp_pcs_comm_set_shard_roots", "dp_pcs_open_set_shard_roots",
-    "dp_logup_build", "dp_logup_num_vars", "dp_logup_outputs", "dp_logup_layer_mles", "dp_logup_free", "dp_logup_layers_fs_next", "dp_logup_run_layers_fs", "dp_mle_linear_combination",
+    "dp_logup_build", "dp_logup_num_vars", "dp_logup_outputs", "dp_logup_layer_mles", "dp_logup_free", "dp_logup_layers_fs_next", "dp_logup_run_layers_fs", "dp_logup_run_layers_fs_blake", "dp_mle_linear_combination",
     "dp_wit_begin", "dp_wit_dense", "dp_wit_matmul", "dp_wit_requant", "dp_wit_relu", "dp_wit_pool", "dp_wit_finish", "dp_wit_free",
     "dp_fft_rows", "dp_pad_rows", "dp_conv_prod", "dp_conv_output_elements", "dp_phi_g_init", "dp_phi_level", "dp_mle_repeat",
 ]
@@ -79,8 +79,10 @@ def lib():
         _lib.dp_sc_destroy.argtypes = [C.c_void_p]
         _lib.dp_sc_tail_fs_next.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
         _lib.dp_sc_run_tail_fs.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+        _lib.dp_sc_run_tail_fs_blake.argtypes = [C.c_void_p] + [C.c_void_p] * 5
         _lib.dp_logup_layers_fs_next.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]
         _lib.dp_logup_run_layers_fs.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 8
+        _lib.dp_logup_run_layers_fs_blake.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 8
     return _lib
 
 
@@ -99,6 +101,8 @@ def host():
         _host.dph_transcript_append_msg.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64]
         _host.dph_transcript_append_e.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
         _host.dph_transcript_challenge.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
+        _host.dph_transcript_save_state.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
+        _host.dph_transcript_load_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _host.dph_poseidon2_permute.argtypes = [C.c_void_p]
         _host.dph_sumcheck_prove_parallel.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(ScProduct), C.c_uint32,
                                                       C.c_uint32, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -38,6 +38,17 @@ void dph_transcript_append_f(void *t, const uint64_t *f, uint64_t n) { for (uint
 void dph_transcript_append_msg(void *t, const uint8_t *m, uint64_t n) { ((DynTranscript *)t)->append_message(m, n); }
 void dph_transcript_append_e(void *t, const uint64_t *e, uint64_t n) { for (uint64_t i = 0; i < n; i++) ((DynTranscript *)t)->append_field_element_ext(Ext(e[2 * i], e[2 * i + 1])); }
 void dph_transcript_challenge(void *t, const char *label, uint64_t *out) { Ext c = ((DynTranscript *)t)->get_and_append_challenge(label); out[0] = c.c0; out[1] = c.c1; }
+// The transcript's device state (what a prover hands to dp_sc_run_tail_fs[_blake] / dp_logup_run_layers_fs[_blake]): *kind = 0 none,
+// 1 the 14-word Poseidon2 sponge, 2 the DP_B3T_WORDS BLAKE3 hasher image; words: DP_B3T_WORDS.  Load takes the same kind back (1 on
+// a mismatch or an invalid image).
+void dph_transcript_save_state(void *t, int *kind, uint64_t *words) { *kind = ((DynTranscript *)t)->save_sponge(words); }
+int dph_transcript_load_state(void *t, int kind, const uint64_t *words) {
+    DPH_TRY
+    if (kind != ((DynTranscript *)t)->state_kind()) throw Error(DP_ERR_INVALID, "dph_transcript_load_state: not this transcript's kind of state");
+    ((DynTranscript *)t)->load_sponge(words);
+    return 0;
+    DPH_CATCH
+}
 
 // VirtualPolynomial numbers MLEs by FIRST USE in the products (virtual_poly.rs:168-177), and get_mle_final_evaluations()
 // returns them in that order; the C entry points below report final evaluations in the CALLER's `mles` order instead.

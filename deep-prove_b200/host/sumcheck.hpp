@@ -254,18 +254,18 @@ class IOPProverState {
     // round's challenge c ([c0, c1]; null in round 0).  Each message goes to the transcript, which draws the next challenge.
     // sc: the single device handle behind `round`, if there is one; when the library says its resident tail runs the transcript
     // on the device from the next round on (dp_sc_tail_fs_next) and the transcript's state can go there, the remaining rounds
-    // are one dp_sc_run_tail_fs call.
+    // are one dp_sc_run_tail_fs (BasicTranscript) or dp_sc_run_tail_fs_blake (BlakeTranscript) call.
     template <class T, class F>
     static void run_rounds(size_t nv, size_t deg, T &transcript, IOPProof &proof, IOPProverState &st, F &&round, dp_sc *sc = nullptr) {
         for (size_t i = 0; i < nv; i++) {
             u64 c[2] = {0, 0};
             if (i > 0) { c[0] = st.challenges.back().c0; c[1] = st.challenges.back().c1; }
-            int dev = 0; u64 sp[Sponge::WORDS];
+            int dev = 0, kind = DS_NONE; u64 sp[DEVICE_STATE_WORDS];
             if (sc) check(dp_sc_tail_fs_next(sc, &dev));
-            if (dev && transcript.save_sponge(sp)) {
+            if (dev && (kind = transcript.save_sponge(sp)) != DS_NONE) {
                 const size_t n = nv - i, w = 2 * (deg + 1);
                 std::vector<u64> msgs(n * w), ch(2 * n);
-                check(dp_sc_run_tail_fs(sc, i > 0 ? c : nullptr, sp, msgs.data(), ch.data(), sp));
+                check((kind == DS_BLAKE3 ? dp_sc_run_tail_fs_blake : dp_sc_run_tail_fs)(sc, i > 0 ? c : nullptr, sp, msgs.data(), ch.data(), sp));
                 transcript.load_sponge(sp);
                 for (size_t k = 0; k < n; k++) {
                     IOPProverMessage msg;

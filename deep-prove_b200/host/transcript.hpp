@@ -6,7 +6,9 @@
 #pragma once
 #include "field.hpp"
 #include "../../include/dp_poseidon2_constants.h"
+#include "../../include/dp_blake3.h"
 #include <cstring>
+#include <stdexcept>
 
 namespace dp {
 
@@ -108,6 +110,13 @@ class Sponge {
     int nin_ = 0, nout_ = 0;
 };
 
+// Which state a transcript hands to the device transcript of the resident kernels (save_sponge's result): none (the host runs every
+// round), BasicTranscript's duplex sponge (Sponge::WORDS words, dp_sc_run_tail_fs / dp_logup_run_layers_fs) or BlakeTranscript's
+// hasher image (dpb3::IMAGE_WORDS words, the _blake entry points).  A buffer of DEVICE_STATE_WORDS holds either.
+enum DeviceState : int { DS_NONE = 0, DS_POSEIDON2 = 1, DS_BLAKE3 = 2 };
+static constexpr size_t DEVICE_STATE_WORDS = dpb3::IMAGE_WORDS;
+static_assert(DEVICE_STATE_WORDS >= (size_t)Sponge::WORDS, "the state buffer holds the Poseidon2 sponge too");
+
 // trait Transcript<E> as implemented by BasicTranscript<E>
 class BasicTranscript {
   public:
@@ -123,8 +132,8 @@ class BasicTranscript {
     void append_field_element_exts(const ExtVec &v) { for (auto &e : v) append_field_element_ext(e); }
     Ext read_challenge() { u64 a = sp_.sample(); u64 b = sp_.sample(); return Ext(a, b); }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
-    // the sponge state for dp_sc_run_tail_fs: true, this transcript can continue on the device
-    bool save_sponge(u64 w[Sponge::WORDS]) const { sp_.save(w); return true; }
+    // the sponge state for dp_sc_run_tail_fs: this transcript can always continue on the device
+    int save_sponge(u64 w[Sponge::WORDS]) const { sp_.save(w); return DS_POSEIDON2; }
     void load_sponge(const u64 w[Sponge::WORDS]) { sp_.load(w); }
   private:
     Sponge sp_;
@@ -136,9 +145,6 @@ class BasicTranscript {
 // update("field_element_ext") + update(bytes(c0) || bytes(c1)); a message goes through the trait default (8-byte chunks -> field
 // elements -> one append each); a challenge is update("challenge") + 16 bytes of finalize_xof read as two little-endian u64, retried
 // until both are canonical (ff_ext/src/lib.rs:29-41,246-254).  BLAKE3 itself: include/dp_blake3.h (pinned against the Python package).
-}  // namespace dp
-#include "../../include/dp_blake3.h"
-namespace dp {
 class BlakeTranscript {
   public:
     explicit BlakeTranscript(const std::string &label) { h_.update(label.data(), label.size()); }   // BlakeTranscript::new: raw label bytes
@@ -158,8 +164,12 @@ class BlakeTranscript {
         }
     }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
-    bool save_sponge(u64 *) const { return false; }                 // BLAKE3: no device counterpart, the host runs every round
-    void load_sponge(const u64 *) { throw std::logic_error("BlakeTranscript has no sponge state"); }
+    // the hasher image for the _blake device entry points; none (the host keeps every round) past 2^16 absorbed chunks
+    int save_sponge(u64 w[dpb3::IMAGE_WORDS]) const { return h_.save(w) ? DS_BLAKE3 : DS_NONE; }
+    void load_sponge(const u64 w[dpb3::IMAGE_WORDS]) {
+        if (!dpb3::image_ok(w)) throw std::invalid_argument("BlakeTranscript::load_sponge: not a BLAKE3 hasher state");
+        h_.load(w);
+    }
   private:
     static size_t le(u64 c, uint8_t b[8]) { size_t n = 0; for (int k = 0; k < 8; k++) { b[k] = (uint8_t)(c >> (8 * k)); if (b[k]) n = k + 1; } return n ? n : 1; }
     dpb3::Hasher h_;
@@ -179,7 +189,9 @@ class DynTranscript {
     void append_field_element_exts(const ExtVec &v) { for (auto &e : v) append_field_element_ext(e); }
     Ext read_challenge() { return blake_ ? k_.read_challenge() : b_.read_challenge(); }
     Ext get_and_append_challenge(const std::string &label) { append_message(label); return read_challenge(); }
-    bool save_sponge(u64 *w) const { return blake_ ? k_.save_sponge(w) : b_.save_sponge(w); }
+    // w: DEVICE_STATE_WORDS; returns which state it holds (DeviceState)
+    int save_sponge(u64 *w) const { return blake_ ? k_.save_sponge(w) : b_.save_sponge(w); }
+    int state_kind() const { return blake_ ? DS_BLAKE3 : DS_POSEIDON2; }          // what load_sponge takes
     void load_sponge(const u64 *w) { blake_ ? k_.load_sponge(w) : b_.load_sponge(w); }
   private:
     bool blake_; BasicTranscript b_; BlakeTranscript k_;

@@ -116,9 +116,10 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals);
  * kernel launches (Nsight Compute, compute-sanitizer): a one-time probe checks that a running kernel can see a word the
  * host posts after the launch call returned. */
 int dp_sc_set_resident_tail(dp_sc *s, int enable);
-/* *out = 1 when the library runs the next round and all later ones with the transcript on the device (dp_sc_run_tail_fs): the
- * next round starts the resident tail and the wait mode is blocking (dp_set_wait_mode(1)).  In spin mode a host round trip is
- * cheaper than the kernel's own Poseidon2 chain, so callers keep calling dp_sc_round there. */
+/* *out = 1 when the library runs the next round and all later ones with the transcript on the device (dp_sc_run_tail_fs, or
+ * dp_sc_run_tail_fs_blake for a BlakeTranscript): the next round starts the resident tail and the wait mode is blocking
+ * (dp_set_wait_mode(1)).  In spin mode a host round trip is cheaper than the kernel's own hash chain, so callers keep calling
+ * dp_sc_round there. */
 int dp_sc_tail_fs_next(dp_sc *s, int *out);
 /* Every remaining round in the resident tail, with BasicTranscript's Fiat-Shamir run by the kernel: each round message is absorbed
  * (append_field_element_exts), then the label "Internal round", and the challenge (c0, c1) is sampled.  prev_challenge: the
@@ -129,6 +130,19 @@ int dp_sc_tail_fs_next(dp_sc *s, int *out);
  * enough rounds). */
 int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
                       uint64_t *sponge_out);
+/* The state of a BlakeTranscript (transcript/src/blake.rs: one running unkeyed BLAKE3 hasher) as DP_B3T_WORDS u64 words, the image
+ * of its blake3::Hasher: [0..3] the chunk chaining value (8 x u32, little-endian pairs), [4] chunk_counter, [5..12] the 64-byte block
+ * buffer (zero past block_len), [13] block_len, [14] blocks_compressed, [15] stack_len, [16 + 4i .. 19 + 4i] chaining-value stack
+ * entry i (8 x u32).  The hasher is lazy: a full block is compressed, and a full chunk pushed, only when more input arrives.  A
+ * valid image has block_len <= 64, blocks_compressed <= 15 (and block_len > 0 when blocks_compressed > 0), zero bytes past
+ * block_len and stack_len == popcount(chunk_counter) <= DP_B3T_STACK; a transcript of more than 2^16 chunks (64 MiB) has no image. */
+#define DP_B3T_STACK 16
+#define DP_B3T_WORDS 80
+/* dp_sc_run_tail_fs with BlakeTranscript's Fiat-Shamir on the device: per round the message (append_field_element_exts), the label
+ * "Internal round" (two 8-byte words, each appended as a field element), then read_challenge.  state_in / state_out: DP_B3T_WORDS
+ * images (may be the same buffer).  Arguments, outputs and DP_ERR_STATE as dp_sc_run_tail_fs; DP_ERR_INVALID for an invalid image. */
+int dp_sc_run_tail_fs_blake(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *state_in, uint64_t *msgs_out, uint64_t *challenges_out,
+                            uint64_t *state_out);
 /* Tail of prove_parallel (prover.rs:544-568) + get_mle_final_evaluations (:474-490): fixes the last
  * challenge and writes n_mles x [c0,c1]. */
 int dp_sc_finish(dp_sc *s, const uint64_t *last_challenge, uint64_t *out_final_evals);
@@ -149,7 +163,8 @@ int dp_logup_outputs(const dp_logup *l, uint64_t out[8]);                    /* 
  * [num_low, num_high, den_low, den_high] (or [den_low, den_high] for the initial lookup layer). */
 int dp_logup_layer_mles(const dp_logup *l, uint32_t layer_vars, dp_mle **out_views, uint32_t *n_views);
 int dp_logup_free(dp_logup *l);
-/* *n_layers = how many layers, from the layer whose halves have first_layer variables upwards, dp_logup_run_layers_fs proves for this
+/* *n_layers = how many layers, from the layer whose halves have first_layer variables upwards, dp_logup_run_layers_fs (or, for a
+ * BlakeTranscript, dp_logup_run_layers_fs_blake) proves for this
  * batch of circuits (0: none, the caller proves each layer with the sumcheck entry points).  Nonzero only in the blocking wait mode
  * (dp_set_wait_mode(1)), for at most 16 circuits of one size and layers whose first sumcheck round is small enough to run resident. */
 int dp_logup_layers_fs_next(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t *n_layers);
@@ -165,6 +180,11 @@ int dp_logup_layers_fs_next(dp_logup *const *circuits, uint32_t n_circuits, uint
 int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
                            uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
                            uint64_t *evals_out);
+/* dp_logup_run_layers_fs with BlakeTranscript's Fiat-Shamir on the device; state: a DP_B3T_WORDS image, in and out.  Arguments,
+ * outputs and DP_ERR_STATE as dp_logup_run_layers_fs; DP_ERR_INVALID for an invalid image. */
+int dp_logup_run_layers_fs_blake(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
+                                 uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *state, uint64_t *msgs_out, uint64_t *challenges_out,
+                                 uint64_t *evals_out);
 /* out = sum_k coefs[k] * mles[k] over Ext MLEs of equal length (same_poly.rs:91-110 final_beta). */
 int dp_mle_linear_combination(dp_mle *const *mles, const uint64_t *coefs, uint32_t n, dp_mle **out);
 

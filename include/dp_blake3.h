@@ -3,7 +3,8 @@
  * Used by the `blake` variant of the path (mpcs/src/util/hash.rs:79-95 BlakeHasher, transcript/src/blake.rs BlakeTranscript),
  * which -- unlike the Poseidon2 variant -- is fully determined by the reference's own sources plus this standard primitive,
  * so it can be PINNED: tests/test_blake.py checks this file against the Python `blake3` package on many lengths, offsets and
- * output sizes.  Header-only, host code (the device has its own single-chunk compression in csrc/blake3.cuh). */
+ * output sizes.  Header-only, host code (the device has its own compression and incremental hasher in csrc/blake3.cuh; Hasher::save /
+ * load exchange the state with it). */
 #ifndef DP_BLAKE3_H
 #define DP_BLAKE3_H
 #include <stdint.h>
@@ -75,9 +76,38 @@ static inline Output parent_output(const uint32_t l[8], const uint32_t r[8], con
     Output o; memcpy(o.cv, key, 32); memcpy(o.block, l, 32); memcpy(o.block + 8, r, 32); o.counter = 0; o.block_len = (uint32_t)BLOCK_LEN; o.flags = PARENT | flags; return o;
 }
 
+/* The hasher's state as IMAGE_WORDS u64 words -- the image a BlakeTranscript hands to the device (include/deepprove_b200.h,
+ * DP_B3T_WORDS): [0..3] chunk chaining value (8 x u32, little-endian pairs), [4] chunk_counter, [5..12] the 64-byte block buffer,
+ * [13] block_len, [14] blocks_compressed, [15] stack_len, [16 + 4i .. 19 + 4i] stack entry i.  Unkeyed hashing only (key = IV,
+ * no mode flags).  image_ok: the image is one a Hasher can be in. */
+static const size_t IMAGE_STACK = 16, IMAGE_WORDS = 16 + 4 * IMAGE_STACK;
+static inline bool image_ok(const uint64_t *w) {
+    if (w[13] > BLOCK_LEN || w[14] > 15 || (w[14] > 0 && w[13] == 0) || w[15] > IMAGE_STACK || w[15] != (uint64_t)__builtin_popcountll(w[4])) return false;
+    for (size_t i = (size_t)w[13]; i < BLOCK_LEN; i++) if ((uint8_t)(w[5 + i / 8] >> (8 * (i % 8))) != 0) return false;
+    return true;
+}
+
 class Hasher {
   public:
     Hasher() { memcpy(key_, IV, 32); chunk_.init(key_, 0, 0); stack_len_ = 0; }
+    /* false (nothing written) when the stack is deeper than IMAGE_STACK: more than 2^16 chunks absorbed */
+    bool save(uint64_t *w) const {
+        if (stack_len_ > IMAGE_STACK) return false;
+        memset(w, 0, 8 * IMAGE_WORDS);
+        put8(w, chunk_.cv); w[4] = chunk_.chunk_counter;
+        for (int i = 0; i < 64; i++) w[5 + i / 8] |= (uint64_t)chunk_.block[i] << (8 * (i % 8));
+        w[13] = chunk_.block_len; w[14] = chunk_.blocks_compressed; w[15] = stack_len_;
+        for (size_t i = 0; i < stack_len_; i++) put8(w + 16 + 4 * i, stack_[i]);
+        return true;
+    }
+    /* an image that passes image_ok */
+    void load(const uint64_t *w) {
+        memcpy(key_, IV, 32); chunk_.init(key_, w[4], 0);
+        get8(w, chunk_.cv);
+        for (int i = 0; i < 64; i++) chunk_.block[i] = (uint8_t)(w[5 + i / 8] >> (8 * (i % 8)));
+        chunk_.block_len = (uint8_t)w[13]; chunk_.blocks_compressed = (uint8_t)w[14]; stack_len_ = (size_t)w[15];
+        for (size_t i = 0; i < stack_len_; i++) get8(w + 16 + 4 * i, stack_[i]);
+    }
     void update(const void *data, size_t n) {
         const uint8_t *in = (const uint8_t *)data;
         while (n > 0) {
@@ -98,6 +128,8 @@ class Hasher {
         o.root_bytes(out, n);
     }
   private:
+    static void put8(uint64_t *w, const uint32_t v[8]) { for (int k = 0; k < 4; k++) w[k] = (uint64_t)v[2 * k] | ((uint64_t)v[2 * k + 1] << 32); }
+    static void get8(const uint64_t *w, uint32_t v[8]) { for (int k = 0; k < 4; k++) { v[2 * k] = (uint32_t)w[k]; v[2 * k + 1] = (uint32_t)(w[k] >> 32); } }
     void add_chunk_cv(uint32_t cv[8], uint64_t total_chunks) {
         while ((total_chunks & 1) == 0) {   /* one merge per trailing zero bit of the chunk count */
             uint32_t p[8]; parent_output(stack_[stack_len_ - 1], cv, key_, 0).chaining_value(p); memcpy(cv, p, 32); stack_len_--; total_chunks >>= 1;

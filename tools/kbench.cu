@@ -11,6 +11,7 @@
 #include <thread>
 #include <atomic>
 #include "../deep-prove_b200/csrc/poseidon2.cuh"
+#include "../deep-prove_b200/csrc/blake3.cuh"
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); exit(1); } } while (0)
 static u64 sm64(u64 &st) { u64 z = (st += 0x9E3779B97F4A7C15ULL); z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL; z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL; return z ^ (z >> 31); }
@@ -432,6 +433,41 @@ static void host_sum_e(const gle *d, int blocks, gle out[4]) {
     for (int t = 0; t < 4; t++) { gle s = e_zero(); for (int b = 0; b < blocks; b++) s = e_add(s, h[4 * b + t]); out[t] = s; }
 }
 
+// ---- fs: one round of the resident tail's device transcript (csrc/sumcheck.cu TrP2 / TrB3) alone, `rounds` rounds back to back in a
+// 1-block kernel: absorb a degree-D message (D + 1 extension elements) and the "Internal round" label, draw the challenge.  The
+// message of round r is derived from the previous challenge, so the rounds form one dependent chain as in the kernel.
+static constexpr u64 FS_LBL0 = 0x6c616e7265746e49ULL, FS_LBL1 = 0x646e756f7220ULL;   // "Internal", " round"
+template <int D> __global__ void k_fs_p2(u64 *w, int rounds) {                        // BasicTranscript: warp 0, 8-lane groups
+    if (threadIdx.x >= 32) return;
+    const int l8 = threadIdx.x & 7;
+    P2Sponge s; p2s_load(s, w, l8);
+    u64 c = 1;
+    for (int r = 0; r < rounds; r++) {
+        for (int t = 0; t < 2 * (D + 1); t++) p2s_observe(s, gl_canon(c * (t + 3)), l8);
+        p2s_observe(s, FS_LBL0, l8); p2s_observe(s, FS_LBL1, l8);
+        const u64 c0 = p2s_sample(s, l8), c1 = p2s_sample(s, l8);
+        c = c0 ^ c1;
+    }
+    __syncwarp();
+    if (threadIdx.x < 8) p2s_store(s, w, l8);
+}
+template <int D> __global__ void k_fs_b3(u64 *w, int rounds) {                        // BlakeTranscript: thread 0, image in shared memory
+    __shared__ u64 img[80];
+    for (int i = threadIdx.x; i < 80; i += blockDim.x) img[i] = w[i];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        u64 c = 1;
+        for (int r = 0; r < rounds; r++) {
+            for (int t = 0; t <= D; t++) b3::t_append_ext(img, gl_canon(c * (2 * t + 3)), gl_canon(c * (2 * t + 4)));
+            b3::t_append_fe(img, FS_LBL0); b3::t_append_fe(img, FS_LBL1);
+            u64 c0, c1; b3::t_challenge(img, c0, c1);
+            c = c0 ^ c1;
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 80; i += blockDim.x) w[i] = img[i];
+}
+
 // =====================================================================================================================
 int main(int argc, char **argv) {
     auto want = [&](const char *s) { if (argc <= 1) return true; for (int i = 1; i < argc; i++) if (!strcmp(argv[i], s)) return true; return false; };
@@ -442,6 +478,19 @@ int main(int argc, char **argv) {
     CK(p2_upload_constants((const u64 *)&DP_P2_EXT_RC[0][0][0], (const u64 *)DP_P2_INT_RC, (const u64 *)DP_P2_DIAG));
     u64 st = 7;
     char *flush = nullptr; CK(cudaMalloc(&flush, 256u << 20));
+
+    if (want("fs")) {
+        const int rounds = 2000;
+        u64 *w; CK(cudaMalloc(&w, 80 * 8)); CK(cudaMemset(w, 0, 80 * 8));
+        printf("[fs] device transcript step alone, one 1-block kernel of %d dependent rounds (256 threads)\n", rounds);
+        auto run = [&](const char *name, auto kern) {
+            const float ms = time_ms([&] { CK(cudaMemset(w, 0, 80 * 8)); kern<<<1, 256>>>(w, rounds); });
+            printf("  %-40s %8.2f us per round\n", name, 1e3 * ms / rounds);
+        };
+        run("Poseidon2 sponge (warp 0), degree 2", k_fs_p2<2>); run("Poseidon2 sponge (warp 0), degree 3", k_fs_p2<3>);
+        run("BLAKE3 hasher (thread 0), degree 2", k_fs_b3<2>); run("BLAKE3 hasher (thread 0), degree 3", k_fs_b3<3>);
+        cudaFree(w);
+    }
 
     if (want("perm")) {
         const u64 n_out = 1ULL << 22;     // 2^22 compressions = 2^23 permutations; 256 MB in, 128 MB out (> L2)

@@ -1,14 +1,23 @@
 #!/usr/bin/env python3
 """Where does multi-proof throughput saturate?  Dense-4M proofs/s and kernel launches/s against the number of proving threads
-(each with its own stream + arena) on one GPU.   usage: throughput_probe.py [workers ...]"""
-import os, sys, time
+(each with its own stream + arena) on one GPU.
+    usage: throughput_probe.py [dense4m|cnn264k] [workers ...] [--hasher poseidon2|blake3] [--wait spin|block]
+--hasher blake3 proves under the `blake` feature (BlakeHasher + BlakeTranscript); --wait block lets the proving threads sleep on the
+library's poller, the configuration in which the resident kernels run the transcript on the device."""
+import argparse, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "deep-prove_b200"))
 import bench, dpb200 as dp
-which = sys.argv[1] if len(sys.argv) > 1 and not sys.argv[1].isdigit() else "dense4m"
-ws = [int(a) for a in sys.argv[1:] if a.isdigit()] or [1, 4, 8, 16, 24, 32, 48, 64]
+ap = argparse.ArgumentParser()
+ap.add_argument("args", nargs="*")
+ap.add_argument("--hasher", default="poseidon2", choices=["poseidon2", "blake3"])
+ap.add_argument("--wait", default="spin", choices=["spin", "block"])
+a = ap.parse_args()
+which = a.args[0] if a.args and not a.args[0].isdigit() else "dense4m"
+ws = [int(x) for x in a.args if x.isdigit()] or [1, 4, 8, 16, 24, 32, 48, 64]
 wl = bench.DenseWorkload() if which == "dense4m" else bench.CnnWorkload()
-dp.init(0); wl.setup_device(dp)
+dp.init(0); dp.set_hasher(1 if a.hasher == "blake3" else 0); wl.setup_device(dp); dp.set_wait_mode(1 if a.wait == "block" else 0)
+print("%s, hasher %s, wait mode %s" % (which, a.hasher, a.wait))
 def cpu_stat():
     d = {}
     try:
