@@ -152,3 +152,17 @@ __device__ __forceinline__ void t_challenge(u64 *w, u64 &a, u64 &b) {
     do { t_absorb(w, le_word("challeng", 8), 8); t_absorb(w, le_word("e", 1), 1); t_finalize16(w, a, b); } while (a >= GL_P || b >= GL_P);
 }
 }  // namespace b3
+
+// TrB3: BlakeTranscript as a transcript policy of the resident sumcheck kernels (see TrP2 in poseidon2.cuh), the hasher above on
+// thread 0, working on the image in place.
+struct TrB3 {
+    static constexpr int WORDS = b3::T_STACK + 4 * b3::T_STACK_MAX;
+    __device__ static bool runs() { return threadIdx.x == 0; }
+    u64 *w;
+    __device__ explicit TrB3(u64 *img) : w(img) {}
+    __device__ void ext(gle e) { b3::t_append_ext(w, e.c0, e.c1); }
+    __device__ void usize(u64 v) { b3::t_append_fe(w, v); }
+    __device__ void label(const u64 (&l)[2]) { b3::t_append_fe(w, l[0]); b3::t_append_fe(w, l[1]); }   // one field element per 8 bytes
+    __device__ gle challenge() { u64 a, b; b3::t_challenge(w, a, b); return e_make(a, b); }
+    __device__ void store(u64 *dst, u64 *also) { for (int i = 0; i < WORDS; i++) { if (dst != w) dst[i] = w[i]; if (also) also[i] = w[i]; } }
+};

@@ -216,6 +216,21 @@ __device__ __forceinline__ u64 p2s_sample(P2Sponge &s, int lane8) {
     return shfl8(s.st, (int)--s.nout);
 }
 
+// The transcripts of the resident sumcheck kernels are compile-time policies (TrP2 here, TrB3 in blake3.cuh).  The threads of a block
+// for which runs() holds build one and call its members together; the state image lives in shared memory between calls and the
+// challenges are valid in thread 0.  TrP2: BasicTranscript, the sponge above on the 8-lane groups of warp 0.
+struct TrP2 {
+    static constexpr int WORDS = P2S_WORDS;
+    __device__ static bool runs() { return threadIdx.x < 32; }
+    P2Sponge s; int l8;
+    __device__ explicit TrP2(const u64 *w) : l8(threadIdx.x & 7) { p2s_load(s, w, l8); }
+    __device__ void ext(gle e) { p2s_observe(s, e.c0, l8); p2s_observe(s, e.c1, l8); }                 // append_field_element_ext
+    __device__ void usize(u64 v) { p2s_observe(s, v, l8); }                                             // append_usize
+    __device__ void label(const u64 (&w)[2]) { p2s_observe(s, w[0], l8); p2s_observe(s, w[1], l8); }   // append_message, 9..16 bytes
+    __device__ gle challenge() { const u64 c0 = p2s_sample(s, l8), c1 = p2s_sample(s, l8); return e_make(c0, c1); }
+    __device__ void store(u64 *w, u64 *also /* or null */) { __syncwarp(); if (threadIdx.x < 8) { p2s_store(s, w, l8); if (also) p2s_store(s, also, l8); } }
+};
+
 // compress(x, y): absorb x -> permute -> overwrite rate with y -> permute -> [s3, s2, s1, s0]  (one copy of the permutation: see above)
 __device__ __forceinline__ void p2_compress(const u64 x[4], const u64 y[4], u64 out[4]) {
     u64 s[8] = {x[0], x[1], x[2], x[3], 0, 0, 0, 0};

@@ -13,7 +13,8 @@
 // partials -- field addition is exact, so the summation order is free and the result is bit-identical
 // to the reference's rayon fold.  The (deg+1) sums per product go back through a pinned buffer; the
 // O(deg^2) glue (2^k multiplicity, coefficient, barycentric extrapolation -- prover.rs:713-724,
-// util.rs:101-136) runs on the host inside dp_sc_round, exactly where the reference has it.
+// util.rs:101-136) is one rule, sc_glue_product: the host applies it inside dp_sc_round, and CTA 0 of
+// the resident kernel applies it when the kernel runs the transcript itself.
 #include "common.cuh"
 #include "poseidon2.cuh"
 #include "blake3.cuh"
@@ -475,14 +476,40 @@ __host__ __device__ inline void sc_desc(ScProd &pd, u32 p, const u32 *idx, u32 n
 }
 
 struct TProd { u32 n_idx; u32 idx[5]; };
-// Fiat-Shamir in the resident kernel (dp_sc_run_tail_fs[_blake]): what sc_glue and the transcript need.  bary[d - 1][i][j]: weight of
-// point j when a degree-d product is extrapolated to point d + 1 + i (exact constants of sc_extrapolate).
+// bary[d - 1][i][j]: weight of point j when a degree-d product's values at 0 .. d are extrapolated to point d + 1 + i (sc_bary)
+typedef u64 ScBary[4][4][5];
+
+// The glue of one product (prover.rs:694-724, sumcheck_macro/src/lib.rs:242): its d + 1 sums v[0..d] times the multiplicity
+// 2^(max_nv - (l2 + R - 1)) of its MLEs' `len` entries in round R (l2 >= 1), times the coefficient, then extrapolated to v[0..max_deg].
+// False: a negative multiplicity, which the host refuses (on the device dp_sc_create's num_vars bound rules it out).  The host's rounds
+// (sc_glue) and the device transcript's (sc_res_fs_round) share it; on the device the multiply stays out of line (see e_mul_ni).
+__host__ __device__ inline gle sc_glue_mul(gle a, gle b) {
+#ifdef __CUDA_ARCH__
+    return e_mul_ni(a, b);
+#else
+    return e_mul(a, b);
+#endif
+}
+__host__ __device__ inline bool sc_glue_product(gle *v, u32 d, u64 len, u32 max_nv, u32 R, gle coef, u32 max_deg, const ScBary &bary) {
+    u32 l2 = 1; while ((1ULL << l2) < len) l2++;
+    const int mult = (int)max_nv - (int)(l2 + R - 1);
+    const u64 scale = gl_canon(1ULL << (mult > 0 ? mult : 0));
+    for (u32 t = 0; t <= d; t++) { gle x = v[t]; if (mult > 0) x = e_mul_base(x, scale); v[t] = sc_glue_mul(x, coef); }
+    for (u32 i = 0; d + 1 + i <= max_deg; i++) {
+        gle x = e_zero();
+        for (u32 j = 0; j <= d; j++) x = e_add(x, e_mul_base(v[j], bary[d - 1][i][j]));
+        v[d + 1 + i] = x;
+    }
+    return mult >= 0;
+}
+
+// Fiat-Shamir in the resident kernels (dp_sc_run_tail_fs[_blake], dp_logup_run_layers_fs[_blake]): what the glue and the transcript need
 static constexpr u32 SC_MAX_ROUNDS = 40;
 // sponge: the transcript's state, the larger of the two images (TrP2: P2S_WORDS, TrB3: DP_B3T_WORDS)
 static constexpr int SC_FS_WORDS = DP_B3T_WORDS;
 static_assert(P2S_WORDS <= SC_FS_WORDS && DP_B3T_WORDS == (int)dpb3::IMAGE_WORDS && DP_B3T_STACK == (int)dpb3::IMAGE_STACK &&
-              DP_B3T_STACK == (int)b3::T_STACK_MAX, "one BLAKE3 state image");
-struct ScTailFs { u32 max_deg, max_nv, round0, pad; u64 label[2]; u64 coef[SC_RES_MAXP][2]; u64 bary[4][4][5]; u64 sponge[SC_FS_WORDS]; };
+              DP_B3T_STACK == (int)b3::T_STACK_MAX && DP_B3T_WORDS == TrB3::WORDS, "one BLAKE3 state image");
+struct ScTailFs { u32 max_deg, max_nv, round0, pad; u64 label[2]; u64 coef[SC_RES_MAXP][2]; ScBary bary; u64 sponge[SC_FS_WORDS]; };
 struct ScTailFsOut { gle msg[SC_MAX_ROUNDS][SC_NACC]; gle chal[SC_MAX_ROUNDS]; u64 sponge[SC_FS_WORDS]; };
 struct ScTail { u32 n_mles, n_products, n_rounds, first_has_challenge; ScMle m[SC_RES_MAXM]; u32 writer[SC_RES_MAXM]; TProd p[SC_RES_MAXP]; ScTailFs fs; };
 
@@ -493,54 +520,16 @@ __device__ __forceinline__ void cl_sync() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// The transcript of the resident kernels, a compile-time policy.  CTA 0's threads for which runs() holds build one and call its
-// members together; the state image lives in shared memory between calls and the challenges are valid in thread 0.
-// TrP2: BasicTranscript, the Poseidon2 duplex sponge on the 8-lane groups of warp 0 (poseidon2.cuh P2Sponge).
-struct TrP2 {
-    static constexpr int WORDS = P2S_WORDS;
-    __device__ static bool runs() { return threadIdx.x < 32; }
-    P2Sponge s; int l8;
-    __device__ explicit TrP2(const u64 *w) : l8(threadIdx.x & 7) { p2s_load(s, w, l8); }
-    __device__ void ext(gle e) { p2s_observe(s, e.c0, l8); p2s_observe(s, e.c1, l8); }                 // append_field_element_ext
-    __device__ void usize(u64 v) { p2s_observe(s, v, l8); }                                             // append_usize
-    __device__ void label(const u64 (&w)[2]) { p2s_observe(s, w[0], l8); p2s_observe(s, w[1], l8); }   // append_message, 9..16 bytes
-    __device__ gle challenge() { const u64 c0 = p2s_sample(s, l8), c1 = p2s_sample(s, l8); return e_make(c0, c1); }
-    __device__ void store(u64 *w, u64 *also /* or null */) { __syncwarp(); if (threadIdx.x < 8) { p2s_store(s, w, l8); if (also) p2s_store(s, also, l8); } }
-};
-// TrB3: BlakeTranscript, the incremental BLAKE3 hasher of blake3.cuh on thread 0, working on the image in place.
-struct TrB3 {
-    static constexpr int WORDS = DP_B3T_WORDS;
-    __device__ static bool runs() { return threadIdx.x == 0; }
-    u64 *w;
-    __device__ explicit TrB3(u64 *img) : w(img) {}
-    __device__ void ext(gle e) { b3::t_append_ext(w, e.c0, e.c1); }
-    __device__ void usize(u64 v) { b3::t_append_fe(w, v); }
-    __device__ void label(const u64 (&l)[2]) { b3::t_append_fe(w, l[0]); b3::t_append_fe(w, l[1]); }   // one field element per 8 bytes
-    __device__ gle challenge() { u64 a, b; b3::t_challenge(w, a, b); return e_make(a, b); }
-    __device__ void store(u64 *dst, u64 *also) { for (int i = 0; i < WORDS; i++) { if (dst != w) dst[i] = w[i]; if (also) also[i] = w[i]; } }
-};
-
 // Round k of the device-transcript tail, in CTA 0 once the product sums are in sprod and this round's folds are committed to sm:
-// sc_glue (one thread per product, on the lengths the host's bookkeeping has after the fold), the sum over products, then the
-// transcript TR -- append_field_element_exts(message), get_and_append_challenge("Internal round") -- and the challenge goes to xctl
-// for the cluster.  Out of line: the round loop keeps its registers (transcript state in shared memory between rounds).
+// the glue (one thread per product, on the lengths the host's bookkeeping has after the fold), the sum over products, then the
+// transcript TR (TrP2 or TrB3) -- append_field_element_exts(message), get_and_append_challenge("Internal round") -- and the challenge
+// goes to xctl for the cluster.  Out of line: the round loop keeps its registers (transcript state in shared memory between rounds).
 template <class TR>
 __device__ __noinline__ void sc_res_fs_round(ScTailFs &f, gle (*sprod)[SC_NACC], const TProd *sp, const ScMle *sm, u32 np, u32 k, bool last,
                                              ScTailFsOut *fsout, u64 *xctl) {
     const u32 R = f.round0 + k + 1, max_deg = f.max_deg;
-    for (u32 p = threadIdx.x; p < np; p += blockDim.x) {
-        const u32 d = sp[p].n_idx; const u64 len = sm[sp[p].idx[0]].len;
-        u32 l2 = 1; while ((1ULL << l2) < len) l2++;
-        const int mult = (int)f.max_nv - (int)(l2 + R - 1);      // >= 0: dp_sc_create bounds every MLE's num_vars by max_nv
-        const gle coef = e_make(f.coef[p][0], f.coef[p][1]);
-        const u64 scale = gl_canon(1ULL << (mult > 0 ? mult : 0));
-        for (u32 t = 0; t <= d; t++) { gle v = sprod[p][t]; if (mult > 0) v = e_mul_base(v, scale); sprod[p][t] = e_mul_ni(v, coef); }
-        for (u32 i = 0; d + 1 + i <= max_deg; i++) {
-            gle v = e_zero();
-            for (u32 j = 0; j <= d; j++) v = e_add(v, e_mul_base(sprod[p][j], f.bary[d - 1][i][j]));
-            sprod[p][d + 1 + i] = v;
-        }
-    }
+    for (u32 p = threadIdx.x; p < np; p += blockDim.x)
+        sc_glue_product(sprod[p], sp[p].n_idx, sm[sp[p].idx[0]].len, f.max_nv, R, e_make(f.coef[p][0], f.coef[p][1]), max_deg, f.bary);
     __syncthreads();
     for (u32 t = threadIdx.x; t <= max_deg; t += blockDim.x) {
         gle v = e_zero();
@@ -707,8 +696,8 @@ struct LgCfg {
     gle point[SC_MAX_ROUNDS + 1];                                  // layer `first`'s point (its last entry is the batching challenge)
     const gle *num[LG_MAXL][LG_MAXC], *den[LG_MAXL][LG_MAXC];     // layer first + l of circuit c: [lo | hi]; num null: numerators all -1
     gle *eq, *work; u64 work_stride;                               // device scratch: the eq table, each MLE's ping-pong tables
-    u64 round_label[2], label[3][2];                               // "Internal round"; "logup_batching", "logup_alpha", "logup_lambda"
-    u64 bary[4][4][5]; u64 sponge[SC_FS_WORDS];
+    u64 label[3][2];                                               // "logup_batching", "logup_alpha", "logup_lambda"
+    ScTailFs fs;                                                   // the rounds' transcript; coef and max_nv are set per layer
 };
 struct LgLayerOut { ScTailFsOut fs; gle evals[SC_RES_MAXM]; };
 struct LgOut { LgLayerOut layer[LG_MAXL]; gle point[SC_MAX_ROUNDS + 1]; gle claim, alpha, lambda; u64 sponge[SC_FS_WORDS]; u64 flag; };
@@ -821,13 +810,10 @@ k_logup_res(const LgCfg *__restrict__ cfg, LgOut *out /* mapped */, gle *xpart, 
     __shared__ ScResSmem S;
     __shared__ LgSmem L;
     if (cl_rank() == 0) {
-        if (threadIdx.x == 0) {
-            L.alpha = cfg->alpha; L.lambda = cfg->lambda; L.claim = cfg->claim;
-            S.sfs.label[0] = cfg->round_label[0]; S.sfs.label[1] = cfg->round_label[1]; S.sfs.max_deg = 3; S.sfs.round0 = 0;
-        }
-        for (u32 i = threadIdx.x; i < TR::WORDS; i += blockDim.x) S.sfs.sponge[i] = cfg->sponge[i];
-        for (u32 i = threadIdx.x; i < 4 * 4 * 5; i += blockDim.x) (&S.sfs.bary[0][0][0])[i] = (&cfg->bary[0][0][0])[i];
+        if (threadIdx.x == 0) { L.alpha = cfg->alpha; L.lambda = cfg->lambda; L.claim = cfg->claim; }
+        for (u32 i = threadIdx.x; i < sizeof(ScTailFs) / 8; i += blockDim.x) ((u64 *)&S.sfs)[i] = ((const u64 *)&cfg->fs)[i];
     }
+    __syncthreads();                                               // the copied state is complete before lg_layer_begin reads and writes it
     for (u32 l = 0; l < cfg->n_layers; l++) {
         lg_layer_begin<TR>(cfg, S, L, l, xpoint);
         cl_sync();                                                 // the eq table of every CTA is visible
@@ -864,28 +850,28 @@ struct dp_sc {
     gle *h_pairs = nullptr; bool have_pairs = false;
     u64 seq = 0; u64 *h_flag = nullptr; u32 *d_done = nullptr;
     int gx = 1;
-    bool tail_enabled = false, tail_active = false; u32 tail_last_round = 0;
+    bool tail_enabled = false, tail_active = false;
     ScTail *h_tail = nullptr; u64 *h_chal = nullptr; ScTailFsOut *h_fs = nullptr;
     gle *d_xpart = nullptr; u64 *d_xctl = nullptr;        // resident cluster kernel: warp partials, [status, c0, c1]
     std::vector<gle> challenges;
 };
 
-static u32 ceil_log2_u64(u64 x) { u32 l = 0; while ((1ULL << l) < x) l++; return l; }
-
-// barycentric extrapolation of a degree-(n-1) polynomial given at 0..n-1 to the point `at`
-// (sumcheck/src/util.rs:19-136; exact arithmetic, so plain Lagrange gives the same element)
-static u64 sc_bary_weight(u32 n, u64 at, u32 j) {
-    u64 num = 1, den = 1;
-    for (u32 i = 0; i < n; i++) if (i != j) {
-        num = gl_mul(num, gl_sub(gl_canon(at), (u64)i));
-        den = gl_mul(den, gl_sub((u64)j, (u64)i));
-    }
-    return gl_mul(num, gl_inv(den));
-}
-static gle sc_extrapolate(const gle *evals, u32 n, u64 at) {
-    gle res = e_zero();
-    for (u32 j = 0; j < n; j++) res = e_add(res, e_mul_base(evals[j], sc_bary_weight(n, at, j)));
-    return res;
+// The weights of ScBary for every degree up to 5 (dp_sc_create's bound): barycentric extrapolation, sumcheck/src/util.rs:19-136 (exact
+// arithmetic, so plain Lagrange gives the same element).  Built once per process.
+static const ScBary &sc_bary() {
+    static const struct Tab {
+        ScBary w = {};
+        Tab() {
+            for (u32 d = 1; d <= 4; d++)
+                for (u32 i = 0; d + 1 + i <= 5; i++)
+                    for (u32 j = 0; j <= d; j++) {
+                        u64 num = 1, den = 1;
+                        for (u32 q = 0; q <= d; q++) if (q != j) { num = gl_mul(num, gl_sub(d + 1 + i, q)); den = gl_mul(den, gl_sub(j, q)); }
+                        w[d - 1][i][j] = gl_mul(num, gl_inv(den));
+                    }
+        }
+    } tab;
+    return tab.w;
 }
 
 static int sc_free_all(dp_sc *s) {
@@ -899,32 +885,21 @@ static int sc_free_all(dp_sc *s) {
     return DP_OK;
 }
 
-// host glue: multiplicity, coefficient, extrapolation, sum over products (prover.rs:694-733)
+// host glue: every product's sums through sc_glue_product, summed over products (prover.rs:694-733)
 static int sc_glue(dp_sc *s, uint64_t *out_evals) {
-    gle msg[SC_NACC + 1];
+    gle msg[SC_NACC];
     for (u32 t = 0; t <= s->max_deg; t++) msg[t] = e_zero();
     for (u32 p = 0; p < s->n_products; p++) {
         const dp_sc_product &pr = s->products[p];
-        u32 d = pr.n_idx;
-        gle sum[16];
-        u64 len = s->mles[pr.idx[0]].len;
-        u32 l2 = std::max<u32>(ceil_log2_u64(len), 1);
-        int mult = (int)s->max_nv - (int)(l2 + s->round - 1);  // sumcheck_macro/src/lib.rs:242
-        DP_CHECK(mult >= 0, DP_ERR_INVALID, "dp_sc_round: negative num_vars multiplicity");
-        gle coef = e_make(pr.coef[0], pr.coef[1]);
-        for (u32 t = 0; t <= d; t++) {
-            gle v = s->h_out[p * SC_NACC + t];
-            if (mult > 0) v = e_mul_base(v, gl_canon(1ULL << mult));
-            sum[t] = e_mul(v, coef);
-        }
-        for (u32 i = 0; i < s->max_deg - d; i++) sum[d + 1 + i] = sc_extrapolate(sum, d + 1, d + 1 + i);
-        for (u32 t = 0; t <= s->max_deg; t++) msg[t] = e_add(msg[t], sum[t]);
+        gle v[SC_NACC];
+        for (u32 t = 0; t <= pr.n_idx; t++) v[t] = s->h_out[p * SC_NACC + t];
+        DP_CHECK(sc_glue_product(v, pr.n_idx, s->mles[pr.idx[0]].len, s->max_nv, s->round, e_make(pr.coef[0], pr.coef[1]), s->max_deg, sc_bary()),
+                 DP_ERR_INVALID, "dp_sc_round: negative num_vars multiplicity");
+        for (u32 t = 0; t <= s->max_deg; t++) msg[t] = e_add(msg[t], v[t]);
     }
     for (u32 t = 0; t <= s->max_deg; t++) { out_evals[2 * t] = msg[t].c0; out_evals[2 * t + 1] = msg[t].c1; }
     return DP_OK;
 }
-
-
 
 // Can a resident kernel talk to the host while it runs?  Not under tools that serialise launches (Nsight Compute blocks the
 // launching thread until the profiled kernel has finished, so the kernel would wait for a challenge its host cannot post).
@@ -975,55 +950,87 @@ static decltype(&k_sc_round<0>) const k_sc_lean_md[4][2] = {{k_sc_lean<2, OPM_B>
                                                               {k_sc_lean<2, OPM_BF>, k_sc_lean<3, OPM_BF>}, {k_sc_lean<2, OPM_EF>, k_sc_lean<3, OPM_EF>}};
 static constexpr int SC_LEAN_BLOCK[4] = {ScLeanShape<OPM_B>::BLOCK, ScLeanShape<OPM_E>::BLOCK, ScLeanShape<OPM_BF>::BLOCK, ScLeanShape<OPM_EF>::BLOCK};
 
+// The cluster of a resident launch whose first round has `work` pair-items over np products: ~512 pair-items per CTA, a power of two
+// <= SC_RES_MAXCTA (portable cluster size); and the warp-partial slots of its xpart scratch (one per warp, at least one per product).
+struct ScResShape { u32 ncta, slots; };
+static ScResShape sc_res_shape(u64 work, u32 np) {
+    u32 ncta = 1; while (ncta < SC_RES_MAXCTA && (u64)ncta * 512 < work) ncta <<= 1;
+    return {ncta, std::max<u32>(ncta * (SC_THREADS / 32), np)};
+}
+// launch a resident kernel as one cluster of ncta CTAs on the context's stream, profiled as `name`
+template <class K, class... A>
+static int sc_res_launch(const char *name, u32 ncta, K kern, A... args) {
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t lc{};
+    lc.gridDim = dim3(ncta); lc.blockDim = dim3(SC_THREADS); lc.dynamicSmemBytes = 0; lc.stream = dp_ctx().stream;
+    lc.attrs = at; lc.numAttrs = 1;
+    DpProfScope prof(name, 0);
+    const cudaError_t ce = cudaLaunchKernelEx(&lc, kern, args...);
+    DP_LAUNCHED();
+    DP_CUDA(ce);
+    DP_CUDA(cudaGetLastError());
+    return DP_OK;
+}
+
+// The previous round's challenge (prover.rs:655-669): none before round 0, one after it; recorded, and the first one refuses constant
+// MLEs.  r: the challenge (zero in round 0); returns whether this round folds by it.
+static int sc_take_challenge(dp_sc *s, const uint64_t *challenge, gle &r, bool &fold) {
+    r = e_zero(); fold = s->round > 0;
+    if (!fold) { DP_CHECK(challenge == nullptr, DP_ERR_STATE, "first round should be prover first."); return DP_OK; }   // prover.rs:655
+    DP_CHECK(challenge != nullptr, DP_ERR_STATE, "verifier message is empty");  // prover.rs:657
+    r = e_from_host(challenge);
+    s->challenges.push_back(r);
+    if (s->challenges.size() == 1)
+        for (auto &m : s->mles) DP_CHECK(m.len > 1, DP_ERR_INVALID, "calling sumcheck on constant");  // prover.rs:667-669
+    return DP_OK;
+}
+// one round's fold done by the resident kernel: the tables now live in its bookkeeping
+static void sc_fold_in_kernel(dp_sc *s) {
+    for (auto &m : s->mles) if (m.len > 1) { m.len >>= 1; m.is_ext = true; m.cur = nullptr; m.where = 3; }
+}
+// wait for the resident kernel's flag with tag s->seq; when it does not come, release the kernel and refuse with `msg`
+static int sc_tail_wait(dp_sc *s, const std::string &msg) {
+    if (dp_wait_flag(s->h_flag, s->seq, true, SC_TAIL_FAILED, 8.0) == s->seq) return DP_OK;
+    s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(dp_ctx().stream);
+    return dp_fail(DP_ERR_CUDA, msg);
+}
+
 // start the resident kernel for all remaining rounds; the first one's message is tagged s->seq.  fs: the kernel runs the transcript
 // (BlakeTranscript when blake, else BasicTranscript) from this state and writes messages, challenges and the final state to s->h_fs
 // (null: the host posts every challenge).
 static int sc_tail_launch(dp_sc *s, gle r, bool fold, const ScTailFs *fs, bool blake = false) {
-    cudaStream_t st = dp_ctx().stream;
-    {
-        int e = 0;
-        if (!s->h_tail && (e = dp_pinned_alloc((void **)&s->h_tail, sizeof(ScTail)))) return e;
-        if (!s->h_chal && (e = dp_pinned_alloc((void **)&s->h_chal, 64))) return e;
-        if (fs && !s->h_fs && (e = dp_pinned_alloc((void **)&s->h_fs, sizeof(ScTailFsOut)))) return e;
-        ScTail &t = *s->h_tail;
-        t.n_mles = s->n_mles; t.n_products = s->n_products; t.n_rounds = s->max_nv - s->round; t.first_has_challenge = fold ? 1 : 0;
-        if (fs) t.fs = *fs;
-        for (u32 i = 0; i < s->n_mles; i++) {
-            ScMle &m = s->mles[i];
-            if (m.len > 1 && !m.work) { if ((e = dp_dev_alloc((void **)&m.work, sizeof(gle) * ((m.len0 >> 1) + (m.len0 >> 2) + 1)))) return e; }
-            t.m[i] = m; t.writer[i] = s->writer[i];
-        }
-        for (u32 p = 0; p < s->n_products; p++) { t.p[p].n_idx = s->products[p].n_idx; for (u32 j = 0; j < 5; j++) t.p[p].idx[j] = s->products[p].idx[j]; }
-        s->h_chal[0] = 0;
-        // cluster size by the first resident round's work: ~512 pair-items per CTA, a power of two <= 8 (portable cluster size)
-        const u64 work = sc_round_work(s, fold);
-        u32 ncta = 1; while (ncta < SC_RES_MAXCTA && (u64)ncta * 512 < work) ncta <<= 1;
-        const u32 slots = std::max<u32>(ncta * (SC_THREADS / 32), s->n_products);
-        if (!s->d_xpart && (e = dp_dev_alloc((void **)&s->d_xpart, sizeof(gle) * SC_NACC * slots))) return e;
-        if (!s->d_xctl && (e = dp_dev_alloc((void **)&s->d_xctl, 64))) return e;
-        u32 dsel = s->products[0].n_idx;
-        for (auto &pr : s->products) if (pr.n_idx != dsel) dsel = 0;
-        cudaLaunchConfig_t lc{};
-        lc.gridDim = dim3(ncta); lc.blockDim = dim3(SC_THREADS); lc.dynamicSmemBytes = 0; lc.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        lc.attrs = at; lc.numAttrs = 1;
-        DpProfScope prof(!fs ? "k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)"
-                         : blake ? "k_sc_res(resident cluster rounds, BLAKE3 device transcript)"
-                                 : "k_sc_res(resident cluster rounds with the device transcript)", 0);
-        const cudaError_t ce = cudaLaunchKernelEx(&lc, k_sc_res_dsel[fs && blake][dsel], (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs, (volatile u64 *)s->h_flag,
-                                                  (volatile u64 *)s->h_chal, s->seq, s->d_xpart, s->d_xctl, fs ? s->h_fs : (ScTailFsOut *)nullptr);
-        DP_LAUNCHED();
-        DP_CUDA(ce);
-        DP_CUDA(cudaGetLastError());
-        s->tail_active = true;
+    int e = 0;
+    if (!s->h_tail && (e = dp_pinned_alloc((void **)&s->h_tail, sizeof(ScTail)))) return e;
+    if (!s->h_chal && (e = dp_pinned_alloc((void **)&s->h_chal, 64))) return e;
+    if (fs && !s->h_fs && (e = dp_pinned_alloc((void **)&s->h_fs, sizeof(ScTailFsOut)))) return e;
+    ScTail &t = *s->h_tail;
+    t.n_mles = s->n_mles; t.n_products = s->n_products; t.n_rounds = s->max_nv - s->round; t.first_has_challenge = fold ? 1 : 0;
+    if (fs) t.fs = *fs;
+    for (u32 i = 0; i < s->n_mles; i++) {
+        ScMle &m = s->mles[i];
+        if (m.len > 1 && !m.work) { if ((e = dp_dev_alloc((void **)&m.work, sizeof(gle) * ((m.len0 >> 1) + (m.len0 >> 2) + 1)))) return e; }
+        t.m[i] = m; t.writer[i] = s->writer[i];
     }
+    for (u32 p = 0; p < s->n_products; p++) { t.p[p].n_idx = s->products[p].n_idx; for (u32 j = 0; j < 5; j++) t.p[p].idx[j] = s->products[p].idx[j]; }
+    s->h_chal[0] = 0;
+    const ScResShape sh = sc_res_shape(sc_round_work(s, fold), s->n_products);
+    if (!s->d_xpart && (e = dp_dev_alloc((void **)&s->d_xpart, sizeof(gle) * SC_NACC * sh.slots))) return e;
+    if (!s->d_xctl && (e = dp_dev_alloc((void **)&s->d_xctl, 64))) return e;
+    u32 dsel = s->products[0].n_idx;
+    for (auto &pr : s->products) if (pr.n_idx != dsel) dsel = 0;
+    if ((e = sc_res_launch(!fs ? "k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)"
+                           : blake ? "k_sc_res(resident cluster rounds, BLAKE3 device transcript)"
+                                   : "k_sc_res(resident cluster rounds with the device transcript)",
+                           sh.ncta, k_sc_res_dsel[fs && blake][dsel], (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs, (volatile u64 *)s->h_flag,
+                           (volatile u64 *)s->h_chal, s->seq, s->d_xpart, s->d_xctl, fs ? s->h_fs : (ScTailFsOut *)nullptr)))
+        return e;
+    s->tail_active = true;
     return DP_OK;
 }
 
 // one round served by the resident kernel (started here on its first round)
 static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
-    cudaStream_t st = dp_ctx().stream;
     s->seq++;
     if (!s->tail_active) {
         if (int e = sc_tail_launch(s, r, fold, nullptr)) return e;
@@ -1031,10 +1038,9 @@ static int sc_tail_round(dp_sc *s, gle r, bool fold, uint64_t *out_evals) {
         s->h_chal[1] = r.c0; s->h_chal[2] = r.c1;
         __atomic_store_n(&s->h_chal[0], s->seq, __ATOMIC_RELEASE);
     }
-    if (fold) for (auto &m : s->mles) if (m.len > 1) { m.len >>= 1; m.is_ext = true; m.cur = nullptr; m.where = 3; }   // the tables now live in the kernel's bookkeeping
+    if (fold) sc_fold_in_kernel(s);
     s->round += 1;
-    const bool ok = dp_wait_flag(s->h_flag, s->seq, true, SC_TAIL_FAILED, 8.0) == s->seq;
-    if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(st); DP_CHECK(false, DP_ERR_CUDA, "dp_sc_round: resident kernel timed out waiting for a challenge (other work queued in the same stream?)"); }
+    if (int e = sc_tail_wait(s, "dp_sc_round: resident kernel timed out waiting for a challenge (other work queued in the same stream?)")) return e;
     if (s->round == s->max_nv) s->have_pairs = true;   // written to mapped memory before the flag
     return sc_glue(s, out_evals);
 }
@@ -1052,6 +1058,65 @@ static cudaError_t sc_fs_constants() {
     return ce;
 }
 
+// The transcript state an entry point takes: BasicTranscript's 14-word sponge (canonical words, counts in range), or a valid image of
+// BlakeTranscript's hasher (dpb3::image_ok), copied into the kernel's SC_FS_WORDS buffer.  False: out of range.
+static bool fs_state_in(const uint64_t *in, bool blake, u64 *dst) {
+    if (blake) { if (!dpb3::image_ok(in)) return false; for (int w = 0; w < DP_B3T_WORDS; w++) dst[w] = in[w]; return true; }
+    if (!(in[12] < 4 && in[13] <= 4)) return false;
+    for (int w = 0; w < P2S_WORDS; w++) dst[w] = w < 12 ? gl_canon(in[w]) : in[w];
+    return true;
+}
+// ... and the state the kernel returns, in dpb3::Hasher::save's form (the stack words past stack_len, which merges leave behind in
+// the kernel, are zero).  False: the BLAKE3 hasher needed more than DP_B3T_STACK stack entries (more than 2^17 chunks).
+static bool fs_state_out(const u64 *src, bool blake, uint64_t *out) {
+    if (blake && (src[b3::T_SLEN] & b3::T_OVERFLOW)) return false;
+    const int n = blake ? b3::T_STACK + 4 * (int)src[b3::T_SLEN] : P2S_WORDS;
+    for (int w = 0; w < (blake ? DP_B3T_WORDS : P2S_WORDS); w++) out[w] = w < n ? src[w] : 0;
+    return true;
+}
+// The transcript part of a device-transcript launch's ScTailFs (fn: the entry point, for the refusal): the caller's state, refused out
+// of range; the Poseidon2 constants unless BLAKE3; the "Internal round" label (Transcript::append_message: 8-byte little-endian words);
+// the extrapolation weights.
+static int sc_fs_setup(ScTailFs &fs, const uint64_t *state_in, bool blake, const char *fn) {
+    DP_CHECK(fs_state_in(state_in, blake, fs.sponge), DP_ERR_INVALID, std::string(fn) + (blake ? ": not a BLAKE3 hasher state" : ": sponge state out of range"));
+    if (!blake) DP_CUDA(sc_fs_constants());
+    static const char label[16] = "Internal round";
+    memcpy(fs.label, label, sizeof label);
+    memcpy(fs.bary, sc_bary(), sizeof(ScBary));
+    return DP_OK;
+}
+
+static int sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
+                          uint64_t *sponge_out, bool blake) {
+    const char *const fn = blake ? "dp_sc_run_tail_fs_blake" : "dp_sc_run_tail_fs";
+    DP_CHECK(s && sponge_in && msgs_out && challenges_out && sponge_out, DP_ERR_INVALID, std::string(fn) + ": null argument");
+    DP_CHECK(!s->finished && s->round < s->max_nv && !s->tail_active, DP_ERR_STATE, "Prover is not active");
+    ScTailFs fs{};
+    if (int e = sc_fs_setup(fs, sponge_in, blake, fn)) return e;
+    DP_CHECK(sc_tail_eligible(s, s->round > 0), DP_ERR_STATE, std::string(fn) + ": the next round does not start the resident tail");
+    gle r; bool fold;
+    if (int e = sc_take_challenge(s, prev_challenge, r, fold)) return e;
+    fs.max_deg = s->max_deg; fs.max_nv = s->max_nv; fs.round0 = s->round;
+    for (u32 p = 0; p < s->n_products; p++) { fs.coef[p][0] = s->products[p].coef[0]; fs.coef[p][1] = s->products[p].coef[1]; }
+    const u32 nr = s->max_nv - s->round;
+    s->seq++;
+    if (int e = sc_tail_launch(s, r, fold, &fs, blake)) return e;
+    s->seq += nr - 1;                                              // the kernel raises the flag once, with the last round's tag
+    for (u32 k = 0; k < nr; k++) if (k > 0 || fold) sc_fold_in_kernel(s);
+    s->round = s->max_nv;
+    if (int e = sc_tail_wait(s, std::string(fn) + ": the resident kernel did not finish")) return e;
+    s->have_pairs = true;
+    const ScTailFsOut &o = *s->h_fs;
+    const u32 w = s->max_deg + 1;
+    for (u32 k = 0; k < nr; k++) {
+        for (u32 t = 0; t < w; t++) { msgs_out[2 * (k * w + t)] = o.msg[k][t].c0; msgs_out[2 * (k * w + t) + 1] = o.msg[k][t].c1; }
+        challenges_out[2 * k] = o.chal[k].c0; challenges_out[2 * k + 1] = o.chal[k].c1;
+        if (k + 1 < nr) s->challenges.push_back(o.chal[k]);     // the last one is dp_sc_finish's
+    }
+    DP_CHECK(fs_state_out(o.sponge, blake, sponge_out), DP_ERR_STATE, std::string(fn) + ": the transcript outgrew the BLAKE3 state image");
+    return DP_OK;
+}
+
 // How many layers from `first` on dp_logup_run_layers_fs takes: blocking waits, a launch that can run resident, at most LG_MAXC equal
 // circuits, and layers whose first round is resident-sized (the same SC_RES_WORK bound as the tail of a single sumcheck).
 static u32 lg_fs_layers(dp_logup *const *c, u32 n, u32 first) {
@@ -1062,6 +1127,62 @@ static u32 lg_fs_layers(dp_logup *const *c, u32 n, u32 first) {
     u32 k = 0;
     while (first + k <= total && k < LG_MAXL && first + k < SC_MAX_ROUNDS && (u64)3 * n * (1ULL << (first + k - 1)) <= SC_RES_WORK) k++;
     return k && sc_tail_supported() ? k : 0;
+}
+
+static int lg_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
+                            uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
+                            uint64_t *evals_out, bool blake) {
+    const char *const fn = blake ? "dp_logup_run_layers_fs_blake" : "dp_logup_run_layers_fs";
+    DP_CHECK(circuits && claim && point && alpha && lambda && sponge && msgs_out && challenges_out && evals_out, DP_ERR_INVALID,
+             std::string(fn) + ": null argument");
+    DP_CHECK(first_layer >= 1 && last_layer >= first_layer && last_layer - first_layer < lg_fs_layers(circuits, n_circuits, first_layer), DP_ERR_STATE,
+             std::string(fn) + ": these layers do not run resident (wait mode, circuit count or layer size)");
+    ScTailFs fs{};
+    if (int e = sc_fs_setup(fs, sponge, blake, fn)) return e;
+    const u32 nl = last_layer - first_layer + 1, n = n_circuits, np = 3 * n, nm_max = 1 + 4 * n;
+    const u64 len_max = 1ULL << last_layer, stride = (len_max >> 1) + (len_max >> 2) + 1;
+    const ScResShape sh = sc_res_shape((u64)np * (len_max >> 1), np);   // sized by the largest layer
+    LgCfg *cfg = nullptr; LgOut *out = nullptr; char *scratch = nullptr;
+    if (int e = dp_pinned_alloc((void **)&cfg, sizeof(LgCfg))) return e;
+    PinnedPtr cfg_owner(cfg);
+    if (int e = dp_pinned_alloc((void **)&out, sizeof(LgOut))) return e;
+    PinnedPtr out_owner(out);
+    const size_t off_point = 64, off_part = off_point + sizeof(gle) * (SC_MAX_ROUNDS + 1), off_eq = off_part + sizeof(gle) * SC_NACC * sh.slots,
+                 off_work = off_eq + sizeof(gle) * len_max, bytes = off_work + sizeof(gle) * stride * nm_max;
+    if (int e = dp_dev_alloc((void **)&scratch, bytes)) return e;
+    DevPtr scratch_owner(scratch);
+    memset(cfg, 0, sizeof(LgCfg));
+    cfg->n_circuits = n; cfg->first = first_layer; cfg->n_layers = nl;
+    cfg->claim = e_from_host(claim); cfg->alpha = e_from_host(alpha); cfg->lambda = e_from_host(lambda);
+    for (u32 i = 0; i < first_layer; i++) cfg->point[i] = e_from_host(point + 2 * i);
+    for (u32 l = 0; l < nl; l++) {
+        const u32 k = circuits[0]->nv - 1 - (first_layer + l);    // circuit layer with 2^(v+1) entries (dp_logup_layer_mles)
+        for (u32 c = 0; c < n; c++) { cfg->num[l][c] = circuits[c]->num[k]; cfg->den[l][c] = circuits[c]->den[k]; }
+    }
+    cfg->eq = (gle *)(scratch + off_eq); cfg->work = (gle *)(scratch + off_work); cfg->work_stride = stride;
+    static const char lbl[3][16] = {"logup_batching", "logup_alpha", "logup_lambda"};   // BasicTranscript::append_message words
+    memcpy(cfg->label, lbl, sizeof lbl);
+    cfg->fs = fs; cfg->fs.max_deg = 3;
+    out->flag = 0;
+    if (int e = sc_res_launch(blake ? "k_logup_res(resident LogUp-GKR layers, BLAKE3 transcript)" : "k_logup_res(resident LogUp-GKR layers, device transcript)",
+                              sh.ncta, blake ? k_logup_res<TrB3> : k_logup_res<TrP2>, (const LgCfg *)cfg, out, (gle *)(scratch + off_part), (u64 *)scratch,
+                              (gle *)(scratch + off_point)))
+        return e;
+    if (dp_wait_flag(&out->flag, 1, false, 0, 8.0) != 1) { dp_stream_sync(dp_ctx().stream); DP_CHECK(out->flag == 1, DP_ERR_CUDA, std::string(fn) + ": the resident kernel did not finish"); }
+    size_t om = 0, oc = 0, oe = 0;
+    for (u32 l = 0; l < nl; l++) {
+        const u32 v = first_layer + l, per = cfg->num[l][0] ? 4 : 2;
+        const LgLayerOut &o = out->layer[l];
+        for (u32 k = 0; k < v; k++) {
+            for (u32 t = 0; t < 4; t++) { msgs_out[om++] = o.fs.msg[k][t].c0; msgs_out[om++] = o.fs.msg[k][t].c1; }
+            challenges_out[oc++] = o.fs.chal[k].c0; challenges_out[oc++] = o.fs.chal[k].c1;
+        }
+        for (u32 i = 0; i < per * n; i++) { evals_out[oe++] = o.evals[i].c0; evals_out[oe++] = o.evals[i].c1; }
+    }
+    for (u32 i = 0; i <= last_layer; i++) { point[2 * i] = out->point[i].c0; point[2 * i + 1] = out->point[i].c1; }
+    claim[0] = out->claim.c0; claim[1] = out->claim.c1; alpha[0] = out->alpha.c0; alpha[1] = out->alpha.c1; lambda[0] = out->lambda.c0; lambda[1] = out->lambda.c1;
+    DP_CHECK(fs_state_out(out->sponge, blake, sponge), DP_ERR_STATE, std::string(fn) + ": the transcript outgrew the BLAKE3 state image");
+    return DP_OK;
 }
 
 extern "C" {
@@ -1130,18 +1251,8 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
     DP_REQUIRE_CTX();
     DP_CHECK(s && out_evals, DP_ERR_INVALID, "dp_sc_round: null argument");
     DP_CHECK(!s->finished && s->round < s->max_nv, DP_ERR_STATE, "Prover is not active");  // prover.rs:636-639
-    gle r = e_zero();
-    bool fold = false;
-    if (s->round == 0) {
-        DP_CHECK(challenge == nullptr, DP_ERR_STATE, "first round should be prover first.");  // prover.rs:655
-    } else {
-        DP_CHECK(challenge != nullptr, DP_ERR_STATE, "verifier message is empty");  // prover.rs:657
-        r = e_from_host(challenge);
-        s->challenges.push_back(r);
-        fold = true;
-        if (s->challenges.size() == 1)
-            for (auto &m : s->mles) DP_CHECK(m.len > 1, DP_ERR_INVALID, "calling sumcheck on constant");  // prover.rs:667-669
-    }
+    gle r; bool fold;
+    if (int e = sc_take_challenge(s, challenge, r, fold)) return e;
     if (s->tail_active || sc_tail_eligible(s, fold)) return sc_tail_round(s, r, fold, out_evals);
     // plan this round's folds: every MLE with >= 1 variable halves (prover.rs:659-684)
     std::vector<gle *> dst(s->n_mles, nullptr);
@@ -1280,73 +1391,6 @@ int dp_sc_tail_fs_next(dp_sc *s, int *out) {
     return DP_OK;
 }
 
-}  // extern "C"
-
-// The transcript state an entry point takes: BasicTranscript's 14-word sponge (canonical words, counts in range), or a valid image of
-// BlakeTranscript's hasher (dpb3::image_ok), copied into the kernel's SC_FS_WORDS buffer.  False: out of range.
-static bool fs_state_in(const uint64_t *in, bool blake, u64 *dst) {
-    if (blake) { if (!dpb3::image_ok(in)) return false; for (int w = 0; w < DP_B3T_WORDS; w++) dst[w] = in[w]; return true; }
-    if (!(in[12] < 4 && in[13] <= 4)) return false;
-    for (int w = 0; w < P2S_WORDS; w++) dst[w] = w < 12 ? gl_canon(in[w]) : in[w];
-    return true;
-}
-// ... and the state the kernel returns, in dpb3::Hasher::save's form (the stack words past stack_len, which merges leave behind in
-// the kernel, are zero).  False: the BLAKE3 hasher needed more than DP_B3T_STACK stack entries (more than 2^17 chunks).
-static bool fs_state_out(const u64 *src, bool blake, uint64_t *out) {
-    if (blake && (src[b3::T_SLEN] & b3::T_OVERFLOW)) return false;
-    const int n = blake ? b3::T_STACK + 4 * (int)src[b3::T_SLEN] : P2S_WORDS;
-    for (int w = 0; w < (blake ? DP_B3T_WORDS : P2S_WORDS); w++) out[w] = w < n ? src[w] : 0;
-    return true;
-}
-
-static int sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
-                          uint64_t *sponge_out, bool blake) {
-    const char *const fn = blake ? "dp_sc_run_tail_fs_blake" : "dp_sc_run_tail_fs";
-    DP_CHECK(s && sponge_in && msgs_out && challenges_out && sponge_out, DP_ERR_INVALID, std::string(fn) + ": null argument");
-    DP_CHECK(!s->finished && s->round < s->max_nv && !s->tail_active, DP_ERR_STATE, "Prover is not active");
-    const bool fold = s->round > 0;
-    DP_CHECK(fold == (prev_challenge != nullptr), DP_ERR_STATE, fold ? "verifier message is empty" : "first round should be prover first.");
-    ScTailFs fs{};
-    DP_CHECK(fs_state_in(sponge_in, blake, fs.sponge), DP_ERR_INVALID, std::string(fn) + (blake ? ": not a BLAKE3 hasher state" : ": sponge state out of range"));
-    DP_CHECK(sc_tail_eligible(s, fold), DP_ERR_STATE, std::string(fn) + ": the next round does not start the resident tail");
-    if (!blake) DP_CUDA(sc_fs_constants());
-    gle r = e_zero();
-    if (fold) {
-        r = e_from_host(prev_challenge);
-        s->challenges.push_back(r);
-        if (s->challenges.size() == 1)
-            for (auto &m : s->mles) DP_CHECK(m.len > 1, DP_ERR_INVALID, "calling sumcheck on constant");  // prover.rs:667-669
-    }
-    fs.max_deg = s->max_deg; fs.max_nv = s->max_nv; fs.round0 = s->round;
-    static const char label[] = "Internal round";                 // Transcript::append_message: 8-byte little-endian words
-    memcpy(fs.label, label, sizeof label - 1);
-    for (u32 p = 0; p < s->n_products; p++) { fs.coef[p][0] = s->products[p].coef[0]; fs.coef[p][1] = s->products[p].coef[1]; }
-    for (u32 d = 1; d < s->max_deg; d++)
-        for (u32 i = 0; d + 1 + i <= s->max_deg; i++)
-            for (u32 j = 0; j <= d; j++) fs.bary[d - 1][i][j] = sc_bary_weight(d + 1, d + 1 + i, j);
-    const u32 nr = s->max_nv - s->round;
-    s->seq++;
-    if (int e = sc_tail_launch(s, r, fold, &fs, blake)) return e;
-    s->seq += nr - 1;                                              // the kernel raises the flag once, with the last round's tag
-    for (u32 k = 0; k < nr; k++)
-        if (k > 0 || fold) for (auto &m : s->mles) if (m.len > 1) { m.len >>= 1; m.is_ext = true; m.cur = nullptr; m.where = 3; }
-    s->round = s->max_nv;
-    const bool ok = dp_wait_flag(s->h_flag, s->seq, true, SC_TAIL_FAILED, 8.0) == s->seq;
-    if (!ok) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(dp_ctx().stream); DP_CHECK(false, DP_ERR_CUDA, std::string(fn) + ": the resident kernel did not finish"); }
-    s->have_pairs = true;
-    const ScTailFsOut &o = *s->h_fs;
-    const u32 w = s->max_deg + 1;
-    for (u32 k = 0; k < nr; k++) {
-        for (u32 t = 0; t < w; t++) { msgs_out[2 * (k * w + t)] = o.msg[k][t].c0; msgs_out[2 * (k * w + t) + 1] = o.msg[k][t].c1; }
-        challenges_out[2 * k] = o.chal[k].c0; challenges_out[2 * k + 1] = o.chal[k].c1;
-        if (k + 1 < nr) s->challenges.push_back(o.chal[k]);     // the last one is dp_sc_finish's
-    }
-    DP_CHECK(fs_state_out(o.sponge, blake, sponge_out), DP_ERR_STATE, std::string(fn) + ": the transcript outgrew the BLAKE3 state image");
-    return DP_OK;
-}
-
-extern "C" {
-
 int dp_sc_run_tail_fs(dp_sc *s, const uint64_t *prev_challenge, const uint64_t *sponge_in, uint64_t *msgs_out, uint64_t *challenges_out,
                       uint64_t *sponge_out) {
     DP_REQUIRE_CTX();
@@ -1358,90 +1402,21 @@ int dp_sc_run_tail_fs_blake(dp_sc *s, const uint64_t *prev_challenge, const uint
     return sc_run_tail_fs(s, prev_challenge, state_in, msgs_out, challenges_out, state_out, true);
 }
 
+int dp_sc_current_mle(dp_sc *s, uint32_t idx, dp_mle **out) {
+    DP_REQUIRE_CTX();
+    DP_CHECK(s && out && idx < s->n_mles, DP_ERR_INVALID, "dp_sc_current_mle: bad argument");
+    const ScMle &m = s->mles[idx];
+    DP_CHECK(!s->tail_active, DP_ERR_STATE, "dp_sc_current_mle: tables are owned by the resident tail kernel");
+    *out = dp_mle_view(const_cast<void *>(m.cur), m.len, m.is_ext);
+    return DP_OK;
+}
+
 int dp_logup_layers_fs_next(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t *n_layers) {
     DP_REQUIRE_CTX();
     DP_CHECK(circuits && n_layers, DP_ERR_INVALID, "dp_logup_layers_fs_next: null argument");
     *n_layers = lg_fs_layers(circuits, n_circuits, first_layer);
     return DP_OK;
 }
-
-}  // extern "C"
-
-static int lg_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
-                            uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
-                            uint64_t *evals_out, bool blake) {
-    const char *const fn = blake ? "dp_logup_run_layers_fs_blake" : "dp_logup_run_layers_fs";
-    DP_CHECK(circuits && claim && point && alpha && lambda && sponge && msgs_out && challenges_out && evals_out, DP_ERR_INVALID,
-             std::string(fn) + ": null argument");
-    DP_CHECK(first_layer >= 1 && last_layer >= first_layer && last_layer - first_layer < lg_fs_layers(circuits, n_circuits, first_layer), DP_ERR_STATE,
-             std::string(fn) + ": these layers do not run resident (wait mode, circuit count or layer size)");
-    u64 state[SC_FS_WORDS] = {};
-    DP_CHECK(fs_state_in(sponge, blake, state), DP_ERR_INVALID, std::string(fn) + (blake ? ": not a BLAKE3 hasher state" : ": sponge state out of range"));
-    if (!blake) DP_CUDA(sc_fs_constants());
-    const u32 nl = last_layer - first_layer + 1, n = n_circuits, np = 3 * n, nm_max = 1 + 4 * n;
-    const u64 len_max = 1ULL << last_layer, stride = (len_max >> 1) + (len_max >> 2) + 1;
-    const u64 work = (u64)np * (len_max >> 1);
-    u32 ncta = 1; while (ncta < SC_RES_MAXCTA && (u64)ncta * 512 < work) ncta <<= 1;      // sized like sc_tail_launch, by the largest layer
-    const u32 slots = std::max<u32>(ncta * (SC_THREADS / 32), np);
-    LgCfg *cfg = nullptr; LgOut *out = nullptr; char *scratch = nullptr;
-    if (int e = dp_pinned_alloc((void **)&cfg, sizeof(LgCfg))) return e;
-    PinnedPtr cfg_owner(cfg);
-    if (int e = dp_pinned_alloc((void **)&out, sizeof(LgOut))) return e;
-    PinnedPtr out_owner(out);
-    const size_t off_point = 64, off_part = off_point + sizeof(gle) * (SC_MAX_ROUNDS + 1), off_eq = off_part + sizeof(gle) * SC_NACC * slots,
-                 off_work = off_eq + sizeof(gle) * len_max, bytes = off_work + sizeof(gle) * stride * nm_max;
-    if (int e = dp_dev_alloc((void **)&scratch, bytes)) return e;
-    DevPtr scratch_owner(scratch);
-    memset(cfg, 0, sizeof(LgCfg));
-    cfg->n_circuits = n; cfg->first = first_layer; cfg->n_layers = nl;
-    cfg->claim = e_from_host(claim); cfg->alpha = e_from_host(alpha); cfg->lambda = e_from_host(lambda);
-    for (u32 i = 0; i < first_layer; i++) cfg->point[i] = e_from_host(point + 2 * i);
-    for (u32 l = 0; l < nl; l++) {
-        const u32 k = circuits[0]->nv - 1 - (first_layer + l);    // circuit layer with 2^(v+1) entries (dp_logup_layer_mles)
-        for (u32 c = 0; c < n; c++) { cfg->num[l][c] = circuits[c]->num[k]; cfg->den[l][c] = circuits[c]->den[k]; }
-    }
-    cfg->eq = (gle *)(scratch + off_eq); cfg->work = (gle *)(scratch + off_work); cfg->work_stride = stride;
-    static const char lbl[4][16] = {"Internal round", "logup_batching", "logup_alpha", "logup_lambda"};   // BasicTranscript::append_message words
-    memcpy(cfg->round_label, lbl[0], 16);
-    for (int q = 0; q < 3; q++) memcpy(cfg->label[q], lbl[q + 1], 16);
-    for (u32 d = 1; d < 3; d++)
-        for (u32 i = 0; d + 1 + i <= 3; i++)
-            for (u32 j = 0; j <= d; j++) cfg->bary[d - 1][i][j] = sc_bary_weight(d + 1, d + 1 + i, j);
-    memcpy(cfg->sponge, state, sizeof state);
-    out->flag = 0;
-    cudaStream_t st = dp_ctx().stream;
-    {
-        cudaLaunchConfig_t lc{};
-        lc.gridDim = dim3(ncta); lc.blockDim = dim3(SC_THREADS); lc.dynamicSmemBytes = 0; lc.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        lc.attrs = at; lc.numAttrs = 1;
-        DpProfScope prof(blake ? "k_logup_res(resident LogUp-GKR layers, BLAKE3 transcript)" : "k_logup_res(resident LogUp-GKR layers, device transcript)", 0);
-        const cudaError_t ce = cudaLaunchKernelEx(&lc, blake ? k_logup_res<TrB3> : k_logup_res<TrP2>, (const LgCfg *)cfg, out, (gle *)(scratch + off_part), (u64 *)scratch,
-                                                  (gle *)(scratch + off_point));
-        DP_LAUNCHED();
-        DP_CUDA(ce);
-        DP_CUDA(cudaGetLastError());
-    }
-    if (dp_wait_flag(&out->flag, 1, false, 0, 8.0) != 1) { dp_stream_sync(st); DP_CHECK(out->flag == 1, DP_ERR_CUDA, std::string(fn) + ": the resident kernel did not finish"); }
-    size_t om = 0, oc = 0, oe = 0;
-    for (u32 l = 0; l < nl; l++) {
-        const u32 v = first_layer + l, per = cfg->num[l][0] ? 4 : 2;
-        const LgLayerOut &o = out->layer[l];
-        for (u32 k = 0; k < v; k++) {
-            for (u32 t = 0; t < 4; t++) { msgs_out[om++] = o.fs.msg[k][t].c0; msgs_out[om++] = o.fs.msg[k][t].c1; }
-            challenges_out[oc++] = o.fs.chal[k].c0; challenges_out[oc++] = o.fs.chal[k].c1;
-        }
-        for (u32 i = 0; i < per * n; i++) { evals_out[oe++] = o.evals[i].c0; evals_out[oe++] = o.evals[i].c1; }
-    }
-    for (u32 i = 0; i <= last_layer; i++) { point[2 * i] = out->point[i].c0; point[2 * i + 1] = out->point[i].c1; }
-    claim[0] = out->claim.c0; claim[1] = out->claim.c1; alpha[0] = out->alpha.c0; alpha[1] = out->alpha.c1; lambda[0] = out->lambda.c0; lambda[1] = out->lambda.c1;
-    DP_CHECK(fs_state_out(out->sponge, blake, sponge), DP_ERR_STATE, std::string(fn) + ": the transcript outgrew the BLAKE3 state image");
-    return DP_OK;
-}
-
-extern "C" {
-
 int dp_logup_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint32_t first_layer, uint32_t last_layer, uint64_t *claim,
                            uint64_t *point, uint64_t *alpha, uint64_t *lambda, uint64_t *sponge, uint64_t *msgs_out, uint64_t *challenges_out,
                            uint64_t *evals_out) {
@@ -1453,15 +1428,6 @@ int dp_logup_run_layers_fs_blake(dp_logup *const *circuits, uint32_t n_circuits,
                                  uint64_t *evals_out) {
     DP_REQUIRE_CTX();
     return lg_run_layers_fs(circuits, n_circuits, first_layer, last_layer, claim, point, alpha, lambda, state, msgs_out, challenges_out, evals_out, true);
-}
-
-int dp_sc_current_mle(dp_sc *s, uint32_t idx, dp_mle **out) {
-    DP_REQUIRE_CTX();
-    DP_CHECK(s && out && idx < s->n_mles, DP_ERR_INVALID, "dp_sc_current_mle: bad argument");
-    const ScMle &m = s->mles[idx];
-    DP_CHECK(!s->tail_active, DP_ERR_STATE, "dp_sc_current_mle: tables are owned by the resident tail kernel");
-    *out = dp_mle_view(const_cast<void *>(m.cur), m.len, m.is_ext);
-    return DP_OK;
 }
 
 }  // extern "C"

@@ -148,6 +148,29 @@ struct IOPProof {
     Ext extract_sum() const { return proofs.at(0).evaluations.at(0) + proofs.at(0).evaluations.at(1); }
 };
 
+// The hand-off to a device-transcript entry point: the transcript's state goes, through call(entry, state), to the Poseidon2 form
+// (p2) or the BLAKE3 form (b3) of the entry point as the state's kind says, and the state the entry point returns is loaded back.
+// False, with nothing called, when the transcript has no device state (DS_NONE).
+template <class T, class F, class C>
+inline bool run_device_transcript(T &transcript, F p2, F b3, C &&call) {
+    u64 sp[DEVICE_STATE_WORDS];
+    const int kind = transcript.save_sponge(sp);
+    if (kind == DS_NONE) return false;
+    check(call(kind == DS_BLAKE3 ? b3 : p2, sp));
+    transcript.load_sponge(sp);
+    return true;
+}
+// n rounds of a device-transcript entry point's flat output appended to proof and challenges: msgs, n messages of deg + 1 elements;
+// ch, n challenges; [c0, c1] words per element
+inline void append_device_rounds(IOPProof &proof, ExtVec &challenges, size_t n, size_t deg, const u64 *msgs, const u64 *ch) {
+    for (size_t k = 0; k < n; k++) {
+        IOPProverMessage msg;
+        for (size_t t = 0; t <= deg; t++, msgs += 2) msg.evaluations.push_back(Ext(msgs[0], msgs[1]));
+        proof.proofs.push_back(std::move(msg));
+        challenges.push_back(Ext(ch[2 * k], ch[2 * k + 1]));
+    }
+}
+
 class IOPProverState {
   public:
     ~IOPProverState() { if (sc_) dp_sc_destroy(sc_); }
@@ -260,20 +283,16 @@ class IOPProverState {
         for (size_t i = 0; i < nv; i++) {
             u64 c[2] = {0, 0};
             if (i > 0) { c[0] = st.challenges.back().c0; c[1] = st.challenges.back().c1; }
-            int dev = 0, kind = DS_NONE; u64 sp[DEVICE_STATE_WORDS];
+            int dev = 0;
             if (sc) check(dp_sc_tail_fs_next(sc, &dev));
-            if (dev && (kind = transcript.save_sponge(sp)) != DS_NONE) {
-                const size_t n = nv - i, w = 2 * (deg + 1);
-                std::vector<u64> msgs(n * w), ch(2 * n);
-                check((kind == DS_BLAKE3 ? dp_sc_run_tail_fs_blake : dp_sc_run_tail_fs)(sc, i > 0 ? c : nullptr, sp, msgs.data(), ch.data(), sp));
-                transcript.load_sponge(sp);
-                for (size_t k = 0; k < n; k++) {
-                    IOPProverMessage msg;
-                    for (size_t t = 0; t <= deg; t++) msg.evaluations.push_back(Ext(msgs[k * w + 2 * t], msgs[k * w + 2 * t + 1]));
-                    proof.proofs.push_back(std::move(msg));
-                    st.challenges.push_back(Ext(ch[2 * k], ch[2 * k + 1]));
+            if (dev) {
+                const size_t n = nv - i;
+                std::vector<u64> msgs(2 * n * (deg + 1)), ch(2 * n);
+                if (run_device_transcript(transcript, dp_sc_run_tail_fs, dp_sc_run_tail_fs_blake, [&](auto run, u64 *sp) {
+                        return run(sc, i > 0 ? c : nullptr, sp, msgs.data(), ch.data(), sp); })) {
+                    append_device_rounds(proof, st.challenges, n, deg, msgs.data(), ch.data());
+                    return;
                 }
-                return;
             }
             IOPProverMessage msg; msg.evaluations.assign(deg + 1, Ext::zero());
             round(i > 0 ? c : nullptr, msg.evaluations);

@@ -106,26 +106,20 @@ LogUpProof logup_batch_prove(const LogUpInput &in, T &t) {
     // the leading small layers in one resident launch that runs the transcript on the device, when the library takes them (blocking
     // waits) and the transcript's state can go there (BasicTranscript's sponge, or BlakeTranscript's hasher up to 2^16 chunks)
     std::vector<dp_logup *> hs; for (auto &c : circuits) hs.push_back(c->h);
-    uint32_t n_dev = 0; int kind = DS_NONE; u64 sp[DEVICE_STATE_WORDS];
+    uint32_t n_dev = 0;
     check(dp_logup_layers_fs_next(hs.data(), (uint32_t)hs.size(), 1, &n_dev));
-    if (n_dev > 0 && (kind = t.save_sponge(sp)) != DS_NONE) {
-        const size_t last = n_dev, n_rounds = last * (last + 1) / 2;
-        auto views = [&](size_t layer) -> size_t { return !in.table && layer == total_layers ? 2 : 4; };   // dp_logup_layer_mles
-        size_t n_evals = 0; for (size_t l = 1; l <= last; l++) n_evals += views(l) * circuits.size();
-        std::vector<u64> pt(2 * (last + 1)), msgs(2 * 4 * n_rounds), ch(2 * n_rounds), ev(2 * n_evals);
-        pt[0] = batching.c0; pt[1] = batching.c1;
-        u64 cl[2] = {claim.c0, claim.c1}, al[2] = {alpha.c0, alpha.c1}, lm[2] = {lambda.c0, lambda.c1};
-        check((kind == DS_BLAKE3 ? dp_logup_run_layers_fs_blake : dp_logup_run_layers_fs)(hs.data(), (uint32_t)hs.size(), 1, (uint32_t)last, cl, pt.data(), al, lm, sp, msgs.data(), ch.data(), ev.data()));
-        t.load_sponge(sp);
-        size_t om = 0, oc = 0, oe = 0;
-        for (size_t l = 1; l <= last; l++) {
+    const size_t last = n_dev, n_rounds = last * (last + 1) / 2;
+    auto views = [&](size_t layer) -> size_t { return !in.table && layer == total_layers ? 2 : 4; };   // dp_logup_layer_mles
+    size_t n_evals = 0; for (size_t l = 1; l <= last; l++) n_evals += views(l) * circuits.size();
+    std::vector<u64> pt(2 * (last + 1)), msgs(2 * 4 * n_rounds), ch(2 * n_rounds), ev(2 * n_evals);
+    pt[0] = batching.c0; pt[1] = batching.c1;
+    u64 cl[2] = {claim.c0, claim.c1}, al[2] = {alpha.c0, alpha.c1}, lm[2] = {lambda.c0, lambda.c1};
+    if (n_dev > 0 && run_device_transcript(t, dp_logup_run_layers_fs, dp_logup_run_layers_fs_blake, [&](auto run, u64 *sp) {
+            return run(hs.data(), (uint32_t)hs.size(), 1, (uint32_t)last, cl, pt.data(), al, lm, sp, msgs.data(), ch.data(), ev.data()); })) {
+        size_t oe = 0;
+        for (size_t l = 1, k = 0; l <= last; k += l, l++) {    // k: rounds before layer l
             IOPProof p;
-            for (size_t k = 0; k < l; k++) {
-                IOPProverMessage m;
-                for (size_t q = 0; q < 4; q++, om += 2) m.evaluations.push_back(Ext(msgs[om], msgs[om + 1]));
-                p.proofs.push_back(std::move(m));
-                p.point.push_back(Ext(ch[oc], ch[oc + 1])); oc += 2;
-            }
+            append_device_rounds(p, p.point, l, 3, msgs.data() + 2 * 4 * k, ch.data() + 2 * k);
             pr.sumcheck_proofs.push_back(std::move(p));
             ExtVec evals; for (size_t i = 0; i < views(l) * circuits.size(); i++, oe += 2) evals.push_back(Ext(ev[oe], ev[oe + 1]));
             pr.round_evaluations.push_back(std::move(evals));

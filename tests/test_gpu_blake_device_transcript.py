@@ -1,5 +1,5 @@
-"""BlakeTranscript on the device (dp_sc_run_tail_fs_blake, dp_logup_run_layers_fs_blake; csrc/sumcheck.cu TrB3 over the incremental
-BLAKE3 of csrc/blake3.cuh).  Under the `blake` hasher a prover in blocking wait mode hands its transcript's hasher image to the resident
+"""BlakeTranscript on the device (dp_sc_run_tail_fs_blake, dp_logup_run_layers_fs_blake; csrc/blake3.cuh TrB3 over the incremental
+BLAKE3 there).  Under the `blake` hasher a prover in blocking wait mode hands its transcript's hasher image to the resident
 sumcheck tail and to the LogUp-GKR layer kernel and takes it back with every message and challenge.  Everything here is pinned: the
 challenges against the Python `blake3` package, the proofs against the checker's BLAKE3 proofs."""
 import ctypes as C

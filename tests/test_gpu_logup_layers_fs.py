@@ -104,7 +104,8 @@ def _circuits(gpu, n_circuits, nv):
 @pytest.mark.gpu
 def test_selection_and_refusals(gpu):
     """the library takes leading layers only in blocking mode, for <= 16 circuits and resident-sized layers; the run entry refuses a
-    range it does not take and a sponge state out of range; BLAKE3 keeps the per-layer path"""
+    range it does not take and a sponge state out of range; under BLAKE3 the Poseidon2 k_logup_res count is 0 because the BLAKE3
+    instantiation runs instead"""
     L = gpu.lib()
     keep, hs = _circuits(gpu, 17, 10)
     n = C.c_uint32()

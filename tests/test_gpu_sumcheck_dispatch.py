@@ -21,17 +21,17 @@ import oracle_py as O
 P = O.P
 
 # ---- constants of sumcheck.cu the model depends on -----------------------------------------------------------------------------
-SC_THREADS = 256            # :25   threads per block of k_sc_round and k_sc_res
+SC_THREADS = 256            # SC_THREADS: threads per block of k_sc_round and k_sc_res
 WARP = 32
-LEAN_MIN_PAIRS = 2048       # :892  lean kernels only when the round has MORE pairs than this
-SC_RES_WORK = 2048          # :442  resident once the round's pair-items, summed over products, are <= this
-SC_RES_CTA_WORK = 512       # :757  ~pair-items per CTA of the resident cluster
-SC_RES_MAXCTA = 8           # :441
-SC_RES_MAXP = 48            # :441
-SC_RES_MAXM = 96            # :441
-COUNTER_POOL_BYTES = 256    # :832  tick counters (n_products + 1 u32) come from a pooled 256-byte block when they fit
-H100_SMS = 132              # common.cuh:15 default; on the device the real count is read from torch
-# sumcheck.cu:705-706: the tail disables itself under tools that serialise launches
+LEAN_MIN_PAIRS = 2048       # dp_sc_round's lean-kernel choice: lean kernels only when the round has MORE pairs than this
+SC_RES_WORK = 2048          # SC_RES_WORK: resident once the round's pair-items, summed over products, are <= this
+SC_RES_CTA_WORK = 512       # sc_res_shape: ~pair-items per CTA of the resident cluster
+SC_RES_MAXCTA = 8           # SC_RES_MAXCTA
+SC_RES_MAXP = 48            # SC_RES_MAXP
+SC_RES_MAXM = 96            # SC_RES_MAXM
+COUNTER_POOL_BYTES = 256    # dp_sc_create's pooled counters: tick counters (n_products + 1 u32) come from a pooled 256-byte block when they fit
+H100_SMS = 132              # common.cuh DpCtx::sm_count default; on the device the real count is read from torch
+# sc_tail_supported: the tail disables itself under tools that serialise launches
 INJECTION_VARS = ("CUDA_INJECTION64_PATH", "CUDA_INJECTION32_PATH", "NV_NSIGHT_INJECTION_TRANSPORT_TYPE",
                   "NV_NSIGHT_INJECTION_PORT_BASE", "NV_COMPUTE_PROFILER_PERFWORKS_DIR")
 
@@ -39,7 +39,7 @@ LEAN_PROFILE_NAME = {"B": "k_sc_lean(msg, Base)", "E": "k_sc_lean(msg, Ext)", "B
                      "EF": "k_sc_lean(fold Ext + msg)"}
 
 
-def _grid_for(work, threads, max_ctas_per_sm, sm_count):          # common.cuh:120-125
+def _grid_for(work, threads, max_ctas_per_sm, sm_count):          # common.cuh dp_grid_for
     return int(max(1, min((work + threads - 1) // threads, sm_count * max_ctas_per_sm)))
 
 

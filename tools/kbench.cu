@@ -433,39 +433,29 @@ static void host_sum_e(const gle *d, int blocks, gle out[4]) {
     for (int t = 0; t < 4; t++) { gle s = e_zero(); for (int b = 0; b < blocks; b++) s = e_add(s, h[4 * b + t]); out[t] = s; }
 }
 
-// ---- fs: one round of the resident tail's device transcript (csrc/sumcheck.cu TrP2 / TrB3) alone, `rounds` rounds back to back in a
-// 1-block kernel: absorb a degree-D message (D + 1 extension elements) and the "Internal round" label, draw the challenge.  The
+// ---- fs: one round of the resident tail's device transcript (TrP2 in poseidon2.cuh, TrB3 in blake3.cuh) alone, `rounds` rounds back
+// to back in a 1-block kernel, with the state image in shared memory and the message loop rolled as in the kernel (whose degree is a
+// run-time value): absorb a degree-D message (D + 1 extension elements) and the "Internal round" label, draw the challenge.  The
 // message of round r is derived from the previous challenge, so the rounds form one dependent chain as in the kernel.
-static constexpr u64 FS_LBL0 = 0x6c616e7265746e49ULL, FS_LBL1 = 0x646e756f7220ULL;   // "Internal", " round"
-template <int D> __global__ void k_fs_p2(u64 *w, int rounds) {                        // BasicTranscript: warp 0, 8-lane groups
-    if (threadIdx.x >= 32) return;
-    const int l8 = threadIdx.x & 7;
-    P2Sponge s; p2s_load(s, w, l8);
-    u64 c = 1;
-    for (int r = 0; r < rounds; r++) {
-        for (int t = 0; t < 2 * (D + 1); t++) p2s_observe(s, gl_canon(c * (t + 3)), l8);
-        p2s_observe(s, FS_LBL0, l8); p2s_observe(s, FS_LBL1, l8);
-        const u64 c0 = p2s_sample(s, l8), c1 = p2s_sample(s, l8);
-        c = c0 ^ c1;
-    }
-    __syncwarp();
-    if (threadIdx.x < 8) p2s_store(s, w, l8);
-}
-template <int D> __global__ void k_fs_b3(u64 *w, int rounds) {                        // BlakeTranscript: thread 0, image in shared memory
-    __shared__ u64 img[80];
-    for (int i = threadIdx.x; i < 80; i += blockDim.x) img[i] = w[i];
+template <class TR, int D> __global__ void k_fs(u64 *w, int rounds) {
+    __shared__ u64 img[TrB3::WORDS];
+    for (int i = threadIdx.x; i < TrB3::WORDS; i += blockDim.x) img[i] = w[i];
     __syncthreads();
-    if (threadIdx.x == 0) {
+    if (TR::runs()) {
+        const u64 label[2] = {b3::le_word("Internal", 8), b3::le_word(" round", 6)};
+        TR t(img);
         u64 c = 1;
         for (int r = 0; r < rounds; r++) {
-            for (int t = 0; t <= D; t++) b3::t_append_ext(img, gl_canon(c * (2 * t + 3)), gl_canon(c * (2 * t + 4)));
-            b3::t_append_fe(img, FS_LBL0); b3::t_append_fe(img, FS_LBL1);
-            u64 c0, c1; b3::t_challenge(img, c0, c1);
-            c = c0 ^ c1;
+#pragma unroll 1
+            for (int k = 0; k <= D; k++) t.ext(e_make(gl_canon(c * (2 * k + 3)), gl_canon(c * (2 * k + 4))));
+            t.label(label);
+            const gle ch = t.challenge();
+            c = ch.c0 ^ ch.c1;
         }
+        t.store(img, nullptr);
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < 80; i += blockDim.x) w[i] = img[i];
+    for (int i = threadIdx.x; i < TrB3::WORDS; i += blockDim.x) w[i] = img[i];
 }
 
 // =====================================================================================================================
@@ -487,8 +477,8 @@ int main(int argc, char **argv) {
             const float ms = time_ms([&] { CK(cudaMemset(w, 0, 80 * 8)); kern<<<1, 256>>>(w, rounds); });
             printf("  %-40s %8.2f us per round\n", name, 1e3 * ms / rounds);
         };
-        run("Poseidon2 sponge (warp 0), degree 2", k_fs_p2<2>); run("Poseidon2 sponge (warp 0), degree 3", k_fs_p2<3>);
-        run("BLAKE3 hasher (thread 0), degree 2", k_fs_b3<2>); run("BLAKE3 hasher (thread 0), degree 3", k_fs_b3<3>);
+        run("Poseidon2 sponge (warp 0), degree 2", k_fs<TrP2, 2>); run("Poseidon2 sponge (warp 0), degree 3", k_fs<TrP2, 3>);
+        run("BLAKE3 hasher (thread 0), degree 2", k_fs<TrB3, 2>); run("BLAKE3 hasher (thread 0), degree 3", k_fs<TrB3, 3>);
         cudaFree(w);
     }
 
