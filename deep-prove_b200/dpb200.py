@@ -14,20 +14,130 @@ HOST_LIB_PATH = os.path.join(_HERE, "libdeepprove_host.so")
 P = 0xFFFFFFFF00000001
 DP_OK, DP_ERR_INVALID, DP_ERR_CUDA, DP_ERR_NO_DEVICE, DP_ERR_STATE, DP_ERR_UNSUPPORTED = range(6)
 
+# Every entry point's C signature, applied once when lib() / host() load the library.  One rule: every pointer, handle, array,
+# out-parameter and callback is VP; a C string is STR; restype is given for every return (INT for `int`, None for `void`).
+VP, STR, U64, I64, U32, INT, F64 = C.c_void_p, C.c_char_p, C.c_uint64, C.c_int64, C.c_uint32, C.c_int, C.c_double
+SIGNATURES = {
+    # ---- libdeepprove_b200.so: include/deepprove_b200.h ----
+    "dp_init": (INT, [INT]),
+    "dp_shutdown": (INT, []),
+    "dp_device_count": (INT, []),
+    "dp_last_error": (STR, []),
+    "dp_version": (STR, []),
+    "dp_set_stream": (INT, [VP]),
+    "dp_synchronize": (INT, []),
+    "dp_kernel_launches": (U64, []),
+    "dp_host_waits": (U64, []),
+    "dp_set_wait_mode": (INT, [INT]),
+    "dp_get_wait_mode": (INT, []),
+    "dp_profile_enable": (INT, [INT]),
+    "dp_profile_reset": (INT, []),
+    "dp_profile_read_ex": (INT, [VP, VP, VP, VP, VP, INT]),
+    "dp_profile_flush": (INT, []),
+    "dp_mle_upload": (INT, [VP, U64, INT, VP]),
+    "dp_mle_wrap_device": (INT, [VP, U64, INT, VP]),
+    "dp_mle_clone": (INT, [VP, VP]),
+    "dp_mle_download": (INT, [VP, VP]),
+    "dp_mle_info": (INT, [VP, VP, VP, VP]),
+    "dp_mle_device_ptr": (VP, [VP]),
+    "dp_mle_free": (INT, [VP]),
+    "dp_mle_fix_high": (INT, [VP, VP, U32]),
+    "dp_mle_fix_high_new": (INT, [VP, VP, U32, VP]),
+    "dp_mle_fix_low": (INT, [VP, VP, U32, VP]),
+    "dp_mle_evaluate": (INT, [VP, VP, U32, VP]),
+    "dp_mle_evaluate_many": (INT, [VP, U32, VP, U32, VP]),
+    "dp_eq_build": (INT, [VP, U32, VP]),
+    "dp_sc_create": (INT, [VP, U32, VP, U32, U32, U32, VP]),
+    "dp_sc_round": (INT, [VP, VP, VP]),
+    "dp_sc_set_resident_tail": (INT, [VP, INT]),
+    "dp_sc_tail_fs_next": (INT, [VP, VP]),
+    "dp_sc_run_tail_fs": (INT, [VP, VP, VP, VP, VP, VP]),
+    "dp_sc_run_tail_fs_blake": (INT, [VP, VP, VP, VP, VP, VP]),
+    "dp_sc_finish": (INT, [VP, VP, VP]),
+    "dp_sc_destroy": (INT, [VP]),
+    "dp_sc_current_mle": (INT, [VP, U32, VP]),
+    "dp_logup_build": (INT, [VP, U32, VP, VP, VP, VP]),
+    "dp_logup_num_vars": (INT, [VP, VP]),
+    "dp_logup_outputs": (INT, [VP, VP]),
+    "dp_logup_layer_mles": (INT, [VP, U32, VP, VP]),
+    "dp_logup_free": (INT, [VP]),
+    "dp_logup_layers_fs_next": (INT, [VP, U32, U32, VP]),
+    "dp_logup_run_layers_fs": (INT, [VP, U32, U32, U32, VP, VP, VP, VP, VP, VP, VP, VP]),
+    "dp_logup_run_layers_fs_blake": (INT, [VP, U32, U32, U32, VP, VP, VP, VP, VP, VP, VP, VP]),
+    "dp_mle_linear_combination": (INT, [VP, VP, U32, VP]),
+    "dp_fft_rows": (INT, [VP, U32, INT]),
+    "dp_pad_rows": (INT, [VP, U64, U32, U32, U64, VP]),
+    "dp_conv_prod": (INT, [VP, VP, U32, U32, U64, VP]),
+    "dp_conv_output_elements": (INT, [VP, U32, U32, VP, VP]),
+    "dp_phi_g_init": (INT, [VP, U32, VP, INT, VP, VP]),
+    "dp_phi_level": (INT, [U32, U32, U32, VP, VP, INT, VP]),
+    "dp_mle_repeat": (INT, [VP, U32, VP]),
+    "dp_set_merkle_hasher": (INT, [INT]),
+    "dp_get_merkle_hasher": (INT, []),
+    "dp_poseidon2_init": (INT, [VP, VP, VP]),
+    "dp_pcs_commit": (INT, [VP, U32, VP]),
+    "dp_pcs_commit_many": (INT, [VP, U32, U32, VP]),
+    "dp_pcs_batch_commit": (INT, [VP, U32, U32, VP]),
+    "dp_pcs_comm_num_polys": (U32, [VP]),
+    "dp_pcs_comm_part": (INT, [VP, U32, VP]),
+    "dp_pcs_comm_info": (INT, [VP, VP, VP, VP, VP]),
+    "dp_pcs_comm_codeword": (INT, [VP, VP]),
+    "dp_pcs_comm_bh_evals": (INT, [VP, VP]),
+    "dp_pcs_comm_free": (INT, [VP]),
+    "dp_pcs_open_begin": (INT, [VP, VP, U32, VP, U32, VP, VP]),
+    "dp_pcs_open_round": (INT, [VP, VP, VP, VP, VP]),
+    "dp_pcs_open_final_message": (INT, [VP, VP]),
+    "dp_pcs_open_query_words": (U64, [VP]),
+    "dp_pcs_open_query": (INT, [VP, VP, U32, VP]),
+    "dp_pcs_open_free": (INT, [VP]),
+    "dp_pcs_commit_shard": (INT, [VP, U32, U32, U32, VP]),
+    "dp_pcs_comm_shard_info": (INT, [VP, VP, VP, VP]),
+    "dp_pcs_comm_set_shard_roots": (INT, [VP, VP, VP]),
+    "dp_pcs_open_set_shard_roots": (INT, [VP, VP, VP]),
+    "dp_wit_begin": (INT, [U32, VP, VP, VP]),
+    "dp_wit_dense": (INT, [VP, VP, VP, U32, U32, VP]),
+    "dp_wit_matmul": (INT, [VP, VP, VP, U32, U32, U32, INT, VP]),
+    "dp_wit_requant": (INT, [VP, VP, U32, I64, U32, U32, U32, VP, U32]),
+    "dp_wit_relu": (INT, [VP, VP, U32, VP]),
+    "dp_wit_pool": (INT, [VP, VP, U32, U32, U32, U32, VP]),
+    "dp_wit_finish": (INT, [VP, VP, VP]),
+    "dp_wit_free": (INT, [VP]),
+    # test hook of libdeepprove_b200.so, not part of the ABI (csrc/context.cu)
+    "dp_debug_wait_flag": (U64, [VP, U64, F64]),
+    # ---- libdeepprove_host.so: host/capi.cpp ----
+    "dph_last_error": (STR, []),
+    "dph_poseidon2_permute": (None, [VP]),
+    "dph_poseidon2_selfcheck": (U64, [U64, U64]),
+    "dph_set_hasher": (INT, [INT]),
+    "dph_transcript_new": (VP, [STR]),
+    "dph_transcript_free": (None, [VP]),
+    "dph_transcript_append_f": (None, [VP, VP, U64]),
+    "dph_transcript_append_msg": (None, [VP, VP, U64]),
+    "dph_transcript_append_e": (None, [VP, VP, U64]),
+    "dph_transcript_challenge": (None, [VP, STR, VP]),
+    "dph_transcript_save_state": (None, [VP, VP, VP]),
+    "dph_transcript_load_state": (INT, [VP, INT, VP]),
+    "dph_sumcheck_prove_parallel": (INT, [VP, U32, VP, U32, U32, STR, VP, VP, VP, VP, VP]),
+    "dph_pcs_open": (INT, [VP, U32, VP, STR, VP, U64, VP, VP]),
+    "dph_zkml_context_free": (None, [VP]),
+    "dph_zkml_prove": (INT, [VP, VP, INT, STR, VP, U64, VP]),
+    "dph_zkml_pool_free": (None, [VP]),
+    "dph_zkml_prove_concurrent": (INT, [VP, INT, U32, U32, INT, STR, VP, VP, U64, VP]),
+    "dph_zkml_prove_concurrent_all": (INT, [VP, INT, U32, U32, INT, STR, VP, VP, U64, VP, VP]),
+    "dph_shm_mailbox_bytes": (U64, []),
+    "dph_shm_allgather": (INT, [VP, U32, U32, VP, VP, U64, VP]),
+    "dph_sumcheck_prove_sharded": (INT, [U32, U32, VP, U32, VP, U32, U32, STR, VP, VP, VP, VP, VP, VP, VP]),
+    "dph_pcs_open_sharded": (INT, [U32, U32, VP, U32, VP, STR, VP, VP, VP, VP, VP, U64, VP, VP, VP]),
+    "dph_sumcheck_prove_batch_polys": (INT, [U32, VP, U32, VP, U32, U32, STR, VP, VP, VP]),
+    "dph_conv_prove": (INT, [U32, U32, U32, U32, VP, VP, VP, VP, STR, VP, VP, VP, U64, VP]),
+    "dph_model_context_new": (INT, [VP, U32, VP, U64, VP]),
+    "dph_pcs_simple_batch": (INT, [VP, U32, U32, VP, U32, VP, STR, VP, VP, U64, VP]),
+    "dph_pcs_batch_open_evals": (INT, [VP, U32, U32, VP, VP, U32, VP, VP, U32, STR, VP, U64, VP]),
+    "dph_logup_prove": (INT, [VP, U32, VP, U32, VP, VP, STR, VP, U64, VP]),
+}
+TEST_HOOKS = {"dp_debug_wait_flag"}
 # every symbol include/deepprove_b200.h declares (tests check the .so exports each one)
-ABI_SYMBOLS = [
-    "dp_init", "dp_shutdown", "dp_device_count", "dp_last_error", "dp_version", "dp_set_stream", "dp_synchronize",
-    "dp_kernel_launches", "dp_host_waits", "dp_set_wait_mode", "dp_get_wait_mode", "dp_profile_enable", "dp_profile_reset", "dp_profile_read_ex", "dp_profile_flush",
-    "dp_mle_upload", "dp_mle_wrap_device", "dp_mle_clone", "dp_mle_download", "dp_mle_info", "dp_mle_device_ptr",
-    "dp_mle_free", "dp_mle_fix_high", "dp_mle_fix_high_new", "dp_mle_fix_low", "dp_mle_evaluate", "dp_mle_evaluate_many", "dp_eq_build",
-    "dp_sc_create", "dp_sc_round", "dp_sc_finish", "dp_sc_destroy", "dp_sc_current_mle", "dp_sc_set_resident_tail",
-    "dp_sc_tail_fs_next", "dp_sc_run_tail_fs", "dp_sc_run_tail_fs_blake", "dp_poseidon2_init", "dp_set_merkle_hasher", "dp_get_merkle_hasher", "dp_pcs_commit", "dp_pcs_commit_many", "dp_pcs_batch_commit", "dp_pcs_comm_num_polys", "dp_pcs_comm_part", "dp_pcs_comm_info", "dp_pcs_comm_codeword", "dp_pcs_comm_bh_evals", "dp_pcs_comm_free",
-    "dp_pcs_open_begin", "dp_pcs_open_round", "dp_pcs_open_final_message", "dp_pcs_open_query_words", "dp_pcs_open_query",
-    "dp_pcs_open_free", "dp_pcs_commit_shard", "dp_pcs_comm_shard_info", "dp_pcs_comm_set_shard_roots", "dp_pcs_open_set_shard_roots",
-    "dp_logup_build", "dp_logup_num_vars", "dp_logup_outputs", "dp_logup_layer_mles", "dp_logup_free", "dp_logup_layers_fs_next", "dp_logup_run_layers_fs", "dp_logup_run_layers_fs_blake", "dp_mle_linear_combination",
-    "dp_wit_begin", "dp_wit_dense", "dp_wit_matmul", "dp_wit_requant", "dp_wit_relu", "dp_wit_pool", "dp_wit_finish", "dp_wit_free",
-    "dp_fft_rows", "dp_pad_rows", "dp_conv_prod", "dp_conv_output_elements", "dp_phi_g_init", "dp_phi_level", "dp_mle_repeat",
-]
+ABI_SYMBOLS = sorted(n for n in SIGNATURES if n.startswith("dp_") and n not in TEST_HOOKS)
 
 
 # must be in the environment before CUDA initialises (see dp_init): 32 hardware work queues instead of 8
@@ -48,41 +158,22 @@ _lib = None
 _host = None
 
 
+def _load(path, prefix, **kw):
+    h = C.CDLL(path, **kw)
+    for name, (res, args) in SIGNATURES.items():
+        if name.startswith(prefix):
+            f = getattr(h, name)
+            f.restype, f.argtypes = res, args
+    return h
+
+
 def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError("%s not built: run `make` (or __graft_entry__.build()); the CUDA extension is "
                               "mandatory, there is no CPU fallback" % LIB_PATH)
-        _lib = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
-        _lib.dp_last_error.restype = C.c_char_p
-        _lib.dp_version.restype = C.c_char_p
-        _lib.dp_kernel_launches.restype = C.c_uint64
-        _lib.dp_host_waits.restype = C.c_uint64
-        _lib.dp_mle_device_ptr.restype = C.c_void_p
-        _lib.dp_mle_device_ptr.argtypes = [C.c_void_p]
-        _lib.dp_set_stream.argtypes = [C.c_void_p]
-        _lib.dp_mle_upload.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_void_p)]
-        _lib.dp_mle_wrap_device.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_void_p)]
-        _lib.dp_mle_clone.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-        _lib.dp_mle_download.argtypes = [C.c_void_p, C.c_void_p]
-        _lib.dp_mle_info.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_int), C.POINTER(C.c_uint32)]
-        _lib.dp_mle_free.argtypes = [C.c_void_p]
-        _lib.dp_mle_fix_high.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
-        _lib.dp_mle_fix_low.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
-        _lib.dp_mle_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
-        _lib.dp_eq_build.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
-        _lib.dp_sc_create.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(ScProduct), C.c_uint32, C.c_uint32,
-                                      C.c_uint32, C.POINTER(C.c_void_p)]
-        _lib.dp_sc_round.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.dp_sc_finish.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.dp_sc_destroy.argtypes = [C.c_void_p]
-        _lib.dp_sc_tail_fs_next.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
-        _lib.dp_sc_run_tail_fs.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-        _lib.dp_sc_run_tail_fs_blake.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-        _lib.dp_logup_layers_fs_next.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]
-        _lib.dp_logup_run_layers_fs.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 8
-        _lib.dp_logup_run_layers_fs_blake.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 8
+        _lib = _load(LIB_PATH, "dp_", mode=C.RTLD_GLOBAL)
     return _lib
 
 
@@ -92,21 +183,7 @@ def host():
         lib()
         if not os.path.exists(HOST_LIB_PATH):
             raise ImportError("%s not built: run `make`" % HOST_LIB_PATH)
-        _host = C.CDLL(HOST_LIB_PATH)
-        _host.dph_last_error.restype = C.c_char_p
-        _host.dph_transcript_new.restype = C.c_void_p
-        _host.dph_transcript_new.argtypes = [C.c_char_p]
-        _host.dph_transcript_free.argtypes = [C.c_void_p]
-        _host.dph_transcript_append_f.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
-        _host.dph_transcript_append_msg.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64]
-        _host.dph_transcript_append_e.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
-        _host.dph_transcript_challenge.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
-        _host.dph_transcript_save_state.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
-        _host.dph_transcript_load_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        _host.dph_poseidon2_permute.argtypes = [C.c_void_p]
-        _host.dph_sumcheck_prove_parallel.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(ScProduct), C.c_uint32,
-                                                      C.c_uint32, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                      C.c_void_p, C.POINTER(C.c_uint32)]
+        _host = _load(HOST_LIB_PATH, "dph_")
     return _host
 
 
@@ -146,6 +223,19 @@ def _u64(a):
 
 def _ptr(a):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def handles(mles):
+    """the C array of the MLEs' handles (None stays a null entry); never empty, so a zero count still passes a valid pointer"""
+    return (C.c_void_p * max(1, len(mles)))(*[None if m is None else m.h for m in mles])
+
+
+def flat_out(cap, call):
+    """call(out, cap, out_len) fills a zeroed buffer of `cap` words and reports the length it wrote: returns those words"""
+    out = np.zeros(cap, dtype=np.uint64)
+    n = C.c_uint64()
+    hcheck(call(_ptr(out), cap, C.byref(n)))
+    return out[: n.value].copy()
 
 
 class Mle:
@@ -277,6 +367,51 @@ def set_hasher(kind):
     hcheck(host().dph_set_hasher(int(kind)))
 
 
+class Transcript:
+    """DynTranscript of the C++ host mirror (host/transcript.hpp): BasicTranscript (Poseidon2 duplex sponge) or BlakeTranscript,
+    whichever set_hasher selected when it was made."""
+
+    def __init__(self, label=b"m2vec"):
+        self.h = C.c_void_p(host().dph_transcript_new(label))
+
+    def append_f(self, f):
+        f = _u64(f).reshape(-1)
+        host().dph_transcript_append_f(self.h, _ptr(f), f.size)
+
+    def append_msg(self, m):
+        host().dph_transcript_append_msg(self.h, bytes(m), len(m))
+
+    def append_e(self, e):
+        e = _u64(e).reshape(-1, 2)
+        host().dph_transcript_append_e(self.h, _ptr(e), e.shape[0])
+
+    def challenge(self, label):
+        out = np.zeros(2, dtype=np.uint64)
+        host().dph_transcript_challenge(self.h, label, _ptr(out))
+        return out
+
+    def save_state(self):
+        """-> (kind, words): kind 0 no device state, 1 the 14-word Poseidon2 sponge, 2 the DP_B3T_WORDS (80) BLAKE3 hasher image"""
+        kind, words = C.c_int(-1), np.zeros(80, dtype=np.uint64)
+        host().dph_transcript_save_state(self.h, C.byref(kind), _ptr(words))
+        return kind.value, words
+
+    def load_state(self, kind, words):
+        w = _u64(words)
+        hcheck(host().dph_transcript_load_state(self.h, int(kind), _ptr(w)))
+
+    def free(self):
+        if self.h:
+            host().dph_transcript_free(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
 def profile_enable(on=True):
     check(lib().dp_profile_enable(int(on)))
 
@@ -314,11 +449,10 @@ class Sumcheck:
 
     def __init__(self, mles, products, max_nv, max_deg):
         self.mles = list(mles)
-        hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
         self.prods = make_products(products)
         self.max_deg = max_deg
         self.h = C.c_void_p()
-        check(lib().dp_sc_create(hs, len(mles), self.prods, len(products), max_nv, max_deg, C.byref(self.h)))
+        check(lib().dp_sc_create(handles(mles), len(mles), self.prods, len(products), max_nv, max_deg, C.byref(self.h)))
 
     def round(self, challenge=None):
         out = np.zeros(2 * (self.max_deg + 1), dtype=np.uint64)
@@ -347,49 +481,29 @@ class Sumcheck:
 def sumcheck_prove_parallel(mles, products, max_nv, label=b"m2vec"):
     """IOPProverState::prove_parallel through the C++ host mirror (host Poseidon2 Fiat-Shamir).
     Returns (point[nv,2], msgs[nv,deg+1,2], final_evals[n_mles,2])."""
-    hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
     prods = make_products(products)
     max_deg = max(len(p[1]) for p in products)
     point = np.zeros((max_nv, 2), dtype=np.uint64)
     msgs = np.zeros((max_nv, max_deg + 1, 2), dtype=np.uint64)
     fin = np.zeros((len(mles), 2), dtype=np.uint64)
     deg = C.c_uint32()
-    hcheck(host().dph_sumcheck_prove_parallel(hs, len(mles), prods, len(products), max_nv, label, None, _ptr(point),
+    hcheck(host().dph_sumcheck_prove_parallel(handles(mles), len(mles), prods, len(products), max_nv, label, None, _ptr(point),
                                               _ptr(msgs), _ptr(fin), C.byref(deg)))
     return point, msgs, fin
 
 
 # ---- mpcs (Basefold) -------------------------------------------------------------------------------
 def _pcs_setup():
-    L = lib()
-    if getattr(L, "_pcs_ready", False):
-        return L
-    L.dp_pcs_commit.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
-    L.dp_pcs_comm_info.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]
-    L.dp_pcs_comm_codeword.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    L.dp_pcs_comm_bh_evals.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    L.dp_pcs_comm_free.argtypes = [C.c_void_p]
-    L.dp_pcs_open_begin.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.c_void_p]
-    L.dp_pcs_open_round.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
-    L.dp_pcs_open_final_message.argtypes = [C.c_void_p, C.c_void_p]
-    L.dp_pcs_open_query_words.argtypes = [C.c_void_p]
-    L.dp_pcs_open_query_words.restype = C.c_uint64
-    L.dp_pcs_open_query.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
-    L.dp_pcs_open_free.argtypes = [C.c_void_p]
-    L.dp_poseidon2_init.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    H = host()
-    H.dph_pcs_open.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p]
-    H.dph_pcs_batch_open.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64,
-                                     C.POINTER(C.c_uint64)]
-    L._pcs_ready = True
-    return L
+    """lib(), for callers that fetch the library through this name before using the Basefold entry points; their signatures are
+    in SIGNATURES like every other"""
+    return lib()
 
 
 class Commitment:
     """BasefoldCommitmentWithWitness on device (dp_pcs_comm)."""
 
     def __init__(self, mle, full_log):
-        L = _pcs_setup()
+        L = lib()
         self.h = C.c_void_p()
         check(L.dp_pcs_commit(mle.h, full_log, C.byref(self.h)))
         nv, b, t = C.c_uint32(), C.c_int(), C.c_int()
@@ -421,57 +535,37 @@ class Commitment:
 
 def pcs_open(mle, full_log, point, label=b"m2vec", cap=1 << 24):
     """Basefold::commit + Basefold::open through the C++ host mirror; returns (root, flat proof)."""
-    _pcs_setup()
     p = _u64(point).reshape(-1)
-    out = np.zeros(cap, dtype=np.uint64)
-    n = C.c_uint64()
     root = np.zeros(4, dtype=np.uint64)
-    hcheck(host().dph_pcs_open(mle.h, full_log, _ptr(p), label, _ptr(out), cap, C.byref(n), _ptr(root)))
-    return root, out[: n.value].copy()
+    flat = flat_out(cap, lambda *o: host().dph_pcs_open(mle.h, full_log, _ptr(p), label, *o, _ptr(root)))
+    return root, flat
 
 
 def pcs_batch_open(mles, full_log, points, label=b"m2vec", cap=1 << 25):
     """commit each polynomial, then Basefold::batch_open with Evaluation::new(i, i, poly_i(point_i))."""
-    _pcs_setup()
-    hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
-    p = np.concatenate([_u64(x).reshape(-1) for x in points])
-    out = np.zeros(cap, dtype=np.uint64)
-    n = C.c_uint64()
-    hcheck(host().dph_pcs_batch_open(hs, len(mles), full_log, _ptr(p), label, _ptr(out), cap, C.byref(n)))
-    return out[: n.value].copy()
+    return pcs_batch_open_evals(mles, full_log, points, range(len(mles)), range(len(mles)), label, cap)
 
 
 def pcs_batch_open_evals(mles, full_log, points, eval_poly, eval_point, label=b"m2vec", cap=1 << 25):
     """commit each polynomial, then Basefold::batch_open with an explicit evaluation list (several polynomials may share a point)"""
-    _pcs_setup()
-    H = host()
-    H.dph_pcs_batch_open_evals.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p,
-                                           C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
-    hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
     p = np.concatenate([_u64(x).reshape(-1) for x in points])
     pnv = np.ascontiguousarray([_u64(x).reshape(-1, 2).shape[0] for x in points], dtype=np.uint32)
     ep = np.ascontiguousarray(eval_poly, dtype=np.uint32); eq = np.ascontiguousarray(eval_point, dtype=np.uint32)
-    out = np.zeros(cap, dtype=np.uint64)
-    n = C.c_uint64()
-    hcheck(H.dph_pcs_batch_open_evals(hs, len(mles), full_log, p.ctypes.data, pnv.ctypes.data, len(pnv), ep.ctypes.data, eq.ctypes.data, len(ep), label, out.ctypes.data, cap, C.byref(n)))
-    return out[: n.value].copy()
+    return flat_out(cap, lambda *o: host().dph_pcs_batch_open_evals(handles(mles), len(mles), full_log, _ptr(p), _ptr(pnv), len(pnv),
+                                                                    _ptr(ep), _ptr(eq), len(ep), label, *o))
 
 
 def pcs_simple_batch(mles, full_log, point=None, evals=None, label=b"m2vec", cap=1 << 24):
     """Basefold::batch_commit of same-size device MLEs (+ simple_batch_open at `point` with the claimed `evals`): (root, flat | None)"""
-    _pcs_setup()
     H = host()
-    H.dph_pcs_simple_batch.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
-    hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
     root = np.zeros(4, dtype=np.uint64)
-    n = C.c_uint64()
     if point is None:
-        hcheck(H.dph_pcs_simple_batch(hs, len(mles), full_log, None, 0, None, label, root.ctypes.data, None, 0, C.byref(n)))
+        hcheck(H.dph_pcs_simple_batch(handles(mles), len(mles), full_log, None, 0, None, label, _ptr(root), None, 0, None))
         return root, None
     pt = _u64(point).reshape(-1); ev = _u64(evals).reshape(-1)
-    out = np.zeros(cap, dtype=np.uint64)
-    hcheck(H.dph_pcs_simple_batch(hs, len(mles), full_log, pt.ctypes.data, pt.size // 2, ev.ctypes.data, label, root.ctypes.data, out.ctypes.data, cap, C.byref(n)))
-    return root, out[: n.value].copy()
+    flat = flat_out(cap, lambda *o: H.dph_pcs_simple_batch(handles(mles), len(mles), full_log, _ptr(pt), pt.size // 2, _ptr(ev), label,
+                                                           _ptr(root), *o))
+    return root, flat
 
 
 # ---- zkml MLP prover (host mirror of zkml::{Context, Prover}) -----------------------------------------
@@ -481,18 +575,22 @@ class ZkmlContext:
     fixed_point_multiplier, intermediate_bit_size."""
 
     def __init__(self, n_layers, width, weights, bias, rq):
-        _pcs_setup()
-        H = host()
-        H.dph_zkml_context_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
-        H.dph_zkml_context_free.argtypes = [C.c_void_p]
-        H.dph_zkml_prove.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
         self.n_layers, self.width = n_layers, width
-        w = np.ascontiguousarray(weights, dtype=np.int64)
-        b = np.ascontiguousarray(bias, dtype=np.int64)
-        r = np.ascontiguousarray(rq, dtype=np.int64)
-        self.h = C.c_void_p()
-        hcheck(H.dph_zkml_context_new(n_layers, width, _ptr(w), _ptr(b), _ptr(r), C.byref(self.h)))
+        w = np.ascontiguousarray(weights, dtype=np.int64).reshape(n_layers, width * width)
+        b = np.ascontiguousarray(bias, dtype=np.int64).reshape(n_layers, width)
+        r = np.ascontiguousarray(rq, dtype=np.int64).reshape(n_layers, 4)
+        desc = np.zeros((3 * n_layers, 9), dtype=np.int64)      # per layer: Dense {width, width}, Requant {rq}, ReLU
+        desc[0::3, 1:3] = width
+        desc[1::3, 0], desc[1::3, 1:5] = 1, r
+        desc[2::3, 0] = 2
+        self._new(desc, np.concatenate([w, b], axis=1), width)
         self._out = np.zeros(1 << 22, dtype=np.uint64)
+
+    def _new(self, desc, data, input_len):
+        d = np.ascontiguousarray(desc, dtype=np.int64).reshape(-1, 9)
+        w = np.ascontiguousarray(data, dtype=np.int64)
+        self.h = C.c_void_p()
+        hcheck(host().dph_model_context_new(_ptr(d), d.shape[0], _ptr(w), int(input_len), C.byref(self.h)))
 
     def prove(self, x, label=b"m2vec"):
         """inference + Prover::prove + flat proof, from a host input vector (end to end)"""
@@ -515,27 +613,21 @@ class ZkmlContext:
         """n_workers persistent host threads (own stream + device arena each) prove until n_proofs are done; returns wall
         seconds, or (seconds, flat proof of the last job handed out) when want_proof.  e2e=False: Prover::prove on the stored
         trace; e2e=True: inference + prove + serialised proof per job."""
-        H = host()
-        H.dph_zkml_prove_concurrent.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_int, C.c_char_p, C.POINTER(C.c_double),
-                                                C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
         sec, n = C.c_double(), C.c_uint64()
         out = _ptr(self._out) if want_proof else None
-        hcheck(H.dph_zkml_prove_concurrent(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
-                                           out, self._out.size, C.byref(n)))
+        hcheck(host().dph_zkml_prove_concurrent(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
+                                                out, self._out.size, C.byref(n)))
         return (sec.value, self._out[: n.value].copy()) if want_proof else sec.value
 
     def prove_concurrent_all(self, n_workers, n_proofs, stride, device=0, e2e=False, label=b"m2vec"):
         """prove_concurrent, keeping every job's flat proof (dph_zkml_prove_concurrent_all).  Returns (seconds, proofs, workers):
         proofs[j] is job j's flat proof (at most `stride` words), workers[j] the index of the worker thread that proved it."""
-        H = host()
-        H.dph_zkml_prove_concurrent_all.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_int, C.c_char_p, C.POINTER(C.c_double),
-                                                    C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
         out = np.zeros(int(n_proofs) * int(stride), dtype=np.uint64)
         lens = np.zeros(int(n_proofs), dtype=np.uint64)
         workers = np.zeros(int(n_proofs), dtype=np.uint32)
         sec = C.c_double()
-        hcheck(H.dph_zkml_prove_concurrent_all(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
-                                               _ptr(out), int(stride), _ptr(lens), _ptr(workers)))
+        hcheck(host().dph_zkml_prove_concurrent_all(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
+                                                    _ptr(out), int(stride), _ptr(lens), _ptr(workers)))
         out = out.reshape(int(n_proofs), int(stride))
         return sec.value, [out[j, : int(lens[j])] for j in range(int(n_proofs))], workers
 
@@ -556,30 +648,18 @@ class ModelContext(ZkmlContext):
     dph_model_context_new: desc (n_nodes, 9) int64, data = weights in node order, input_len = padded input length."""
 
     def __init__(self, desc, data, input_len):
-        _pcs_setup()
-        H = host()
-        H.dph_model_context_new.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]
-        H.dph_zkml_context_free.argtypes = [C.c_void_p]
-        H.dph_zkml_prove.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
-        d = np.ascontiguousarray(desc, dtype=np.int64).reshape(-1, 9)
-        w = np.ascontiguousarray(data, dtype=np.int64)
-        self.h = C.c_void_p()
-        hcheck(H.dph_model_context_new(_ptr(d), d.shape[0], _ptr(w), int(input_len), C.byref(self.h)))
+        self._new(desc, data, input_len)
         self._out = np.zeros(1 << 23, dtype=np.uint64)
 
 
 def sumcheck_prove_batch_polys(T, mles, products, max_nv, label=b"m2vec"):
     """IOPProverState::prove_batch_polys (devirgo split into T contiguous slices) through the C++ host mirror."""
-    H = host()
-    H.dph_sumcheck_prove_batch_polys.argtypes = [C.c_uint32, C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(ScProduct), C.c_uint32, C.c_uint32,
-                                                 C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
     prods = make_products(products)
     max_deg = max(len(p[1]) for p in products)
     point = np.zeros((max_nv, 2), dtype=np.uint64)
     msgs = np.zeros((max_nv, max_deg + 1, 2), dtype=np.uint64)
     fin = np.zeros((len(mles), 2), dtype=np.uint64)
-    hcheck(H.dph_sumcheck_prove_batch_polys(T, hs, len(mles), prods, len(products), max_nv, label, _ptr(point), _ptr(msgs), _ptr(fin)))
+    hcheck(host().dph_sumcheck_prove_batch_polys(T, handles(mles), len(mles), prods, len(products), max_nv, label, _ptr(point), _ptr(msgs), _ptr(fin)))
     return point, msgs, fin
 
 
@@ -587,16 +667,17 @@ def sumcheck_prove_batch_polys(T, mles, products, max_nv, label=b"m2vec"):
 def conv_prove(filt, bias, unpadded_out, x, label=b"m2vec", cap=1 << 20, prove=True):
     """Convolution::op (+ prove_convolution_step when `prove`) on a padded layer: filt [kw, kx, real_nw, real_nw],
     bias [kw], x [kx, n_x, n_x] (int64).  Returns (after_bias, cleared, flat_proof | None)."""
-    H = host()
     filt = np.ascontiguousarray(filt, dtype=np.int64); bias = np.ascontiguousarray(bias, dtype=np.int64); x = np.ascontiguousarray(x, dtype=np.int64)
     kw, kx, rn, _ = filt.shape
     n_x = x.shape[1]
     uo = np.ascontiguousarray(unpadded_out, dtype=np.uint32)
     after = np.zeros((kw, n_x, n_x), dtype=np.int64)
     cleared = np.zeros((kw, n_x, n_x), dtype=np.int64)
-    out = np.zeros(cap if prove else 1, dtype=np.uint64)
-    n = C.c_uint64()
-    H.dph_conv_prove.argtypes = [C.c_uint32] * 4 + [C.c_void_p] * 4 + [C.c_char_p] + [C.c_void_p] * 3 + [C.c_uint64, C.c_void_p]
-    hcheck(H.dph_conv_prove(kw, kx, n_x, rn, filt.ctypes.data, bias.ctypes.data, uo.ctypes.data, x.ctypes.data, label, after.ctypes.data, cleared.ctypes.data,
-                            out.ctypes.data if prove else None, cap, C.addressof(n) if prove else None))
-    return after, cleared, (out[:n.value].copy() if prove else None)
+
+    def call(out, cap, out_len):
+        return host().dph_conv_prove(kw, kx, n_x, rn, _ptr(filt), _ptr(bias), _ptr(uo), _ptr(x), label, _ptr(after), _ptr(cleared),
+                                     out, cap, out_len)
+    if not prove:
+        hcheck(call(None, 0, None))
+        return after, cleared, None
+    return after, cleared, flat_out(cap, call)

@@ -7,6 +7,27 @@ static thread_local std::string g_herr;
 #define DPH_TRY try {
 #define DPH_CATCH } catch (const Error &e) { g_herr = e.what(); return e.code ? e.code : 1; } catch (const std::exception &e) { g_herr = e.what(); return 1; }
 
+// A caller's device MLE as a DeviceMle (a view, no copy); with T > 1, its slice t of T (the t-th contiguous part)
+static DeviceMle view(const dp_mle *m, uint32_t t = 0, uint32_t T = 1) {
+    uint64_t len; int ext; check(dp_mle_info(m, &len, &ext, nullptr));
+    const uint64_t sl = len / T;
+    return DeviceMle::wrap_device((char *)dp_mle_device_ptr(m) + (size_t)t * sl * (ext ? 16 : 8), sl, ext != 0);
+}
+// n extension elements given as [c0, c1] word pairs (a point, claimed evaluations)
+static ExtVec exts(const u64 *w, size_t n) {
+    ExtVec v;
+    for (size_t i = 0; i < n; i++) v.push_back(Ext(w[2 * i], w[2 * i + 1]));
+    return v;
+}
+// The flat-output rule: *out_len = the words the output needs; a null `out` only asks for that length, a `cap` below it is refused.
+static int put_flat(const char *entry, const std::vector<u64> &words, uint64_t *out, uint64_t cap, uint64_t *out_len) {
+    *out_len = words.size();
+    if (!out) return 0;
+    if (words.size() > cap) throw Error(DP_ERR_INVALID, std::string(entry) + ": output buffer too small");
+    memcpy(out, words.data(), 8 * words.size());
+    return 0;
+}
+
 extern "C" {
 
 const char *dph_last_error() { return g_herr.c_str(); }
@@ -63,11 +84,7 @@ static VirtualPolynomial make_poly(dp_mle *const *mles, uint32_t n_mles, const d
                                    uint32_t t = 0, uint32_t T = 1) {
     VirtualPolynomial vp(max_nv);
     std::vector<DeviceMle> views;
-    for (uint32_t i = 0; i < n_mles; i++) {
-        uint64_t len; int ext; check(dp_mle_info(mles[i], &len, &ext, nullptr));
-        uint64_t sl = len / T;
-        views.push_back(DeviceMle::wrap_device((char *)dp_mle_device_ptr(mles[i]) + (size_t)t * sl * (ext ? 16 : 8), sl, ext));
-    }
+    for (uint32_t i = 0; i < n_mles; i++) views.push_back(view(mles[i], t, T));
     for (uint32_t p = 0; p < n_products; p++) {
         std::vector<DeviceMle> l;
         for (uint32_t j = 0; j < products[p].n_idx; j++) l.push_back(views.at(products[p].idx[j]));
@@ -115,44 +132,13 @@ extern "C" {
 // Basefold::commit + Basefold::open with BasefoldProof flattened (BasefoldProof::flatten layout)
 int dph_pcs_open(dp_mle *poly, uint32_t full_log, const uint64_t *point, const char *label, uint64_t *out, uint64_t cap, uint64_t *out_len, uint64_t *out_root) {
     DPH_TRY
-    uint64_t len; int ext; uint32_t nv; check(dp_mle_info(poly, &len, &ext, &nv));
-    DeviceMle m = DeviceMle::wrap_device(dp_mle_device_ptr(poly), len, ext);
+    DeviceMle m = view(poly);
     BasefoldProverParams pp; pp.full_message_size_log = full_log;
     auto comm = Basefold::commit(pp, m);
     if (out_root) memcpy(out_root, comm.root.v, 32);
-    ExtVec pt; for (uint32_t i = 0; i < nv; i++) pt.push_back(Ext(point[2 * i], point[2 * i + 1]));
     DynTranscript t(label);
-    BasefoldProof pr = Basefold::open(pp, m, comm, pt, t);
-    std::vector<uint64_t> f = pr.flatten();
-    *out_len = f.size();
-    if (f.size() > cap) { g_herr = "dph_pcs_open: output buffer too small"; return 2; }
-    memcpy(out, f.data(), 8 * f.size());
-    return 0;
-    DPH_CATCH
-}
-
-int dph_pcs_batch_open(dp_mle *const *polys, uint32_t n, uint32_t full_log, const uint64_t *points, const char *label, uint64_t *out, uint64_t cap,
-                       uint64_t *out_len) {
-    DPH_TRY
-    BasefoldProverParams pp; pp.full_message_size_log = full_log;
-    std::vector<DeviceMle> ms; std::vector<BasefoldCommitmentWithWitness> comms; std::vector<ExtVec> pts; std::vector<Evaluation> evals;
-    size_t o = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        uint64_t len; int ext; uint32_t nv; check(dp_mle_info(polys[i], &len, &ext, &nv));
-        ms.push_back(DeviceMle::wrap_device(dp_mle_device_ptr(polys[i]), len, ext));
-        comms.push_back(Basefold::commit(pp, ms.back()));
-        ExtVec pt; for (uint32_t k = 0; k < nv; k++) pt.push_back(Ext(points[2 * (o + k)], points[2 * (o + k) + 1]));
-        o += nv; pts.push_back(pt);
-        Evaluation ev; ev.poly = i; ev.point = i; ev.value = ms.back().evaluate(pt);
-        evals.push_back(ev);
-    }
-    DynTranscript t(label);
-    BasefoldProof pr = Basefold::batch_open(pp, ms, comms, pts, evals, t);
-    std::vector<uint64_t> f = pr.flatten();
-    *out_len = f.size();
-    if (f.size() > cap) { g_herr = "dph_pcs_batch_open: output buffer too small"; return 2; }
-    memcpy(out, f.data(), 8 * f.size());
-    return 0;
+    BasefoldProof pr = Basefold::open(pp, m, comm, exts(point, m.num_vars()), t);
+    return put_flat("dph_pcs_open", pr.flatten(), out, cap, out_len);
     DPH_CATCH
 }
 
@@ -166,28 +152,6 @@ struct ZkHandle { dp::zkml::Model model; dp::zkml::Context ctx; dp::zkml::Device
 }
 extern "C" {
 
-// Model = n_layers x [Dense(width x width)+bias -> Requant -> ReLU]; rq = n_layers x {right_shift, fp_scale, fpm, intermediate_bits}.
-// Builds the Context: uploads weights/bias/tables and commits them (CommitmentContext::new) -- setup, not proving.
-int dph_zkml_context_new(uint32_t n_layers, uint32_t width, const int64_t *weights, const int64_t *bias, const int64_t *rq, void **out) {
-    DPH_TRY
-    using namespace dp::zkml;
-    auto *h = new ZkHandle();
-    h->model.input_len = width;
-    for (uint32_t l = 0; l < n_layers; l++) {
-        Node d; d.op = Op::Dense; d.nrows = d.ncols = width;
-        d.weights.assign(weights + (size_t)l * width * width, weights + (size_t)(l + 1) * width * width);
-        d.bias.assign(bias + (size_t)l * width, bias + (size_t)(l + 1) * width);
-        h->model.nodes.push_back(std::move(d));
-        Node r; r.op = Op::Requant; r.rq.right_shift = rq[4 * l]; r.rq.fp_scale = rq[4 * l + 1]; r.rq.fixed_point_multiplier = rq[4 * l + 2]; r.rq.intermediate_bit_size = rq[4 * l + 3];
-        h->model.nodes.push_back(r);
-        Node a; a.op = Op::Relu; h->model.nodes.push_back(a);
-    }
-    h->ctx = Context::generate(h->model);
-    check(dp_synchronize());
-    *out = h;
-    return 0;
-    DPH_CATCH
-}
 extern "C" void dph_zkml_pool_free(void *handle);
 void dph_zkml_context_free(void *h) { dph_zkml_pool_free(h); delete (ZkHandle *)h; }
 
@@ -203,13 +167,7 @@ int dph_zkml_prove(void *handle, const int64_t *input, int mode, const char *lab
     DynTranscript t(label);
     Prover<DynTranscript> prover(h->ctx, t);
     Proof p = prover.prove(h->trace);
-    if (out) {
-        std::vector<uint64_t> f = p.flatten(h->model.nodes.size());
-        *out_len = f.size();
-        if (f.size() > cap) { g_herr = "dph_zkml_prove: output buffer too small"; return 2; }
-        memcpy(out, f.data(), 8 * f.size());
-    }
-    return 0;
+    return out ? put_flat("dph_zkml_prove", p.flatten(h->model.nodes.size()), out, cap, out_len) : 0;
     DPH_CATCH
 }
 
@@ -332,6 +290,19 @@ extern "C" int dph_shm_allgather(void *shm_region, uint32_t world, uint32_t rank
     return 0;
     DPH_CATCH
 }
+// Runs fn(ex) over this rank's exchange: the shared-memory mailbox when shm_region is given (its sequence number carried in and out
+// through shm_seq; when fn throws the mailbox is poisoned, so peers fail fast instead of spinning on this rank's slot), else the callback.
+template <class Fn>
+static auto with_exchange(void *shm_region, uint64_t *shm_seq, CallbackExchange::Fn cb, void *user, uint32_t world, uint32_t rank, const char *entry, Fn fn) {
+    if (shm_region) {
+        ShmExchange ex(shm_region, world, rank); if (shm_seq) ex.seq = *shm_seq;
+        try { auto r = fn(ex); if (shm_seq) *shm_seq = ex.seq; return r; }
+        catch (...) { ex.poison(); if (shm_seq) *shm_seq = ex.seq; throw; }
+    }
+    if (!cb && world > 1) throw Error(DP_ERR_INVALID, std::string(entry) + ": no exchange given");
+    CallbackExchange ex(cb, user, world, rank);
+    return fn(ex);
+}
 extern "C" int dph_sumcheck_prove_sharded(uint32_t world, uint32_t rank, dp_mle *const *mles, uint32_t n_mles, const dp_sc_product *products, uint32_t n_products,
                                           uint32_t nv_total, const char *label, void *shm_region, uint64_t *shm_seq, CallbackExchange::Fn cb, void *user,
                                           uint64_t *out_point, uint64_t *out_msgs, uint64_t *out_final) {
@@ -339,14 +310,8 @@ extern "C" int dph_sumcheck_prove_sharded(uint32_t world, uint32_t rank, dp_mle 
     uint32_t logG = 0; while ((1u << logG) < world) logG++;
     VirtualPolynomial vp = make_poly(mles, n_mles, products, n_products, nv_total - logG);
     DynTranscript tr(label);
-    std::pair<IOPProof, IOPProverState> res;
-    if (shm_region) {
-        ShmExchange ex(shm_region, world, rank); if (shm_seq) ex.seq = *shm_seq;
-        try { res = IOPProverState::prove_sharded(std::move(vp), nv_total, ex, tr); }
-        catch (...) { ex.poison(); if (shm_seq) *shm_seq = ex.seq; throw; }   // peers fail fast instead of spinning on this rank's slot
-        if (shm_seq) *shm_seq = ex.seq;
-    }
-    else { if (!cb && world > 1) throw Error(DP_ERR_INVALID, "prove_sharded: no exchange given"); CallbackExchange ex(cb, user, world, rank); res = IOPProverState::prove_sharded(std::move(vp), nv_total, ex, tr); }
+    auto res = with_exchange(shm_region, shm_seq, cb, user, world, rank, "prove_sharded",
+                             [&](Exchange &ex) { return IOPProverState::prove_sharded(std::move(vp), nv_total, ex, tr); });
     write_proof(res, products, n_products, n_mles, out_point, out_msgs, out_final);
     return 0;
     DPH_CATCH
@@ -359,10 +324,9 @@ extern "C" int dph_pcs_open_sharded(uint32_t world, uint32_t rank, dp_mle *poly,
                                     void *shm_region, uint64_t *shm_seq, CallbackExchange::Fn cb, void *user,
                                     uint64_t *out, uint64_t cap, uint64_t *out_len, uint64_t *out_root, double *times_ms) {
     DPH_TRY
-    uint64_t len; int ext; uint32_t nv; check(dp_mle_info(poly, &len, &ext, &nv));
-    DeviceMle m = DeviceMle::wrap_device(dp_mle_device_ptr(poly), len, ext);
+    DeviceMle m = view(poly);
     BasefoldProverParams pp; pp.full_message_size_log = full_log;
-    ExtVec pt; for (uint32_t i = 0; i < nv; i++) pt.push_back(Ext(point[2 * i], point[2 * i + 1]));
+    const ExtVec pt = exts(point, m.num_vars());
     DynTranscript t(label);
     auto run = [&](Exchange &ex) {
         auto t0 = std::chrono::steady_clock::now();
@@ -374,16 +338,7 @@ extern "C" int dph_pcs_open_sharded(uint32_t world, uint32_t rank, dp_mle *poly,
         if (times_ms) { times_ms[0] = std::chrono::duration<double, std::milli>(t1 - t0).count(); times_ms[1] = std::chrono::duration<double, std::milli>(t2 - t1).count(); }
         return pr.flatten();
     };
-    std::vector<uint64_t> f;
-    if (shm_region) {
-        ShmExchange ex(shm_region, world, rank); if (shm_seq) ex.seq = *shm_seq;
-        try { f = run(ex); } catch (...) { ex.poison(); if (shm_seq) *shm_seq = ex.seq; throw; }
-        if (shm_seq) *shm_seq = ex.seq;
-    } else { if (!cb && world > 1) throw Error(DP_ERR_INVALID, "dph_pcs_open_sharded: no exchange given"); CallbackExchange ex(cb, user, world, rank); f = run(ex); }
-    *out_len = f.size();
-    if (f.size() > cap) { g_herr = "dph_pcs_open_sharded: output buffer too small"; return 2; }
-    memcpy(out, f.data(), 8 * f.size());
-    return 0;
+    return put_flat("dph_pcs_open_sharded", with_exchange(shm_region, shm_seq, cb, user, world, rank, "dph_pcs_open_sharded", run), out, cap, out_len);
     DPH_CATCH
 }
 
@@ -422,21 +377,19 @@ extern "C" int dph_conv_prove(uint32_t kw, uint32_t kx, uint32_t n_x, uint32_t r
     Claim cl; for (size_t i = 0; i < ceil_log2(cleared.size()); i++) cl.point.push_back(t.read_challenge());
     cl.eval = DeviceMle::from_evaluations_vec(to_base(cleared)).evaluate(cl.point);
     ConvProof pr; Claim in_claim = c.prove_convolution_step(t, cl, pd, pr);
-    std::vector<u64> fl = flatten_conv_proof(pr, in_claim);
-    *out_len = fl.size();
-    if (out) { if (fl.size() > cap) throw Error(DP_ERR_INVALID, "dph_conv_prove: output buffer too small"); memcpy(out, fl.data(), 8 * fl.size()); }
-    return 0;
+    return put_flat("dph_conv_prove", flatten_conv_proof(pr, in_claim), out, cap, out_len);
     DPH_CATCH
 }
 
 // General model builder: `desc` holds 9 int64 per node {kind, 8 shape words} and `data` the weights in node order
 // (kind 5 MatMul {rows, inner, cols, transposed, has_bias}: the constant right matrix then the bias; kind 0 Dense {nrows, ncols}: weights then bias; 1 Requant {right_shift, fp_scale, multiplier, intermediate_bits};
-//  2 ReLU; 3 Conv {kw, kx, nw, real_nw, unpadded_out[3]}: filter then bias; 4 Maxpool {C, H, W}).  Same handle type as
-// dph_zkml_context_new: dph_zkml_prove / dph_zkml_prove_concurrent / dph_zkml_context_free apply.
+//  2 ReLU; 3 Conv {kw, kx, nw, real_nw, unpadded_out[3]}: filter then bias; 4 Maxpool {C, H, W}).  Builds the Context: uploads
+// weights, bias and tables and commits them (CommitmentContext::new) -- setup, not proving.  dph_zkml_prove /
+// dph_zkml_prove_concurrent / dph_zkml_context_free take the handle.
 extern "C" int dph_model_context_new(const int64_t *desc, uint32_t n_nodes, const int64_t *data, uint64_t input_len, void **out) {
     DPH_TRY
     using namespace dp::zkml;
-    auto *h = new ZkHandle();
+    auto h = std::make_unique<ZkHandle>();
     h->model.input_len = input_len;
     const int64_t *w = data;
     for (uint32_t i = 0; i < n_nodes; i++) {
@@ -450,13 +403,13 @@ extern "C" int dph_model_context_new(const int64_t *desc, uint32_t n_nodes, cons
         case 4: n.op = Op::Pool; n.pool_c = d[1]; n.pool_h = d[2]; n.pool_w = d[3]; break;
         case 5: n.op = Op::MatMul; n.mm_r = d[1]; n.mm_k = d[2]; n.mm_c = d[3]; n.mm_t = d[4] != 0; n.mm_bias = d[5] != 0; n.weights.assign(w, w + n.mm_k * n.mm_c); w += n.mm_k * n.mm_c;
                 if (n.mm_bias) { n.bias.assign(w, w + n.mm_c); w += n.mm_c; } break;
-        default: delete h; throw Error(DP_ERR_INVALID, "dph_model_context_new: unknown node kind");
+        default: throw Error(DP_ERR_INVALID, "dph_model_context_new: unknown node kind");
         }
         h->model.nodes.push_back(std::move(n));
     }
     h->ctx = Context::generate(h->model);
     check(dp_synchronize());
-    *out = h;
+    *out = h.release();
     return 0;
     DPH_CATCH
 }
@@ -467,19 +420,13 @@ extern "C" int dph_pcs_simple_batch(dp_mle *const *polys, uint32_t n, uint32_t f
     DPH_TRY
     BasefoldProverParams pp; pp.full_message_size_log = full_log;
     std::vector<DeviceMle> ps;
-    for (uint32_t i = 0; i < n; i++) { uint64_t len; int ext; check(dp_mle_info(polys[i], &len, &ext, nullptr)); ps.push_back(DeviceMle::wrap_device(dp_mle_device_ptr(polys[i]), len, ext)); }
+    for (uint32_t i = 0; i < n; i++) ps.push_back(view(polys[i]));
     BasefoldCommitmentWithWitness comm = Basefold::batch_commit(pp, ps);
     memcpy(out_root, comm.root.v, 32);
     if (!point) return 0;
-    ExtVec pt, ev; for (uint32_t i = 0; i < nv; i++) pt.push_back(Ext(point[2 * i], point[2 * i + 1]));
-    for (uint32_t i = 0; i < n; i++) ev.push_back(Ext(evals[2 * i], evals[2 * i + 1]));
     DynTranscript t(label);
-    SimpleBatchProof sp = Basefold::simple_batch_open(pp, comm, pt, ev, t);
-    std::vector<uint64_t> f = sp.flatten();
-    *out_len = f.size();
-    if (f.size() > cap) throw Error(DP_ERR_INVALID, "dph_pcs_simple_batch: output buffer too small");
-    memcpy(out, f.data(), 8 * f.size());
-    return 0;
+    SimpleBatchProof sp = Basefold::simple_batch_open(pp, comm, exts(point, nv), exts(evals, n), t);
+    return put_flat("dph_pcs_simple_batch", sp.flatten(), out, cap, out_len);
     DPH_CATCH
 }
 
@@ -490,17 +437,13 @@ extern "C" int dph_pcs_batch_open_evals(dp_mle *const *polys, uint32_t n, uint32
     DPH_TRY
     BasefoldProverParams pp; pp.full_message_size_log = full_log;
     std::vector<DeviceMle> ms; std::vector<BasefoldCommitmentWithWitness> comms; std::vector<ExtVec> pts; std::vector<Evaluation> evals;
-    for (uint32_t i = 0; i < n; i++) { uint64_t len; int ext; check(dp_mle_info(polys[i], &len, &ext, nullptr)); ms.push_back(DeviceMle::wrap_device(dp_mle_device_ptr(polys[i]), len, ext)); comms.push_back(Basefold::commit(pp, ms.back())); }
+    for (uint32_t i = 0; i < n; i++) { ms.push_back(view(polys[i])); comms.push_back(Basefold::commit(pp, ms.back())); }
     size_t o = 0;
-    for (uint32_t k = 0; k < n_points; k++) { ExtVec pt; for (uint32_t j = 0; j < point_nv[k]; j++) pt.push_back(Ext(points[2 * (o + j)], points[2 * (o + j) + 1])); o += point_nv[k]; pts.push_back(pt); }
+    for (uint32_t k = 0; k < n_points; k++) { pts.push_back(exts(points + 2 * o, point_nv[k])); o += point_nv[k]; }
     for (uint32_t j = 0; j < n_evals; j++) { Evaluation ev; ev.poly = eval_poly[j]; ev.point = eval_point[j]; ev.value = ms.at(ev.poly).evaluate(pts.at(ev.point)); evals.push_back(ev); }
     DynTranscript t(label);
     BasefoldProof pr = Basefold::batch_open(pp, ms, comms, pts, evals, t);
-    std::vector<uint64_t> f = pr.flatten();
-    *out_len = f.size();
-    if (f.size() > cap) throw Error(DP_ERR_INVALID, "dph_pcs_batch_open_evals: output buffer too small");
-    memcpy(out, f.data(), 8 * f.size());
-    return 0;
+    return put_flat("dph_pcs_batch_open_evals", pr.flatten(), out, cap, out_len);
     DPH_CATCH
 }
 
@@ -513,7 +456,6 @@ extern "C" int dph_logup_prove(dp_mle *const *cols, uint32_t n_cols, dp_mle *mul
     DPH_TRY
     zkml::LogUpInput in;
     in.table = mult != nullptr;
-    auto view = [](dp_mle *m) { u64 len; int ext; check(dp_mle_info(m, &len, &ext, nullptr)); return DeviceMle::wrap_device(dp_mle_device_ptr(m), len, ext != 0); };
     for (uint32_t i = 0; i < n_cols; i++) in.column_evals.push_back(view(cols[i]));
     if (mult) in.multiplicities = view(mult);
     in.constant_challenge = Ext(cc[0], cc[1]); in.column_separation_challenge = Ext(sc[0], sc[1]); in.columns_per_instance = columns_per_instance;
@@ -526,9 +468,7 @@ extern "C" int dph_logup_prove(dp_mle *const *cols, uint32_t n_cols, dp_mle *mul
     for (auto &ev : pr.round_evaluations) { w.push_back(ev.size()); for (auto &e : ev) put(e); }
     for (auto &c : pr.output_claims) { for (auto &e : c.point) put(e); put(c.eval); }
     put(t.get_and_append_challenge("after"));
-    if (w.size() > cap) throw Error(DP_ERR_INVALID, "dph_logup_prove: output buffer too small");
-    std::copy(w.begin(), w.end(), out); *out_len = w.size();
-    return 0;
+    return put_flat("dph_logup_prove", w, out, cap, out_len);
     DPH_CATCH
 }
 

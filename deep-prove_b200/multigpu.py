@@ -16,9 +16,13 @@ After the local rounds the G residual values per MLE are all-gathered and the la
 The exchange is injected (`allgather`) so the same code runs over NCCL (device tensors over NVLink), over gloo
 (CPU tests) or in-process; the per-slice engine is injected as well (product: the CUDA library's dp_sc_*).
 """
+import ctypes as C
+
 import numpy as np
 
 P = 0xFFFFFFFF00000001
+# the exchange callback of the sharded entry points (host/sumcheck.hpp CallbackExchange::Fn): cb(user, send, n_words, recv) -> 0 on success
+_ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint64))
 
 
 def _sum_mod_p(parts):
@@ -98,43 +102,7 @@ def prove_sharded(make_engine, local_mles, products, nv_total, max_deg, rank, wo
     return np.array(point), np.array(msgs), fin
 
 
-# ---- product engine / transcript (CUDA library + C++ host mirror) -----------------------------------
-class HostTranscript:
-    """BasicTranscript of the C++ host mirror (host/transcript.hpp) -- Poseidon2 duplex sponge on the host CPU."""
-
-    def __init__(self, label=b"m2vec"):
-        import ctypes as C
-        import dpb200 as dp
-        self._C, self._dp = C, dp
-        H = dp.host()
-        H.dph_transcript_new.restype = C.c_void_p
-        H.dph_transcript_new.argtypes = [C.c_char_p]
-        H.dph_transcript_free.argtypes = [C.c_void_p]
-        H.dph_transcript_append_msg.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64]
-        H.dph_transcript_append_e.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
-        H.dph_transcript_challenge.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
-        self.H = H
-        self.h = C.c_void_p(H.dph_transcript_new(label))
-
-    def append_msg(self, m):
-        self.H.dph_transcript_append_msg(self.h, bytes(m), len(m))
-
-    def append_e(self, e):
-        e = np.ascontiguousarray(e, dtype=np.uint64).reshape(-1, 2)
-        self.H.dph_transcript_append_e(self.h, e.ctypes.data, e.shape[0])
-
-    def challenge(self, label):
-        out = np.zeros(2, dtype=np.uint64)
-        self.H.dph_transcript_challenge(self.h, label, out.ctypes.data)
-        return out
-
-    def __del__(self):
-        try:
-            self.H.dph_transcript_free(self.h)
-        except Exception:
-            pass
-
-
+# ---- product engine (CUDA library; the transcript is dpb200.Transcript of the C++ host mirror) ------------------------
 def device_engine(mles, products, nv, max_deg):
     """per-slice engine on this rank's GPU: mles are dpb200.Mle handles, or (array, is_ext) pairs that get uploaded"""
     import dpb200 as dp
@@ -144,23 +112,39 @@ def device_engine(mles, products, nv, max_deg):
 
 def prove_sharded_device(local_mles, products, nv_total, rank, world, allgather, label=b"m2vec"):
     """the product entry: this rank's slices are resident on its GPU (dp_init done by the caller)"""
+    import dpb200 as dp
     max_deg = max(len(p[1]) for p in products)
-    return prove_sharded(device_engine, local_mles, products, nv_total, max_deg, rank, world, allgather, HostTranscript(label))
+    return prove_sharded(device_engine, local_mles, products, nv_total, max_deg, rank, world, allgather, dp.Transcript(label))
 
 
 # ---- native path: the whole sharded proof inside the C++ host mirror, exchange through shared memory -----------
+def _exchange_args(mailbox, allgather, world):
+    """the (shm_region, shm_seq, cb, user) arguments of a sharded entry point: the mailbox, or a callback over `allgather` (keep the
+    tuple until the call returns: it holds the callback)."""
+    if mailbox is not None:
+        return C.c_void_p(mailbox.addr), C.byref(mailbox.seq), None, None
+    if allgather is None:
+        return None, None, None, None
+
+    def cb(user, send, n, recv):
+        try:
+            got = allgather(np.ctypeslib.as_array(send, shape=(int(n),)).copy())
+            np.ctypeslib.as_array(recv, shape=(world * int(n),))[:] = np.asarray(got, dtype=np.uint64).reshape(-1)
+            return 0
+        except Exception:
+            return 1
+    return None, None, _ALLGATHER_FN(cb), None
+
+
 class ShmMailbox:
     """Same-node mailbox for IOPProverState::prove_sharded (host/sumcheck.hpp ShmExchange): one zero-initialised POSIX
     shared-memory region mapped by every rank.  The per-round message must reach the host for Fiat-Shamir anyway, so
     the ranks exchange it host-to-host (~1 us) instead of through a device collective."""
 
     def __init__(self, name, rank, world, barrier):
-        import ctypes as C
         from multiprocessing import shared_memory, resource_tracker
         import dpb200 as dp
-        H = dp.host()
-        H.dph_shm_mailbox_bytes.restype = C.c_uint64
-        size = int(H.dph_shm_mailbox_bytes())
+        size = int(dp.host().dph_shm_mailbox_bytes())
         self.rank, self.world = rank, world
         if rank == 0:
             self.shm = shared_memory.SharedMemory(name=name, create=True, size=size)
@@ -189,31 +173,15 @@ class ShmMailbox:
 def prove_sharded_native(local_mles, products, nv_total, rank, world, mailbox=None, allgather=None, label=b"m2vec"):
     """IOPProverState::prove_sharded in the C++ host mirror (no Python in the round loop).  Exchange: `mailbox`
     (ShmMailbox, same node) or `allgather` (callable(words)->[world, n], e.g. TorchAllGather over NCCL)."""
-    import ctypes as C
     import dpb200 as dp
-    H = dp.host()
-    CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint64))
-    H.dph_sumcheck_prove_sharded.argtypes = [C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(dp.ScProduct), C.c_uint32, C.c_uint32,
-                                             C.c_char_p, C.c_void_p, C.POINTER(C.c_uint64), CB, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    hs = (C.c_void_p * len(local_mles))(*[m.h for m in local_mles])
     prods = dp.make_products(products)
     max_deg = max(len(p[1]) for p in products)
     point = np.zeros((nv_total, 2), dtype=np.uint64)
     msgs = np.zeros((nv_total, max_deg + 1, 2), dtype=np.uint64)
     fin = np.zeros((len(local_mles), 2), dtype=np.uint64)
-
-    def _cb(user, send, n, recv):
-        try:
-            got = allgather(np.ctypeslib.as_array(send, shape=(int(n),)).copy())
-            np.ctypeslib.as_array(recv, shape=(world * int(n),))[:] = np.asarray(got, dtype=np.uint64).reshape(-1)
-            return 0
-        except Exception:
-            return 1
-    cb = CB(_cb) if (mailbox is None and allgather is not None) else C.cast(None, CB)
-    dp.hcheck(H.dph_sumcheck_prove_sharded(world, rank, hs, len(local_mles), prods, len(products), nv_total, label,
-                                           C.c_void_p(mailbox.addr) if mailbox is not None else None,
-                                           C.byref(mailbox.seq) if mailbox is not None else None, cb, None,
-                                           point.ctypes.data, msgs.ctypes.data, fin.ctypes.data))
+    ex = _exchange_args(mailbox, allgather, world)
+    dp.hcheck(dp.host().dph_sumcheck_prove_sharded(world, rank, dp.handles(local_mles), len(local_mles), prods, len(products), nv_total, label,
+                                                   *ex, point.ctypes.data, msgs.ctypes.data, fin.ctypes.data))
     return point, msgs, fin
 
 
@@ -223,16 +191,11 @@ class LocalMailbox:
     same GPU) can play the ranks -- how the single-GPU tests exercise the sharded protocol end to end."""
 
     def __init__(self):
-        import ctypes as C
         import dpb200 as dp
-        H = dp.host()
-        H.dph_shm_mailbox_bytes.restype = C.c_uint64
-        self.buf = (C.c_char * int(H.dph_shm_mailbox_bytes()))()
+        self.buf = (C.c_char * int(dp.host().dph_shm_mailbox_bytes()))()
         self.addr = C.addressof(self.buf)
 
     def for_rank(self):
-        import ctypes as C
-
         class _View:
             pass
         v = _View(); v.addr = self.addr; v.seq = C.c_uint64(0)
@@ -244,27 +207,10 @@ def basefold_commit_open_sharded(mle, full_log, point, rank, world, mailbox=None
     this rank's GPU; this rank keeps the slice [rank/world, (rank+1)/world) of the bit-reversed evaluations, codeword, oracles and
     Merkle trees.  Exchange: `mailbox` (ShmMailbox / LocalMailbox view) or `allgather` (callable(words) -> [world, n]).
     Returns (root[4], flat proof (same image as dpb200.pcs_open), (commit_ms, open_ms)) -- identical on every rank."""
-    import ctypes as C
     import dpb200 as dp
-    dp._pcs_setup()
-    H = dp.host()
-    CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint64))
-    H.dph_pcs_open_sharded.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_uint64), CB, C.c_void_p,
-                                       C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p]
     p = np.ascontiguousarray(point, dtype=np.uint64).reshape(-1)
-    out = np.zeros(cap, dtype=np.uint64); n = C.c_uint64(); root = np.zeros(4, dtype=np.uint64); times = np.zeros(2, dtype=np.float64)
-
-    def cb_impl(user, send, n_words, recv):
-        try:
-            w = np.ctypeslib.as_array(send, shape=(n_words,)).copy()
-            got = np.ascontiguousarray(allgather(w), dtype=np.uint64).reshape(-1)
-            C.memmove(recv, got.ctypes.data, 8 * got.size)
-            return 0
-        except Exception:
-            return 1
-    cb = CB(cb_impl) if (mailbox is None and allgather is not None) else CB()
-    rc = H.dph_pcs_open_sharded(world, rank, mle.h, full_log, p.ctypes.data, label,
-                                C.c_void_p(mailbox.addr) if mailbox is not None else None, C.byref(mailbox.seq) if mailbox is not None else None, cb, None,
-                                out.ctypes.data, cap, C.byref(n), root.ctypes.data, times.ctypes.data)
-    dp.hcheck(rc)
-    return root, out[: n.value].copy(), (float(times[0]), float(times[1]))
+    root, times = np.zeros(4, dtype=np.uint64), np.zeros(2, dtype=np.float64)
+    ex = _exchange_args(mailbox, allgather, world)
+    flat = dp.flat_out(cap, lambda *o: dp.host().dph_pcs_open_sharded(world, rank, mle.h, full_log, p.ctypes.data, label, *ex, *o,
+                                                                      root.ctypes.data, times.ctypes.data))
+    return root, flat, (float(times[0]), float(times[1]))

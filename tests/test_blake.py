@@ -82,6 +82,14 @@ def _script(t_new, t_f, t_msg, t_e, t_ch, t_read):
     return out
 
 
+def host_transcript_ops():
+    """_script's operations on dpb200.Transcript, challenges as int pairs; read_challenge is a challenge with an empty label, which
+    appends nothing"""
+    def ch(t, label):
+        return tuple(int(x) for x in t.challenge(label))
+    return (lambda t, f: t.append_f(f), lambda t, m: t.append_msg(m), lambda t, e: t.append_e(e), ch, lambda t: ch(t, b""))
+
+
 def test_checker_and_host_blake_transcripts_match_the_python_restatement(blake_checker):
     py = _script(lambda l: PyBlakeTranscript(l), lambda t, f: [t.append_f(x) for x in f], lambda t, m: t.append_msg(m),
                  lambda t, e: [t.append_e(*x) for x in e], lambda t, l: t.challenge(l), lambda t: t.read_challenge())
@@ -93,26 +101,13 @@ def test_checker_and_host_blake_transcripts_match_the_python_restatement(blake_c
     assert orc == py
     # the product's host library (no GPU needed for the transcript)
     import dpb200 as dp
-    H = dp.host()
-    H.dph_set_hasher.argtypes = [C.c_int]
-    # dph_set_hasher also switches the device library's Merkle hasher flag (a plain flag: no device needed)
-    assert H.dph_set_hasher(1) == 0
+    # set_hasher also switches the device library's Merkle hasher flag (a plain flag: no device needed)
+    dp.set_hasher(1)
     try:
-        def h_f(t, f):
-            a = np.asarray(f, dtype=np.uint64); H.dph_transcript_append_f(t, a.ctypes.data_as(C.c_void_p), a.size)
-
-        def h_e(t, e):
-            a = np.asarray(e, dtype=np.uint64).reshape(-1); H.dph_transcript_append_e(t, a.ctypes.data_as(C.c_void_p), a.size // 2)
-
-        def h_ch(t, l):
-            o = np.zeros(2, dtype=np.uint64); H.dph_transcript_challenge(t, l, o.ctypes.data_as(C.c_void_p)); return (int(o[0]), int(o[1]))
-
-        def h_read(t):      # read_challenge without a label: an empty label appends nothing
-            return h_ch(t, b"")
-        host = _script(lambda l: C.c_void_p(H.dph_transcript_new(l)), h_f, lambda t, m: H.dph_transcript_append_msg(t, m, len(m)), h_e, h_ch, h_read)
+        host = _script(dp.Transcript, *host_transcript_ops())
         assert host == py
     finally:
-        H.dph_set_hasher(0)
+        dp.set_hasher(0)
 
 
 def test_blake_hasher_digests(blake_checker):

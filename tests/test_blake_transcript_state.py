@@ -2,8 +2,6 @@
 the DP_B3T_WORDS words a prover hands to the device transcript (dp_sc_run_tail_fs_blake, dp_logup_run_layers_fs_blake).  A
 transcript saved after any prefix and loaded into a fresh one continues exactly as the Python `blake3` package does, the image
 follows blake3::Hasher's lazy rules, a transcript of more than 2^16 chunks has no image, and load refuses images no hasher can be in."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -23,30 +21,9 @@ def _label(n):
 @pytest.fixture()
 def host():
     import dpb200 as dp
-    H = dp.host()
-    H.dph_set_hasher.argtypes = [C.c_int]
-    assert H.dph_set_hasher(1) == 0
-    yield H
-    H.dph_set_hasher(0)
-
-
-def _save(H, t):
-    kind = C.c_int(-1)
-    w = np.zeros(WORDS, dtype=np.uint64)
-    H.dph_transcript_save_state(t, C.byref(kind), w.ctypes.data_as(C.c_void_p))
-    return kind.value, w
-
-
-def _host_ops(H):
-    def h_f(t, f):
-        a = np.asarray(f, dtype=np.uint64); H.dph_transcript_append_f(t, a.ctypes.data_as(C.c_void_p), a.size)
-
-    def h_e(t, e):
-        a = np.asarray(e, dtype=np.uint64).reshape(-1); H.dph_transcript_append_e(t, a.ctypes.data_as(C.c_void_p), a.size // 2)
-
-    def h_ch(t, lbl):
-        o = np.zeros(2, dtype=np.uint64); H.dph_transcript_challenge(t, lbl, o.ctypes.data_as(C.c_void_p)); return (int(o[0]), int(o[1]))
-    return h_f, lambda t, m: H.dph_transcript_append_msg(t, m, len(m)), h_e, h_ch, lambda t: h_ch(t, b"")
+    dp.set_hasher(1)
+    yield dp
+    dp.set_hasher(0)
 
 
 def _expected_image_fields(n):
@@ -60,26 +37,25 @@ def _expected_image_fields(n):
 
 @pytest.mark.parametrize("n", PREFIXES)
 def test_saved_state_continues_like_the_package(host, n):
-    H = host
     label = _label(n)
-    t = C.c_void_p(H.dph_transcript_new(label))
+    t = host.Transcript(label)
     try:
-        kind, w = _save(H, t)
+        kind, w = t.save_state()
     finally:
-        H.dph_transcript_free(t)
+        t.free()
     assert kind == 2
     ctr, blen, nblk, slen = _expected_image_fields(n)
     assert [int(w[4]), int(w[13]), int(w[14]), int(w[15])] == [ctr, blen, nblk, slen]
     block = w[5:13].tobytes()
     assert block[:blen] == label[n - blen:n] and block[blen:] == b"\0" * (64 - blen)
     assert not w[16 + 4 * slen:].any()
-    fresh = C.c_void_p(H.dph_transcript_new(b"something else"))
+    fresh = host.Transcript(b"something else")
     try:
-        assert H.dph_transcript_load_state(fresh, 2, w.ctypes.data_as(C.c_void_p)) == 0
-        got = TB._script(lambda _: fresh, *_host_ops(H))
-        kind2, w2 = _save(H, fresh)
+        fresh.load_state(2, w)
+        got = TB._script(lambda _: fresh, *TB.host_transcript_ops())
+        kind2, w2 = fresh.save_state()
     finally:
-        H.dph_transcript_free(fresh)
+        fresh.free()
     py = TB._script(lambda _: TB.PyBlakeTranscript(label), lambda t, f: [t.append_f(x) for x in f], lambda t, m: t.append_msg(m),
                     lambda t, e: [t.append_e(*x) for x in e], lambda t, lbl: t.challenge(lbl), lambda t: t.read_challenge())
     assert got == py
@@ -88,29 +64,28 @@ def test_saved_state_continues_like_the_package(host, n):
 
 def test_sixteen_stack_entries_save_and_seventeen_refuse(host):
     """2^16 - 1 pushed chunks: 16 stack entries, the deepest image; 2^17 - 1: 17 entries, no image (the host keeps the transcript)"""
-    H = host
     n16 = (2 ** 16 - 1) * 1024 + 1
     label = _label(n16)
-    t = C.c_void_p(H.dph_transcript_new(label))
+    t = host.Transcript(label)
     try:
-        kind, w = _save(H, t)
+        kind, w = t.save_state()
         assert kind == 2 and int(w[15]) == 16 and int(w[4]) == 2 ** 16 - 1
-        fresh = C.c_void_p(H.dph_transcript_new(b""))
+        fresh = host.Transcript(b"")
         try:
-            assert H.dph_transcript_load_state(fresh, 2, w.ctypes.data_as(C.c_void_p)) == 0
-            got = TB._script(lambda _: fresh, *_host_ops(H))
+            fresh.load_state(2, w)
+            got = TB._script(lambda _: fresh, *TB.host_transcript_ops())
         finally:
-            H.dph_transcript_free(fresh)
+            fresh.free()
     finally:
-        H.dph_transcript_free(t)
+        t.free()
     py = TB._script(lambda _: TB.PyBlakeTranscript(label), lambda t, f: [t.append_f(x) for x in f], lambda t, m: t.append_msg(m),
                     lambda t, e: [t.append_e(*x) for x in e], lambda t, lbl: t.challenge(lbl), lambda t: t.read_challenge())
     assert got == py
-    t = C.c_void_p(H.dph_transcript_new(_label((2 ** 17 - 1) * 1024 + 1)))
+    t = host.Transcript(_label((2 ** 17 - 1) * 1024 + 1))
     try:
-        kind, w = _save(H, t)
+        kind, w = t.save_state()
     finally:
-        H.dph_transcript_free(t)
+        t.free()
     assert kind == 0
 
 
@@ -129,13 +104,17 @@ def malformed_images():
 
 
 def test_load_refuses_malformed_images(host):
-    H = host
     ok, bad = malformed_images()
-    t = C.c_void_p(H.dph_transcript_new(b"x"))
+    t = host.Transcript(b"x")
     try:
-        assert H.dph_transcript_load_state(t, 2, ok.ctypes.data_as(C.c_void_p)) == 0
+        t.load_state(2, ok)
         for name, w in bad:
-            assert H.dph_transcript_load_state(t, 2, w.ctypes.data_as(C.c_void_p)) != 0, name
-        assert H.dph_transcript_load_state(t, 1, ok.ctypes.data_as(C.c_void_p)) != 0, "a Poseidon2 state into a BLAKE3 transcript"
+            try:
+                t.load_state(2, w)
+            except host.DpError:
+                continue
+            pytest.fail("a malformed image was loaded: " + name)
+        with pytest.raises(host.DpError):         # a Poseidon2 state into a BLAKE3 transcript
+            t.load_state(1, ok)
     finally:
-        H.dph_transcript_free(t)
+        t.free()

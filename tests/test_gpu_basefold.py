@@ -127,20 +127,13 @@ def test_batch_open_with_shared_points(gpu):
 
 
 # ---- refusals of the Basefold C ABI ------------------------------------------------------------------------------------------------
-def _abi(gpu):
-    L = gpu._pcs_setup()
-    L.dp_pcs_commit_shard.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
-    L.dp_pcs_batch_commit.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
-    return L
-
-
 def _commit(gpu, nv, full_log):
     return gpu.Commitment(gpu.Mle.upload(rnd_poly(600 + nv, nv, False), False), full_log)
 
 
 def _open_begin(gpu, handles, num_vars, batch=False):
     """dp_pcs_open_begin over raw commitment handles -> return code (an opening that starts is freed again)"""
-    L = _abi(gpu)
+    L = gpu.lib()
     hs = (C.c_void_p * len(handles))(*handles)
     pt = gpu._u64(O.splitmix_e(610, num_vars)).reshape(-1)
     coeffs = np.ones(2 * len(handles), dtype=np.uint64) if batch else None
@@ -173,7 +166,7 @@ def _open_single_wrong_vars(gpu):
 
 
 def _sharded(gpu, nv=13):
-    L = _abi(gpu)
+    L = gpu.lib()
     m, h = gpu.Mle.upload(rnd_poly(620, nv, False), False), C.c_void_p()
     gpu.check(L.dp_pcs_commit_shard(m.h, nv, 0, 2, C.byref(h)))
     return h
@@ -184,7 +177,7 @@ def _open_sharded_in_batch(gpu):
     try:
         return _open_begin(gpu, [h.value], 13, batch=True)
     finally:
-        _abi(gpu).dp_pcs_comm_free(h)
+        gpu.lib().dp_pcs_comm_free(h)
 
 
 def _open_sharded_without_roots(gpu):
@@ -192,11 +185,11 @@ def _open_sharded_without_roots(gpu):
     try:
         return _open_begin(gpu, [h.value], 13)
     finally:
-        _abi(gpu).dp_pcs_comm_free(h)
+        gpu.lib().dp_pcs_comm_free(h)
 
 
 def _shard(gpu, nv, rank, world, hasher=0):
-    L = _abi(gpu)
+    L = gpu.lib()
     m, h = gpu.Mle.upload(rnd_poly(630, nv, False), False), C.c_void_p()
     gpu.set_hasher(hasher)
     try:
@@ -209,11 +202,10 @@ def _shard(gpu, nv, rank, world, hasher=0):
 
 
 def _batch(gpu, nvs):
-    L = _abi(gpu)
+    L = gpu.lib()
     mles = [gpu.Mle.upload(rnd_poly(640 + i, nv, False), False) for i, nv in enumerate(nvs)]
-    hs = (C.c_void_p * max(1, len(mles)))(*[m.h for m in mles])
     h = C.c_void_p()
-    rc = L.dp_pcs_batch_commit(hs, len(mles), 10, C.byref(h))
+    rc = L.dp_pcs_batch_commit(gpu.handles(mles), len(mles), 10, C.byref(h))
     if rc == 0:
         L.dp_pcs_comm_free(h)
     return rc

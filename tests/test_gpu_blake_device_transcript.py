@@ -39,29 +39,18 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
-class HostT:
-    """a host BlakeTranscript through the C entry points (the `blake` hasher must be selected)"""
+def _host_t(gpu, label=b"", image=None):
+    """a host BlakeTranscript (the `blake` hasher must be selected), continued from `image` when given"""
+    t = gpu.Transcript(label)
+    if image is not None:
+        t.load_state(2, image)
+    return t
 
-    def __init__(self, gpu, label=b"", image=None):
-        self.H = gpu.host()
-        self.t = C.c_void_p(self.H.dph_transcript_new(label))
-        if image is not None:
-            w = np.ascontiguousarray(image, dtype=np.uint64)
-            assert self.H.dph_transcript_load_state(self.t, 2, _p(w)) == 0
 
-    def image(self):
-        kind, w = TS._save(self.H, self.t)
-        assert kind == 2
-        return w
-
-    def append_e(self, c0, c1):
-        a = np.array([c0, c1], dtype=np.uint64); self.H.dph_transcript_append_e(self.t, _p(a), 1)
-
-    def challenge(self, label):
-        o = np.zeros(2, dtype=np.uint64); self.H.dph_transcript_challenge(self.t, label, _p(o)); return (int(o[0]), int(o[1]))
-
-    def free(self):
-        self.H.dph_transcript_free(self.t)
+def _image(t):
+    kind, w = t.save_state()
+    assert kind == 2
+    return w
 
 
 def _run_tail(gpu, sc, nv, max_deg, image, prev=None, entry="dp_sc_run_tail_fs_blake"):
@@ -100,9 +89,8 @@ def _continue(t, msgs):
     """what the host transcript t draws for these round messages"""
     out = []
     for m in msgs:
-        for e in m:
-            t.append_e(int(e[0]), int(e[1]))
-        out.append(t.challenge(b"Internal round"))
+        t.append_e(m)
+        out.append(tuple(int(x) for x in t.challenge(b"Internal round")))
     return out
 
 
@@ -114,12 +102,12 @@ def test_device_hasher_continues_a_handed_over_state(blake, n, max_deg):
     challenges equal the package's, the image coming back equals the host hasher's after the same bytes, and the messages equal the
     oracle's at those challenges"""
     label = TS._label(n)
-    src = HostT(blake, label)
+    src = _host_t(blake, label)
     try:
-        image = src.image()
+        image = _image(src)
         msgs, ch, w_out = _tail_case(blake, image, max_deg)
         host = _continue(src, msgs)
-        host_image = src.image()
+        host_image = _image(src)
     finally:
         src.free()
     py = TB.PyBlakeTranscript(label)
@@ -144,18 +132,18 @@ def _synthetic_high_counter():
 @pytest.mark.parametrize("kind", ["stack16", "counter_above_2e32"])
 def test_device_hasher_on_synthetic_images(blake, kind):
     if kind == "stack16":
-        src = HostT(blake, TS._label((2 ** 16 - 1) * 1024 + 1))
-        image = src.image()
+        src = _host_t(blake, TS._label((2 ** 16 - 1) * 1024 + 1))
+        image = _image(src)
         assert int(image[15]) == 16
         src.free()
     else:
         image = _synthetic_high_counter()
-    t = HostT(blake, b"", image)
+    t = _host_t(blake, b"", image)
     try:
-        assert (t.image() == image).all()
+        assert (_image(t) == image).all()
         msgs, ch, w_out = _tail_case(blake, image, 3, nv=6)
         host = _continue(t, msgs)
-        host_image = t.image()
+        host_image = _image(t)
     finally:
         t.free()
     assert [(int(a), int(b)) for a, b in ch] == host
@@ -170,11 +158,11 @@ def test_retry_path(blake):
     label = g["label"].encode()
     mles = [(O.splitmix_e(s, 1 << g["nv"]) if ext else O.splitmix_f(s, 1 << g["nv"]), ext) for s, ext in g["mles"]]
     products = [(tuple(g["product"][0]), g["product"][1])]
-    src = HostT(blake, label)
+    src = _host_t(blake, label)
     try:
-        msgs, ch, w_out = _tail_case(blake, src.image(), g["max_deg"], nv=g["nv"], mles=mles, products=products)
+        msgs, ch, w_out = _tail_case(blake, _image(src), g["max_deg"], nv=g["nv"], mles=mles, products=products)
         host = _continue(src, msgs)
-        host_image = src.image()
+        host_image = _image(src)
     finally:
         src.free()
     py = TB.PyBlakeTranscript(label)
@@ -240,12 +228,11 @@ def test_blake_device_layers_match_the_host_path(blake, case):
         H = gpu.host()
         dm = [gpu.Mle.upload(c, False) for c in cols]
         dmult = gpu.Mle.upload(mult, False) if mult is not None else None
-        hs = (C.c_void_p * len(dm))(*[m.h for m in dm])
         cc = np.array(O.splitmix_f(91, 2), dtype=np.uint64)
         sc = np.array(O.splitmix_f(92, 2), dtype=np.uint64)
         out = np.zeros(1 << 20, dtype=np.uint64)
         n = C.c_uint64()
-        gpu.hcheck(H.dph_logup_prove(hs, len(dm), dmult.h if dmult else None, cpi, _p(cc), _p(sc), LABEL, _p(out), out.size, C.byref(n)))
+        gpu.hcheck(H.dph_logup_prove(gpu.handles(dm), len(dm), dmult.h if dmult else None, cpi, _p(cc), _p(sc), LABEL, _p(out), out.size, C.byref(n)))
         b3 = _launches(gpu, B3_LAYERS)
     finally:
         gpu.profile_enable(False)

@@ -127,21 +127,19 @@ RESIDENT_CASES = [c.name for c in D.CASES if any(r["family"] == "resident" for r
 
 def _prove(gpu, mles, products, nv):
     """prove_parallel through the host library with an explicit transcript; returns the proof and one challenge drawn after it"""
-    H = gpu.host()
-    hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
     prods = gpu.make_products(products)
     max_deg = max(len(p[1]) for p in products)
     point = np.zeros((nv, 2), dtype=np.uint64)
     msgs = np.zeros((nv, max_deg + 1, 2), dtype=np.uint64)
     fin = np.zeros((len(mles), 2), dtype=np.uint64)
     deg = C.c_uint32()
-    t = H.dph_transcript_new(LABEL)
+    t = gpu.Transcript(LABEL)
     try:
-        gpu.hcheck(H.dph_sumcheck_prove_parallel(hs, len(mles), prods, len(products), nv, LABEL, t, _p(point), _p(msgs), _p(fin), C.byref(deg)))
-        after = np.zeros(2, dtype=np.uint64)
-        H.dph_transcript_challenge(t, b"after", _p(after))
+        gpu.hcheck(gpu.host().dph_sumcheck_prove_parallel(gpu.handles(mles), len(mles), prods, len(products), nv, LABEL, t.h, _p(point), _p(msgs),
+                                                          _p(fin), C.byref(deg)))
+        after = t.challenge(b"after")
     finally:
-        H.dph_transcript_free(t)
+        t.free()
     return point, msgs, fin, after
 
 

@@ -31,7 +31,6 @@ def _prove(gpu, cols, mult, cpi, mode):
     H = gpu.host()
     dm = [gpu.Mle.upload(c, False) for c in cols]
     dmult = gpu.Mle.upload(mult, False) if mult is not None else None
-    hs = (C.c_void_p * len(dm))(*[m.h for m in dm])
     cc = np.array(O.splitmix_f(91, 2), dtype=np.uint64)
     sc = np.array(O.splitmix_f(92, 2), dtype=np.uint64)
     out = np.zeros(1 << 20, dtype=np.uint64)
@@ -41,9 +40,7 @@ def _prove(gpu, cols, mult, cpi, mode):
     gpu.profile_enable(True)
     gpu.profile_reset()
     try:
-        H.dph_logup_prove.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_char_p, C.c_void_p,
-                                      C.c_uint64, C.POINTER(C.c_uint64)]
-        gpu.hcheck(H.dph_logup_prove(hs, len(dm), dmult.h if dmult else None, cpi, _p(cc), _p(sc), LABEL, _p(out), out.size, C.byref(n)))
+        gpu.hcheck(H.dph_logup_prove(gpu.handles(dm), len(dm), dmult.h if dmult else None, cpi, _p(cc), _p(sc), LABEL, _p(out), out.size, C.byref(n)))
         gpu.lib().dp_profile_flush()
         fs = gpu.profile_read().get(LAYERS_PROFILE, (0,))[0]
     finally:
@@ -86,9 +83,6 @@ def test_device_layers_match_the_host_path(gpu, case):
 
 def _circuits(gpu, n_circuits, nv):
     L = gpu.lib()
-    L.dp_logup_build.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
-    L.dp_logup_layers_fs_next.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]
-    L.dp_logup_run_layers_fs.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 8
     cc = np.array([3, 0], dtype=np.uint64)
     sc = np.array([5, 0], dtype=np.uint64)
     keep, hs = [], []

@@ -270,31 +270,12 @@ def test_reference_matches_the_oracle_circuit(name):
 
 
 # ---- device wrappers (C ABI, include/deepprove_b200.h) ---------------------------------------------------------------------
-def _abi(gpu):
-    L = gpu.lib()
-    if not getattr(L, "_lookup_abi", False):
-        L.dp_logup_build.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
-        L.dp_logup_num_vars.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
-        L.dp_logup_outputs.argtypes = [C.c_void_p, C.c_void_p]
-        L.dp_logup_layer_mles.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]
-        L.dp_logup_free.argtypes = [C.c_void_p]
-        L.dp_mle_linear_combination.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
-        L.dp_mle_evaluate_many.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
-        L.dp_wit_matmul.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(C.c_void_p)]
-        L._lookup_abi = True
-    return L
-
-
-def _handles(mles):
-    return (C.c_void_p * max(1, len(mles)))(*[None if m is None else m.h for m in mles])
-
-
 class Logup:
     def __init__(self, gpu, cols, mult, c, gamma, n_columns=None):
-        self.gpu, self.L = gpu, _abi(gpu)
+        self.gpu, self.L = gpu, gpu.lib()
         self._c, self._g = O.u64(c), O.u64(gamma)
         self.h = C.c_void_p()
-        gpu.check(self.L.dp_logup_build(_handles(cols), len(cols) if n_columns is None else n_columns,
+        gpu.check(self.L.dp_logup_build(gpu.handles(cols), len(cols) if n_columns is None else n_columns,
                                         None if mult is None else mult.h, self._c.ctypes.data, self._g.ctypes.data, C.byref(self.h)))
 
     def num_vars(self):
@@ -321,20 +302,20 @@ class Logup:
 def linear_combination(gpu, mles, coefs, n=None):
     cf = O.u64(coefs).reshape(-1)
     out = C.c_void_p()
-    gpu.check(_abi(gpu).dp_mle_linear_combination(_handles(mles), cf.ctypes.data, len(mles) if n is None else n, C.byref(out)))
+    gpu.check(gpu.lib().dp_mle_linear_combination(gpu.handles(mles), cf.ctypes.data, len(mles) if n is None else n, C.byref(out)))
     return gpu.Mle(out.value)
 
 
 def evaluate_many(gpu, mles, point, num_vars):
     pt = O.u64(point).reshape(-1)
     out = np.zeros(2 * len(mles), dtype=np.uint64)
-    gpu.check(_abi(gpu).dp_mle_evaluate_many(_handles(mles), len(mles), pt.ctypes.data if pt.size else None, num_vars, out.ctypes.data))
+    gpu.check(gpu.lib().dp_mle_evaluate_many(gpu.handles(mles), len(mles), pt.ctypes.data if pt.size else None, num_vars, out.ctypes.data))
     return out.reshape(-1, 2)
 
 
 def matmul(gpu, left, right, bias, R, K, Cc, transposed):
     out = C.c_void_p()
-    gpu.check(_abi(gpu).dp_wit_matmul(left.h, right.h, None if bias is None else bias.h, R, K, Cc, int(transposed), C.byref(out)))
+    gpu.check(gpu.lib().dp_wit_matmul(left.h, right.h, None if bias is None else bias.h, R, K, Cc, int(transposed), C.byref(out)))
     return gpu.Mle(out.value)
 
 
@@ -541,7 +522,7 @@ def test_evaluate_many_refusals(gpu):
     a, b = gpu.Mle.upload(O.splitmix_f(1, 16), False), gpu.Mle.upload(O.splitmix_f(2, 8), False)
     _refused(gpu, lambda: evaluate_many(gpu, [a, b], O.splitmix_e(3, 4), 4), "MLE size does not match the point")
     with pytest.raises(gpu.DpError) as e:
-        gpu.check(_abi(gpu).dp_mle_evaluate_many(_handles([a]), 0, O.splitmix_e(3, 4).ctypes.data, 4, np.zeros(2, np.uint64).ctypes.data))
+        gpu.check(gpu.lib().dp_mle_evaluate_many(gpu.handles([a]), 0, O.splitmix_e(3, 4).ctypes.data, 4, np.zeros(2, np.uint64).ctypes.data))
     assert e.value.code == gpu.DP_ERR_INVALID
 
 

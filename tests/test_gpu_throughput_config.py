@@ -360,24 +360,15 @@ def _comm_data(gpu, h):
     return root, cw, gpu.Mle(v.value).download()
 
 
-def _api(gpu):
-    L = gpu._pcs_setup()
-    L.dp_pcs_batch_commit.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
-    L.dp_pcs_commit_many.argtypes = [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
-    L.dp_pcs_comm_part.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
-    return L
-
-
 def commit_on_device(gpu, case, polys):
     """one dp_pcs_commit (or dp_pcs_batch_commit) -> (root, [(codeword, evaluations) per polynomial])"""
-    L = _api(gpu)
+    L = gpu.lib()
     mles = [gpu.Mle.upload(p, case.ext) for p in polys]
     h = C.c_void_p()
     if case.n_polys == 1:
         gpu.check(L.dp_pcs_commit(mles[0].h, case.full_log, C.byref(h)))
     else:
-        hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
-        gpu.check(L.dp_pcs_batch_commit(hs, len(mles), case.full_log, C.byref(h)))
+        gpu.check(L.dp_pcs_batch_commit(gpu.handles(mles), len(mles), case.full_log, C.byref(h)))
     try:
         if case.n_polys == 1:
             root, cw, bh = _comm_data(gpu, h)
@@ -482,11 +473,10 @@ def _many_polys(seed):
 
 def commit_many_on_device(gpu, polys):
     """one dp_pcs_commit_many call -> [(root, codeword, evaluations)]"""
-    L = _api(gpu)
+    L = gpu.lib()
     mles = [gpu.Mle.upload(a, e) for a, e in polys]
-    hs = (C.c_void_p * len(mles))(*[m.h for m in mles])
     out = (C.c_void_p * len(mles))()
-    gpu.check(L.dp_pcs_commit_many(hs, len(mles), MANY_FULL_LOG, out))
+    gpu.check(L.dp_pcs_commit_many(gpu.handles(mles), len(mles), MANY_FULL_LOG, out))
     try:
         return [_comm_data(gpu, out[i]) for i in range(len(mles))]
     finally:

@@ -72,35 +72,27 @@ def test_hash_or_noop():
 
 def test_host_transcript_equals_oracle_transcript():
     import dpb200
-    h = dpb200.host()
     to = O.Transcript(b"m2vec")
-    th = C.c_void_p(h.dph_transcript_new(b"m2vec"))
+    th = dpb200.Transcript(b"m2vec")
     f = O.splitmix_f(5, 11)
     e = O.splitmix_e(6, 3)
-    out = np.zeros(2, dtype=np.uint64)
     for rnd in range(5):
-        to.append_f(f)
-        h.dph_transcript_append_f(th, f.ctypes.data_as(C.c_void_p), f.size)
-        to.append_e(e)
-        h.dph_transcript_append_e(th, e.ctypes.data_as(C.c_void_p), e.shape[0])
-        to.append_msg(b"some label!")
-        h.dph_transcript_append_msg(th, b"some label!", 11)
+        for t in (to, th):
+            t.append_f(f)
+            t.append_e(e)
+            t.append_msg(b"some label!")
         c1 = to.challenge(b"Internal round")
-        h.dph_transcript_challenge(th, b"Internal round", out.ctypes.data_as(C.c_void_p))
+        out = th.challenge(b"Internal round")
         assert (c1 == out).all()
         assert int(c1[0]) < O.P and int(c1[1]) < O.P
-    h.dph_transcript_free(th)
+    th.free()
 
 
 def test_fast_host_permutation_equals_the_canonical_formulation():
     """the weak-form host permutation (host/transcript.hpp) against the plain canonical one on 300k seeded states incl. edge
     values (0, 1, p-1, 2^32-1, 2^32, 2^63, ...) and a chained sponge-like sequence: identical, canonical outputs"""
-    import ctypes as C
     import dpb200 as dp
-    H = dp.host()
-    H.dph_poseidon2_selfcheck.restype = C.c_uint64
-    H.dph_poseidon2_selfcheck.argtypes = [C.c_uint64, C.c_uint64]
-    assert H.dph_poseidon2_selfcheck(300000, 12345) == 0
+    assert dp.host().dph_poseidon2_selfcheck(300000, 12345) == 0
 
 
 def test_fast_checker_permutation_equals_the_plain_restatement():

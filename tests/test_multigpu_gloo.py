@@ -119,7 +119,6 @@ dist.init_process_group("gloo")
 rank, world = dist.get_rank(), dist.get_world_size()
 mb = mg.ShmMailbox("dpb200_cpu_%%d" %% os.getppid(), rank, world, dist.barrier)
 H = dp.host()
-H.dph_shm_allgather.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64), C.c_void_p, C.c_uint64, C.c_void_p]
 ok = True
 for it in range(2000):
     n = [8, 1, 2046, 2047, 5000][it %% 5]         # one slot, a full slot, and multi-chunk payloads (the sharded Basefold query rows)

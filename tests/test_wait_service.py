@@ -19,8 +19,6 @@ def _wait(lib, word, want, timeout, out, k):
 @pytest.fixture
 def lib():
     L = dpb200.lib()
-    L.dp_debug_wait_flag.restype = C.c_uint64
-    L.dp_debug_wait_flag.argtypes = [C.c_void_p, C.c_uint64, C.c_double]
     before = L.dp_get_wait_mode()
     yield L
     L.dp_set_wait_mode(before)

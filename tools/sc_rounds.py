@@ -31,7 +31,7 @@ for rep in range(3):
     import ctypes as C
     out = np.zeros(2 * (deg + 1), dtype=np.uint64); po = out.ctypes.data_as(C.c_void_p)
     chp = [np.ascontiguousarray(ch[r]).ctypes.data_as(C.c_void_p) for r in range(nv)]
-    f = dp.lib().dp_sc_round; f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    f = dp.lib().dp_sc_round
     pc = time.perf_counter
     for r in range(nv):
         t0 = pc()
