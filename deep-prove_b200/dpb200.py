@@ -66,10 +66,14 @@ SIGNATURES = {
     "dp_logup_run_layers_fs_blake": (INT, [VP, U32, U32, U32, VP, VP, VP, VP, VP, VP, VP, VP]),
     "dp_mle_linear_combination": (INT, [VP, VP, U32, VP]),
     "dp_fft_rows": (INT, [VP, U32, INT]),
+    "dp_fft_rows_long": (INT, [VP, U32, INT]),
     "dp_pad_rows": (INT, [VP, U64, U32, U32, U64, VP]),
     "dp_conv_prod": (INT, [VP, VP, U32, U32, U64, VP]),
     "dp_conv_output_elements": (INT, [VP, U32, U32, VP, VP]),
+    "dp_conv_output": (INT, [VP, U32, U32, VP, VP, VP, VP]),
+    "dp_reverse_rows": (INT, [VP, U64, VP]),
     "dp_phi_g_init": (INT, [VP, U32, VP, INT, VP, VP]),
+    "dp_phi_g_init_long": (INT, [VP, U32, VP, INT, VP, VP]),
     "dp_phi_level": (INT, [U32, U32, U32, VP, VP, INT, VP]),
     "dp_mle_repeat": (INT, [VP, U32, VP]),
     "dp_set_merkle_hasher": (INT, [INT]),

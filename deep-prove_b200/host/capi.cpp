@@ -370,7 +370,7 @@ extern "C" int dph_conv_prove(uint32_t kw, uint32_t kx, uint32_t n_x, uint32_t r
     std::vector<Element> x(input, input + (size_t)kx * n_x * n_x);
     ConvData pd;
     std::vector<Element> cleared = c.op(x, pd);
-    if (out_after_bias) memcpy(out_after_bias, pd.output_as_element.data(), 8 * pd.output_as_element.size());
+    if (out_after_bias) { std::vector<Element> a = to_elements(pd.output_as_element); memcpy(out_after_bias, a.data(), 8 * a.size()); }
     if (out_cleared) memcpy(out_cleared, cleared.data(), 8 * cleared.size());
     if (!out_len) return 0;
     DynTranscript t(label);

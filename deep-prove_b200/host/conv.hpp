@@ -11,7 +11,8 @@
 namespace dp {
 namespace zkml {
 
-inline DeviceMle fft_rows(DeviceMle m, uint32_t log_n, bool inverse) { check(dp_fft_rows(m.handle(), log_n, inverse ? 1 : 0)); return m; }
+// rows up to 2^13 one block per row, longer rows (images wider than 64) through the two-pass kernel
+inline DeviceMle fft_rows(DeviceMle m, uint32_t log_n, bool inverse) { check((log_n <= 13 ? dp_fft_rows : dp_fft_rows_long)(m.handle(), log_n, inverse ? 1 : 0)); return m; }
 inline DeviceMle pad_rows(const DeviceMle &src, u64 rows, uint32_t n_real, uint32_t n, u64 out_len) { dp_mle *o; check(dp_pad_rows(src.handle(), rows, n_real, n, out_len, &o)); return DeviceMle(o); }
 inline DeviceMle repeat(const DeviceMle &src, uint32_t times) { dp_mle *o; check(dp_mle_repeat(src.handle(), times, &o)); return DeviceMle(o); }
 inline ExtVec download_ext(const DeviceMle &m) {
@@ -26,11 +27,12 @@ inline Ext mle_eval_host(ExtVec v, const ExtVec &point) {          // evaluate (
 }
 
 struct HadamardProof { IOPProof sumcheck; ExtVec individual_claim; };
-// hadamard::prove (hadamard.rs:83-126)
+// hadamard::prove (hadamard.rs:83-126) on two resident tensors
 template <class T>
-HadamardProof hadamard_prove(T &t, const Claim &output_claim, const std::vector<Element> &v1, const std::vector<Element> &v2) {
-    if (v1.size() != v2.size() || (v1.size() & (v1.size() - 1)) || output_claim.point.size() != ceil_log2(v1.size())) throw Error(DP_ERR_INVALID, "hadamard: shapes / claim point do not match");
-    DeviceMle a = DeviceMle::from_evaluations_vec(to_base(v1)), b = DeviceMle::from_evaluations_vec(to_base(v2)), beta = DeviceMle::build_eq_x_r(output_claim.point);
+HadamardProof hadamard_prove(T &t, const Claim &output_claim, const DeviceMle &a, const DeviceMle &b) {
+    const u64 n = a.len();
+    if (n != b.len() || (n & (n - 1)) || output_claim.point.size() != ceil_log2(n)) throw Error(DP_ERR_INVALID, "hadamard: shapes / claim point do not match");
+    DeviceMle beta = DeviceMle::build_eq_x_r(output_claim.point);
     VirtualPolynomial vp(output_claim.point.size());
     vp.add_mle_list({a, b, beta}, Ext::one());
     auto res = IOPProverState::prove_parallel(std::move(vp), t);
@@ -44,7 +46,7 @@ struct PhiTables { DeviceMle w_red; std::vector<DeviceMle> mid; };
 inline PhiTables phi_g_init(const ExtVec &rx, Ext scale, size_t n, bool is_fft) {
     auto f = flatten(rx); u64 sc[2] = {scale.c0, scale.c1};
     dp_mle *w = nullptr; std::vector<dp_mle *> mid(n - 1, nullptr);
-    check(dp_phi_g_init(f.data(), (uint32_t)n, sc, is_fft ? 1 : 0, &w, mid.data()));
+    check((n <= 14 ? dp_phi_g_init : dp_phi_g_init_long)(f.data(), (uint32_t)n, sc, is_fft ? 1 : 0, &w, mid.data()));
     PhiTables p; p.w_red = DeviceMle(w); for (auto *m : mid) p.mid.push_back(DeviceMle(m));
     return p;
 }
@@ -88,7 +90,7 @@ BatchFFTProof prove_batch_matrix(T &t, const ExtVec &r, const DeviceMle &rows, s
 struct ConvData {                                                   // tensor.rs:326-337, the parts the prover reads
     DeviceMle input;                                                // [kx][n_x^2] Base: index_x(real_input) = each channel reversed
     DeviceMle input_fft, prod;                                      // [kx][2 n_x^2], [kw][2 n_w^2] Ext
-    std::vector<Element> output_as_element;                         // conv output after bias, before clearing, [kw][n_x][n_x]
+    DeviceMle output_as_element;                                    // conv output after bias, before clearing, [kw][n_x][n_x] Base
 };
 struct BatchFFTWeightsProof { IOPProof proof; ExtVec claims, partial_evals; MatrixEvalProof matrix_evaluation; };
 struct ConvProof {                                                  // convolution.rs:97-121
@@ -106,14 +108,16 @@ struct Convolution {
     size_t kw = 0, kx = 0, nw = 0, real_nw = 0;
     std::vector<Element> filter, bias;
     size_t unpadded_out[3] = {0, 0, 0};
-    DeviceMle filter_mle, bias_mle, w_fft;                          // resident: weights (Base), bias (Base), FFT(index_w(filter)) [kw][kx][2 nw^2]
+    DeviceMle filter_mle, bias_mle, w_fft, mask;                    // resident: weights (Base), bias (Base), FFT(index_w(filter)) [kw][kx][2 nw^2],
+                                                                    // clearing tensor (Base 0/1) [kw][nw][nw]
     size_t filter_size() const { return nw * nw; }
     size_t row_len() const { return 2 * nw * nw; }
     void load() {
         if (filter.size() != kw * kx * real_nw * real_nw || bias.size() != kw) throw Error(DP_ERR_INVALID, "Convolution: filter/bias shape mismatch");
         filter_mle = DeviceMle::from_evaluations_vec(to_base(filter));
-        if (kw > 1) bias_mle = DeviceMle::from_evaluations_vec(to_base(bias));
+        bias_mle = DeviceMle::from_evaluations_vec(to_base(bias));
         w_fft = fft_rows(pad_rows(filter_mle, kw * kx, (uint32_t)real_nw, (uint32_t)nw, row_len()), (uint32_t)ceil_log2(row_len()), false);   // tensor.rs:492-503, hoisted out of the inference
+        mask = DeviceMle::from_evaluations_vec(to_base(clearing_tensor()));
     }
     std::vector<Element> clearing_tensor() const {                  // new_clearing_tensor (convolution.rs:1508-1530)
         std::vector<Element> d(kw * nw * nw, 0);
@@ -121,23 +125,24 @@ struct Convolution {
             if (i < unpadded_out[0] && j < unpadded_out[1] && k < unpadded_out[2]) d[(i * nw + j) * nw + k] = 1;
         return d;
     }
-    // Convolution::op (convolution.rs:320-350) over Tensor::fft_conv (tensor.rs:458-523): returns the cleared output
-    std::vector<Element> op(const std::vector<Element> &x, ConvData &pd) const {
+    // Convolution::op (convolution.rs:320-350) over Tensor::fft_conv (tensor.rs:458-523) on a resident input tensor (Base,
+    // canonical field elements): returns the cleared output, resident too
+    DeviceMle op(const DeviceMle &x, ConvData &pd) const {
         size_t n_x = nw, chunk = n_x * n_x;
-        if (x.size() != kx * chunk) throw Error(DP_ERR_INVALID, "Convolution::op: input is not [kx, n_x, n_x]");
-        std::vector<u64> rev(x.size());
-        for (size_t c = 0; c < kx; c++) for (size_t i = 0; i < chunk; i++) rev[c * chunk + i] = from_i64(x[c * chunk + (chunk - 1 - i)]);
-        pd.input = DeviceMle::from_evaluations_vec(rev);
+        if (x.is_ext() || x.len() != kx * chunk) throw Error(DP_ERR_INVALID, "Convolution::op: input is not [kx, n_x, n_x]");
+        dp_mle *rev; check(dp_reverse_rows(x.handle(), chunk, &rev));
+        pd.input = DeviceMle(rev);
         pd.input_fft = fft_rows(pad_rows(pd.input, kx, (uint32_t)n_x, (uint32_t)n_x, 2 * chunk), (uint32_t)ceil_log2(2 * chunk), false);
         dp_mle *pr; check(dp_conv_prod(pd.input_fft.handle(), w_fft.handle(), (uint32_t)kw, (uint32_t)kx, row_len(), &pr));
         pd.prod = DeviceMle(pr);
         DeviceMle out = fft_rows(pd.prod.clone(), (uint32_t)ceil_log2(row_len()), true);
-        pd.output_as_element.assign(kw * chunk, 0);
-        check(dp_conv_output_elements(out.handle(), (uint32_t)kw, (uint32_t)n_x, bias.data(), pd.output_as_element.data()));
-        std::vector<Element> clr = clearing_tensor(), cleared(pd.output_as_element.size());
-        for (size_t i = 0; i < cleared.size(); i++) cleared[i] = pd.output_as_element[i] * clr[i];
-        return cleared;
+        dp_mle *after, *cleared;
+        check(dp_conv_output(out.handle(), (uint32_t)kw, (uint32_t)n_x, bias_mle.handle(), mask.handle(), &after, &cleared));
+        pd.output_as_element = DeviceMle(after);
+        return DeviceMle(cleared);
     }
+    // the same from and to host tensors (the host-trace path)
+    std::vector<Element> op(const std::vector<Element> &x, ConvData &pd) const { return to_elements(op(DeviceMle::from_evaluations_vec(to_base(x)), pd)); }
     // Convolution::prove_batch_fft_weights (convolution.rs:368-458)
     template <class T>
     BatchFFTWeightsProof prove_batch_fft_weights(T &t, const ExtVec &r) const {
@@ -158,7 +163,7 @@ struct Convolution {
     template <class T>
     Claim prove_convolution_step(T &t, const Claim &last_claim_in, const ConvData &pd, ConvProof &out) const {
         size_t lfs = ceil_log2(filter_size()), lkw = ceil_log2(kw), lrow = ceil_log2(row_len());
-        out.clearing_proof = hadamard_prove(t, last_claim_in, pd.output_as_element, clearing_tensor());
+        out.clearing_proof = hadamard_prove(t, last_claim_in, pd.output_as_element, mask);
         Claim last_claim{out.clearing_proof.sumcheck.point, out.clearing_proof.individual_claim[0]};
         if (lfs + lkw != last_claim.point.size()) throw Error(DP_ERR_INVALID, "Inconsistent random point size");
         ExtVec r(last_claim.point.size() + 1, Ext::zero()), bias_point(lkw, Ext::zero());

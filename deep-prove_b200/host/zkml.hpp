@@ -61,6 +61,7 @@ struct TableType {
 };
 inline Element relu(Element e) { return e < 0 ? 0 : e; }
 inline std::vector<u64> to_base(const std::vector<Element> &v) { std::vector<u64> o(v.size()); for (size_t i = 0; i < v.size(); i++) o[i] = from_i64(v[i]); return o; }
+inline std::vector<Element> to_elements(const DeviceMle &m) { std::vector<u64> f = m.download(); std::vector<Element> o(f.size()); for (size_t i = 0; i < f.size(); i++) o[i] = f[i] > (P >> 1) ? -(Element)(P - f[i]) : (Element)f[i]; return o; }
 
 // (PCS::CommitmentWithWitness, DenseMultilinearExtension) -- lookup/context.rs:38-41
 struct ProverCommitment { BasefoldCommitmentWithWitness comm; DeviceMle poly; };
@@ -316,9 +317,8 @@ inline void wit_check(uint32_t bits) {
     if (bits & 1) throw Error(DP_ERR_INVALID, "Could not apply requantisation, tensor element had absolute value too large");
     if (bits) throw Error(DP_ERR_INVALID, "lookup witness: a value is not in its table (clamping / relu / pooling range)");
 }
-inline std::vector<Element> to_elements(const DeviceMle &m) { std::vector<u64> f = m.download(); std::vector<Element> o(f.size()); for (size_t i = 0; i < f.size(); i++) o[i] = f[i] > (P >> 1) ? -(Element)(P - f[i]) : (Element)f[i]; return o; }
-// Model::run on the device (Dense / Requant / Relu / Maxpool2D kernels of csrc/witness.cu; the FFT convolution keeps its
-// host-vector interface: its input comes down and its output goes back up once per convolution node)
+// Model::run on the device (Dense / Requant / Relu / Maxpool2D kernels of csrc/witness.cu, the FFT convolution of csrc/conv.cu):
+// only the model input crosses PCIe
 inline DeviceTrace run_device(const Context &ctx, const std::vector<Element> &input) {
     const Model &m = *ctx.model;
     DeviceTrace tr; tr.input = DeviceMle::from_evaluations_vec(to_base(input));
@@ -332,7 +332,7 @@ inline DeviceTrace run_device(const Context &ctx, const std::vector<Element> &in
         else if (n.op == Op::Relu) { dp_mle *h; check(dp_wit_relu(wh.w, cur.handle(), ti.at(TableType::relu()), &h)); o = wit_own(h); }
         else if (n.op == Op::Pool) o = wit_pool(wh.w, cur, n, ti)[4];
         else if (n.op == Op::MatMul) { const auto &c = ctx.model_comms.at(id); dp_mle *h; check(dp_wit_matmul(cur.handle(), c.at("MatMulWeight").poly.handle(), n.mm_bias ? c.at("MatMulBias").poly.handle() : nullptr, (uint32_t)n.mm_r, (uint32_t)n.mm_k, (uint32_t)n.mm_c, n.mm_t ? 1 : 0, &h)); o = wit_own(h); }
-        else { ConvData cd; std::vector<Element> out = ctx.convs.at(id).op(to_elements(cur), cd); tr.conv[id] = std::move(cd); o = DeviceMle::from_evaluations_vec(to_base(out)); }
+        else { ConvData cd; o = ctx.convs.at(id).op(cur, cd); tr.conv[id] = std::move(cd); }
         tr.outs.push_back(o); cur = o;
     }
     if (wh.w) { std::vector<dp_mle *> mu(kinds.size(), nullptr); uint32_t bits = 0; check(dp_wit_finish(wh.w, mu.data(), &bits)); for (dp_mle *h : mu) wit_own(h); wit_check(bits); }

@@ -77,6 +77,59 @@ def cnn_small(seed=1):
     return cnn(seed, img=16, c0=3, c1=4, c2=6, f1=24, f2=16, f3=10, k=3)
 
 
+def covid(seed=1, img=224, channels=(32, 64, 64, 128, 128), fc=64, k=3):
+    """The reference's vision model (zkml/assets/scripts/covid/covid.py, CNNModel.forward) in the padded layout, same rules as
+    cnn():  [3,img,img] -> conv(c1) -> requant -> relu -> conv(c2) -> requant -> relu -> maxpool -> [conv -> requant -> relu
+    -> maxpool] x 3 -> flatten -> dense fc -> requant -> relu -> dense 1 -> requant -> relu.  Dropout is the identity at
+    inference.  The one-output dense layer is padded to 4 rows (rows 2-4 and their bias are zero): the requant and ReLU
+    lookups that follow it need tensors of at least 4 entries (their LogUp circuits refuse a 2-entry column).  At img = 224
+    the padded widths are 256, 256, 128, 64, 32 (FFT rows of 2^17, 2^17, 2^15, 2^13, 2^11).
+    Returns (desc, data, input, n_real_params); the defaults have 1,457,537 real parameters."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    desc, data, n_params = [], [], 0
+    c0 = 3
+    kx_u, n_u, n_p = c0, img, _p2(img)
+    x = np.zeros((_p2(c0), n_p, n_p), dtype=np.int64)
+    x[:c0, :img, :img] = rng.integers(-127, 128, size=(c0, img, img))
+    for li, kw_u in enumerate(channels):
+        kx, kw, rn = _p2(kx_u), _p2(kw_u), _p2(k)
+        filt = np.zeros((kw, kx, rn, rn), dtype=np.int64)
+        filt[:kw_u, :kx_u, :k, :k] = rng.integers(-127, 128, size=(kw_u, kx_u, k, k))
+        bias = np.zeros(kw, dtype=np.int64)
+        bias[:kw_u] = rng.integers(-1000, 1001, size=kw_u)
+        n_params += kw_u * kx_u * k * k + kw_u
+        h_out = n_u - k + 1
+        desc.append([CONV, kw, kx, n_p, rn, kw_u, h_out, h_out, 0])
+        data += [filt.reshape(-1), bias]
+        terms = k * k * kx_u
+        desc.append(_requant(_clog2(terms) + 2, 2 * (BIT_LEN - 1) + _clog2(terms + 1)))
+        desc.append([RELU] + [0] * 8)
+        kx_u, n_u = kw_u, h_out
+        if li > 0:                                  # conv1 feeds conv2 directly
+            desc.append([POOL, kw, n_p, n_p, 0, 0, 0, 0, 0])
+            n_u, n_p = n_u // 2, n_p // 2
+    ncols, prev_real = _p2(kx_u) * n_p * n_p, None
+    for li, out_u in enumerate((fc, 1)):
+        nrows = max(4, _p2(out_u))
+        w = np.zeros((nrows, ncols), dtype=np.int64)
+        if li == 0:
+            mask = np.zeros((_p2(kx_u), n_p, n_p), dtype=bool)
+            mask[:kx_u, :n_u, :n_u] = True
+            real = mask.reshape(-1)
+        else:
+            real = np.arange(ncols) < prev_real
+        w[:out_u, real] = rng.integers(-127, 128, size=(out_u, int(real.sum())))
+        b = np.zeros(nrows, dtype=np.int64)
+        b[:out_u] = rng.integers(-127, 128, size=out_u)
+        n_params += out_u * int(real.sum()) + out_u
+        desc.append([DENSE, nrows, ncols, 0, 0, 0, 0, 0, 0])
+        data += [w.reshape(-1), b]
+        desc.append(_requant(_clog2(ncols), 2 * (BIT_LEN - 1) + _clog2(ncols) + 1))
+        desc.append([RELU] + [0] * 8)
+        ncols, prev_real = nrows, out_u
+    return np.asarray(desc, dtype=np.int64), np.concatenate(data).astype(np.int64), x.reshape(-1), n_params
+
+
 def token_mlp(seed=1, tokens=8, d_model=64, d_hidden=128, transposed=(False, True), bias=(True, False)):
     """A token-wise MLP as the transformer feed-forward block uses it (zkml/src/layers/matrix_mul.rs: OperandMatrix::Input x
     OperandMatrix::Weight): X [tokens, d_model] -> MatMul(W1 [d_model, d_hidden] or its transpose, + bias) -> requant -> relu

@@ -194,6 +194,9 @@ int dp_mle_linear_combination(dp_mle *const *mles, const uint64_t *coefs, uint32
 /* tensor.rs:261-323 `fft(v, flag)` applied to every row of an Ext MLE viewed as [len >> log_n][2^log_n], in place;
  * natural order in and out, root = get_root_of_unity(log_n) (tensor.rs:220), inverse includes the 1/n scaling. */
 int dp_fft_rows(dp_mle *m, uint32_t log_n, int inverse);
+/* dp_fft_rows for rows of 2^14..2^21 (padded image widths 128..1024): the same transform, contract and root table, as a
+ * four-step FFT in two passes over HBM with a scratch tensor the size of the MLE.  The caller picks by the row length. */
+int dp_fft_rows_long(dp_mle *m, uint32_t log_n, int inverse);
 /* index_w / index_wf (tensor.rs:236-253, convolution.rs:1535-1550): every source row holds an n_real x n_real block that is
  * placed top-left in an n x n grid and zero-padded to out_len; the result is Ext, rows * out_len long. */
 int dp_pad_rows(const dp_mle *src, uint64_t rows, uint32_t n_real, uint32_t n, uint64_t out_len, dp_mle **out);
@@ -202,9 +205,18 @@ int dp_conv_prod(const dp_mle *x_fft, const dp_mle *w_fft, uint32_t kw, uint32_t
 /* index_u + to_element + add_bias (tensor.rs:255-259,343-361; convolution.rs:152-162): out_host[i][t] =
  * to_element(out_rows[i][n_x^2 - 1 - t]) + bias[i], out_rows = iFFT(prod) as [kw][2 n_x^2]; bias and out_host are HOST arrays. */
 int dp_conv_output_elements(const dp_mle *out_rows, uint32_t kw, uint32_t n_x, const int64_t *bias, int64_t *out_host);
+/* the same tensor kept on the device: *after = to_field(index_u + to_element + add_bias) as a Base MLE [kw][n_x^2], and
+ * *cleared = after * mask, the layer's clearing tensor (convolution.rs:1484-1530); bias [kw] and mask [kw][n_x^2] are Base MLEs
+ * of canonical field elements. */
+int dp_conv_output(const dp_mle *out_rows, uint32_t kw, uint32_t n_x, const dp_mle *bias, const dp_mle *mask, dp_mle **after, dp_mle **cleared);
+/* index_x (tensor.rs:343-361): every row of `row_len` values of a Base MLE reversed, into a new MLE. */
+int dp_reverse_rows(const dp_mle *src, uint64_t row_len, dp_mle **out);
 /* Prover::phi_g_init (iop/prover.rs:231-289): w_red = W(rx, .) of the FFT (is_fft = 0) or iFFT (is_fft = 1, the reference's
  * flag value in prove_batch_ifft) matrix scaled by `scale`, length 2^n, plus the n - 1 intermediate tables mid[i] (2^(i+1) values). */
 int dp_phi_g_init(const uint64_t *rx, uint32_t n, const uint64_t scale[2], int is_fft, dp_mle **w_red, dp_mle **mid);
+/* dp_phi_g_init for 15 <= n <= 21 (the FFT rows of dp_fft_rows_long): same arguments and outputs; the levels wider than one
+ * block run as one grid launch each. */
+int dp_phi_g_init_long(const uint64_t *rx, uint32_t n, const uint64_t scale[2], int is_fft, dp_mle **w_red, dp_mle **mid);
 /* one level of delegate_matrix_evaluation (iop/prover.rs:182-195): out[i] = A + B * omega^(i << shift), omega =
  * get_root_of_unity(n_total) (its inverse when `inverse`), i < 2^len_log; A, B are Ext scalars the host derives from r1, r2. */
 int dp_phi_level(uint32_t len_log, uint32_t n_total, uint32_t shift, const uint64_t A[2], const uint64_t B[2], int inverse, dp_mle **out);
