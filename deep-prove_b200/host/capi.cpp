@@ -358,7 +358,7 @@ extern "C" int dph_sumcheck_prove_batch_polys(uint32_t T, dp_mle *const *mles, u
 
 // ---- FFT-convolution layer in isolation (host/conv.hpp): inference + layer proof ----------------------------------
 // The output claim is drawn as Prover::prove draws the model-output claim (iop/prover.rs:423-436): point from the
-// transcript, eval = MLE(cleared output)(point).  Flat layout: host/conv.hpp flatten_conv_proof.
+// transcript, eval = MLE(cleared output)(point).  Flat layout: host/zkml.hpp flatten_conv_proof.
 extern "C" int dph_conv_prove(uint32_t kw, uint32_t kx, uint32_t n_x, uint32_t real_nw, const int64_t *filter, const int64_t *bias, const uint32_t *unpadded_out,
                               const int64_t *input, const char *label, int64_t *out_after_bias, int64_t *out_cleared, uint64_t *out, uint64_t cap, uint64_t *out_len) {
     DPH_TRY
@@ -369,15 +369,16 @@ extern "C" int dph_conv_prove(uint32_t kw, uint32_t kx, uint32_t n_x, uint32_t r
     c.load();
     std::vector<Element> x(input, input + (size_t)kx * n_x * n_x);
     ConvData pd;
-    std::vector<Element> cleared = c.op(x, pd);
+    DeviceMle cleared = c.op(DeviceMle::from_evaluations_vec(to_base(x)), pd);
     if (out_after_bias) { std::vector<Element> a = to_elements(pd.output_as_element); memcpy(out_after_bias, a.data(), 8 * a.size()); }
-    if (out_cleared) memcpy(out_cleared, cleared.data(), 8 * cleared.size());
+    if (out_cleared) { std::vector<Element> a = to_elements(cleared); memcpy(out_cleared, a.data(), 8 * a.size()); }
     if (!out_len) return 0;
     DynTranscript t(label);
-    Claim cl; for (size_t i = 0; i < ceil_log2(cleared.size()); i++) cl.point.push_back(t.read_challenge());
-    cl.eval = DeviceMle::from_evaluations_vec(to_base(cleared)).evaluate(cl.point);
+    Claim cl; for (size_t i = 0; i < ceil_log2(cleared.len()); i++) cl.point.push_back(t.read_challenge());
+    cl.eval = cleared.evaluate(cl.point);
     ConvProof pr; Claim in_claim = c.prove_convolution_step(t, cl, pd, pr);
-    return put_flat("dph_conv_prove", flatten_conv_proof(pr, in_claim), out, cap, out_len);
+    ProofImage w; flatten_conv_proof(w, pr, in_claim);
+    return put_flat("dph_conv_prove", w.words, out, cap, out_len);
     DPH_CATCH
 }
 
@@ -461,14 +462,13 @@ extern "C" int dph_logup_prove(dp_mle *const *cols, uint32_t n_cols, dp_mle *mul
     in.constant_challenge = Ext(cc[0], cc[1]); in.column_separation_challenge = Ext(sc[0], sc[1]); in.columns_per_instance = columns_per_instance;
     DynTranscript t(label ? label : "");
     zkml::LogUpProof pr = zkml::logup_batch_prove(in, t);
-    std::vector<u64> w;
-    auto put = [&](const Ext &e) { w.push_back(e.c0); w.push_back(e.c1); };
-    w.push_back(pr.sumcheck_proofs.size());
-    for (auto &p : pr.sumcheck_proofs) { w.push_back(p.proofs.size()); for (auto &m : p.proofs) { w.push_back(m.evaluations.size()); for (auto &e : m.evaluations) put(e); } for (auto &e : p.point) put(e); }
-    for (auto &ev : pr.round_evaluations) { w.push_back(ev.size()); for (auto &e : ev) put(e); }
-    for (auto &c : pr.output_claims) { for (auto &e : c.point) put(e); put(c.eval); }
-    put(t.get_and_append_challenge("after"));
-    return put_flat("dph_logup_prove", w, out, cap, out_len);
+    ProofImage w;
+    w.put(pr.sumcheck_proofs.size());
+    for (auto &p : pr.sumcheck_proofs) { w.put(p.proofs.size()); for (auto &m : p.proofs) w.exts(m.evaluations); for (auto &e : p.point) w.ext(e); }
+    for (auto &ev : pr.round_evaluations) w.exts(ev);
+    for (auto &c : pr.output_claims) { for (auto &e : c.point) w.ext(e); w.ext(c.eval); }
+    w.ext(t.get_and_append_challenge("after"));
+    return put_flat("dph_logup_prove", w.words, out, cap, out_len);
     DPH_CATCH
 }
 

@@ -141,8 +141,6 @@ struct Convolution {
         pd.output_as_element = DeviceMle(after);
         return DeviceMle(cleared);
     }
-    // the same from and to host tensors (the host-trace path)
-    std::vector<Element> op(const std::vector<Element> &x, ConvData &pd) const { return to_elements(op(DeviceMle::from_evaluations_vec(to_base(x)), pd)); }
     // Convolution::prove_batch_fft_weights (convolution.rs:368-458)
     template <class T>
     BatchFFTWeightsProof prove_batch_fft_weights(T &t, const ExtVec &r) const {

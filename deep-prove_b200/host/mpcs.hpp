@@ -35,6 +35,21 @@ struct CodewordQuery { Ext p0, p1; u64 index = 0; bool is_base = false; std::vec
 struct SingleQueryResult { u64 x_index = 0; CodewordQuery commitment_query; std::vector<CodewordQuery> oracle_query; };
 struct BatchedQueryResult { u64 x_index = 0; std::vector<CodewordQuery> oracle_query, commitments_query; };
 
+// Writer of the flat u64 proof images the parity tests compare word for word with the CPU checker's flatteners
+struct ProofImage {
+    std::vector<u64> words;
+    void put(u64 w) { words.push_back(w); }
+    void ext(const Ext &e) { put(e.c0); put(e.c1); }
+    void exts(const ExtVec &v) { put(v.size()); for (auto &e : v) ext(e); }        // length, then the elements
+    void digest(const Digest &d) { for (u64 w : d.v) put(w); }
+    void query(const CodewordQuery &q) {                                            // a base-field leaf pair as one word per leaf
+        put(q.index); put(q.is_base ? 1 : 0);
+        if (q.is_base) { put(q.p0.c0); put(q.p1.c0); } else { ext(q.p0); ext(q.p1); }
+        put(q.merkle_path.size()); for (auto &d : q.merkle_path) digest(d);
+    }
+    void iop(const IOPProof &p) { exts(p.point); put(p.proofs.size()); for (auto &m : p.proofs) exts(m.evaluations); }
+};
+
 // BasefoldProof (structure.rs:329-345)
 struct BasefoldProof {
     std::vector<ExtVec> sumcheck_messages;
@@ -46,23 +61,16 @@ struct BasefoldProof {
     bool is_trivial = false; std::vector<u64> trivial_proof; bool trivial_is_ext = false;
     // flat u64 image used by the parity tests (layout documented in tests/test_oracle_basefold.py parse_flat)
     std::vector<u64> flatten() const {
-        std::vector<u64> o;
-        auto fe = [&](const Ext &e) { o.push_back(e.c0); o.push_back(e.c1); };
-        auto fd = [&](const Digest &d) { for (int i = 0; i < 4; i++) o.push_back(d.v[i]); };
-        auto fq = [&](const CodewordQuery &q) {
-            o.push_back(q.index); o.push_back(q.is_base ? 1 : 0);
-            if (q.is_base) { o.push_back(q.p0.c0); o.push_back(q.p1.c0); } else { fe(q.p0); fe(q.p1); }
-            o.push_back(q.merkle_path.size()); for (auto &d : q.merkle_path) fd(d);
-        };
-        o.push_back(sumcheck_proof.size()); for (auto &m : sumcheck_proof) for (auto &e : m) fe(e);
-        o.push_back(sumcheck_messages.size()); for (auto &m : sumcheck_messages) for (auto &e : m) fe(e);
-        o.push_back(roots.size()); for (auto &d : roots) fd(d);
-        o.push_back(final_message.size()); for (auto &e : final_message) fe(e);
-        o.push_back(single_queries.size());
-        for (auto &q : single_queries) { o.push_back(q.x_index); fq(q.commitment_query); o.push_back(q.oracle_query.size()); for (auto &x : q.oracle_query) fq(x); }
-        o.push_back(batched_queries.size());
-        for (auto &q : batched_queries) { o.push_back(q.x_index); o.push_back(q.oracle_query.size()); for (auto &x : q.oracle_query) fq(x); o.push_back(q.commitments_query.size()); for (auto &x : q.commitments_query) fq(x); }
-        return o;
+        ProofImage w;
+        w.put(sumcheck_proof.size()); for (auto &m : sumcheck_proof) for (auto &e : m) w.ext(e);
+        w.put(sumcheck_messages.size()); for (auto &m : sumcheck_messages) for (auto &e : m) w.ext(e);
+        w.put(roots.size()); for (auto &d : roots) w.digest(d);
+        w.exts(final_message);
+        w.put(single_queries.size());
+        for (auto &q : single_queries) { w.put(q.x_index); w.query(q.commitment_query); w.put(q.oracle_query.size()); for (auto &x : q.oracle_query) w.query(x); }
+        w.put(batched_queries.size());
+        for (auto &q : batched_queries) { w.put(q.x_index); w.put(q.oracle_query.size()); for (auto &x : q.oracle_query) w.query(x); w.put(q.commitments_query.size()); for (auto &x : q.commitments_query) w.query(x); }
+        return w.words;
     }
 };
 
@@ -72,21 +80,18 @@ struct SimpleBatchProof {
     std::vector<ExtVec> sumcheck_messages; std::vector<Digest> roots; ExtVec final_message; std::vector<SimpleBatchQueryResult> queries;
     bool is_trivial = false;
     std::vector<u64> flatten() const {   // same image as the CPU checker's flatten_simple_batch_proof
-        std::vector<u64> o;
-        auto fe = [&](const Ext &e) { o.push_back(e.c0); o.push_back(e.c1); };
-        auto fd = [&](const Digest &d) { for (int i = 0; i < 4; i++) o.push_back(d.v[i]); };
-        o.push_back(sumcheck_messages.size()); for (auto &m : sumcheck_messages) for (auto &e : m) fe(e);
-        o.push_back(roots.size()); for (auto &d : roots) fd(d);
-        o.push_back(final_message.size()); for (auto &e : final_message) fe(e);
-        o.push_back(queries.size());
+        ProofImage w;
+        w.put(sumcheck_messages.size()); for (auto &m : sumcheck_messages) for (auto &e : m) w.ext(e);
+        w.put(roots.size()); for (auto &d : roots) w.digest(d);
+        w.exts(final_message);
+        w.put(queries.size());
         for (auto &q : queries) {
-            o.push_back(q.x_index); o.push_back(q.index); o.push_back(q.is_base ? 1 : 0); o.push_back(q.left.size());
-            for (size_t k = 0; k < q.left.size(); k++) { if (q.is_base) { o.push_back(q.left[k].c0); o.push_back(q.right[k].c0); } else { fe(q.left[k]); fe(q.right[k]); } }
-            o.push_back(q.merkle_path.size()); for (auto &d : q.merkle_path) fd(d);
-            o.push_back(q.oracle_query.size());
-            for (auto &x : q.oracle_query) { o.push_back(x.index); o.push_back(x.is_base ? 1 : 0); if (x.is_base) { o.push_back(x.p0.c0); o.push_back(x.p1.c0); } else { fe(x.p0); fe(x.p1); } o.push_back(x.merkle_path.size()); for (auto &d : x.merkle_path) fd(d); }
+            w.put(q.x_index); w.put(q.index); w.put(q.is_base ? 1 : 0); w.put(q.left.size());
+            for (size_t k = 0; k < q.left.size(); k++) { if (q.is_base) { w.put(q.left[k].c0); w.put(q.right[k].c0); } else { w.ext(q.left[k]); w.ext(q.right[k]); } }
+            w.put(q.merkle_path.size()); for (auto &d : q.merkle_path) w.digest(d);
+            w.put(q.oracle_query.size()); for (auto &x : q.oracle_query) w.query(x);
         }
-        return o;
+        return w.words;
     }
 };
 

@@ -7,6 +7,8 @@
 // in the reference; every polynomial lives in HBM and every O(n) loop goes through include/deepprove_b200.h.
 #pragma once
 #include "mpcs.hpp"
+#include <optional>
+#include <set>
 #include <unordered_map>
 #include <cstdlib>
 #include <cstdio>
@@ -26,12 +28,6 @@ struct Requant {                                            // layers/requant.rs
     size_t right_shift = 0, fp_scale = 0, intermediate_bit_size = 0; Element fixed_point_multiplier = 0;
     size_t shift() const { return fp_scale + right_shift; }
     size_t clamping_size() const { return intermediate_bit_size + ceil_log2((size_t)fixed_point_multiplier) - shift(); }
-    Element apply(Element e) const {
-        Element rounding = (Element)1 << (shift() - 1);
-        Element unclamped = (rounding + e * fixed_point_multiplier) >> shift();
-        Element sign = unclamped >= 0 ? 1 : -1, a = unclamped < 0 ? -unclamped : unclamped;
-        return a >= QMAX ? QMAX * sign : unclamped;
-    }
     Ext recombine_claims(Ext clamping_claim, const ExtVec &shifted) const {   // requant.rs:483-515
         Ext full = Ext::from_base(canon(1ULL << shift())) * clamping_claim, p2 = Ext::one();
         for (auto &v : shifted) { full += v * p2; p2 *= Ext::from_base(1ULL << BIT_LEN); }
@@ -65,6 +61,10 @@ inline std::vector<Element> to_elements(const DeviceMle &m) { std::vector<u64> f
 
 // (PCS::CommitmentWithWitness, DenseMultilinearExtension) -- lookup/context.rs:38-41
 struct ProverCommitment { BasefoldCommitmentWithWitness comm; DeviceMle poly; };
+// A Dense / MatMul / Conv node's model polynomials, committed at setup: `weight` is the dense weight matrix, the MatMul constant
+// matrix or the conv filter; `bias` is absent for a MatMul without bias.  Bias goes before weight in the transcript and in the
+// claims: the reference keys them by PolyId in a BTreeMap (commit/context.rs:59-103).
+struct ModelCommitment { std::optional<ProverCommitment> bias; ProverCommitment weight; };
 
 struct TableData { std::vector<Element> merged; std::map<Element, u64> table_count; std::vector<DeviceMle> columns; };
 
@@ -211,25 +211,23 @@ class Context {
         for (auto &kv : tabs) max_len = std::max(max_len, (size_t)1 << kv.first.multiplicity_poly_vars());   // context.rs:171-175
         size_t p2 = 1; while (p2 < max_len) p2 <<= 1;
         c.pp = Basefold::setup_and_trim(p2);
-        for (size_t id = 0; id < m.nodes.size(); id++) if (m.nodes[id].op == Op::Dense) {   // CommitmentContext::new (commit/context.rs:59-103)
-            for (auto &kv : std::map<std::string, const std::vector<Element> *>{{"DenseBias", &m.nodes[id].bias}, {"DenseWeight", &m.nodes[id].weights}}) {
-                DeviceMle poly = DeviceMle::from_evaluations_vec(to_base(*kv.second));
-                c.model_comms[id][kv.first] = {Basefold::commit(c.pp, poly), poly};
+        // CommitmentContext::new (commit/context.rs:59-103); a braced list evaluates in order, so the bias is committed first
+        auto commit = [&](const DeviceMle &poly) { return ProverCommitment{Basefold::commit(c.pp, poly), poly}; };
+        auto upload = [](const std::vector<Element> &v) { return DeviceMle::from_evaluations_vec(to_base(v)); };
+        for (size_t id = 0; id < m.nodes.size(); id++) {
+            const Node &n = m.nodes[id];
+            if (n.op == Op::Dense) c.model_comms[id] = {commit(upload(n.bias)), commit(upload(n.weights))};
+            else if (n.op == Op::MatMul) {   // MatMul::ctx (matrix_mul.rs:951-963): the constant matrix and the bias are model polynomials
+                ModelCommitment &mc = c.model_comms[id];
+                if (n.mm_bias) mc.bias = commit(upload(n.bias));
+                mc.weight = commit(upload(n.weights));
+            } else if (n.op == Op::Conv) {   // convolution.rs:532-540
+                Convolution cv; cv.kw = n.kw; cv.kx = n.kx; cv.nw = n.nw; cv.real_nw = n.real_nw; cv.filter = n.weights; cv.bias = n.bias;
+                for (int i = 0; i < 3; i++) cv.unpadded_out[i] = n.unpadded_out[i];
+                cv.load();
+                c.model_comms[id] = {commit(upload(n.bias)), commit(cv.filter_mle)};
+                c.convs[id] = std::move(cv);
             }
-        } else if (m.nodes[id].op == Op::MatMul) {   // MatMul::ctx (matrix_mul.rs:951-963): the constant matrix and the bias are model polynomials
-            const Node &n = m.nodes[id];
-            if (n.mm_bias) { DeviceMle poly = DeviceMle::from_evaluations_vec(to_base(n.bias)); c.model_comms[id]["MatMulBias"] = {Basefold::commit(c.pp, poly), poly}; }
-            DeviceMle poly = DeviceMle::from_evaluations_vec(to_base(n.weights));
-            c.model_comms[id]["MatMulWeight"] = {Basefold::commit(c.pp, poly), poly};
-        } else if (m.nodes[id].op == Op::Conv) {   // convolution.rs:532-540: ConvBias, ConvFilter (BTreeMap order)
-            const Node &n = m.nodes[id];
-            Convolution cv; cv.kw = n.kw; cv.kx = n.kx; cv.nw = n.nw; cv.real_nw = n.real_nw; cv.filter = n.weights; cv.bias = n.bias;
-            for (int i = 0; i < 3; i++) cv.unpadded_out[i] = n.unpadded_out[i];
-            cv.load();
-            DeviceMle bias_poly = DeviceMle::from_evaluations_vec(to_base(n.bias));
-            c.model_comms[id]["ConvBias"] = {Basefold::commit(c.pp, bias_poly), bias_poly};
-            c.model_comms[id]["ConvFilter"] = {Basefold::commit(c.pp, cv.filter_mle), cv.filter_mle};
-            c.convs[id] = std::move(cv);
         }
         for (auto &kv : tabs) {   // get_merged_table_column (lookup/context.rs:158-296), resident for every proof
             TableData td; std::vector<std::vector<u64>> cols;
@@ -243,105 +241,86 @@ class Context {
         }
         return c;
     }
-    template <class T> void write_to_transcript(T &t) const { for (auto &nk : model_comms) for (auto &pk : nk.second) Basefold::write_commitment(pk.second.comm.root, t); }   // commit/context.rs:181-190
+    template <class T> void write_to_transcript(T &t) const {   // commit/context.rs:181-190
+        for (auto &kv : model_comms) { if (kv.second.bias) Basefold::write_commitment(kv.second.bias->comm.root, t); Basefold::write_commitment(kv.second.weight.comm.root, t); }
+    }
     const Model *model = nullptr; BasefoldProverParams pp;
-    std::map<size_t, std::map<std::string, ProverCommitment>> model_comms;
+    std::map<size_t, ModelCommitment> model_comms;
     std::map<TableType, TableData> tables;
     std::map<size_t, Convolution> convs;                      // resident conv layers (weights, FFT'd filters)
 };
 
 struct LogUpWitness { bool table = false; std::vector<ProverCommitment> commits; std::vector<DeviceMle> column_evals; DeviceMle multiplicity_evals; size_t columns_per_instance = 1; TableType tt{0, 0}; };
 
-// quantised inference (model run): outputs[i] = output tensor of node i
-// Maxpool2D::op (pooling.rs:667-677) on a padded [C][H][W] tensor
-inline std::vector<Element> maxpool2d(const std::vector<Element> &x, size_t C, size_t H, size_t W) {
-    std::vector<Element> o(C * (H / 2) * (W / 2));
-    for (size_t c = 0; c < C; c++) for (size_t r = 0; r < H / 2; r++) for (size_t cc = 0; cc < W / 2; cc++) {
-        Element mx = x[(c * H + 2 * r) * W + 2 * cc];
-        for (size_t a = 0; a < 2; a++) for (size_t b = 0; b < 2; b++) mx = std::max(mx, x[(c * H + 2 * r + a) * W + 2 * cc + b]);
-        o[(c * (H / 2) + r) * (W / 2) + cc] = mx;
-    }
-    return o;
-}
-inline std::vector<std::vector<Element>> run(const Model &m, const std::vector<Element> &input, const Context *ctx = nullptr, std::map<size_t, ConvData> *conv_data = nullptr) {
-    std::vector<std::vector<Element>> outs; std::vector<Element> cur = input;
-    for (auto &n : m.nodes) {
-        std::vector<Element> o;
-        if (n.op == Op::Dense) { o.resize(n.nrows); for (size_t r = 0; r < n.nrows; r++) { Element a = n.bias[r]; const Element *w = &n.weights[r * n.ncols]; for (size_t c = 0; c < n.ncols; c++) a += w[c] * cur[c]; o[r] = a; } }
-        else if (n.op == Op::Requant) { Element lim = (Element)1 << n.rq.intermediate_bit_size; for (Element e : cur) { if (e > lim || e < -lim) throw Error(DP_ERR_INVALID, "Could not apply requantisation, tensor element had absolute value too large"); o.push_back(n.rq.apply(e)); } }
-        else if (n.op == Op::Relu) for (Element e : cur) o.push_back(relu(e));
-        else if (n.op == Op::Pool) o = maxpool2d(cur, n.pool_c, n.pool_h, n.pool_w);
-        else if (n.op == Op::MatMul) {
-            if (cur.size() != n.mm_r * n.mm_k) throw Error(DP_ERR_INVALID, "Incompatible shape found for input matrix");
-            o.assign(n.mm_r * n.mm_c, 0);
-            for (size_t r = 0; r < n.mm_r; r++) for (size_t c = 0; c < n.mm_c; c++) {
-                Element a = n.mm_bias ? n.bias[c] : 0;
-                for (size_t k = 0; k < n.mm_k; k++) a += cur[r * n.mm_k + k] * (n.mm_t ? n.weights[c * n.mm_k + k] : n.weights[k * n.mm_c + c]);
-                o[r * n.mm_c + c] = a;
-            }
-        }
-        else {
-            if (!ctx || !conv_data) throw Error(DP_ERR_INVALID, "run: a convolution needs the Context (resident FFT'd filters)");
-            ConvData cd; o = ctx->convs.at(outs.size()).op(cur, cd); (*conv_data)[outs.size()] = std::move(cd);
-        }
-        outs.push_back(o); cur = o;
-    }
-    return outs;
-}
-inline std::vector<std::vector<Element>> run(const Context &ctx, const std::vector<Element> &input, std::map<size_t, ConvData> *conv_data) { return run(*ctx.model, input, &ctx, conv_data); }
+// The inference trace on the device: every tensor is a Base MLE of canonical field elements of signed integers (Tensor::to_field),
+// so a trace tensor doubles as a lookup column.  Built by run_device only (quantised inference on the device: only the model input
+// crosses PCIe); read-only afterwards, shared by concurrent provers.
+struct DeviceTrace {
+    DeviceMle input; std::vector<DeviceMle> outs; std::map<size_t, ConvData> conv;
+    bool valid() const { return input.valid(); }
+    const DeviceMle &node_input(size_t id) const { return id == 0 ? input : outs[id - 1]; }
+};
 
-// The inference trace ON THE DEVICE: every tensor is a Base MLE of canonical field elements of signed integers (Tensor::to_field),
-// so a trace tensor doubles as a lookup column.  Built by run_device (quantised inference on the device: only the model input
-// crosses PCIe) or by uploading a host trace once (upload_trace); read-only afterwards, shared by concurrent provers.
-struct DeviceTrace { DeviceMle input; std::vector<DeviceMle> outs; std::map<size_t, ConvData> conv; bool valid() const { return input.valid(); } };
-struct WitHandle { dp_wit *w = nullptr; ~WitHandle() { if (w) dp_wit_free(w); } };
-// the tables of a Context in TableType order (the reference's BTreeMap order) as the dp_wit_begin arguments
-inline void wit_tables(const Context &ctx, std::vector<uint32_t> &kinds, std::vector<uint32_t> &sizes, std::map<TableType, uint32_t> &index) {
-    for (auto &kv : ctx.tables) { index[kv.first] = (uint32_t)kinds.size(); kinds.push_back((uint32_t)kv.first.kind); sizes.push_back((uint32_t)kv.first.size); }
-}
-inline DeviceMle wit_own(dp_mle *h) { return DeviceMle(h); }
-inline std::vector<DeviceMle> wit_requant(dp_wit *w, const DeviceMle &x, const Requant &rq, const std::map<TableType, uint32_t> &ti) {
-    size_t nc = 2 + rq.shift() / BIT_LEN; std::vector<dp_mle *> raw(nc, nullptr);
-    check(dp_wit_requant(w, x.handle(), (uint32_t)rq.shift(), rq.fixed_point_multiplier, (uint32_t)rq.intermediate_bit_size,
-                         ti.at(TableType::clamping(rq.clamping_size())), ti.at(TableType::range()), raw.data(), (uint32_t)nc));
-    std::vector<DeviceMle> cols; for (dp_mle *h : raw) cols.push_back(wit_own(h));
-    return cols;
-}
-inline std::vector<DeviceMle> wit_pool(dp_wit *w, const DeviceMle &x, const Node &n, const std::map<TableType, uint32_t> &ti) {
-    dp_mle *raw[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    check(dp_wit_pool(w, x.handle(), (uint32_t)n.pool_c, (uint32_t)n.pool_h, (uint32_t)n.pool_w, ti.at(TableType::range()), raw));
-    std::vector<DeviceMle> cols; for (dp_mle *h : raw) cols.push_back(wit_own(h));
-    return cols;
-}
-inline void wit_check(uint32_t bits) {
-    if (bits & 1) throw Error(DP_ERR_INVALID, "Could not apply requantisation, tensor element had absolute value too large");
-    if (bits) throw Error(DP_ERR_INVALID, "lookup witness: a value is not in its table (clamping / relu / pooling range)");
-}
+// One lookup-witness pass (csrc/witness.cu): a dp_wit over the Context's tables in TableType order (the reference's BTreeMap
+// order), whose histograms the node kernels fill; finish() turns them into the multiplicity polynomials.
+class LookupPass {
+  public:
+    explicit LookupPass(const Context &ctx) {
+        std::vector<uint32_t> kinds, sizes;
+        for (auto &kv : ctx.tables) { index_[kv.first] = (uint32_t)kinds.size(); kinds.push_back((uint32_t)kv.first.kind); sizes.push_back((uint32_t)kv.first.size); }
+        if (!kinds.empty()) check(dp_wit_begin((uint32_t)kinds.size(), kinds.data(), sizes.data(), &w_));
+    }
+    ~LookupPass() { if (w_) dp_wit_free(w_); }
+    LookupPass(const LookupPass &) = delete;
+    LookupPass &operator=(const LookupPass &) = delete;
+
+    // The lookup columns of a Requant / ReLU / Maxpool2D node over its input x, in commit order; the node's output is column 1
+    // (Requant, ReLU) or 4 (Maxpool2D).
+    //   Requant (requant.rs:208-330): the clamping (input, output) pair, then the byte chunks of the shifted-out bits
+    //   ReLU (activation.rs:238-323): the node's input and output tensors
+    //   Maxpool2D (pooling.rs:210-271, compute_polys :686-771): the four (output - input) differences, then the output
+    std::vector<DeviceMle> columns(const Node &n, const DeviceMle &x) {
+        if (n.op == Op::Relu) { dp_mle *h; check(dp_wit_relu(w_, x.handle(), table(TableType::relu()), &h)); return {x, DeviceMle(h)}; }
+        const Requant &rq = n.rq;
+        std::vector<dp_mle *> raw(n.op == Op::Pool ? 5 : 2 + rq.shift() / BIT_LEN, nullptr);
+        if (n.op == Op::Requant) check(dp_wit_requant(w_, x.handle(), (uint32_t)rq.shift(), rq.fixed_point_multiplier, (uint32_t)rq.intermediate_bit_size,
+                                                      table(TableType::clamping(rq.clamping_size())), table(TableType::range()), raw.data(), (uint32_t)raw.size()));
+        else if (n.op == Op::Pool) check(dp_wit_pool(w_, x.handle(), (uint32_t)n.pool_c, (uint32_t)n.pool_h, (uint32_t)n.pool_w, table(TableType::range()), raw.data()));
+        else throw Error(DP_ERR_INVALID, "lookup witness: the node has no lookup columns");
+        std::vector<DeviceMle> cols; for (dp_mle *h : raw) cols.push_back(DeviceMle(h));
+        return cols;
+    }
+    // the multiplicity polynomial of every table; refuses a trace with a value outside its table
+    std::map<TableType, DeviceMle> finish() {
+        if (!w_) return {};
+        std::vector<dp_mle *> raw(index_.size(), nullptr); uint32_t bits = 0;
+        check(dp_wit_finish(w_, raw.data(), &bits));
+        std::map<TableType, DeviceMle> mults; for (auto &kv : index_) mults[kv.first] = DeviceMle(raw[kv.second]);
+        if (bits & 1) throw Error(DP_ERR_INVALID, "Could not apply requantisation, tensor element had absolute value too large");
+        if (bits) throw Error(DP_ERR_INVALID, "lookup witness: a value is not in its table (clamping / relu / pooling range)");
+        return mults;
+    }
+  private:
+    uint32_t table(const TableType &tt) const { return index_.at(tt); }
+    dp_wit *w_ = nullptr; std::map<TableType, uint32_t> index_;
+};
+
 // Model::run on the device (Dense / Requant / Relu / Maxpool2D kernels of csrc/witness.cu, the FFT convolution of csrc/conv.cu):
 // only the model input crosses PCIe
 inline DeviceTrace run_device(const Context &ctx, const std::vector<Element> &input) {
     const Model &m = *ctx.model;
     DeviceTrace tr; tr.input = DeviceMle::from_evaluations_vec(to_base(input));
-    std::vector<uint32_t> kinds, sizes; std::map<TableType, uint32_t> ti; wit_tables(ctx, kinds, sizes, ti);
-    WitHandle wh; if (!kinds.empty()) check(dp_wit_begin((uint32_t)kinds.size(), kinds.data(), sizes.data(), &wh.w));
+    LookupPass wit(ctx);
     DeviceMle cur = tr.input;
     for (size_t id = 0; id < m.nodes.size(); id++) {
         const Node &n = m.nodes[id]; DeviceMle o;
-        if (n.op == Op::Dense) { const auto &c = ctx.model_comms.at(id); dp_mle *h; check(dp_wit_dense(c.at("DenseWeight").poly.handle(), c.at("DenseBias").poly.handle(), cur.handle(), (uint32_t)n.nrows, (uint32_t)n.ncols, &h)); o = wit_own(h); }
-        else if (n.op == Op::Requant) o = wit_requant(wh.w, cur, n.rq, ti)[1];
-        else if (n.op == Op::Relu) { dp_mle *h; check(dp_wit_relu(wh.w, cur.handle(), ti.at(TableType::relu()), &h)); o = wit_own(h); }
-        else if (n.op == Op::Pool) o = wit_pool(wh.w, cur, n, ti)[4];
-        else if (n.op == Op::MatMul) { const auto &c = ctx.model_comms.at(id); dp_mle *h; check(dp_wit_matmul(cur.handle(), c.at("MatMulWeight").poly.handle(), n.mm_bias ? c.at("MatMulBias").poly.handle() : nullptr, (uint32_t)n.mm_r, (uint32_t)n.mm_k, (uint32_t)n.mm_c, n.mm_t ? 1 : 0, &h)); o = wit_own(h); }
-        else { ConvData cd; o = ctx.convs.at(id).op(cur, cd); tr.conv[id] = std::move(cd); }
+        if (n.op == Op::Dense) { const ModelCommitment &c = ctx.model_comms.at(id); dp_mle *h; check(dp_wit_dense(c.weight.poly.handle(), c.bias->poly.handle(), cur.handle(), (uint32_t)n.nrows, (uint32_t)n.ncols, &h)); o = DeviceMle(h); }
+        else if (n.op == Op::MatMul) { const ModelCommitment &c = ctx.model_comms.at(id); dp_mle *h; check(dp_wit_matmul(cur.handle(), c.weight.poly.handle(), c.bias ? c.bias->poly.handle() : nullptr, (uint32_t)n.mm_r, (uint32_t)n.mm_k, (uint32_t)n.mm_c, n.mm_t ? 1 : 0, &h)); o = DeviceMle(h); }
+        else if (n.op == Op::Conv) { ConvData cd; o = ctx.convs.at(id).op(cur, cd); tr.conv[id] = std::move(cd); }
+        else o = wit.columns(n, cur)[n.op == Op::Pool ? 4 : 1];
         tr.outs.push_back(o); cur = o;
     }
-    if (wh.w) { std::vector<dp_mle *> mu(kinds.size(), nullptr); uint32_t bits = 0; check(dp_wit_finish(wh.w, mu.data(), &bits)); for (dp_mle *h : mu) wit_own(h); wit_check(bits); }
-    return tr;
-}
-inline DeviceTrace upload_trace(const std::vector<Element> &input, const std::vector<std::vector<Element>> &outs, const std::map<size_t, ConvData> *conv_data) {
-    DeviceTrace tr; tr.input = DeviceMle::from_evaluations_vec(to_base(input));
-    for (auto &o : outs) tr.outs.push_back(DeviceMle::from_evaluations_vec(to_base(o)));
-    if (conv_data) tr.conv = *conv_data;
+    wit.finish();
     return tr;
 }
 
@@ -353,16 +332,10 @@ class Prover {
 
     // end to end from the host input vector: inference on the device, then prove
     Proof prove(const std::vector<Element> &input) { DeviceTrace tr = run_device(ctx_, input); return prove(tr); }
-    // a host trace (the reference's InferenceTrace): uploaded once, tensor by tensor
-    Proof prove(const std::vector<Element> &input, const std::vector<std::vector<Element>> &outs, const std::map<size_t, ConvData> *conv_data = nullptr) {
-        DeviceTrace tr = upload_trace(input, outs, conv_data); return prove(tr);
-    }
     // Prover::prove(full_trace): the inference trace is an INPUT of proving (zkml/src/bin/bench.rs:390-408 times only this)
     Proof prove(const DeviceTrace &tr) {
         const Model &m = *ctx_.model;
         if (tr.outs.size() != m.nodes.size()) throw Error(DP_ERR_INVALID, "prove: the trace does not match the model");
-        const std::map<size_t, ConvData> *conv_data = &tr.conv;
-        auto node_input = [&](size_t id) -> const DeviceMle & { return id == 0 ? tr.input : tr.outs[id - 1]; };
         ctx_.write_to_transcript(t_);
         instantiate_witness_ctx(m, tr);
         // output claim (prover.rs:423-436)
@@ -371,15 +344,12 @@ class Prover {
         last.eval = fo.evaluate(last.point);
         for (size_t id = m.nodes.size(); id-- > 0;) {
             const Node &n = m.nodes[id];
-            if (n.op == Op::Dense) last = prove_dense(id, n, last, node_input(id));
+            if (n.op == Op::Dense) last = prove_dense(id, n, last, tr.node_input(id));
             else if (n.op == Op::Requant) last = prove_requant(id, n, last);
             else if (n.op == Op::Relu) last = prove_activation(id, last);
             else if (n.op == Op::Pool) last = prove_pooling(id, n, last);
-            else if (n.op == Op::MatMul) last = prove_matmul(id, n, last, node_input(id));
-            else {
-                if (!conv_data || !conv_data->count(id)) throw Error(DP_ERR_INVALID, "prove: no convolution proving data in the trace");
-                last = prove_convolution(id, last, conv_data->at(id));
-            }
+            else if (n.op == Op::MatMul) last = prove_matmul(id, n, last, tr.node_input(id));
+            else last = prove_convolution(id, last, tr.conv.at(id));
         }
         prove_tables();
         commit_prove();
@@ -388,56 +358,49 @@ class Prover {
 
   private:
     void add_witness_claim(const ProverCommitment &pc, const Claim &c) { (pc.poly.num_vars() <= Basefold::trivial_num_vars() ? trivial_claims_ : claims_).push_back({pc, c}); }   // commit/context.rs:290-310
-    ProverCommitment commit_column(const std::vector<u64> &ev) { DeviceMle p = DeviceMle::from_evaluations_vec(ev); return {Basefold::commit(ctx_.pp, p), p}; }
+    // a node's model-polynomial claims, bias first (ModelCommitment); a MatMul without bias has no bias claim
+    void add_model_claims(size_t id, const Claim &bias, const Claim &weight) {
+        const ModelCommitment &mc = ctx_.model_comms.at(id);
+        if (mc.bias) add_witness_claim(*mc.bias, bias);
+        add_witness_claim(mc.weight, weight);
+    }
 
     // generate_lookup_witnesses (lookup/context.rs:631-756) + initialise_from_table_set (:758-781).
     // The reference commits every witness column from rayon workers before any challenge is drawn; here all
     // columns are gathered first and committed with ONE Basefold::commit_many call (concurrent on the device).
     void instantiate_witness_ctx(const Model &m, const DeviceTrace &tr) {
-        auto node_input = [&](size_t id) -> const DeviceMle & { return id == 0 ? tr.input : tr.outs[id - 1]; };
         std::vector<DeviceMle> polys;                            // every column to commit, in creation order (all device-resident)
         struct Slot { size_t node; size_t witness; bool table; bool column = true; };  // where commitment k goes (column: also a lookup column)
         std::vector<Slot> slots;
-        std::vector<uint32_t> kinds, sizes; std::map<TableType, uint32_t> ti; wit_tables(ctx_, kinds, sizes, ti);
-        WitHandle wh; if (!kinds.empty()) check(dp_wit_begin((uint32_t)kinds.size(), kinds.data(), sizes.data(), &wh.w));
-        std::map<TableType, bool> used;
+        LookupPass wit(ctx_);
+        std::set<TableType> used;
+        auto witness = [&](TableType tt, size_t columns_per_instance) { LogUpWitness w; w.tt = tt; w.columns_per_instance = columns_per_instance; used.insert(tt); return w; };
         for (size_t id = 0; id < m.nodes.size(); id++) {
             const Node &n = m.nodes[id];
-            if (n.op == Op::Requant) {   // requant.rs:208-330: clamping (input, output) columns + the byte chunks of the shifted-out bits
-                TableType tc = TableType::clamping(n.rq.clamping_size()), trg = TableType::range();
-                used[tc] = used[trg] = true;
-                std::vector<DeviceMle> c = wit_requant(wh.w, node_input(id), n.rq, ti);
-                LogUpWitness wc; wc.tt = tc; wc.columns_per_instance = 2;
-                LogUpWitness ws; ws.tt = trg; ws.columns_per_instance = 1;
-                lookup_witness_[id] = {wc, ws};
-                for (size_t k = 0; k < c.size(); k++) { polys.push_back(c[k]); slots.push_back({id, k < 2 ? (size_t)0 : (size_t)1, false}); }
-            } else if (n.op == Op::Relu) {   // activation.rs:238-323: the node's input and output tensors ARE the two columns
-                TableType tt = TableType::relu(); LogUpWitness w; w.tt = tt; w.columns_per_instance = 2; used[tt] = true;
-                dp_mle *h; check(dp_wit_relu(wh.w, node_input(id).handle(), ti.at(tt), &h)); DeviceMle out = wit_own(h);
-                lookup_witness_[id] = {w};
-                polys.push_back(node_input(id)); slots.push_back({id, 0, false});
-                polys.push_back(out); slots.push_back({id, 0, false});
-            } else if (n.op == Op::Pool) {   // pooling.rs:210-271 + compute_polys (:686-771)
-                TableType trg = TableType::range(); LogUpWitness w; w.tt = trg; w.columns_per_instance = 1; used[trg] = true;
-                std::vector<DeviceMle> c = wit_pool(wh.w, node_input(id), n, ti);
-                lookup_witness_[id] = {w};
-                for (size_t k = 0; k < 4; k++) { polys.push_back(c[k]); slots.push_back({id, 0, false}); }
-                polys.push_back(c[4]); slots.push_back({id, 0, false, false});   // the output poly: committed, not a lookup column
+            if (n.op != Op::Requant && n.op != Op::Relu && n.op != Op::Pool) continue;
+            const std::vector<DeviceMle> c = wit.columns(n, tr.node_input(id));
+            auto add = [&](size_t k, size_t which, bool column = true) { polys.push_back(c[k]); slots.push_back({id, which, false, column}); };
+            if (n.op == Op::Requant) {   // the clamping (input, output) pair goes to the clamping table, the byte chunks to the range table
+                lookup_witness_[id] = {witness(TableType::clamping(n.rq.clamping_size()), 2), witness(TableType::range(), 1)};
+                for (size_t k = 0; k < c.size(); k++) add(k, k < 2 ? 0 : 1);
+            } else if (n.op == Op::Relu) {
+                lookup_witness_[id] = {witness(TableType::relu(), 2)};
+                add(0, 0); add(1, 0);
+            } else {
+                lookup_witness_[id] = {witness(TableType::range(), 1)};
+                for (size_t k = 0; k < 4; k++) add(k, 0);
+                add(4, 0, false);   // the output poly: committed, not a lookup column
             }
         }
+        // table multiplicities (lookup/context.rs:675-737): histograms the node kernels filled, every table row distinct
+        std::map<TableType, DeviceMle> mults = wit.finish();
         std::vector<TableType> table_order;
-        if (wh.w) {   // table multiplicities (lookup/context.rs:675-737): histograms the node kernels filled, every table row distinct
-            std::vector<dp_mle *> mu(kinds.size(), nullptr); uint32_t bits = 0;
-            check(dp_wit_finish(wh.w, mu.data(), &bits));
-            std::vector<DeviceMle> mults; for (dp_mle *h : mu) mults.push_back(wit_own(h));
-            wit_check(bits);
-            for (auto &kv : ctx_.tables) {
-                if (!used.count(kv.first)) continue;
-                for (auto &tc : kv.second.table_count) if (tc.second != 1) throw Error(DP_ERR_UNSUPPORTED, "device multiplicities need distinct table rows");
-                LogUpWitness w; w.table = true; w.tt = kv.first; w.column_evals = kv.second.columns;
-                table_witness_.push_back(w); table_order.push_back(kv.first);
-                polys.push_back(mults[ti.at(kv.first)]); slots.push_back({0, table_witness_.size() - 1, true});
-            }
+        for (auto &kv : ctx_.tables) {
+            if (!used.count(kv.first)) continue;
+            for (auto &tc : kv.second.table_count) if (tc.second != 1) throw Error(DP_ERR_UNSUPPORTED, "device multiplicities need distinct table rows");
+            LogUpWitness w; w.table = true; w.tt = kv.first; w.column_evals = kv.second.columns;
+            table_witness_.push_back(w); table_order.push_back(kv.first);
+            polys.push_back(mults.at(kv.first)); slots.push_back({0, table_witness_.size() - 1, true});
         }
         std::vector<BasefoldCommitmentWithWitness> comms = Basefold::commit_many(ctx_.pp, polys);
         for (size_t k = 0; k < slots.size(); k++) {
@@ -456,8 +419,8 @@ class Prover {
 
     // Dense::prove_step (layers/dense.rs:423-551)
     Claim prove_dense(size_t id, const Node &n, const Claim &last_claim, const DeviceMle &input) {
-        const auto &comms = ctx_.model_comms.at(id);
-        const DeviceMle &weights = comms.at("DenseWeight").poly, &bias = comms.at("DenseBias").poly;
+        const ModelCommitment &mc = ctx_.model_comms.at(id);
+        const DeviceMle &weights = mc.weight.poly, &bias = mc.bias->poly;
         if (ceil_log2(n.nrows) != last_claim.point.size()) throw Error(DP_ERR_INVALID, "something's wrong with the randomness");
         Ext bias_eval = bias.evaluate(last_claim.point);
         DeviceMle mat = weights.fix_high_variables(last_claim.point);      // rows are the HIGH variables (dense.rs:471-475)
@@ -467,8 +430,7 @@ class Prover {
         auto res = IOPProverState::prove_parallel(std::move(vp), t_);
         const ExtVec &fe = res.second.get_mle_final_evaluations();
         ExtVec wp = res.first.point; wp.insert(wp.end(), last_claim.point.begin(), last_claim.point.end());
-        add_witness_claim(comms.at("DenseBias"), {last_claim.point, bias_eval});   // BTreeMap order of PolyId
-        add_witness_claim(comms.at("DenseWeight"), {wp, fe[0]});
+        add_model_claims(id, {last_claim.point, bias_eval}, {wp, fe[0]});
         proof_.dense[id] = {res.first, bias_eval, fe};
         return {res.first.point, fe[1]};
     }
@@ -477,14 +439,14 @@ class Prover {
     // the left = input matrix) and the column part (fixes the LOW variables of the constant matrix, or its HIGH ones when it is stored
     // transposed); one degree-2 sumcheck over the shared inner dimension; the left evaluation is the claim handed to the previous node
     Claim prove_matmul(size_t id, const Node &n, const Claim &last_claim, const DeviceMle &input) {
-        const auto &comms = ctx_.model_comms.at(id);
+        const ModelCommitment &mc = ctx_.model_comms.at(id);
         const size_t vr = ceil_log2(n.mm_r), vc = ceil_log2(n.mm_c), vk = ceil_log2(n.mm_k);
         if (last_claim.point.size() != vr + vc) throw Error(DP_ERR_INVALID, "Wrong length of last claim point");
         const ExtVec p_right(last_claim.point.begin(), last_claim.point.begin() + vc), p_left(last_claim.point.begin() + vc, last_claim.point.end());   // split_claim
         Ext bias_eval = Ext::zero();
-        if (n.mm_bias) bias_eval = comms.at("MatMulBias").poly.evaluate(p_right);
+        if (mc.bias) bias_eval = mc.bias->poly.evaluate(p_right);
         DeviceMle left = input.fix_high_variables(p_left);
-        const DeviceMle &w = comms.at("MatMulWeight").poly;
+        const DeviceMle &w = mc.weight.poly;
         DeviceMle right = n.mm_t ? w.fix_high_variables(p_right) : w.fix_variables(p_right);
         if (left.num_vars() != vk || right.num_vars() != vk) throw Error(DP_ERR_INVALID, "matmul: free variables of the two matrices differ");
         VirtualPolynomial vp(vk);
@@ -494,8 +456,7 @@ class Prover {
         ExtVec pl = res.first.point; pl.insert(pl.end(), p_left.begin(), p_left.end());                      // full_points
         ExtVec pr;
         if (n.mm_t) { pr = res.first.point; pr.insert(pr.end(), p_right.begin(), p_right.end()); } else { pr = p_right; pr.insert(pr.end(), res.first.point.begin(), res.first.point.end()); }
-        if (n.mm_bias) add_witness_claim(comms.at("MatMulBias"), {p_right, bias_eval});                       // BTreeMap order of PolyId
-        add_witness_claim(comms.at("MatMulWeight"), {pr, fe[1]});
+        add_model_claims(id, {p_right, bias_eval}, {pr, fe[1]});
         proof_.dense[id] = {res.first, bias_eval, fe};                                                         // MatMulProof has DenseProof's shape
         return {pl, fe[0]};
     }
@@ -545,9 +506,7 @@ class Prover {
     // Convolution::prove (convolution.rs:609-636) -> prove_convolution_step, then add_common_claims (:1003-1010)
     Claim prove_convolution(size_t id, const Claim &last_claim, const ConvData &pd) {
         ConvProof cp; Claim in_claim = ctx_.convs.at(id).prove_convolution_step(t_, last_claim, pd, cp);
-        const auto &comms = ctx_.model_comms.at(id);
-        add_witness_claim(comms.at("ConvBias"), cp.bias_poly_claim);                  // BTreeMap order of PolyId
-        add_witness_claim(comms.at("ConvFilter"), cp.filter_claim);
+        add_model_claims(id, cp.bias_poly_claim, cp.filter_claim);
         proof_.conv[id] = cp;
         return in_claim;
     }
@@ -607,49 +566,40 @@ class Prover {
     std::vector<std::pair<ProverCommitment, Claim>> claims_, trivial_claims_;
 };
 
-// flat u64 image for the parity tests (layout documented in tests/test_gpu_zkml.py)
-inline void flat_e(std::vector<u64> &o, const Ext &e) { o.push_back(e.c0); o.push_back(e.c1); }
-inline void flat_iop(std::vector<u64> &o, const IOPProof &p) { o.push_back(p.point.size()); for (auto &e : p.point) flat_e(o, e); o.push_back(p.proofs.size()); for (auto &m : p.proofs) { o.push_back(m.evaluations.size()); for (auto &e : m.evaluations) flat_e(o, e); } }
-inline void flat_logup(std::vector<u64> &o, const LogUpProof &p) {
-    o.push_back(p.sumcheck_proofs.size()); for (auto &s : p.sumcheck_proofs) flat_iop(o, s);
-    o.push_back(p.round_evaluations.size()); for (auto &r : p.round_evaluations) { o.push_back(r.size()); for (auto &e : r) flat_e(o, e); }
-    o.push_back(p.output_claims.size()); for (auto &c : p.output_claims) { o.push_back(c.point.size()); for (auto &e : c.point) flat_e(o, e); flat_e(o, c.eval); }
-    o.push_back(p.circuit_outputs.size()); for (auto &r : p.circuit_outputs) { o.push_back(r.size()); for (auto &e : r) flat_e(o, e); }
-    o.push_back(p.table ? 1 : 0);
+// flat u64 images for the parity tests, word for word the CPU checker's
+inline void flat_logup(ProofImage &w, const LogUpProof &p) {
+    w.put(p.sumcheck_proofs.size()); for (auto &s : p.sumcheck_proofs) w.iop(s);
+    w.put(p.round_evaluations.size()); for (auto &r : p.round_evaluations) w.exts(r);
+    w.put(p.output_claims.size()); for (auto &c : p.output_claims) { w.exts(c.point); w.ext(c.eval); }
+    w.put(p.circuit_outputs.size()); for (auto &r : p.circuit_outputs) w.exts(r);
+    w.put(p.table ? 1 : 0);
 }
-inline void flat_evec(std::vector<u64> &o, const ExtVec &v) { o.push_back(v.size()); for (auto &e : v) flat_e(o, e); }
-// same layout as the CPU checker's flattening: ConvProof field order (convolution.rs:97-121), the two commitment claims, the input claim
-inline std::vector<u64> flatten_conv_proof(const ConvProof &p, const Claim &input_claim) {
-    std::vector<u64> o;
-    flat_iop(o, p.fft_proof); flat_evec(o, p.fft_claims); flat_iop(o, p.fft_proof_weights); flat_iop(o, p.ifft_proof);
-    o.push_back(p.fft_delegation.proofs.size()); for (auto &q : p.fft_delegation.proofs) flat_iop(o, q);
-    o.push_back(p.fft_delegation_weights.proofs.size()); for (auto &q : p.fft_delegation_weights.proofs) flat_iop(o, q);
-    o.push_back(p.ifft_delegation.proofs.size()); for (auto &q : p.ifft_delegation.proofs) flat_iop(o, q);
-    flat_iop(o, p.hadamard_proof); flat_evec(o, p.ifft_claims); flat_evec(o, p.fft_weight_claims);
-    o.push_back(p.fft_delegation.claims.size()); for (auto &c : p.fft_delegation.claims) flat_evec(o, c);
-    o.push_back(p.fft_delegation_weights.claims.size()); for (auto &c : p.fft_delegation_weights.claims) flat_evec(o, c);
-    o.push_back(p.ifft_delegation.claims.size()); for (auto &c : p.ifft_delegation.claims) flat_evec(o, c);
-    flat_evec(o, p.hadamard_claims); flat_e(o, p.bias_claim); flat_evec(o, p.partial_evals);
-    flat_iop(o, p.clearing_proof.sumcheck); flat_evec(o, p.clearing_proof.individual_claim);
-    flat_evec(o, p.filter_claim.point); flat_e(o, p.filter_claim.eval); flat_evec(o, p.bias_poly_claim.point); flat_e(o, p.bias_poly_claim.eval);
-    flat_evec(o, input_claim.point); flat_e(o, input_claim.eval);
-    return o;
+// ConvProof field order (convolution.rs:97-121), the two commitment claims, the input claim
+inline void flatten_conv_proof(ProofImage &w, const ConvProof &p, const Claim &input_claim) {
+    const MatrixEvalProof *delegations[3] = {&p.fft_delegation, &p.fft_delegation_weights, &p.ifft_delegation};
+    w.iop(p.fft_proof); w.exts(p.fft_claims); w.iop(p.fft_proof_weights); w.iop(p.ifft_proof);
+    for (auto *d : delegations) { w.put(d->proofs.size()); for (auto &q : d->proofs) w.iop(q); }
+    w.iop(p.hadamard_proof); w.exts(p.ifft_claims); w.exts(p.fft_weight_claims);
+    for (auto *d : delegations) { w.put(d->claims.size()); for (auto &c : d->claims) w.exts(c); }
+    w.exts(p.hadamard_claims); w.ext(p.bias_claim); w.exts(p.partial_evals);
+    w.iop(p.clearing_proof.sumcheck); w.exts(p.clearing_proof.individual_claim);
+    w.exts(p.filter_claim.point); w.ext(p.filter_claim.eval); w.exts(p.bias_poly_claim.point); w.ext(p.bias_poly_claim.eval);
+    w.exts(input_claim.point); w.ext(input_claim.eval);
 }
 
 inline std::vector<u64> Proof::flatten(size_t n_nodes) const {
-    std::vector<u64> o;
-    auto fd = [&](const Digest &d) { for (int i = 0; i < 4; i++) o.push_back(d.v[i]); };
+    ProofImage w;
     for (size_t id = 0; id < n_nodes; id++) {
-        if (dense.count(id)) { const auto &d = dense.at(id); o.push_back(100 + id); flat_iop(o, d.sumcheck); flat_e(o, d.bias_eval); o.push_back(d.individual_claims.size()); for (auto &e : d.individual_claims) flat_e(o, e); }
-        if (requant.count(id)) { const auto &r = requant.at(id); o.push_back(200 + id); flat_iop(o, r.io_accumulation); o.push_back(r.accumulation_evals.size()); for (auto &e : r.accumulation_evals) flat_e(o, e); flat_logup(o, r.clamping_lookup); flat_logup(o, r.shifted_lookup); o.push_back(r.commitments.size()); for (auto &d : r.commitments) fd(d); }
-        if (activation.count(id)) { const auto &a = activation.at(id); o.push_back(300 + id); flat_iop(o, a.io_accumulation.sumcheck); o.push_back(a.io_accumulation.evals.size()); for (auto &e : a.io_accumulation.evals) flat_e(o, e); flat_logup(o, a.lookup); o.push_back(a.commits.size()); for (auto &d : a.commits) fd(d); }
-        if (conv.count(id)) { o.push_back(400 + id); std::vector<u64> c = flatten_conv_proof(conv.at(id), Claim()); o.insert(o.end(), c.begin(), c.end()); }
-        if (pooling.count(id)) { const auto &q = pooling.at(id); o.push_back(500 + id); flat_iop(o, q.sumcheck); flat_logup(o, q.lookup); flat_evec(o, q.zerocheck_evals); o.push_back(q.variable_gap); o.push_back(q.commitments.size()); for (auto &d : q.commitments) fd(d); }
+        if (dense.count(id)) { const auto &d = dense.at(id); w.put(100 + id); w.iop(d.sumcheck); w.ext(d.bias_eval); w.exts(d.individual_claims); }
+        if (requant.count(id)) { const auto &r = requant.at(id); w.put(200 + id); w.iop(r.io_accumulation); w.exts(r.accumulation_evals); flat_logup(w, r.clamping_lookup); flat_logup(w, r.shifted_lookup); w.put(r.commitments.size()); for (auto &d : r.commitments) w.digest(d); }
+        if (activation.count(id)) { const auto &a = activation.at(id); w.put(300 + id); w.iop(a.io_accumulation.sumcheck); w.exts(a.io_accumulation.evals); flat_logup(w, a.lookup); w.put(a.commits.size()); for (auto &d : a.commits) w.digest(d); }
+        if (conv.count(id)) { w.put(400 + id); flatten_conv_proof(w, conv.at(id), Claim()); }
+        if (pooling.count(id)) { const auto &q = pooling.at(id); w.put(500 + id); w.iop(q.sumcheck); flat_logup(w, q.lookup); w.exts(q.zerocheck_evals); w.put(q.variable_gap); w.put(q.commitments.size()); for (auto &d : q.commitments) w.digest(d); }
     }
-    o.push_back(table_proofs.size()); for (auto &t : table_proofs) { fd(t.multiplicity_commit); flat_logup(o, t.lookup); }
-    o.push_back(trivial_proofs.size());
-    std::vector<u64> b = batch_proof.flatten(); o.push_back(b.size()); o.insert(o.end(), b.begin(), b.end());
-    return o;
+    w.put(table_proofs.size()); for (auto &t : table_proofs) { w.digest(t.multiplicity_commit); flat_logup(w, t.lookup); }
+    w.put(trivial_proofs.size());
+    std::vector<u64> b = batch_proof.flatten(); w.put(b.size()); w.words.insert(w.words.end(), b.begin(), b.end());
+    return w.words;
 }
 
 }  // namespace zkml

@@ -93,3 +93,27 @@ def test_end_to_end_proof_uses_device_inference(gpu):
     assert (ctx.prove(x) == exp).all()
     ctx.run_inference(x)
     assert (ctx.prove_trace(want_proof=True) == exp).all()
+
+
+def test_model_refuses_values_outside_the_lookups(gpu):
+    """the model-level refusals of the witness pass: a Dense output past 2^intermediate_bit_size refuses the requant, a ReLU input
+    past its table refuses the lookup; a refused proof leaves the context able to prove the next input bit for bit"""
+    import oracle_py as O
+    nl, width = 2, 128
+    w, b, rq = O.synthetic_mlp(nl, width, 21)
+    x = O.synthetic_input(width, 22)
+    bad = x * (1 << 20)
+    assert np.abs(w[: width * width].reshape(width, width) @ bad + b[:width]).max() > 1 << int(rq[0][3])
+    ctx = gpu.ZkmlContext(nl, width, w, b, rq)
+    with pytest.raises(gpu.DpError, match="absolute value too large"):
+        ctx.prove(bad)
+    exp, _ = O.zkml_prove(nl, width, 21, 22)
+    assert (ctx.prove(x) == exp).all()
+
+    n = 16
+    desc = np.zeros((2, 9), dtype=np.int64)
+    desc[0, :3] = 0, n, n                   # Dense n x n
+    desc[1, 0] = 2                          # ReLU
+    data = np.concatenate([np.ones(n * n, dtype=np.int64), np.zeros(n, dtype=np.int64)])
+    with pytest.raises(gpu.DpError, match="not in its table"):
+        gpu.ModelContext(desc, data, n).prove(np.full(n, 100, dtype=np.int64))     # outputs 1600 > 127
