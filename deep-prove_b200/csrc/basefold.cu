@@ -25,6 +25,7 @@
 #include <atomic>
 #include <map>
 #include <memory>
+#include <mutex>
 
 static constexpr u32 BF_RATE_LOG = 1;            // RSCodeDefaultSpec (rs.rs:192-214)
 static constexpr u32 BF_BASECODE_LOG = 7;
@@ -44,8 +45,7 @@ static PowTab powtab_at(const u64 *t) { PowTab p; p.t0 = t; p.t1 = t + 2048; p.t
 static int pow_table_build(u64 base, const u64 **out) {
     u64 *tab = nullptr;
     DP_CUDA(cudaMalloc((void **)&tab, sizeof(u64) * 3 * 2048));
-    k_pow_table<<<24, 256, 0, dp_ctx().stream>>>(base, tab); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_pow_table, 24, 256, 0, dp_ctx().stream, base, tab));
     DP_CUDA(dp_stream_sync(dp_ctx().stream));
     *out = tab;
     return DP_OK;
@@ -153,9 +153,8 @@ static int run_levels(T *data, u32 n_log, u32 from, u32 to) {
         size_t smem = sizeof(T) << (lv + c_log);
         if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_tile_pass<T, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         DpProfScope prof(MODE ? "k_tile_pass(ntt)" : "k_tile_pass(moebius)", (sizeof(T) << n_log) * 2);
-        k_tile_pass<T, MODE><<<(unsigned)tiles, 256, smem, c.stream>>>(data, n_log, ch.first, ch.second, c_log, tab); DP_LAUNCHED();
+        DP_CUDA(dp_launch(k_tile_pass<T, MODE>, (unsigned)tiles, 256, smem, c.stream, data, n_log, ch.first, ch.second, c_log, tab));
     }
-    DP_CUDA(cudaGetLastError());
     return DP_OK;
 }
 
@@ -298,7 +297,7 @@ __device__ __forceinline__ void mk_publish_root(const RootOut &rt, const u64 *ro
     if (!rt.root_host) return;
 #pragma unroll
     for (int k = 0; k < 4; k++) rt.root_host[k] = __ldcg(root_dev + k);
-    if (rt.flag) { __threadfence_system(); *(volatile u64 *)rt.flag = rt.seq; }
+    if (rt.flag) dp_publish(rt.flag, rt.seq);
 }
 template <bool EXT, bool FROM_LEAVES>
 __global__ void __launch_bounds__(256) k_merkle_small(const void *src, u32 first_level, u32 lg, u64 nl_first, u64 *levels, LvlOff lo, u32 *ticket, RootOut rt, u32 sub_max, u32 tph_min) {
@@ -484,27 +483,23 @@ static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64
         if (!l0) {
             u64 *own = nullptr; if (int e = dp_dev_alloc((void **)&own, sizeof(u64) * 4 * (n >> 1))) return e;
             DpProfScope prof("k_b3_leaves(blake3)", n * (ext ? 16 : 8) + (n >> 1) * 32);
-            const unsigned g = (unsigned)(((n >> 1) + 255) / 256);
-            const auto kern = ext ? k_b3_leaves<true> : k_b3_leaves<false>;
-            kern<<<g, 256, 0, c.stream>>>(leaves, n >> 1, own); DP_LAUNCHED();
             t.level0 = l0 = own; t.own_level0 = true;
+            DP_CUDA(dp_launch(ext ? k_b3_leaves<true> : k_b3_leaves<false>, (unsigned)(((n >> 1) + 255) / 256), 256, 0, c.stream, leaves, n >> 1, own));
         }
-        if (t.lg == 1) { t.root_dev = const_cast<u64 *>(l0); DP_CUDA(cudaGetLastError()); return DP_OK; }
+        if (t.lg == 1) { t.root_dev = const_cast<u64 *>(l0); return DP_OK; }
         for (u32 l = 1; l < t.lg; l++) {
             const u64 nl = n >> (l + 1);
             const u64 *in = l == 1 ? l0 : t.levels + 4 * t.lvl_off[l - 1];
-            if (nl <= 1024 && t.lg < 36) { DpProfScope prof("k_b3_tail(blake3)", nl * 96); k_b3_tail<<<1, 1024, 0, c.stream>>>(in, l, t.lg, nl, t.levels, lo_all); DP_LAUNCHED(); break; }
+            if (nl <= 1024 && t.lg < 36) { DpProfScope prof("k_b3_tail(blake3)", nl * 96); DP_CUDA(dp_launch(k_b3_tail, 1, 1024, 0, c.stream, in, l, t.lg, nl, t.levels, lo_all)); break; }
             DpProfScope prof("k_b3_up(blake3)", nl * 96);
-            k_b3_up<<<(unsigned)((nl + 255) / 256), 256, 0, c.stream>>>(in, nl, t.levels + 4 * t.lvl_off[l]); DP_LAUNCHED();
+            DP_CUDA(dp_launch(k_b3_up, (unsigned)((nl + 255) / 256), 256, 0, c.stream, in, nl, t.levels + 4 * t.lvl_off[l]));
         }
         t.root_dev = t.levels + 4 * t.lvl_off[t.lg - 1];
-        DP_CUDA(cudaGetLastError());
         return DP_OK;
     }
     if (t.lg == 1 && lvl0) { t.root_dev = const_cast<u64 *>(lvl0); }
     else if (t.lg == 1) {
-        const auto kern = ext ? k_leafpair_root<true> : k_leafpair_root<false>;
-        kern<<<1, 1, 0, c.stream>>>(leaves, t.levels); DP_LAUNCHED();
+        DP_CUDA(dp_launch(ext ? k_leafpair_root<true> : k_leafpair_root<false>, 1, 1, 0, c.stream, leaves, t.levels));
         t.root_dev = t.levels;
     } else {
         for (u32 l = 1; l < t.lg; l++) {
@@ -521,7 +516,7 @@ static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64
                 u32 *ticket = nullptr; if (int e = mk_ticket(&ticket)) return e;
                 RootOut ro = rt ? *rt : RootOut{nullptr, nullptr, 0};
                 const auto kern = from_leaves ? (ext ? k_merkle_small<true, true> : k_merkle_small<false, true>) : k_merkle_small<false, false>;
-                kern<<<g, 256, 0, c.stream>>>(src, l, t.lg, nl, t.levels, lo_all, ticket, ro, sub_max, tph_min); DP_LAUNCHED();
+                DP_CUDA(dp_launch(kern, g, 256, 0, c.stream, src, l, t.lg, nl, t.levels, lo_all, ticket, ro, sub_max, tph_min));
                 if (rt && rt_done) *rt_done = true;
                 break;
             }
@@ -532,20 +527,18 @@ static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64
                 // instructions, so the mid levels of many proofs' trees overlap instead of queueing behind each other.
                 DpProfScope prof("k_merkle_mid(poseidon2 compress, thread per hash)", in_bytes + nl * 32, 2 * nl);
                 const auto kern = from_leaves ? (ext ? k_merkle_mid<true, true> : k_merkle_mid<false, true>) : k_merkle_mid<false, false>;
-                kern<<<(unsigned)((nl + 63) / 64), 64, 0, c.stream>>>(src, nl, out); DP_LAUNCHED();
+                DP_CUDA(dp_launch(kern, (unsigned)((nl + 63) / 64), 64, 0, c.stream, src, nl, out));
                 continue;
             }
             DpProfScope prof("k_merkle(poseidon2 compress)", in_bytes + nl * 32, 2 * nl);
             const unsigned mgrid = (unsigned)std::min<u64>((nl + 127) / 128, 1u << 22);
             // one hash per thread, many SHORT blocks (no persistent grid-stride blocks): with 16 proofs in flight the block
             // scheduler can interleave other streams' latency-critical single-block kernels every few microseconds
-            if (from_leaves) { const auto kern = ext ? k_merkle_l1<true> : k_merkle_l1<false>; kern<<<mgrid, 128, 0, c.stream>>>(src, nl, out); }
-            else k_merkle_up<<<mgrid, 128, 0, c.stream>>>((const u64 *)src, nl, out);
-            DP_LAUNCHED();
+            if (from_leaves) DP_CUDA(dp_launch(ext ? k_merkle_l1<true> : k_merkle_l1<false>, mgrid, 128, 0, c.stream, src, nl, out));
+            else DP_CUDA(dp_launch(k_merkle_up, mgrid, 128, 0, c.stream, (const u64 *)src, nl, out));
         }
         t.root_dev = t.levels + 4 * t.lvl_off[t.lg - 1];
     }
-    DP_CUDA(cudaGetLastError());
     return DP_OK;
 }
 static void tree_free(DevTree &t) { if (t.own_levels) dp_dev_free(t.levels); t.levels = nullptr; if (t.own_level0) { dp_dev_free(const_cast<u64 *>(t.level0)); t.level0 = nullptr; t.own_level0 = false; } t.leaves = nullptr; }
@@ -616,10 +609,8 @@ static int lincomb_bcast(gle *out, const gle *base, const std::vector<LcTerm> &t
         for (u32 k = 0; k < a.n; k++) { const LcTerm &t = terms[o + k]; a.s[k].p = t.p; a.s[k].c0 = t.coef.c0; a.s[k].c1 = t.coef.c1; a.s[k].ext = t.ext ? 1 : 0; a.s[k].rep_log = t.rep_log; src_bytes += (n >> t.rep_log) * (t.ext ? 16 : 8); }
         const gle *b = o == 0 ? base : out;
         DpProfScope p("k_lincomb_bcast", src_bytes + n * (b ? 32 : 16));
-        if (b) k_lincomb_bcast<true><<<g, 256, 0, c.stream>>>(out, b, a, n); else k_lincomb_bcast<false><<<g, 256, 0, c.stream>>>(out, nullptr, a, n);
-        DP_LAUNCHED();
+        DP_CUDA(dp_launch(b ? k_lincomb_bcast<true> : k_lincomb_bcast<false>, g, 256, 0, c.stream, out, b, a, n));
     }
-    DP_CUDA(cudaGetLastError());
     return DP_OK;
 }
 __global__ void k_lift(const u64 *__restrict__ src, gle *__restrict__ out, u64 n) {
@@ -717,8 +708,7 @@ static int encode_small(const void *evals, void *bh_evals, void *codeword, u32 n
     const size_t smem = sizeof(T) << (nv + BF_RATE_LOG);
     DpProfScope p("k_encode_small(bitrev+moebius+expand+ntt)", sizeof(T) * m * 2 + smem);
     if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_encode_small<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_encode_small<T><<<1, 512, smem, dp_ctx().stream>>>((const T *)evals, (T *)bh_evals, (T *)codeword, nv, shift, root_tab()); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_encode_small<T>, 1, 512, smem, dp_ctx().stream, (const T *)evals, (T *)bh_evals, (T *)codeword, nv, shift, root_tab()));
     return DP_OK;
 }
 
@@ -737,20 +727,18 @@ static int encode_tiled(const void *evals, void *bh_evals, void *codeword, u32 n
     DevPtr coef_owner(coef);
     PowTab st; if (int e = shift_powtab(shift, &st)) return e;
     const int g = dp_grid_for(m, 256, 8);
-    { DpProfScope p("k_bitrev", esz * m * 2); k_bitrev<T><<<g, 256, 0, c.stream>>>((const T *)evals, logG ? coef : bh, nv); DP_LAUNCHED(); }
+    { DpProfScope p("k_bitrev", esz * m * 2); DP_CUDA(dp_launch(k_bitrev<T>, g, 256, 0, c.stream, (const T *)evals, logG ? coef : bh, nv)); }
     if (!logG) DP_CUDA(cudaMemcpyAsync(coef, bh, esz * m, cudaMemcpyDeviceToDevice, c.stream));
     else if (cudaMemcpyAsync(bh, coef + Ml * rank, esz * Ml, cudaMemcpyDeviceToDevice, c.stream) != cudaSuccess)
         return dp_fail(DP_ERR_CUDA, "dp_pcs_commit_shard: copy of the evaluation slice failed");
     if (int e = run_levels<T, 0>(coef, nv, 0, nv)) return e;
-    if (!logG) { DpProfScope p("k_expand", esz * m * 3); k_expand<T><<<g, 256, 0, c.stream>>>(coef, cw, nv, st, root_tab()); DP_LAUNCHED(); }
+    if (!logG) { DpProfScope p("k_expand", esz * m * 3); DP_CUDA(dp_launch(k_expand<T>, g, 256, 0, c.stream, coef, cw, nv, st, root_tab())); }
     else {
         u32 rev_rank = 0; for (u32 b = 0; b < logG; b++) if (rank >> b & 1) rev_rank |= 1u << (logG - 1 - b);
         DpProfScope p("k_shard_expand", esz * (m + S));
-        k_shard_expand<T><<<dp_grid_for(S, 256, 8), 256, 0, c.stream>>>(coef, cw, nv, logG, rev_rank, st, root_tab()); DP_LAUNCHED();
+        DP_CUDA(dp_launch(k_shard_expand<T>, dp_grid_for(S, 256, 8), 256, 0, c.stream, coef, cw, nv, logG, rev_rank, st, root_tab()));
     }
-    if (int e = run_levels<T, 1>(cw, n_log - logG, logG ? 0 : 1, n_log - logG)) return e;
-    DP_CUDA(cudaGetLastError());
-    return DP_OK;
+    return run_levels<T, 1>(cw, n_log - logG, logG ? 0 : 1, n_log - logG);
 }
 
 extern "C" {
@@ -927,7 +915,7 @@ int dp_pcs_batch_commit(const dp_mle *const *polys, uint32_t n, uint32_t full_lo
         const bool blake = blake_on();
         if (blake) DP_CHECK((b->is_base ? n : 2 * n) <= 128, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: BLAKE3 batch leaves are limited to one 1024-byte chunk (128 base / 64 extension polynomials)");
         const auto kern = blake ? (b->is_base ? k_b3_batch_l0<false> : k_b3_batch_l0<true>) : (b->is_base ? k_merkle_batch_l0<false> : k_merkle_batch_l0<true>);
-        kern<<<(unsigned)((n0 + 127) / 128), 128, 0, c.stream>>>(bp, n, n0, b->level0); DP_LAUNCHED();
+        DP_CUDA(dp_launch(kern, (unsigned)((n0 + 127) / 128), 128, 0, c.stream, bp, n, n0, b->level0));
     }
     if (int e = tree_build(b->tree, b->parts[0]->codeword, !b->is_base, N, b->level0)) return e;
     for (auto *part : b->parts) { part->tree = tree_view(b->tree); part->tree.leaves = part->codeword; }   // own leaves, the batch tree's digests
@@ -1016,7 +1004,6 @@ int dp_pcs_comm_bh_evals(const dp_pcs_comm *cm, dp_mle **view) {
 }
 int dp_pcs_comm_free(dp_pcs_comm *cm) {
     if (!cm) return DP_OK;
-    std::lock_guard<std::recursive_mutex> lk(dp_ctx().mu);
     if (dp_ctx().ready) { tree_free(cm->tree); if (!cm->trivial) dp_dev_free(cm->codeword); dp_dev_free(cm->bh_evals); dp_dev_free(cm->level0); tree_free(cm->top); dp_dev_free(cm->top_lvl0); }
     for (auto *p : cm->parts) dp_pcs_comm_free(p);
     delete cm;
@@ -1028,7 +1015,7 @@ static int open_oracle_from_codeword(dp_pcs_open *o, const dp_pcs_comm *cm) {
     DpCtx &c = dp_ctx();
     o->n0 = cm->cw_len;
     if (int e = dp_dev_alloc((void **)&o->oracle0, sizeof(gle) * o->n0)) return e;
-    if (cm->is_base) { k_lift<<<dp_grid_for(o->n0, 256, 8), 256, 0, c.stream>>>((const u64 *)cm->codeword, o->oracle0, o->n0); DP_LAUNCHED(); }
+    if (cm->is_base) DP_CUDA(dp_launch(k_lift, dp_grid_for(o->n0, 256, 8), 256, 0, c.stream, (const u64 *)cm->codeword, o->oracle0, o->n0));
     else DP_CUDA(cudaMemcpyAsync(o->oracle0, cm->codeword, sizeof(gle) * o->n0, cudaMemcpyDeviceToDevice, c.stream));
     return DP_OK;
 }
@@ -1101,7 +1088,6 @@ int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, u
             if (int e = lincomb_bcast(o->scratch_sum_evals, nullptr, terms, M)) return e;
             o->evals = dp_mle_view(o->scratch_sum_evals, M, true);
         }
-        DP_CUDA(cudaGetLastError());
         if (int e = dp_eq_build(rp.data(), num_vars, &o->eq)) return e;
     }
     // the Basefold-internal sumcheck (basefold/sumcheck.rs) is a degree-2 LSB-first sumcheck of eq * evals on
@@ -1148,8 +1134,8 @@ int dp_pcs_open_round(dp_pcs_open *o, const uint64_t challenge[2], uint64_t next
         u64 gamma = 7; for (u32 k = 0; k < gexp; k++) gamma = gl_sqr(gamma);
         u64 nhgi = gl_neg(gl_mul(gl_inv(gamma), 0x7FFFFFFF80000001ULL));   // -(1/gamma_lvl)/2
         DpProfScope p("k_fri_fold", len * 16 + (len >> 1) * 16);
-        k_fri_fold<<<dp_grid_for(len >> 1, 256, 8), 256, 0, c.stream>>>(o->oracle0, folded, level, len >> 1, (u64)o->shard_rank * (len >> 1), r, gamma, nhgi, root_tab()); DP_LAUNCHED();
-        DP_CUDA(cudaGetLastError());
+        DP_CUDA(dp_launch(k_fri_fold, dp_grid_for(len >> 1, 256, 8), 256, 0, c.stream, o->oracle0, folded, level, len >> 1, (u64)o->shard_rank * (len >> 1), r, gamma,
+                          nhgi, root_tab()));
     }
     // the oracle just consumed is either round i-1's tree leaves (kept) or the initial / merged buffer (freed)
     bool consumed_is_tree_leaves = !o->rounds.empty() && o->rounds.back().oracle == o->oracle0;
@@ -1165,7 +1151,7 @@ int dp_pcs_open_round(dp_pcs_open *o, const uint64_t challenge[2], uint64_t next
         RootOut ro{o->h_root, o->h_root + 8, ++o->root_seq}; bool published = false;
         if (int e = tree_build(rd.tree, folded, true, rd.len, nullptr, &ro, &published)) return e;   // compute_inner_ext
         if (published) {   // the tree's last launch stores the root and then the sequence number in mapped memory
-            if (dp_wait_flag(o->h_root + 8, o->root_seq, false, 0, 30.0) != o->root_seq) { DP_CUDA(dp_stream_sync(c.stream)); DP_CHECK(o->h_root[8] == o->root_seq, DP_ERR_CUDA, "dp_pcs_open_round: tree kernel finished without publishing its root"); }
+            if (int e = dp_await(o->h_root + 8, o->root_seq, 30.0, "dp_pcs_open_round: tree kernel finished without publishing its root")) return e;
             memcpy(root, o->h_root, 32);
         } else if (int e = dp_d2h(root, rd.tree.root_dev, 32, c.stream)) return e;
         o->rounds.push_back(rd);
@@ -1252,8 +1238,7 @@ int dp_pcs_open_query(dp_pcs_open *o, const uint64_t *x_indices, uint32_t n, uin
     DP_CUDA(cudaMemcpyAsync(dx, x_indices, 8 * (size_t)n, cudaMemcpyHostToDevice, c.stream));
     DP_CUDA(dp_stream_sync(c.stream));   // qt/off are stack-owned host buffers
     if (logG) DP_CUDA(cudaMemsetAsync(dout, 0, 8 * w * n, c.stream));   // rows of queries other ranks own stay zero
-    k_query_gather<<<dim3(n, nt), 32, 0, c.stream>>>(dq, nt, dx, doff, w, dout); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_query_gather, dim3(n, nt), 32, 0, c.stream, dq, nt, dx, doff, w, dout));
     if (int e = dp_d2h(out, dout, 8 * w * n, c.stream)) return e;
     dp_dev_free(dq); dp_dev_free(doff); dp_dev_free(dx); dp_dev_free(dout);
     return DP_OK;
@@ -1261,7 +1246,6 @@ int dp_pcs_open_query(dp_pcs_open *o, const uint64_t *x_indices, uint32_t n, uin
 
 int dp_pcs_open_free(dp_pcs_open *o) {
     if (!o) return DP_OK;
-    std::lock_guard<std::recursive_mutex> lk(dp_ctx().mu);
     if (dp_ctx().ready) {
         if (o->sc) dp_sc_destroy(o->sc);
         bool oracle_in_rounds = false;

@@ -1,10 +1,12 @@
-// Library-internal context: one per host thread, with its own stream and device arena.
+// Library-internal context: one per host thread, with its own stream and device arena.  A context belongs to the thread that
+// made it and is only ever touched from that thread, so it needs no lock; a device block may still be released on another thread,
+// through the arena's foreign-free path (dp_dev_free), which takes the slab registry's lock.
 #pragma once
 #include "gl.cuh"
 #include "../../include/deepprove_b200.h"
 #include <memory>
-#include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 #include <cstdio>
 #include <cstring>
@@ -15,7 +17,6 @@ struct DpCtx {
     int sm_count = 132;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    std::recursive_mutex mu;
     u64 *sync_flag = nullptr; u64 sync_seq = 0;   // dp_stream_sync: this thread's pinned completion word
     std::vector<void *> zero_blocks;               // 256-byte device blocks known to hold zeros (dp_zero_block_get/put)
 };
@@ -27,13 +28,33 @@ int dp_fail(int code, const std::string &s);
         cudaError_t e_ = (x);                                                                               \
         if (e_ != cudaSuccess) return dp_fail(DP_ERR_CUDA, std::string(#x) + ": " + cudaGetErrorString(e_)); \
     } while (0)
-#define DP_REQUIRE_CTX()                                                                    \
-    std::lock_guard<std::recursive_mutex> lk_(dp_ctx().mu);                                 \
-    if (!dp_ctx().ready) return dp_fail(DP_ERR_NO_DEVICE, "dp_init() has not succeeded: no CUDA device context")
 #define DP_CHECK(cond, code, msg) \
     do { if (!(cond)) return dp_fail((code), (msg)); } while (0)
+#define DP_REQUIRE_CTX() DP_CHECK(dp_ctx().ready, DP_ERR_NO_DEVICE, "dp_init() has not succeeded: no CUDA device context")
+
+// ---- launching kernels -------------------------------------------------------------------------------------------------
+// Every kernel of the library is launched by one of these two: they count the launch (dp_kernel_launches) and return its error,
+// for the caller's DP_CUDA.
 void dp_count_launch();
-#define DP_LAUNCHED() dp_count_launch()
+template <class... P, class... A>
+cudaError_t dp_launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A &&...args) {
+    kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+    dp_count_launch();
+    return cudaGetLastError();
+}
+// ... and as one thread-block cluster of ncta CTAs (the resident sumcheck kernels)
+template <class... P, class... A>
+cudaError_t dp_launch_cluster(void (*kernel)(P...), unsigned ncta, dim3 block, cudaStream_t st, A &&...args) {
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t lc{};
+    lc.gridDim = dim3(ncta); lc.blockDim = block; lc.dynamicSmemBytes = 0; lc.stream = st;
+    lc.attrs = at; lc.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&lc, kernel, std::forward<A>(args)...);
+    dp_count_launch();
+    const cudaError_t last = cudaGetLastError();   // also clears the error a refused launch leaves there
+    return e != cudaSuccess ? e : last;
+}
 
 // optional per-kernel timing with CUDA events on the launch stream (bench.py's roofline leg)
 int dp_prof_begin(const char *name, u64 algorithmic_bytes, u64 units = 0);   // returns a token (or -1 when disabled); units: permutations / field ops
@@ -58,6 +79,10 @@ u64 dp_wait_flag(volatile u64 *flag, u64 want, bool has_fail, u64 fail, double t
 // cudaStreamSynchronize for the hot path: in DP_WAIT_BLOCK mode a one-thread kernel raises this thread's pinned word at the
 // end of the stream's queued work and the thread sleeps on it (cudaStreamSynchronize itself spins in the driver).
 cudaError_t dp_stream_sync(cudaStream_t st);
+// A completion word: a kernel publishes `v` with dp_publish after its results, and the host waits for it with dp_await.  When the
+// word does not come within timeout_s, dp_await drains the context's stream, looks once more and refuses with `refusal`.
+__device__ __forceinline__ void dp_publish(volatile u64 *word, u64 v) { __threadfence_system(); *word = v; }
+int dp_await(volatile u64 *word, u64 want, double timeout_s, const std::string &refusal);
 
 // Device -> caller's (pageable) host memory, then wait: staged through pinned memory so that the copy call returns at once
 // and the wait goes through the wait service.  (cudaMemcpyAsync into pageable memory blocks INSIDE the driver, spinning, until

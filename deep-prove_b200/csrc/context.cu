@@ -6,7 +6,8 @@
 
 static thread_local std::string g_err;
 // One context PER HOST THREAD (own stream, device arena, pinned cache): independent proofs run concurrently
-// from several host threads on one GPU and share only read-only device data (model, tables, twiddles).
+// from several host threads on one GPU and share only read-only device data (model, tables, twiddles).  Only the owning thread
+// reaches its context, so nothing in it is locked.
 static thread_local DpCtx g_ctx;
 DpCtx &dp_ctx() { return g_ctx; }
 static std::atomic<unsigned long long> g_total_launches{0};
@@ -239,17 +240,21 @@ u64 dp_wait_flag(volatile u64 *flag, u64 want, bool has_fail, u64 fail, double t
         }
     }
 }
-__global__ void k_signal(u64 *flag, u64 seq) { __threadfence_system(); *(volatile u64 *)flag = seq; }
+__global__ void k_signal(u64 *flag, u64 seq) { dp_publish(flag, seq); }
 cudaError_t dp_stream_sync(cudaStream_t st) {
     if (dp_wait_mode() == DP_WAIT_SPIN) { g_host_waits.fetch_add(1, std::memory_order_relaxed); return cudaStreamSynchronize(st); }
     DpCtx &c = g_ctx;
     if (!c.sync_flag) { void *p = nullptr; if (dp_pinned_alloc(&p, 64) != DP_OK) return cudaErrorMemoryAllocation; c.sync_flag = (u64 *)p; *c.sync_flag = 0; c.sync_seq = 0; }
     const u64 seq = ++c.sync_seq;
-    k_signal<<<1, 1, 0, st>>>(c.sync_flag, seq); dp_count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+    if (cudaError_t e = dp_launch(k_signal, 1, 1, 0, st, c.sync_flag, seq)) return e;
     if (dp_wait_flag(c.sync_flag, seq, false, 0, 30.0) != seq) return cudaStreamSynchronize(st);   // timeout: let the runtime report what happened
     return cudaSuccess;
+}
+int dp_await(volatile u64 *word, u64 want, double timeout_s, const std::string &refusal) {
+    if (dp_wait_flag(word, want, false, 0, timeout_s) == want) return DP_OK;
+    DP_CUDA(dp_stream_sync(g_ctx.stream));
+    DP_CHECK(*word == want, DP_ERR_CUDA, refusal);
+    return DP_OK;
 }
 
 DpD2H::DpD2H(cudaStream_t s, size_t reserve_bytes) : st(s) { cap = reserve_bytes < 64 ? 64 : reserve_bytes; if (dp_pinned_alloc(&pin, cap) != DP_OK) { pin = nullptr; cap = 0; } }
@@ -331,30 +336,26 @@ int dp_set_wait_mode(int mode) {
 int dp_get_wait_mode(void) { return dp_wait_mode(); }
 
 int dp_profile_enable(int on) {
-    std::lock_guard<std::recursive_mutex> lk(g_ctx.mu);
     prof_resolve();
     g_prof_on.store(on != 0);
     return DP_OK;
 }
 int dp_profile_flush(void) {   // fold this thread's pending events into the process-wide table (cheap no-op when idle)
     if (g_prof_pending.empty()) return DP_OK;
-    std::lock_guard<std::recursive_mutex> lk(g_ctx.mu);
     prof_resolve();
     return DP_OK;
 }
 int dp_profile_reset(void) {
-    std::lock_guard<std::recursive_mutex> lk(g_ctx.mu);
     prof_resolve();
-    std::lock_guard<std::mutex> lk2(g_prof_mu);
+    std::lock_guard<std::mutex> lk(g_prof_mu);
     g_prof_stats.clear();
     return DP_OK;
 }
 // Writes up to `cap` entries; returns the number of distinct kernel names seen.  `units` (may be NULL) = the kernel's own
 // work unit summed over launches: Poseidon2 permutations for the Merkle kernels, field operations for the sumcheck rounds.
 int dp_profile_read_ex(char (*names)[64], uint64_t *counts, double *total_ms, uint64_t *bytes, uint64_t *units, int cap) {
-    std::lock_guard<std::recursive_mutex> lk(g_ctx.mu);
     prof_resolve();
-    std::lock_guard<std::mutex> lk2(g_prof_mu);
+    std::lock_guard<std::mutex> lk(g_prof_mu);
     int i = 0;
     for (auto &kv : g_prof_stats) {
         if (i < cap) {
@@ -381,7 +382,6 @@ int dp_init(int device) {
     // other (a resident tail kernel in a shared queue stalls its neighbours); 32 is the hardware maximum.  Only effective
     // if CUDA is not initialised yet in this process -- hosts that initialise CUDA first should export it themselves.
     setenv("CUDA_DEVICE_MAX_CONNECTIONS", "32", 0);
-    std::lock_guard<std::recursive_mutex> lk(g_ctx.mu);
     int n = dp_device_count();
     if (n <= 0) return dp_fail(DP_ERR_NO_DEVICE, "no CUDA device visible: deepprove_b200 has no CPU fallback");
     if (device < 0 || device >= n) return dp_fail(DP_ERR_INVALID, "dp_init: device index out of range");
@@ -399,7 +399,6 @@ int dp_init(int device) {
 }
 
 int dp_shutdown(void) {
-    std::lock_guard<std::recursive_mutex> lk(g_ctx.mu);
     if (!g_ctx.ready) return DP_OK;
     cudaStreamSynchronize(g_ctx.stream);
     if (g_ctx.own_stream) cudaStreamDestroy(g_ctx.stream);

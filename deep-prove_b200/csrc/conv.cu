@@ -42,8 +42,7 @@ extern "C" int dp_fft_rows(dp_mle *m, uint32_t log_n, int inverse) {
     size_t smem = sizeof(gle) << log_n;
     if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_fft_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     DpProfScope prof("k_fft_rows", m->bytes() * 2);
-    k_fft_rows<<<(unsigned)(m->len >> log_n), 256, smem, dp_ctx().stream>>>((gle *)m->data, log_n, inverse, tab); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_fft_rows, (unsigned)(m->len >> log_n), 256, smem, dp_ctx().stream, (gle *)m->data, log_n, inverse, tab));
     return DP_OK;
 }
 
@@ -127,9 +126,9 @@ extern "C" int dp_fft_rows_long(dp_mle *m, uint32_t log_n, int inverse) {
     DP_CUDA(cudaFuncSetAttribute(k_fft_long_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
     cudaStream_t st = dp_ctx().stream;
     DpProfScope prof("k_fft_long", m->bytes() * 4);
-    k_fft_long_cols<<<(unsigned)((rows << lg2) / FFT_G), 512, smem1, st>>>((const gle *)m->data, (gle *)tmp, lg1, lg2, inverse, tab); DP_LAUNCHED();
-    k_fft_long_rows<<<(unsigned)((rows << lg1) / FFT_G), 512, smem2, st>>>((const gle *)tmp, (gle *)m->data, lg1, lg2, inverse, inverse ? gl_inv(1ULL << log_n) : 1ULL, tab); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_fft_long_cols, (unsigned)((rows << lg2) / FFT_G), 512, smem1, st, (const gle *)m->data, (gle *)tmp, lg1, lg2, inverse, tab));
+    DP_CUDA(dp_launch(k_fft_long_rows, (unsigned)((rows << lg1) / FFT_G), 512, smem2, st, (const gle *)tmp, (gle *)m->data, lg1, lg2, inverse,
+                      inverse ? gl_inv(1ULL << log_n) : 1ULL, tab));
     return DP_OK;
 }
 
@@ -151,10 +150,8 @@ extern "C" int dp_pad_rows(const dp_mle *src, uint64_t rows, uint32_t n_real, ui
     u64 total = rows * out_len;
     DP_CHECK(total && (total & (total - 1)) == 0, DP_ERR_INVALID, "dp_pad_rows: rows * out_len must be a power of two");
     MlePtr m; if (int e = dp_mle_alloc(total, true, m)) return e;
-    int g = dp_grid_for(total, 256, 8);
-    if (src->is_ext) k_pad_rows<true><<<g, 256, 0, dp_ctx().stream>>>(src->data, rows, n_real, n, out_len, (gle *)m->data);
-    else k_pad_rows<false><<<g, 256, 0, dp_ctx().stream>>>(src->data, rows, n_real, n, out_len, (gle *)m->data);
-    DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(src->is_ext ? k_pad_rows<true> : k_pad_rows<false>, dp_grid_for(total, 256, 8), 256, 0, dp_ctx().stream, src->data, rows, n_real, n,
+                      out_len, (gle *)m->data));
     *out = m.release(); return DP_OK;
 }
 
@@ -174,8 +171,8 @@ extern "C" int dp_conv_prod(const dp_mle *x_fft, const dp_mle *w_fft, uint32_t k
     DP_CHECK(x_fft->len == (u64)kx * row_len && w_fft->len == (u64)kw * kx * row_len, DP_ERR_INVALID, "dp_conv_prod: operand shapes do not match [kx, n] / [kw, kx, n]");
     MlePtr m; if (int e = dp_mle_alloc((u64)kw * row_len, true, m)) return e;
     DpProfScope prof("k_conv_prod", (w_fft->bytes() + x_fft->bytes() + m->bytes()));
-    k_conv_prod<<<dp_grid_for((u64)kw * row_len, 128, 8), 128, 0, dp_ctx().stream>>>((const gle *)x_fft->data, (const gle *)w_fft->data, kw, kx, row_len, (gle *)m->data); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_conv_prod, dp_grid_for((u64)kw * row_len, 128, 8), 128, 0, dp_ctx().stream, (const gle *)x_fft->data, (const gle *)w_fft->data, kw, kx,
+                      row_len, (gle *)m->data));
     *out = m.release(); return DP_OK;
 }
 
@@ -200,8 +197,7 @@ extern "C" int dp_conv_output_elements(const dp_mle *out_rows, uint32_t kw, uint
     DevPtr db_owner(db);
     cudaStream_t st = dp_ctx().stream;
     DP_CUDA(cudaMemcpyAsync(db, bias, 8 * (size_t)kw, cudaMemcpyHostToDevice, st));
-    k_conv_out_elems<<<dp_grid_for(nx2 * kw, 256, 8), 256, 0, st>>>((const gle *)out_rows->data, kw, (u32)nx2, db, d); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_conv_out_elems, dp_grid_for(nx2 * kw, 256, 8), 256, 0, st, (const gle *)out_rows->data, kw, (u32)nx2, db, d));
     return dp_d2h(out_host, d, 8 * nx2 * kw, st);
 }
 // The same tensor as a device Base MLE of canonical field elements (Tensor::to_field of the Element tensor: from_i64(to_element(c) + b)
@@ -222,9 +218,8 @@ extern "C" int dp_conv_output(const dp_mle *out_rows, uint32_t kw, uint32_t n_x,
     MlePtr a, c;
     if (int e = dp_mle_alloc(nx2 * kw, false, a)) return e;
     if (int e = dp_mle_alloc(nx2 * kw, false, c)) return e;
-    k_conv_output<<<dp_grid_for(nx2 * kw, 256, 8), 256, 0, dp_ctx().stream>>>((const gle *)out_rows->data, kw, (u32)nx2, (const u64 *)bias->data,
-                                                                               (const u64 *)mask->data, (u64 *)a->data, (u64 *)c->data); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_conv_output, dp_grid_for(nx2 * kw, 256, 8), 256, 0, dp_ctx().stream, (const gle *)out_rows->data, kw, (u32)nx2, (const u64 *)bias->data,
+                      (const u64 *)mask->data, (u64 *)a->data, (u64 *)c->data));
     *after = a.release(); *cleared = c.release(); return DP_OK;
 }
 
@@ -237,8 +232,7 @@ extern "C" int dp_reverse_rows(const dp_mle *src, uint64_t row_len, dp_mle **out
     DP_REQUIRE_CTX();
     DP_CHECK(src && out && !src->is_ext && row_len && src->len % row_len == 0, DP_ERR_INVALID, "dp_reverse_rows: need a Base MLE of whole rows");
     MlePtr m; if (int e = dp_mle_alloc(src->len, false, m)) return e;
-    k_reverse_rows<<<dp_grid_for(src->len, 256, 8), 256, 0, dp_ctx().stream>>>((const u64 *)src->data, src->len, row_len, (u64 *)m->data); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_reverse_rows, dp_grid_for(src->len, 256, 8), 256, 0, dp_ctx().stream, (const u64 *)src->data, src->len, row_len, (u64 *)m->data));
     *out = m.release(); return DP_OK;
 }
 
@@ -295,12 +289,10 @@ static int phi_g_init_run(const uint64_t *rx, uint32_t n, const uint64_t *scale,
     for (u32 i = 0; i + 1 < n; i++) { if (int e = dp_mle_alloc(2ULL << i, true, own[i])) return e; a.mid[i] = (gle *)own[i]->data; }
     const u32 last = is_fft ? n : n - 1, head = std::min(last, max_head);
     gle *phi = (gle *)w->data;
-    k_phi_g_init<<<1, 1024, 0, st>>>(phi, a, n, head, is_fft, tab); DP_LAUNCHED();
-    for (u32 i = head + 1; i <= last; i++) {
-        k_phi_g_level<<<((1u << (i - 1)) + 255) / 256, 256, 0, st>>>(phi, a.rx[n - i], n, i, is_fft, i < n ? a.mid[i - 1] : nullptr, tab); DP_LAUNCHED();
-    }
-    if (!is_fft && head < last) { k_phi_g_scale<<<((1u << (n - 1)) + 255) / 256, 256, 0, st>>>(phi, a.rx[0], n, tab); DP_LAUNCHED(); }
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_phi_g_init, 1, 1024, 0, st, phi, a, n, head, is_fft, tab));
+    for (u32 i = head + 1; i <= last; i++)
+        DP_CUDA(dp_launch(k_phi_g_level, ((1u << (i - 1)) + 255) / 256, 256, 0, st, phi, a.rx[n - i], n, i, is_fft, i < n ? a.mid[i - 1] : nullptr, tab));
+    if (!is_fft && head < last) DP_CUDA(dp_launch(k_phi_g_scale, ((1u << (n - 1)) + 255) / 256, 256, 0, st, phi, a.rx[0], n, tab));
     for (u32 i = 0; i + 1 < n; i++) mid[i] = own[i].release();
     *w_red = w.release(); return DP_OK;
 }
@@ -329,8 +321,7 @@ extern "C" int dp_phi_level(uint32_t len_log, uint32_t n_total, uint32_t shift, 
     PowTab tab; if (int e = dp_root_powtab(&tab)) return e;
     MlePtr m; if (int e = dp_mle_alloc(1ULL << len_log, true, m)) return e;
     u32 len = 1u << len_log;
-    k_phi_level<<<(len + 255) / 256, 256, 0, dp_ctx().stream>>>((gle *)m->data, len, n_total, shift, e_from_host(A), e_from_host(B), inverse, tab); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_phi_level, (len + 255) / 256, 256, 0, dp_ctx().stream, (gle *)m->data, len, n_total, shift, e_from_host(A), e_from_host(B), inverse, tab));
     *out = m.release(); return DP_OK;
 }
 
@@ -343,7 +334,6 @@ extern "C" int dp_mle_repeat(const dp_mle *src, uint32_t times, dp_mle **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(src && out && src->is_ext && times && (times & (times - 1)) == 0, DP_ERR_INVALID, "dp_mle_repeat: need an Ext MLE and a power-of-two count");
     MlePtr m; if (int e = dp_mle_alloc(src->len * times, true, m)) return e;
-    k_repeat<<<dp_grid_for(m->len, 256, 8), 256, 0, dp_ctx().stream>>>((const gle *)src->data, src->len, m->len, (gle *)m->data); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_repeat, dp_grid_for(m->len, 256, 8), 256, 0, dp_ctx().stream, (const gle *)src->data, src->len, m->len, (gle *)m->data));
     *out = m.release(); return DP_OK;
 }

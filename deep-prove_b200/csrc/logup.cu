@@ -55,8 +55,7 @@ __global__ void __launch_bounds__(256) k_logup_tail(LayerPtrs lp, u32 from_layer
         const gle *num = lp.num[n_layers - 1], *den = lp.den[n_layers - 1];
         const gle a = num[0], b = num[1], c = den[0], d = den[1];
         out_host[0] = a.c0; out_host[1] = a.c1; out_host[2] = b.c0; out_host[3] = b.c1; out_host[4] = c.c0; out_host[5] = c.c1; out_host[6] = d.c0; out_host[7] = d.c1;
-        __threadfence_system();
-        *(volatile u64 *)(out_host + 8) = seq;
+        dp_publish(out_host + 8, seq);
     }
 }
 // out[i] = sum_k coef_k * m_k[i]
@@ -98,16 +97,15 @@ int dp_logup_build(dp_mle *const *columns, uint32_t n_columns, const dp_mle *mul
     for (u32 k = 0; k < n_columns; k++) { ca.col[k] = (const u64 *)columns[k]->data; ca.pw[k] = pw; pw = e_mul(pw, sep); }
     gle cc = e_from_host(constant_challenge);
     int g = dp_grid_for(len, 256, 8);
-    { DpProfScope prof("k_logup_den", len * (8 * n_columns + 16)); k_logup_den<<<g, 256, 0, c.stream>>>(ca, cc, len, L->den[0]); DP_LAUNCHED(); }
-    if (L->table) { k_lift_b2e<<<g, 256, 0, c.stream>>>((const u64 *)multiplicities->data, L->num[0], len); DP_LAUNCHED(); }
+    { DpProfScope prof("k_logup_den", len * (8 * n_columns + 16)); DP_CUDA(dp_launch(k_logup_den, g, 256, 0, c.stream, ca, cc, len, L->den[0])); }
+    if (L->table) DP_CUDA(dp_launch(k_lift_b2e, g, 256, 0, c.stream, (const u64 *)multiplicities->data, L->num[0], len));
     u32 k = 0;
     for (; k + 1 < L->nv && (len >> (k + 1)) > 1024; k++) {
         u64 half = len >> (k + 1);
-        int gg = dp_grid_for(half, 256, 8);
+        const bool init_lookup = k == 0 && !L->table;       // a lookup circuit's first numerators are all -1: L->num[0] holds none
         DpProfScope prof("k_logup_layer", half * 96);
-        if (k == 0 && !L->table) k_logup_layer<true><<<gg, 256, 0, c.stream>>>(nullptr, L->den[0], half, L->num[1], L->den[1]);
-        else k_logup_layer<false><<<gg, 256, 0, c.stream>>>(L->num[k], L->den[k], half, L->num[k + 1], L->den[k + 1]);
-        DP_LAUNCHED();
+        DP_CUDA(dp_launch(init_lookup ? k_logup_layer<true> : k_logup_layer<false>, dp_grid_for(half, 256, 8), 256, 0, c.stream,
+                          init_lookup ? nullptr : L->num[k], L->den[k], half, L->num[k + 1], L->den[k + 1]));
     }
     if (k + 1 < L->nv) {
         LayerPtrs lp; memset(&lp, 0, sizeof lp);
@@ -115,9 +113,8 @@ int dp_logup_build(dp_mle *const *columns, uint32_t n_columns, const dp_mle *mul
         DpProfScope prof("k_logup_tail", (len >> k) * 96);
         void *hp = nullptr;
         if (L->nv - 1 > k && dp_pinned_alloc(&hp, 128) == DP_OK) { L->h_out = (u64 *)hp; L->h_out[8] = 0; }
-        k_logup_tail<<<1, 256, 0, c.stream>>>(lp, k, L->nv, len, !L->table, L->h_out, 1); DP_LAUNCHED();
+        DP_CUDA(dp_launch(k_logup_tail, 1, 256, 0, c.stream, lp, k, L->nv, len, !L->table, L->h_out, 1));
     }
-    DP_CUDA(cudaGetLastError());
     if (!L->table) L->num[0] = nullptr;
     *out = L.release();
     return DP_OK;
@@ -136,7 +133,7 @@ int dp_logup_outputs(const dp_logup *L, uint64_t out[8]) {
     u32 last = L->nv - 1;
     DP_CHECK(L->num[last] != nullptr, DP_ERR_INVALID, "dp_logup_outputs: circuit too small");
     if (L->h_out) {   // stored by the tail kernel itself
-        if (dp_wait_flag(L->h_out + 8, 1, false, 0, 30.0) != 1) { DP_CUDA(dp_stream_sync(dp_ctx().stream)); DP_CHECK(L->h_out[8] == 1, DP_ERR_CUDA, "dp_logup_outputs: the tail kernel did not publish the outputs"); }
+        if (int e = dp_await(L->h_out + 8, 1, 30.0, "dp_logup_outputs: the tail kernel did not publish the outputs")) return e;
         memcpy(out, L->h_out, 64);
         return DP_OK;
     }
@@ -163,7 +160,6 @@ int dp_logup_layer_mles(const dp_logup *L, uint32_t layer_vars, dp_mle **out_vie
 
 int dp_logup_free(dp_logup *L) {
     if (!L) return DP_OK;
-    std::lock_guard<std::recursive_mutex> lk(dp_ctx().mu);
     if (dp_ctx().ready) {
         if (L->h_out && L->h_out[8] != 1) dp_stream_sync(dp_ctx().stream);   // the tail kernel still owns the pinned block
         dp_dev_free(L->block);
@@ -186,8 +182,7 @@ int dp_mle_linear_combination(dp_mle *const *mles, const uint64_t *coefs, uint32
     }
     MlePtr r;
     if (int e = dp_mle_alloc(len, true, r)) return e;
-    k_lincomb<<<dp_grid_for(len, 256, 8), 256, 0, dp_ctx().stream>>>(a, len, (gle *)r->data); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_lincomb, dp_grid_for(len, 256, 8), 256, 0, dp_ctx().stream, a, len, (gle *)r->data));
     *out = r.release();
     return DP_OK;
 }

@@ -40,8 +40,7 @@ static int dpk_eq_build(const gle *point, u32 nv, gle *out) {
     const u32 L = 10;
     if (nv <= L + 2) {
         u32 n = 1u << nv;
-        k_eq_small<<<(n + 127) / 128, 128, 0, c.stream>>>(pa, 0, nv, out); DP_LAUNCHED();
-        DP_CUDA(cudaGetLastError());
+        DP_CUDA(dp_launch(k_eq_small, (n + 127) / 128, 128, 0, c.stream, pa, 0, nv, out));
         return DP_OK;
     }
     u32 H = nv - L;
@@ -50,16 +49,15 @@ static int dpk_eq_build(const gle *point, u32 nv, gle *out) {
     DevPtr lo_owner(lo);
     if (int e = dp_dev_alloc((void **)&hi, sizeof(gle) << H)) return e;
     DevPtr hi_owner(hi);
-    k_eq_small<<<((1u << L) + 127) / 128, 128, 0, c.stream>>>(pa, 0, L, lo); DP_LAUNCHED();
-    if (H <= 14) { k_eq_small<<<((1u << H) + 127) / 128, 128, 0, c.stream>>>(pa, L, H, hi); DP_LAUNCHED(); }
+    DP_CUDA(dp_launch(k_eq_small, ((1u << L) + 127) / 128, 128, 0, c.stream, pa, 0, L, lo));
+    if (H <= 14) DP_CUDA(dp_launch(k_eq_small, ((1u << H) + 127) / 128, 128, 0, c.stream, pa, L, H, hi));
     else {  // recurse once for very large tables
         gle sub[32];
         for (u32 i = 0; i < H; i++) sub[i] = point[L + i];
         if (int e = dpk_eq_build(sub, H, hi)) return e;
     }
     u64 n = 1ULL << nv;
-    k_eq_expand<<<dp_grid_for(n, 256, 8), 256, 0, c.stream>>>(lo, hi, L, n, out); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_eq_expand, dp_grid_for(n, 256, 8), 256, 0, c.stream, lo, hi, L, n, out));
     return DP_OK;
 }
 
@@ -81,11 +79,7 @@ __global__ void k_fold_low(const void *__restrict__ src, u64 half, gle r, gle *_
 int dpk_fold_low(const void *src, bool src_ext, u64 len, gle r, gle *out) {
     DpCtx &c = dp_ctx();
     u64 half = len >> 1;
-    int g = dp_grid_for(half, 256, 8);
-    if (src_ext) k_fold_low<true><<<g, 256, 0, c.stream>>>(src, half, r, out);
-    else k_fold_low<false><<<g, 256, 0, c.stream>>>(src, half, r, out);
-    DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(src_ext ? k_fold_low<true> : k_fold_low<false>, dp_grid_for(half, 256, 8), 256, 0, c.stream, src, half, r, out));
     return DP_OK;
 }
 
@@ -173,9 +167,7 @@ static int dpk_fix_high(const void *src, bool src_ext, u64 len, const gle *point
     if (int e = dpk_eq_build(point, k, w)) return e;
     DpProfScope prof(S < 32 ? "k_fixhigh_dot" : "k_fixhigh_cols", len * (src_ext ? 16 : 8) + S * 16);
     if (S < 32) {
-        if (src_ext) k_fixhigh_dot<true><<<(unsigned)S, 256, 0, c.stream>>>(src, w, S, J, out);
-        else k_fixhigh_dot<false><<<(unsigned)S, 256, 0, c.stream>>>(src, w, S, J, out);
-        DP_LAUNCHED();
+        DP_CUDA(dp_launch(src_ext ? k_fixhigh_dot<true> : k_fixhigh_dot<false>, (unsigned)S, 256, 0, c.stream, src, w, S, J, out));
     } else {
         const int T = 128;
         u64 gx = (S + T - 1) / T;
@@ -187,13 +179,9 @@ static int dpk_fix_high(const void *src, bool src_ext, u64 len, const gle *point
         gle *part = out;
         DevPtr part_owner;
         if (ny > 1) { if (int e = dp_dev_alloc((void **)&part, sizeof(gle) * S * ny)) return e; part_owner.reset(part); }
-        dim3 grid((unsigned)gx, (unsigned)ny);
-        if (src_ext) k_fixhigh_cols<true><<<grid, T, 0, c.stream>>>(src, w, S, J, rows, part);
-        else k_fixhigh_cols<false><<<grid, T, 0, c.stream>>>(src, w, S, J, rows, part);
-        DP_LAUNCHED();
-        if (ny > 1) { k_sum_parts<<<(unsigned)((S + 255) / 256), 256, 0, c.stream>>>(part, S, (u32)ny, out); DP_LAUNCHED(); }
+        DP_CUDA(dp_launch(src_ext ? k_fixhigh_cols<true> : k_fixhigh_cols<false>, dim3((unsigned)gx, (unsigned)ny), T, 0, c.stream, src, w, S, J, rows, part));
+        if (ny > 1) DP_CUDA(dp_launch(k_sum_parts, (unsigned)((S + 255) / 256), 256, 0, c.stream, part, S, (u32)ny, out));
     }
-    DP_CUDA(cudaGetLastError());
     return DP_OK;
 }
 
@@ -222,8 +210,7 @@ int dp_mle_upload(const uint64_t *evals, uint64_t len, int is_ext, dp_mle **out)
     if (int e = dp_mle_alloc(len, is_ext != 0, m)) return e;
     DP_CUDA(cudaMemcpyAsync(m->data, evals, m->bytes(), cudaMemcpyHostToDevice, dp_ctx().stream));
     u64 n = len * (is_ext ? 2 : 1);
-    k_canonicalize<<<dp_grid_for(n, 256, 8), 256, 0, dp_ctx().stream>>>((u64 *)m->data, n); DP_LAUNCHED();
-    DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_canonicalize, dp_grid_for(n, 256, 8), 256, 0, dp_ctx().stream, (u64 *)m->data, n));
     *out = m.release();
     return DP_OK;
 }
@@ -264,7 +251,6 @@ void *dp_mle_device_ptr(const dp_mle *m) { return m ? m->data : nullptr; }
 
 int dp_mle_free(dp_mle *m) {
     if (!m) return DP_OK;
-    std::lock_guard<std::recursive_mutex> lk(dp_ctx().mu);
     if (m->owned && dp_ctx().ready) dp_dev_free(m->data);
     delete m;
     return DP_OK;
@@ -362,9 +348,8 @@ int dp_mle_evaluate_many(const dp_mle *const *mles, uint32_t n, const uint64_t *
         EvalArg a; memset(&a, 0, sizeof a);
         u32 cnt = std::min<u32>(16, n - base);
         for (u32 i = 0; i < cnt; i++) { a.src[i] = mles[base + i]->data; a.ext[i] = mles[base + i]->is_ext; }
-        k_eval_many<<<cnt, 256, 0, dp_ctx().stream>>>(a, w, J, res + base); DP_LAUNCHED();
+        DP_CUDA(dp_launch(k_eval_many, cnt, 256, 0, dp_ctx().stream, a, w, J, res + base));
     }
-    DP_CUDA(cudaGetLastError());
     DP_CUDA(cudaMemcpyAsync(hres, res, sizeof(gle) * n, cudaMemcpyDeviceToHost, dp_ctx().stream));
     DP_CUDA(dp_stream_sync(dp_ctx().stream));
     for (u32 i = 0; i < n; i++) { out[2 * i] = hres[i].c0; out[2 * i + 1] = hres[i].c1; }

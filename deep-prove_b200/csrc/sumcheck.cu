@@ -209,10 +209,10 @@ __device__ __forceinline__ void sc_body_split_dsel(const ScProd &pd, gle r, gle 
 // Called by ONE thread after a block barrier that follows the message stores of its block mates: its system-scope fence
 // orders those stores (observed through the barrier) before the flag.
 __device__ __forceinline__ void sc_signal(u64 seq, u64 *flag, u32 *done) {
-    if (gridDim.y == 1) { __threadfence_system(); *(volatile u64 *)flag = seq; return; }
+    if (gridDim.y == 1) { dp_publish(flag, seq); return; }
     __threadfence_system();
     u32 t = atomicAdd(done, 1u);
-    if (t == gridDim.y - 1) { *done = 0; __threadfence_system(); *(volatile u64 *)flag = seq; }
+    if (t == gridDim.y - 1) { *done = 0; dp_publish(flag, seq); }
 }
 
 // Block + grid reduction of the per-thread accumulators of one product (blockIdx.y) and hand-over to the host:
@@ -599,7 +599,7 @@ __device__ __forceinline__ void sc_res_rounds(ScResSmem &S, const u32 nm, const 
             }
             cl_sync();
             const u64 status = __ldcg(xctl);
-            if (status) { if (rank == 0 && threadIdx.x == 0 && status == 2) { __threadfence_system(); *flag = SC_TAIL_FAILED; } return; }   // uniform over the cluster
+            if (status) { if (rank == 0 && threadIdx.x == 0 && status == 2) dp_publish(flag, SC_TAIL_FAILED); return; }   // uniform over the cluster
             r = e_make(__ldcg(xctl + 1), __ldcg(xctl + 2));
             if (CHAIN && threadIdx.x == 0) schal[k - 1] = r;
         }
@@ -660,7 +660,7 @@ __device__ __forceinline__ void sc_res_rounds(ScResSmem &S, const u32 nm, const 
                 }
                 __syncthreads();
             }
-            if (threadIdx.x == 0 && (!fs || k == nr - 1)) { __threadfence_system(); *flag = seq; }   // device transcript: once, at the end
+            if (threadIdx.x == 0 && (!fs || k == nr - 1)) dp_publish(flag, seq);   // device transcript: once, at the end
         }
         if (k + 1 < nr) build_descs(true);                     // next round's descriptors while the host hashes
         // CTAs other than 0 run ahead to the next cluster barrier; xpart is not rewritten before it (the work phase follows it)
@@ -800,7 +800,7 @@ __device__ __noinline__ void lg_layer_end(const LgCfg *cfg, LgOut *out, ScResSme
         for (u32 i = threadIdx.x; i < TR::WORDS; i += blockDim.x) out->sponge[i] = S.sfs.sponge[i];
         if (threadIdx.x == 0) { st_e(&out->claim, L.claim); st_e(&out->alpha, L.alpha); st_e(&out->lambda, L.lambda); }
         __syncthreads();
-        if (threadIdx.x == 0) { __threadfence_system(); *(volatile u64 *)&out->flag = 1; }
+        if (threadIdx.x == 0) dp_publish(&out->flag, 1);
     }
 }
 
@@ -908,8 +908,7 @@ static int sc_glue(dp_sc *s, uint64_t *out_evals) {
 __global__ void k_tail_probe(volatile u64 *mailbox, volatile u64 *result, long long limit_cycles) {
     long long t0 = clock64(); u64 ok = 2;
     while (clock64() - t0 < limit_cycles) { if (mailbox[0] == 1) { ok = 1; break; } }
-    __threadfence_system();
-    result[0] = ok;
+    dp_publish(result, ok);
 }
 static bool sc_tail_supported() {
     static std::once_flag once; static bool supported = false;
@@ -920,9 +919,10 @@ static bool sc_tail_supported() {
         if (dp_pinned_alloc((void **)&pin, 128) != DP_OK) return;
         pin[0] = 0; pin[8] = 0;
         cudaStream_t st = dp_ctx().stream;
-        k_tail_probe<<<1, 1, 0, st>>>(pin, pin + 8, 100000000LL); dp_count_launch();
-        __atomic_store_n(&pin[0], (u64)1, __ATOMIC_RELEASE);          // reached at once unless the launch call itself waits for the kernel
-        if (dp_stream_sync(st) == cudaSuccess) supported = (pin[8] == 1);
+        if (dp_launch(k_tail_probe, 1, 1, 0, st, pin, pin + 8, 100000000LL) == cudaSuccess) {
+            __atomic_store_n(&pin[0], (u64)1, __ATOMIC_RELEASE);      // reached at once unless the launch call itself waits for the kernel
+            if (dp_stream_sync(st) == cudaSuccess) supported = (pin[8] == 1);
+        }
         dp_pinned_free(pin);
     });
     return supported;
@@ -956,21 +956,6 @@ struct ScResShape { u32 ncta, slots; };
 static ScResShape sc_res_shape(u64 work, u32 np) {
     u32 ncta = 1; while (ncta < SC_RES_MAXCTA && (u64)ncta * 512 < work) ncta <<= 1;
     return {ncta, std::max<u32>(ncta * (SC_THREADS / 32), np)};
-}
-// launch a resident kernel as one cluster of ncta CTAs on the context's stream, profiled as `name`
-template <class K, class... A>
-static int sc_res_launch(const char *name, u32 ncta, K kern, A... args) {
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(ncta); lc.blockDim = dim3(SC_THREADS); lc.dynamicSmemBytes = 0; lc.stream = dp_ctx().stream;
-    lc.attrs = at; lc.numAttrs = 1;
-    DpProfScope prof(name, 0);
-    const cudaError_t ce = cudaLaunchKernelEx(&lc, kern, args...);
-    DP_LAUNCHED();
-    DP_CUDA(ce);
-    DP_CUDA(cudaGetLastError());
-    return DP_OK;
 }
 
 // The previous round's challenge (prover.rs:655-669): none before round 0, one after it; recorded, and the first one refuses constant
@@ -1019,12 +1004,13 @@ static int sc_tail_launch(dp_sc *s, gle r, bool fold, const ScTailFs *fs, bool b
     if (!s->d_xctl && (e = dp_dev_alloc((void **)&s->d_xctl, 64))) return e;
     u32 dsel = s->products[0].n_idx;
     for (auto &pr : s->products) if (pr.n_idx != dsel) dsel = 0;
-    if ((e = sc_res_launch(!fs ? "k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)"
-                           : blake ? "k_sc_res(resident cluster rounds, BLAKE3 device transcript)"
-                                   : "k_sc_res(resident cluster rounds with the device transcript)",
-                           sh.ncta, k_sc_res_dsel[fs && blake][dsel], (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs, (volatile u64 *)s->h_flag,
-                           (volatile u64 *)s->h_chal, s->seq, s->d_xpart, s->d_xctl, fs ? s->h_fs : (ScTailFsOut *)nullptr)))
-        return e;
+    {
+        DpProfScope prof(!fs ? "k_sc_res(resident cluster rounds; time includes the host's Fiat-Shamir between rounds)"
+                         : blake ? "k_sc_res(resident cluster rounds, BLAKE3 device transcript)"
+                                 : "k_sc_res(resident cluster rounds with the device transcript)", 0);
+        DP_CUDA(dp_launch_cluster(k_sc_res_dsel[fs && blake][dsel], sh.ncta, SC_THREADS, dp_ctx().stream, (const ScTail *)s->h_tail, r, s->h_out, s->h_pairs,
+                                  s->h_flag, s->h_chal, s->seq, s->d_xpart, s->d_xctl, fs ? s->h_fs : nullptr));
+    }
     s->tail_active = true;
     return DP_OK;
 }
@@ -1164,11 +1150,12 @@ static int lg_run_layers_fs(dp_logup *const *circuits, uint32_t n_circuits, uint
     memcpy(cfg->label, lbl, sizeof lbl);
     cfg->fs = fs; cfg->fs.max_deg = 3;
     out->flag = 0;
-    if (int e = sc_res_launch(blake ? "k_logup_res(resident LogUp-GKR layers, BLAKE3 transcript)" : "k_logup_res(resident LogUp-GKR layers, device transcript)",
-                              sh.ncta, blake ? k_logup_res<TrB3> : k_logup_res<TrP2>, (const LgCfg *)cfg, out, (gle *)(scratch + off_part), (u64 *)scratch,
-                              (gle *)(scratch + off_point)))
-        return e;
-    if (dp_wait_flag(&out->flag, 1, false, 0, 8.0) != 1) { dp_stream_sync(dp_ctx().stream); DP_CHECK(out->flag == 1, DP_ERR_CUDA, std::string(fn) + ": the resident kernel did not finish"); }
+    {
+        DpProfScope prof(blake ? "k_logup_res(resident LogUp-GKR layers, BLAKE3 transcript)" : "k_logup_res(resident LogUp-GKR layers, device transcript)", 0);
+        DP_CUDA(dp_launch_cluster(blake ? k_logup_res<TrB3> : k_logup_res<TrP2>, sh.ncta, SC_THREADS, dp_ctx().stream, (const LgCfg *)cfg, out,
+                                  (gle *)(scratch + off_part), (u64 *)scratch, (gle *)(scratch + off_point)));
+    }
+    if (int e = dp_await(&out->flag, 1, 8.0, std::string(fn) + ": the resident kernel did not finish")) return e;
     size_t om = 0, oc = 0, oe = 0;
     for (u32 l = 0; l < nl; l++) {
         const u32 v = first_layer + l, per = cfg->num[l][0] ? 4 : 2;
@@ -1316,10 +1303,8 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
         // one small kernel per uniform degree keeps the instruction footprint low
         const auto kern = lean_mode >= 0 ? k_sc_lean_md[lean_mode][dsel - 2] : k_sc_round_dsel[dsel];
         const int block = lean_mode >= 0 ? SC_LEAN_BLOCK[lean_mode] : SC_THREADS;
-        kern<<<grid, block, 0, st>>>(descs_arg, s->h_descs[0], r, s->d_partials, s->d_counters, s->h_out, s->seq, s->h_flag, s->d_done);
-        DP_LAUNCHED();
+        DP_CUDA(dp_launch(kern, grid, block, 0, st, descs_arg, s->h_descs[0], r, s->d_partials, s->d_counters, s->h_out, s->seq, s->h_flag, s->d_done));
     }
-    DP_CUDA(cudaGetLastError());
     // commit the folds to the bookkeeping while the GPU works
     for (u32 i = 0; i < s->n_mles; i++) if (folds[i]) sc_commit_fold(s->mles[i], dst[i]);
     s->round += 1;
@@ -1329,17 +1314,15 @@ int dp_sc_round(dp_sc *s, const uint64_t *challenge, uint64_t *out_evals) {
         if (ok) {
             gle *d_pairs = (gle *)((char *)s->d_fin + sizeof(ScFin) * s->n_mles);
             DP_CUDA(cudaMemcpyAsync(s->d_fin, s->h_fin, sizeof(ScFin) * s->n_mles, cudaMemcpyHostToDevice, st));
-            k_sc_gather<<<(s->n_mles + 127) / 128, 128, 0, st>>>(s->d_fin, s->n_mles, d_pairs); DP_LAUNCHED();
+            DP_CUDA(dp_launch(k_sc_gather, (s->n_mles + 127) / 128, 128, 0, st, s->d_fin, s->n_mles, d_pairs));
             DP_CUDA(cudaMemcpyAsync(s->h_pairs, d_pairs, sizeof(gle) * 2 * s->n_mles, cudaMemcpyDeviceToHost, st));
             s->have_pairs = true;
         }
     }
     if (s->have_pairs) { DP_CUDA(dp_stream_sync(st)); s->round_in_flight = false; }      // last round: the gathered pairs follow the kernel
     else {
-        volatile u64 *f = s->h_flag;
-        const bool ok = dp_wait_flag(f, s->seq, false, 0, 2.0) == s->seq;
-        if (ok) s->round_in_flight = false;
-        if (!ok) { DP_CUDA(dp_stream_sync(st)); DP_CHECK(*f == s->seq, DP_ERR_CUDA, "dp_sc_round: kernel finished without signalling"); s->round_in_flight = false; }
+        if (int e = dp_await(s->h_flag, s->seq, 2.0, "dp_sc_round: kernel finished without signalling")) return e;
+        s->round_in_flight = false;
     }
     return sc_glue(s, out_evals);
 }
@@ -1364,7 +1347,6 @@ int dp_sc_finish(dp_sc *s, const uint64_t *last_challenge, uint64_t *out_final) 
 
 int dp_sc_destroy(dp_sc *s) {
     if (!s) return DP_OK;
-    std::lock_guard<std::recursive_mutex> lk(dp_ctx().mu);
     if (dp_ctx().ready) {
         if (s->tail_active && s->round < s->max_nv) { s->h_chal[0] = SC_TAIL_ABORT; dp_stream_sync(dp_ctx().stream); }   // release the waiting kernel
         sc_free_all(s);

@@ -145,9 +145,9 @@ int dp_wit_dense(const dp_mle *weights, const dp_mle *bias, const dp_mle *x, uin
     DP_CHECK(weights->len == (u64)nrows * ncols && bias->len == nrows && x->len == ncols, DP_ERR_INVALID, "dp_wit_dense: shape mismatch");
     MlePtr o; if (int e = dp_mle_alloc(nrows, false, o)) return e;
     DpProfScope prof("k_wit_dense", weights->bytes() + x->bytes() + 16ull * nrows);
-    if (ncols >= 2) k_wit_dense<<<(nrows * 32 + 255) / 256, 256, 0, dp_ctx().stream>>>((const u64 *)weights->data, (const u64 *)bias->data, (const u64 *)x->data, nrows, ncols, (u64 *)o->data);
-    else k_wit_dense_small<<<(nrows + 255) / 256, 256, 0, dp_ctx().stream>>>((const u64 *)weights->data, (const u64 *)bias->data, (const u64 *)x->data, nrows, ncols, (u64 *)o->data);
-    DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    const bool wide = ncols >= 2;
+    DP_CUDA(dp_launch(wide ? k_wit_dense : k_wit_dense_small, wide ? (nrows * 32 + 255) / 256 : (nrows + 255) / 256, 256, 0, dp_ctx().stream,
+                      (const u64 *)weights->data, (const u64 *)bias->data, (const u64 *)x->data, nrows, ncols, (u64 *)o->data));
     *out = o.release();
     return DP_OK;
 }
@@ -159,8 +159,8 @@ int dp_wit_matmul(const dp_mle *left, const dp_mle *right, const dp_mle *bias, u
     DP_CHECK(left->len == (u64)R * K && right->len == (u64)K * C && (!bias || bias->len == C), DP_ERR_INVALID, "Incompatible shape found for input matrix");   // matrix_mul.rs:277-283
     MlePtr o; if (int e = dp_mle_alloc((u64)R * C, false, o)) return e;
     DpProfScope prof("k_wit_matmul", left->bytes() + right->bytes() + 8ull * R * C);
-    k_wit_matmul<<<(unsigned)(((u64)R * C + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)left->data, (const u64 *)right->data, bias ? (const u64 *)bias->data : nullptr, R, K, C, transposed, (u64 *)o->data);
-    DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_wit_matmul, (unsigned)(((u64)R * C + 255) / 256), 256, 0, dp_ctx().stream, (const u64 *)left->data, (const u64 *)right->data,
+                      bias ? (const u64 *)bias->data : nullptr, R, K, C, transposed, (u64 *)o->data));
     *out = o.release();
     return DP_OK;
 }
@@ -186,9 +186,9 @@ int dp_wit_requant(dp_wit *w, const dp_mle *x, uint32_t shift, int64_t fixed_poi
     c.cin = (u64 *)own[0]->data; c.cout = (u64 *)own[1]->data;
     for (u32 j = 0; j < c.n_chunks; j++) c.chunk[j] = (u64 *)own[2 + j]->data;
     DpProfScope prof("k_wit_requant", x->bytes() * (1 + n_cols));
-    k_wit_requant<<<(unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)x->data, x->len, shift, (long long)fixed_point_multiplier, 1LL << intermediate_bit_size, c,
-                                                                               w->counts + w->off[clamp_table], w->size[clamp_table], w->counts + w->off[range_table], w->counts + w->off[w->n_tables]);
-    DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_wit_requant, (unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream, (const u64 *)x->data, x->len, shift, (long long)fixed_point_multiplier,
+                      1LL << intermediate_bit_size, c, w->counts + w->off[clamp_table], w->size[clamp_table], w->counts + w->off[range_table],
+                      w->counts + w->off[w->n_tables]));
     wit_hand_over(own, cols);
     return DP_OK;
 }
@@ -199,8 +199,8 @@ int dp_wit_relu(dp_wit *w, const dp_mle *x, uint32_t relu_table, dp_mle **out) {
     if (int e = wit_table(w, relu_table, 0, "dp_wit_relu")) return e;
     MlePtr o; if (int e = dp_mle_alloc(x->len, false, o)) return e;
     DpProfScope prof("k_wit_relu", x->bytes() * 2);
-    k_wit_relu<<<(unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)x->data, x->len, (u64 *)o->data, w->counts + w->off[relu_table], w->counts + w->off[w->n_tables]);
-    DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_wit_relu, (unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream, (const u64 *)x->data, x->len, (u64 *)o->data,
+                      w->counts + w->off[relu_table], w->counts + w->off[w->n_tables]));
     *out = o.release();
     return DP_OK;
 }
@@ -218,8 +218,8 @@ int dp_wit_pool(dp_wit *w, const dp_mle *x, uint32_t C, uint32_t H, uint32_t Wd,
     for (u32 k = 0; k < 4; k++) p.diff[k] = (u64 *)own[k]->data;
     p.out = (u64 *)own[4]->data;
     DpProfScope prof("k_wit_pool", x->bytes() + 5 * n * 8);
-    k_wit_pool<<<(unsigned)((n + 255) / 256), 256, 0, dp_ctx().stream>>>((const u64 *)x->data, C, H, Wd, p, w->counts + w->off[range_table], w->counts + w->off[w->n_tables]);
-    DP_LAUNCHED(); DP_CUDA(cudaGetLastError());
+    DP_CUDA(dp_launch(k_wit_pool, (unsigned)((n + 255) / 256), 256, 0, dp_ctx().stream, (const u64 *)x->data, C, H, Wd, p, w->counts + w->off[range_table],
+                      w->counts + w->off[w->n_tables]));
     wit_hand_over(own, cols);
     return DP_OK;
 }
@@ -234,7 +234,7 @@ int dp_wit_finish(dp_wit *w, dp_mle **mults, uint32_t *error_bits) {
     for (u32 t = 0; t < w->n_tables; t++) { if (int e = dp_mle_alloc(w->off[t + 1] - w->off[t], false, own[t])) return e; o.m[t] = (u64 *)own[t]->data; }
     for (u32 t = 0; t <= w->n_tables; t++) o.off[t] = w->off[t];
     cudaStream_t st = dp_ctx().stream;
-    k_wit_mult<<<(unsigned)((w->off[w->n_tables] + 255) / 256), 256, 0, st>>>(w->counts, o); DP_LAUNCHED();
+    DP_CUDA(dp_launch(k_wit_mult, (unsigned)((w->off[w->n_tables] + 255) / 256), 256, 0, st, w->counts, o));
     DP_CUDA(cudaMemcpyAsync(w->err_pinned, w->counts + w->off[w->n_tables], 4, cudaMemcpyDeviceToHost, st));
     DP_CUDA(dp_stream_sync(st));
     wit_hand_over(own, mults);
@@ -244,7 +244,6 @@ int dp_wit_finish(dp_wit *w, dp_mle **mults, uint32_t *error_bits) {
 
 int dp_wit_free(dp_wit *w) {
     if (!w) return DP_OK;
-    std::lock_guard<std::recursive_mutex> lk(dp_ctx().mu);
     if (dp_ctx().ready) { dp_dev_free(w->counts); dp_pinned_free(w->err_pinned); }
     delete w;
     return DP_OK;
