@@ -1,15 +1,12 @@
-// Basefold multilinear PCS on device: commit (K7 hypercube interpolation, K8 RS/NTT encode, K9 Poseidon2
-// Merkle), open / batch_open commit phase (K10 FRI fold, K11 coefficient-form sumcheck via the sumcheck
-// engine, K12 batch prelude) and query gathering (K13).
+// Basefold multilinear PCS on device: commit (K7 hypercube interpolation, K8 RS/NTT encode, K9 Merkle tree:
+// merkle.cu), open / batch_open commit phase (K10 FRI fold, K11 coefficient-form sumcheck via the sumcheck
+// engine, K12 batch prelude) and query gathering (K13: merkle.cu).
 // Reference: mpcs/src/basefold.rs:86-154,304-354,466-770; basefold/{commit_phase.rs,sumcheck.rs,
-// encoding/rs.rs,query_phase.rs:31-138,373-534}; util/{merkle_tree.rs,hash.rs,arithmetic.rs:120-132,
-// arithmetic/hypercube.rs}.
+// encoding/rs.rs,query_phase.rs:31-138,373-534}; util/{arithmetic.rs:120-132,arithmetic/hypercube.rs}.
 //
 // Data layout in HBM (per commitment of a 2^nu polynomial): bh_evals = bit-reversed evaluations (8 or
-// 16 B/elt), codeword = bit-reversed RS codeword of 2^(nu+1) elements, digests = Merkle levels >= 1
-// (4 x u64 each; level 0 of the reference is a zero-padded copy of the leaf pair -- hash_or_noop of <= 4
-// elements, poseidon_hash.rs:22-28 -- so it is recomputed from the leaves on demand, never stored).
-// Everything stays resident until the opening: roots and round messages are the only D2H traffic.
+// 16 B/elt), codeword = bit-reversed RS codeword of 2^(nu+1) elements, the Merkle tree over the codeword
+// (merkle.cuh).  Everything stays resident until the opening: roots and round messages are the only D2H traffic.
 //
 // Linear-algebra shortcuts (exact arithmetic, identical field elements):
 //  * interpolate_over_boolean_hypercube commutes with the bit-reversal permutation, so the coefficient
@@ -19,8 +16,7 @@
 //  * the zero-padded upper half makes the first DIF level a pure copy-and-scale (k_expand).
 #include "common.cuh"
 #include "powtab.cuh"
-#include "poseidon2.cuh"
-#include "blake3.cuh"
+#include "merkle.cuh"
 #include <algorithm>
 #include <atomic>
 #include <map>
@@ -50,24 +46,19 @@ static int pow_table_build(u64 base, const u64 **out) {
     *out = tab;
     return DP_OK;
 }
-struct BfGlobals { std::atomic<const u64 *> root_tab{nullptr}; std::atomic<bool> p2_ready{false}; };
-static BfGlobals g_bf;          // process-wide, read-only once built (shared by every host thread's context)
+static std::atomic<const u64 *> g_root_tab{nullptr};   // process-wide, read-only once built (shared by every host thread's context)
 static std::mutex g_bf_mu;
 static int bf_prepare() {
-    if (g_bf.p2_ready.load() && g_bf.root_tab.load()) return DP_OK;
+    if (g_root_tab.load()) return DP_OK;
     std::lock_guard<std::mutex> lk(g_bf_mu);
-    if (!g_bf.p2_ready.load()) {
-        DP_CUDA(p2_upload_constants((const u64 *)&DP_P2_EXT_RC[0][0][0], (const u64 *)DP_P2_INT_RC, (const u64 *)DP_P2_DIAG));
-        g_bf.p2_ready.store(true);
-    }
-    if (!g_bf.root_tab.load()) {
+    if (!g_root_tab.load()) {
         const u64 *tab = nullptr;
         if (int e = pow_table_build(GL_ROOT32, &tab)) return e;
-        g_bf.root_tab.store(tab);
+        g_root_tab.store(tab);
     }
     return DP_OK;
 }
-static PowTab root_tab() { return powtab_at(g_bf.root_tab.load()); }
+static PowTab root_tab() { return powtab_at(g_root_tab.load()); }
 int dp_root_powtab(PowTab *out) { if (int e = bf_prepare()) return e; *out = root_tab(); return DP_OK; }
 // shift^j tables, one per coset shift (i.e. per full_log - nv), built on first use and kept
 static int shift_powtab(u64 shift, PowTab *out) {
@@ -227,324 +218,6 @@ __global__ void __launch_bounds__(512) k_encode_small(const T *__restrict__ in, 
     for (u32 k = threadIdx.x; k < N; k += blockDim.x) cw[k] = sm[k];
 }
 
-// ---- K9 Merkle ----
-template <bool EXT> __device__ __forceinline__ void leaf_pair_digest(const void *leaves, u64 pair, u64 d[4]) {
-    if (EXT) { const gle *l = (const gle *)leaves + 2 * pair; gle a = ld_e(l), b = ld_e(l + 1); d[0] = a.c0; d[1] = a.c1; d[2] = b.c0; d[3] = b.c1; }
-    else { ulonglong2 v = ld_b2((const u64 *)leaves + 2 * pair); d[0] = v.x; d[1] = v.y; d[2] = 0; d[3] = 0; }
-}
-// the two children of hash i on the first level of a single-polynomial tree: leaf pairs 2i and 2i + 1
-template <bool EXT> __device__ __forceinline__ void mk_leaf_children(const void *leaves, u64 i, u64 x[4], u64 y[4]) {
-    leaf_pair_digest<EXT>(leaves, 2 * i, x); leaf_pair_digest<EXT>(leaves, 2 * i + 1, y);
-}
-// the two children of a hash on a higher level: the 8 digest words at `in`
-__device__ __forceinline__ void mk_node_children(const u64 *in, u64 x[4], u64 y[4]) {
-    ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(in), b = *reinterpret_cast<const ulonglong2 *>(in + 2);
-    ulonglong2 c = *reinterpret_cast<const ulonglong2 *>(in + 4), d = *reinterpret_cast<const ulonglong2 *>(in + 6);
-    x[0] = a.x; x[1] = a.y; x[2] = b.x; x[3] = b.y; y[0] = c.x; y[1] = c.y; y[2] = d.x; y[3] = d.y;
-}
-__device__ __forceinline__ void mk_store(u64 *out, u64 i, const u64 d[4]) {
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i) = make_ulonglong2(d[0], d[1]);
-    *reinterpret_cast<ulonglong2 *>(out + 4 * i + 2) = make_ulonglong2(d[2], d[3]);
-}
-template <bool EXT>
-__global__ void k_merkle_l1(const void *__restrict__ leaves, u64 n_out, u64 *__restrict__ out) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
-    for (; i < n_out; i += stride) {
-        u64 x[4], y[4], o[4];
-        mk_leaf_children<EXT>(leaves, i, x, y);
-        p2_compress(x, y, o);
-        mk_store(out, i, o);
-    }
-}
-__global__ void k_merkle_up(const u64 *__restrict__ in, u64 n_out, u64 *__restrict__ out) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
-    for (; i < n_out; i += stride) {
-        u64 x[4], y[4], o[4];
-        mk_node_children(in + 8 * i, x, y);
-        p2_compress(x, y, o);
-        mk_store(out, i, o);
-    }
-}
-template <bool EXT, bool FROM_LEAVES>
-__global__ void __launch_bounds__(64) k_merkle_mid(const void *__restrict__ src, u64 n_out, u64 *__restrict__ out) {
-    const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_out) return;
-    u64 x[4], y[4], o[4];
-    if (FROM_LEAVES) mk_leaf_children<EXT>(src, i, x, y);
-    else mk_node_children((const u64 *)src + 8 * i, x, y);
-    p2_compress_lat(x, y, o);
-    mk_store(out, i, o);
-}
-// 8 lanes per hash (poseidon2.cuh): word w of the leaf-pair digest `pair`
-template <bool EXT> __device__ __forceinline__ u64 leaf_pair_word(const void *leaves, u64 pair, int w) {
-    if (EXT) return ((const u64 *)leaves)[4 * pair + w];
-    return w < 2 ? ((const u64 *)leaves)[2 * pair + w] : 0ULL;
-}
-// Every remaining level of a tree whose current level has <= MK_SMALL hashes, in ONE launch.  Each block owns MK_SUB hashes of the
-// first level and walks that subtree up to its root with a block barrier per level; the last block to finish (ticket) folds the
-// <= 8 subtree roots.  A level with >= 64 hashes per block runs one THREAD per hash (latency-optimised permutation): the same
-// ~40 us per level as a single-warp chain costs anyway, at 1/5 of the issue slots of the lane-parallel form -- with dozens of proofs
-// in flight these small trees were as much GPU work as all the wide Merkle levels together (8 lanes x ~4.5 k instructions per
-// permutation against 12.8 k for one thread).  Levels with <= 32 hashes per block use 8 lanes per hash (shorter dependent chain,
-// ~27 us per level); 88 % of a 2048-hash tree's permutations are in the thread-per-hash levels.
-struct LvlOff { u64 off[36]; };
-static constexpr u32 MK_SUB = 256;
-static constexpr u64 MK_SMALL = 2048;
-// `rt`: optional hand-over of the root to the host with the kernel's own stores (mapped pinned memory): root words, then a system
-// fence, then the sequence number the host waits for -- no D2H copy node and no separate signal launch per tree.
-struct RootOut { u64 *root_host; u64 *flag; u64 seq; };
-__device__ __forceinline__ void mk_publish_root(const RootOut &rt, const u64 *root_dev) {   // one thread, after the barrier that follows the root's stores
-    if (!rt.root_host) return;
-#pragma unroll
-    for (int k = 0; k < 4; k++) rt.root_host[k] = __ldcg(root_dev + k);
-    if (rt.flag) dp_publish(rt.flag, rt.seq);
-}
-template <bool EXT, bool FROM_LEAVES>
-__global__ void __launch_bounds__(256) k_merkle_small(const void *src, u32 first_level, u32 lg, u64 nl_first, u64 *levels, LvlOff lo, u32 *ticket, RootOut rt, u32 sub_max, u32 tph_min) {
-    // (sub_max, tph_min) = (256, 64) with many proofs in flight (see above); (32, never) for a single proof: 64 blocks x one 8-lane pass
-    // per level is the shortest chain (~20 us per level against ~40 us for a thread per hash) and nothing else wants the issue slots
-    const int lane8 = threadIdx.x & 7; const u32 grp = threadIdx.x >> 3;
-    const u32 sub = (u32)(nl_first < sub_max ? nl_first : sub_max);
-    u32 l = first_level;
-    for (u32 k = 0; (sub >> k) >= 1 && l < lg; k++, l++) {
-        const u32 cnt = sub >> k; const u64 base = (u64)blockIdx.x * cnt;
-        u64 *out = levels + 4 * lo.off[l];
-        const u64 *prev = k == 0 ? (const u64 *)src : levels + 4 * lo.off[l - 1];
-        if (cnt >= tph_min) {                              // one thread per hash
-            if (threadIdx.x < cnt) {
-                const u64 i = base + threadIdx.x;
-                u64 x[4], y[4], o[4];
-                if (k == 0 && FROM_LEAVES) mk_leaf_children<EXT>(src, i, x, y);
-                else {   // the 8 words inline: through mk_node_children this kernel's instruction order changes
-                    const u64 *in = prev + 8 * i;
-                    ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(in), b = *reinterpret_cast<const ulonglong2 *>(in + 2);
-                    ulonglong2 c = *reinterpret_cast<const ulonglong2 *>(in + 4), d = *reinterpret_cast<const ulonglong2 *>(in + 6);
-                    x[0] = a.x; x[1] = a.y; x[2] = b.x; x[3] = b.y; y[0] = c.x; y[1] = c.y; y[2] = d.x; y[3] = d.y;
-                }
-                p2_compress_lat(x, y, o);
-                mk_store(out, i, o);
-            }
-        } else for (u32 b = 0; b < cnt; b += 32) {         // 8 lanes per hash, 32 hashes per pass
-            if (b + (grp & ~3u) >= cnt) continue;          // warp-uniform (a warp holds 4 lane groups): idle warps skip the permutations
-            const bool live = b + grp < cnt; const u64 i = base + b + grp;
-            u64 xw = 0, yw = 0;
-            if (live && lane8 < 4) {
-                if (k == 0 && FROM_LEAVES) { xw = leaf_pair_word<EXT>(src, 2 * i, lane8); yw = leaf_pair_word<EXT>(src, 2 * i + 1, lane8); }
-                else { const u64 *in = prev + 8 * i; xw = in[lane8]; yw = in[4 + lane8]; }
-            }
-            const u64 sres = p2x8_compress(xw, yw, lane8);
-            if (live && lane8 < 4) out[4 * i + (3 - lane8)] = sres;
-        }
-        __syncthreads();
-    }
-    if (gridDim.x == 1) { if (threadIdx.x == 0) mk_publish_root(rt, levels + 4 * lo.off[lg - 1]); return; }
-    __shared__ bool last;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) { const u32 t = atomicAdd(ticket, 1u); last = (t == gridDim.x - 1); if (last) *ticket = 0; }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    for (u32 cnt = gridDim.x >> 1; cnt >= 1 && l < lg; cnt >>= 1, l++) {
-        u64 *out = levels + 4 * lo.off[l];
-        const u64 *in0 = levels + 4 * lo.off[l - 1];
-        for (u32 b = 0; b < cnt; b += 32) {
-            if (b + (grp & ~3u) >= cnt) continue;
-            const u32 j = b + grp; const bool live = j < cnt;
-            u64 xw = 0, yw = 0;
-            if (live && lane8 < 4) { xw = __ldcg(in0 + 8 * (u64)j + lane8); yw = __ldcg(in0 + 8 * (u64)j + 4 + lane8); }   // written by other blocks / an earlier pass
-            const u64 sres = p2x8_compress(xw, yw, lane8);
-            if (live && lane8 < 4) out[4 * (u64)j + (3 - lane8)] = sres;
-        }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) mk_publish_root(rt, levels + 4 * lo.off[lg - 1]);
-}
-// process-wide pool of zeroed ticket counters (each k_merkle_small launch takes the next one and leaves it zero again)
-static std::atomic<u32 *> g_mk_tickets{nullptr}; static std::atomic<u32> g_mk_next{0}; static constexpr u32 MK_TICKETS = 4096;
-static int mk_ticket(u32 **out) {
-    u32 *tickets = g_mk_tickets.load();
-    if (!tickets) {
-        std::lock_guard<std::mutex> lk(g_bf_mu);
-        tickets = g_mk_tickets.load();
-        if (!tickets) {
-            DP_CUDA(cudaMalloc((void **)&tickets, sizeof(u32) * MK_TICKETS));
-            DP_CUDA(cudaMemset(tickets, 0, sizeof(u32) * MK_TICKETS));
-            g_mk_tickets.store(tickets);
-        }
-    }
-    *out = tickets + (g_mk_next.fetch_add(1, std::memory_order_relaxed) % MK_TICKETS);
-    return DP_OK;
-}
-
-// batch_commit leaf level (merkle_tree.rs:286-312, util/hash.rs:30-41): digest_i = compress(hash(values of all m polynomials at
-// index 2i), hash(... at 2i+1)), hash = hash_or_noop over the base-field limbs
-struct BatchPtrs { const void *p[64]; };
-template <bool EXT>
-__global__ void k_merkle_batch_l0(BatchPtrs bp, u32 m, u64 n_out, u64 *__restrict__ out) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_out) return;
-    u64 x[4], y[4], o[4];
-    const int n = EXT ? 2 * (int)m : (int)m;
-    auto ga = [&](int k) -> u64 { return EXT ? ((const u64 *)bp.p[k >> 1])[2 * (2 * i) + (k & 1)] : ((const u64 *)bp.p[k])[2 * i]; };
-    auto gb = [&](int k) -> u64 { return EXT ? ((const u64 *)bp.p[k >> 1])[2 * (2 * i + 1) + (k & 1)] : ((const u64 *)bp.p[k])[2 * i + 1]; };
-    p2_hash_or_noop(ga, n, x); p2_hash_or_noop(gb, n, y);
-    p2_compress(x, y, o);
-    mk_store(out, i, o);
-}
-template <bool EXT> __global__ void k_leafpair_root(const void *leaves, u64 *out) { u64 d[4]; leaf_pair_digest<EXT>(leaves, 0, d); for (int i = 0; i < 4; i++) out[i] = d[i]; }
-
-// ---- the `blake` MerkleHasher (mpcs/src/util/hash.rs:79-95): leaf pair -> BLAKE3(LE bytes), inner node -> BLAKE3(left || right) ----
-// Selected process-wide with dp_set_merkle_hasher (the reference selects at compile time: feature `blake`, mpcs/src/lib.rs:339-342).
-static std::atomic<int> g_hasher{0};          // 0 Poseidon2 (default), 1 BLAKE3
-static inline bool blake_on() { return g_hasher.load(std::memory_order_relaxed) == 1; }
-template <bool EXT> __device__ __forceinline__ void b3_leaf_pair(const void *leaves, u64 pair, u64 d[4]) {
-    u64 w[4];
-    if (EXT) { const gle *l = (const gle *)leaves + 2 * pair; gle a = ld_e(l), b = ld_e(l + 1); w[0] = a.c0; w[1] = a.c1; w[2] = b.c0; w[3] = b.c1; b3::hash_words(w, 4, d); }
-    else { ulonglong2 v = ld_b2((const u64 *)leaves + 2 * pair); w[0] = v.x; w[1] = v.y; b3::hash_words(w, 2, d); }
-}
-// level 0 (hash_two_leaves) of a single-polynomial tree: one digest per leaf pair.  Stored (unlike the Poseidon variant, whose
-// level 0 is a zero-padded copy of the pair and is recomputed on demand).
-template <bool EXT> __global__ void k_b3_leaves(const void *__restrict__ leaves, u64 n_out, u64 *__restrict__ out) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_out) return;
-    u64 d[4]; b3_leaf_pair<EXT>(leaves, i, d);
-    mk_store(out, i, d);
-}
-__global__ void k_b3_up(const u64 *__restrict__ in, u64 n_out, u64 *__restrict__ out) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_out) return;
-    u64 w[8];
-#pragma unroll
-    for (int k = 0; k < 8; k += 2) { ulonglong2 v = *reinterpret_cast<const ulonglong2 *>(in + 8 * i + k); w[k] = v.x; w[k + 1] = v.y; }
-    u64 d[4]; b3::hash_words(w, 8, d);
-    mk_store(out, i, d);
-}
-// every remaining level (<= 1024 hashes at the first one) in one single-block launch
-__global__ void __launch_bounds__(1024) k_b3_tail(const u64 *__restrict__ in0, u32 first_level, u32 lg, u64 nl_first, u64 *levels, LvlOff lo) {
-    const u64 *in = in0; u64 nl = nl_first;
-    for (u32 l = first_level; l < lg; l++, nl >>= 1) {
-        u64 *out = levels + 4 * lo.off[l];
-        if (threadIdx.x < nl) {
-            u64 w[8];
-#pragma unroll
-            for (int k = 0; k < 8; k++) w[k] = in[8 * (u64)threadIdx.x + k];
-            u64 d[4]; b3::hash_words(w, 8, d);
-#pragma unroll
-            for (int k = 0; k < 4; k++) out[4 * (u64)threadIdx.x + k] = d[k];
-        }
-        __syncthreads();
-        in = out;
-    }
-}
-
-// batch_commit leaf level under BLAKE3: digest_i = H( H(values of all polynomials at 2i) || H(... at 2i+1) )  (hash_two_leaves_batch_*)
-template <bool EXT>
-__global__ void k_b3_batch_l0(BatchPtrs bp, u32 m, u64 n_out, u64 *__restrict__ out) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_out) return;
-    const int n = EXT ? 2 * (int)m : (int)m;
-    auto ga = [&](int k) -> u64 { return EXT ? ((const u64 *)bp.p[k >> 1])[2 * (2 * i) + (k & 1)] : ((const u64 *)bp.p[k])[2 * i]; };
-    auto gb = [&](int k) -> u64 { return EXT ? ((const u64 *)bp.p[k >> 1])[2 * (2 * i + 1) + (k & 1)] : ((const u64 *)bp.p[k])[2 * i + 1]; };
-    u64 w[8], d[4];
-    b3::hash_stream(ga, n, w); b3::hash_stream(gb, n, w + 4);
-    b3::hash_words(w, 8, d);
-#pragma unroll
-    for (int k = 0; k < 4; k++) out[4 * i + k] = d[k];
-}
-
-// A Merkle tree over `n` leaves living in HBM: levels >= 1 packed back to back.
-struct DevTree {
-    const void *leaves = nullptr; bool ext = false; u64 n = 0; u32 lg = 0;
-    u64 *levels = nullptr;            // level l (1-based) at offset lvl_off[l] (in digests)
-    std::vector<u64> lvl_off;         // lvl_off[l] for l = 1..lg-1
-    u64 *root_dev = nullptr;          // 4 limbs
-    const u64 *level0 = nullptr;      // batch trees only: stored digests of the leaf pairs (single-polynomial trees recompute them)
-    bool own_levels = true;           // false for the per-polynomial views of a batch commitment
-    bool own_level0 = false;          // BLAKE3 trees of one polynomial store their leaf-pair digests (Poseidon2 recomputes them: zero-padded copies)
-};
-// `lvl0` != NULL: a batch tree -- the digests of the leaf pairs are given (k_merkle_batch_l0) instead of being packed from `leaves`
-// `rt` (optional): the launch that produces the root also stores it (and then rt->flag = rt->seq) in mapped host memory; *rt_done
-// tells the caller whether that happened (single-level and BLAKE3 trees do not: the caller copies the root as before)
-static int tree_build(DevTree &t, const void *leaves, bool ext, u64 n, const u64 *lvl0 = nullptr, const RootOut *rt = nullptr, bool *rt_done = nullptr) {
-    if (rt_done) *rt_done = false;
-    DpCtx &c = dp_ctx();
-    t.level0 = lvl0;
-    t.leaves = leaves; t.ext = ext; t.n = n; t.lg = 0; while ((1ULL << t.lg) < n) t.lg++;
-    DP_CHECK(t.lg >= 1, DP_ERR_INVALID, "merkle tree needs at least two leaves");
-    t.lvl_off.assign(t.lg + 1, 0);
-    u64 total = 0;
-    for (u32 l = 1; l < t.lg; l++) { t.lvl_off[l] = total; total += n >> (l + 1); }
-    if (int e = dp_dev_alloc((void **)&t.levels, sizeof(u64) * 4 * (total + 1))) return e;
-    LvlOff lo_all; memset(&lo_all, 0, sizeof lo_all);
-    for (u32 k = 1; k < t.lg && k < 36; k++) lo_all.off[k] = t.lvl_off[k];
-    if (blake_on()) {
-        const u64 *l0 = lvl0;
-        if (!l0) {
-            u64 *own = nullptr; if (int e = dp_dev_alloc((void **)&own, sizeof(u64) * 4 * (n >> 1))) return e;
-            DpProfScope prof("k_b3_leaves(blake3)", n * (ext ? 16 : 8) + (n >> 1) * 32);
-            t.level0 = l0 = own; t.own_level0 = true;
-            DP_CUDA(dp_launch(ext ? k_b3_leaves<true> : k_b3_leaves<false>, (unsigned)(((n >> 1) + 255) / 256), 256, 0, c.stream, leaves, n >> 1, own));
-        }
-        if (t.lg == 1) { t.root_dev = const_cast<u64 *>(l0); return DP_OK; }
-        for (u32 l = 1; l < t.lg; l++) {
-            const u64 nl = n >> (l + 1);
-            const u64 *in = l == 1 ? l0 : t.levels + 4 * t.lvl_off[l - 1];
-            if (nl <= 1024 && t.lg < 36) { DpProfScope prof("k_b3_tail(blake3)", nl * 96); DP_CUDA(dp_launch(k_b3_tail, 1, 1024, 0, c.stream, in, l, t.lg, nl, t.levels, lo_all)); break; }
-            DpProfScope prof("k_b3_up(blake3)", nl * 96);
-            DP_CUDA(dp_launch(k_b3_up, (unsigned)((nl + 255) / 256), 256, 0, c.stream, in, nl, t.levels + 4 * t.lvl_off[l]));
-        }
-        t.root_dev = t.levels + 4 * t.lvl_off[t.lg - 1];
-        return DP_OK;
-    }
-    if (t.lg == 1 && lvl0) { t.root_dev = const_cast<u64 *>(lvl0); }
-    else if (t.lg == 1) {
-        DP_CUDA(dp_launch(ext ? k_leafpair_root<true> : k_leafpair_root<false>, 1, 1, 0, c.stream, leaves, t.levels));
-        t.root_dev = t.levels;
-    } else {
-        for (u32 l = 1; l < t.lg; l++) {
-            const u64 nl = n >> (l + 1);
-            const bool from_leaves = (l == 1 && !lvl0);
-            const u64 in_bytes = from_leaves ? nl * (ext ? 64 : 32) : nl * 64;
-            const void *src = l == 1 ? (lvl0 ? (const void *)lvl0 : leaves) : (const void *)(t.levels + 4 * t.lvl_off[l - 1]);
-            u64 *out = t.levels + 4 * t.lvl_off[l];
-            if (nl <= MK_SMALL && t.lg < 36) {   // this and every remaining level in one launch
-                DpProfScope prof("k_merkle_small(poseidon2 compress, all remaining levels)", in_bytes + (2 * nl - 1) * 32 * 2, 2 * (2 * nl - 1));
-                const bool many = dp_wait_mode() == DP_WAIT_BLOCK;     // the throughput configuration (many proofs in flight)
-                const u32 sub_max = many ? MK_SUB : 32, tph_min = many ? 64 : 0xFFFFFFFFu;
-                const unsigned g = (unsigned)((nl + sub_max - 1) / sub_max);
-                u32 *ticket = nullptr; if (int e = mk_ticket(&ticket)) return e;
-                RootOut ro = rt ? *rt : RootOut{nullptr, nullptr, 0};
-                const auto kern = from_leaves ? (ext ? k_merkle_small<true, true> : k_merkle_small<false, true>) : k_merkle_small<false, false>;
-                DP_CUDA(dp_launch(kern, g, 256, 0, c.stream, src, l, t.lg, nl, t.levels, lo_all, ticket, ro, sub_max, tph_min));
-                if (rt && rt_done) *rt_done = true;
-                break;
-            }
-            if (nl <= 32768) {
-                // Mid levels (2 k .. 32 k hashes): one thread per hash in 64-thread blocks, with the latency-optimised permutation.  A
-                // level is one wave of single-warp chains either way (46 us per compress per warp, 39 us in this formulation vs 52 us
-                // for the 8-lanes-per-hash kernel used before), but it now holds 1/8 of the thread slots and issues ~1/5 of the
-                // instructions, so the mid levels of many proofs' trees overlap instead of queueing behind each other.
-                DpProfScope prof("k_merkle_mid(poseidon2 compress, thread per hash)", in_bytes + nl * 32, 2 * nl);
-                const auto kern = from_leaves ? (ext ? k_merkle_mid<true, true> : k_merkle_mid<false, true>) : k_merkle_mid<false, false>;
-                DP_CUDA(dp_launch(kern, (unsigned)((nl + 63) / 64), 64, 0, c.stream, src, nl, out));
-                continue;
-            }
-            DpProfScope prof("k_merkle(poseidon2 compress)", in_bytes + nl * 32, 2 * nl);
-            const unsigned mgrid = (unsigned)std::min<u64>((nl + 127) / 128, 1u << 22);
-            // one hash per thread, many SHORT blocks (no persistent grid-stride blocks): with 16 proofs in flight the block
-            // scheduler can interleave other streams' latency-critical single-block kernels every few microseconds
-            if (from_leaves) DP_CUDA(dp_launch(ext ? k_merkle_l1<true> : k_merkle_l1<false>, mgrid, 128, 0, c.stream, src, nl, out));
-            else DP_CUDA(dp_launch(k_merkle_up, mgrid, 128, 0, c.stream, (const u64 *)src, nl, out));
-        }
-        t.root_dev = t.levels + 4 * t.lvl_off[t.lg - 1];
-    }
-    return DP_OK;
-}
-static void tree_free(DevTree &t) { if (t.own_levels) dp_dev_free(t.levels); t.levels = nullptr; if (t.own_level0) { dp_dev_free(const_cast<u64 *>(t.level0)); t.level0 = nullptr; t.own_level0 = false; } t.leaves = nullptr; }
-// the same tree, owning nothing (the per-polynomial views of a batch commitment)
-static DevTree tree_view(const DevTree &t) { DevTree v = t; v.own_levels = false; v.own_level0 = false; return v; }
-
 // ---- K10 FRI fold (commit_phase.rs:511-526, rs.rs:377-410, arithmetic.rs:120-132) ----
 // out[i] = y0 + (r - x0) * (y1 - y0) * w,  x0 = w_{2^(level+1)}^{rev(i, level)} * gamma_lvl,  w = -1/(2 x0)
 // (`n` outputs starting at global index `off`: a rank of a sharded opening folds its own contiguous slice)
@@ -618,69 +291,28 @@ __global__ void k_lift(const u64 *__restrict__ src, gle *__restrict__ out, u64 n
     for (; i < n; i += stride) st_e(out + i, e_from_base(src[i]));
 }
 
-// ---- K13 query gather: per (query, tree): [p0.c0 p0.c1 p1.c0 p1.c1][path digests x (lg-1)] ----
-// Sharded trees (logG > 0): `leaves` / `levels` are this rank's subtree over 2^lg_local leaves, `top_*` the replicated tree over the G
-// subtree roots; a query whose leaf pair another rank owns leaves its row untouched (zero) -- the ranks' rows are summed afterwards.
-struct QTree { const void *leaves; const u64 *levels; const u64 *level0; u64 off[34]; u32 lg; u32 ext; u32 shift; u32 logG;
-               u32 lg_local; u32 rank; const u64 *top_lvl0; const u64 *top_levels; u64 top_off[9]; };
-__global__ void k_query_gather(const QTree *__restrict__ trees, u32 n_trees, const u64 *__restrict__ xs, const u64 *__restrict__ out_off, u64 per_query, u64 *__restrict__ out) {
-    u32 q = blockIdx.x, ti = blockIdx.y;
-    QTree t = trees[ti];
-    u64 idx = xs[q] >> t.shift;
-    u64 p0 = (idx | 1) - 1;
-    u64 *o = out + (u64)q * per_query + out_off[ti];
-    u64 owner = 0;
-    if (t.logG) { owner = p0 >> t.lg_local; if (owner != t.rank) return; p0 &= (1ULL << t.lg_local) - 1; }
-    const u32 lgl = t.logG ? t.lg_local : t.lg;
-    for (u32 k = threadIdx.x; k < t.lg; k += blockDim.x) {
-        if (k == 0) {
-            if (t.ext) { gle a = ld_e((const gle *)t.leaves + p0), b = ld_e((const gle *)t.leaves + p0 + 1); o[0] = a.c0; o[1] = a.c1; o[2] = b.c0; o[3] = b.c1; }
-            else { const u64 *l = (const u64 *)t.leaves; o[0] = l[p0]; o[1] = 0; o[2] = l[p0 + 1]; o[3] = 0; }
-        }
-        if (k + 1 < t.lg && k + 1 >= lgl) {   // above this rank's subtree: the sibling subtree root, then the replicated top levels
-            const u32 kk = k + 1 - lgl;
-            const u64 *sd = kk == 0 ? t.top_lvl0 + 4 * (owner ^ 1) : t.top_levels + 4 * (t.top_off[kk] + ((owner >> kk) ^ 1));
-            u64 *d = o + 4 + 4 * k;
-            d[0] = sd[0]; d[1] = sd[1]; d[2] = sd[2]; d[3] = sd[3];
-        } else
-        if (k + 1 < t.lg) {   // path entry k = inner[k][(p0 >> (k+1)) ^ 1]
-            u64 node = (p0 >> (k + 1)) ^ 1;
-            u64 *d = o + 4 + 4 * k;
-            if (k == 0 && t.level0) { const u64 *sd = t.level0 + 4 * node; d[0] = sd[0]; d[1] = sd[1]; d[2] = sd[2]; d[3] = sd[3]; }
-            else if (k == 0) {
-                if (t.ext) { const gle *l = (const gle *)t.leaves + 2 * node; gle a = ld_e(l), b = ld_e(l + 1); d[0] = a.c0; d[1] = a.c1; d[2] = b.c0; d[3] = b.c1; }
-                else { const u64 *l = (const u64 *)t.leaves + 2 * node; d[0] = l[0]; d[1] = l[1]; d[2] = 0; d[3] = 0; }
-            } else {
-                const u64 *s = t.levels + 4 * (t.off[k] + node);
-                d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
-            }
-        }
-    }
-}
-
 // =====================================================================================================
 struct dp_pcs_comm {
     u32 num_vars = 0, full_log = 0; bool is_base = true, trivial = false;
     void *bh_evals = nullptr;   // bit-reversed evals (raw evals when trivial)
     void *codeword = nullptr;   // bit-reversed codeword (== bh_evals when trivial)
     u64 cw_len = 0;
-    DevTree tree;
-    u64 root[4] = {0, 0, 0, 0};
-    std::vector<dp_pcs_comm *> parts;   // batch_commit: one (encode-only) commitment per polynomial; their trees are views of `tree`
-    u64 *level0 = nullptr;              // batch_commit: digests of the leaf pairs
+    DevTree tree;                       // over `codeword`; empty for the parts of a batch commitment
+    const DevTree *batch_tree = nullptr;   // a part of a batch commitment: the batch's tree, over all the parts' codewords
+    uint64_t root[4] = {0, 0, 0, 0};
+    std::vector<dp_pcs_comm *> parts;   // batch_commit: one (encode-only) commitment per polynomial
     // dp_pcs_commit_shard: `codeword` / `bh_evals` / `tree` are this rank's contiguous slice (cw_len = local length); `top` is the
     // replicated tree over the world's subtree roots (dp_pcs_comm_set_shard_roots), `root` the global root once it is set
-    u32 shard_rank = 0, shard_log = 0; DevTree top; u64 *top_lvl0 = nullptr; u64 local_root[4] = {0, 0, 0, 0};
+    u32 shard_rank = 0, shard_log = 0; DevTree top; uint64_t local_root[4] = {0, 0, 0, 0};
 };
 
-struct OpenRound { gle *oracle = nullptr; u64 len = 0; DevTree tree; DevTree top; u64 *top_lvl0 = nullptr; };
+struct OpenRound { gle *oracle = nullptr; DevTree tree; DevTree top; };   // tree over `oracle`; top: sharded openings
 struct dp_pcs_open {
     u32 num_vars = 0, full_log = 0, num_rounds = 0, round = 0;
     std::vector<const dp_pcs_comm *> comms; std::vector<gle> coeffs; bool batch = false;
     gle *oracle0 = nullptr; u64 n0 = 0;        // running oracle of the current round (E)
     bool oracle0_owned = true;
     std::vector<OpenRound> rounds;             // trees over the folded oracles (pre-addition copies)
-    gle *pending = nullptr; u64 pending_len = 0;  // folded oracle awaiting its tree/addition
     dp_mle *eq = nullptr, *evals = nullptr; bool evals_owned = false;
     dp_sc *sc = nullptr;
     gle final_msg[1 << BF_BASECODE_LOG]; bool have_final = false;
@@ -743,34 +375,13 @@ static int encode_tiled(const void *evals, void *bh_evals, void *codeword, u32 n
 
 extern "C" {
 
-int dp_set_merkle_hasher(int kind) {
-    DP_CHECK(kind == 0 || kind == 1, DP_ERR_INVALID, "dp_set_merkle_hasher: 0 = Poseidon2 (PoseidonHasher), 1 = BLAKE3 (BlakeHasher)");
-    g_hasher.store(kind);
-    return DP_OK;
-}
-int dp_get_merkle_hasher(void) { return g_hasher.load(); }
-
-int dp_poseidon2_init(const uint64_t *ext_rc /*2x4x8*/, const uint64_t *int_rc /*22*/, const uint64_t *diag /*8*/) {
-    DP_REQUIRE_CTX();
-    DP_CHECK(ext_rc && int_rc && diag, DP_ERR_INVALID, "dp_poseidon2_init: null argument");
-    u64 a[64], b[22], d[8];
-    for (int i = 0; i < 64; i++) a[i] = gl_canon(ext_rc[i]);
-    for (int i = 0; i < 22; i++) b[i] = gl_canon(int_rc[i]);
-    for (int i = 0; i < 8; i++) d[i] = gl_canon(diag[i]);
-    DP_CUDA(dp_stream_sync(dp_ctx().stream));
-    DP_CUDA(p2_upload_constants(a, b, d));
-    g_bf.p2_ready.store(true);
-    return DP_OK;
-}
-
-// enqueue every kernel of one commitment on the context's CURRENT stream; the root lands in `root_pinned`
-static int commit_enqueue(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **out, u64 *root_pinned, bool with_tree = true) {
+// enqueue every kernel of one commitment on the context's CURRENT stream; the root lands in `root_pinned` (null: no tree, a batch part)
+static int commit_enqueue(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **out, u64 *root_pinned) {
     u32 nv = poly->num_vars();
     DP_CHECK(nv <= full_log, DP_ERR_INVALID, "PolynomialTooLarge");                 // basefold.rs:97-99
     DP_CHECK(nv >= 1, DP_ERR_INVALID, "dp_pcs_commit: need at least one variable");
     if (int e = bf_prepare()) return e;
     DpCtx &c = dp_ctx();
-    if (!root_pinned && with_tree) return dp_fail(DP_ERR_INVALID, "commit_enqueue: no root buffer");
     CommPtr cm(new dp_pcs_comm());
     cm->num_vars = nv; cm->full_log = full_log; cm->is_base = !poly->is_ext;
     size_t esz = poly->is_ext ? 16 : 8;
@@ -790,10 +401,10 @@ static int commit_enqueue(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **o
         else rc = poly->is_ext ? encode_tiled<gle>(poly->data, cm->bh_evals, cm->codeword, nv, shift, 0, 0) : encode_tiled<u64>(poly->data, cm->bh_evals, cm->codeword, nv, shift, 0, 0);
         if (rc) return rc;
     }
-    if (with_tree) {
-        RootOut ro{root_pinned, nullptr, 0}; bool published = false;
-        if (int e = tree_build(cm->tree, cm->codeword, poly->is_ext, cm->cw_len, nullptr, &ro, &published)) return e;   // K9
-        if (!published) DP_CUDA(cudaMemcpyAsync(root_pinned, cm->tree.root_dev, 32, cudaMemcpyDeviceToHost, c.stream));
+    if (root_pinned) {
+        RootOut ro{root_pinned, nullptr, 0};
+        if (int e = tree_build(cm->tree, {cm->codeword}, poly->is_ext, cm->cw_len, &ro)) return e;   // K9
+        if (!cm->tree.root_published) DP_CUDA(cudaMemcpyAsync(root_pinned, cm->tree.root_dev, 32, cudaMemcpyDeviceToHost, c.stream));
     }
     *out = cm.release();
     return DP_OK;
@@ -811,22 +422,6 @@ int dp_pcs_commit(const dp_mle *poly, uint32_t full_log, dp_pcs_comm **out) {
 }
 
 
-// the replicated tree over the world's subtree roots: level "0" = the G roots, then log G levels of compress
-static int top_tree_build(DevTree &top, u64 **top_lvl0, const uint64_t *roots, u32 logG, u64 out_root[4]) {
-    DpCtx &c = dp_ctx();
-    const u64 G = 1ULL << logG;
-    if (int e = dp_dev_alloc((void **)top_lvl0, 32 * G)) return e;
-    u64 *pin = nullptr;
-    if (int e = dp_pinned_alloc((void **)&pin, 32 * G + 64)) return e;
-    for (u64 k = 0; k < 4 * G; k++) pin[k] = gl_canon(roots[k]);
-    DP_CUDA(cudaMemcpyAsync(*top_lvl0, pin, 32 * G, cudaMemcpyHostToDevice, c.stream));
-    int rc = tree_build(top, nullptr, false, 2 * G, *top_lvl0);
-    if (rc == DP_OK) rc = dp_d2h(out_root, top.root_dev, 32, c.stream);
-    else cudaStreamSynchronize(c.stream);
-    dp_pinned_free(pin);
-    return rc;
-}
-
 // Basefold::commit of ONE polynomial sharded over `world` = 2^k ranks (one process per GPU).  Every rank passes the whole
 // polynomial (resident on its GPU) and keeps only its contiguous slice of the bit-reversed evaluations, of the bit-reversed
 // codeword and the Merkle subtree over that slice; (*out)'s root is the SUBTREE root until dp_pcs_comm_set_shard_roots has been
@@ -836,7 +431,7 @@ int dp_pcs_commit_shard(const dp_mle *poly, uint32_t full_log, uint32_t rank, ui
     DP_CHECK(poly && out, DP_ERR_INVALID, "dp_pcs_commit_shard: null argument");
     u32 logG = 0; while ((1u << logG) < world) logG++;
     DP_CHECK(world >= 2 && (1u << logG) == world && rank < world, DP_ERR_INVALID, "dp_pcs_commit_shard: world must be a power of two >= 2 and rank < world");
-    DP_CHECK(!blake_on(), DP_ERR_UNSUPPORTED, "dp_pcs_commit_shard: Poseidon2 trees only");
+    DP_CHECK(!mk_blake3(), DP_ERR_UNSUPPORTED, "dp_pcs_commit_shard: Poseidon2 trees only");
     const u32 nv = poly->num_vars();
     DP_CHECK(nv <= full_log, DP_ERR_INVALID, "PolynomialTooLarge");
     DP_CHECK(logG <= 6 && nv >= BF_BASECODE_LOG + 4 && nv > logG + 11, DP_ERR_INVALID, "dp_pcs_commit_shard: polynomial too small to shard over this many ranks");
@@ -851,7 +446,7 @@ int dp_pcs_commit_shard(const dp_mle *poly, uint32_t full_log, uint32_t rank, ui
     const u64 shift = coset_shift(full_log, nv);
     if (int e = poly->is_ext ? encode_tiled<gle>(poly->data, cm->bh_evals, cm->codeword, nv, shift, logG, rank)
                              : encode_tiled<u64>(poly->data, cm->bh_evals, cm->codeword, nv, shift, logG, rank)) return e;
-    if (int e = tree_build(cm->tree, cm->codeword, poly->is_ext, cm->cw_len)) return e;
+    if (int e = tree_build(cm->tree, {cm->codeword}, poly->is_ext, cm->cw_len)) return e;
     if (int e = dp_d2h(cm->local_root, cm->tree.root_dev, 32, c.stream)) return e;
     memcpy(cm->root, cm->local_root, 32);
     *out = cm.release();
@@ -862,9 +457,9 @@ int dp_pcs_commit_shard(const dp_mle *poly, uint32_t full_log, uint32_t rank, ui
 int dp_pcs_comm_set_shard_roots(dp_pcs_comm *cm, const uint64_t *roots, uint64_t out_root[4]) {
     DP_REQUIRE_CTX();
     DP_CHECK(cm && roots && cm->shard_log > 0, DP_ERR_INVALID, "dp_pcs_comm_set_shard_roots: not a sharded commitment");
-    DP_CHECK(!cm->top_lvl0, DP_ERR_STATE, "dp_pcs_comm_set_shard_roots: roots already set");
+    DP_CHECK(!cm->top.level0, DP_ERR_STATE, "dp_pcs_comm_set_shard_roots: roots already set");
     for (int k = 0; k < 4; k++) DP_CHECK(gl_canon(roots[4 * cm->shard_rank + k]) == cm->local_root[k], DP_ERR_INVALID, "dp_pcs_comm_set_shard_roots: this rank's entry is not its own subtree root");
-    if (int e = top_tree_build(cm->top, &cm->top_lvl0, roots, cm->shard_log, cm->root)) return e;
+    if (int e = top_tree_build(cm->top, roots, cm->shard_log, cm->root)) return e;
     if (out_root) memcpy(out_root, cm->root, 32);
     return DP_OK;
 }
@@ -882,43 +477,30 @@ int dp_pcs_comm_shard_info(const dp_pcs_comm *cm, uint32_t *rank, uint32_t *worl
 int dp_pcs_batch_commit(const dp_mle *const *polys, uint32_t n, uint32_t full_log, dp_pcs_comm **out) {
     DP_REQUIRE_CTX();
     DP_CHECK(polys && out && n >= 1, DP_ERR_INVALID, "cannot batch commit to zero polynomials");      // basefold.rs:367-371
-    DP_CHECK(n <= 64, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: at most 64 polynomials per batch");
+    DP_CHECK(n <= MK_BATCH_MAX, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: at most 64 polynomials per batch");
     for (u32 i = 0; i < n; i++) DP_CHECK(polys[i] && polys[i]->len == polys[0]->len && polys[i]->is_ext == polys[0]->is_ext, DP_ERR_INVALID,
                                          "cannot batch commit to polynomials with different number of variables");   // :379-386
+    if (mk_blake3()) DP_CHECK((polys[0]->is_ext ? 2 * n : n) <= MK_B3_BATCH_WORDS, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: BLAKE3 batch leaves are limited to one 1024-byte chunk (128 base / 64 extension polynomials)");
     if (int e = bf_prepare()) return e;
     DpCtx &c = dp_ctx();
     CommPtr b(new dp_pcs_comm());
     b->num_vars = polys[0]->num_vars(); b->full_log = full_log; b->is_base = !polys[0]->is_ext;
-    if (n == 1) {   // merkelize with one value vector is the plain tree (merkle_tree.rs:274-285): the batch is a view of an ordinary commitment
-        dp_pcs_comm *part = nullptr; u64 *pin1 = nullptr;
-        if (int e = dp_pinned_alloc((void **)&pin1, 32)) return e;
-        int rc = commit_enqueue(polys[0], full_log, &part, pin1, true);
-        if (rc == DP_OK) { dp_stream_sync(c.stream); memcpy(part->root, pin1, 32); memcpy(b->root, pin1, 32); }
-        dp_pinned_free(pin1);
-        if (rc != DP_OK) return rc;
-        b->parts.push_back(part); b->trivial = part->trivial; b->cw_len = part->cw_len;
-        b->tree = tree_view(part->tree);
+    if (n == 1) {   // merkelize with one value vector is the plain tree (merkle_tree.rs:274-285): the batch holds an ordinary commitment
+        dp_pcs_comm *part = nullptr;
+        if (int e = dp_pcs_commit(polys[0], full_log, &part)) return e;
+        b->parts.push_back(part); b->trivial = part->trivial; b->cw_len = part->cw_len; memcpy(b->root, part->root, 32);
         *out = b.release();
         return DP_OK;
     }
-    BatchPtrs bp; memset(&bp, 0, sizeof bp);
+    std::vector<const void *> codewords;
     for (u32 i = 0; i < n; i++) {
         dp_pcs_comm *part = nullptr;
-        if (int e = commit_enqueue(polys[i], full_log, &part, nullptr, false)) return e;
-        b->parts.push_back(part); bp.p[i] = part->codeword;
+        if (int e = commit_enqueue(polys[i], full_log, &part, nullptr)) return e;
+        b->parts.push_back(part); codewords.push_back(part->codeword);
     }
     b->trivial = b->parts[0]->trivial; b->cw_len = b->parts[0]->cw_len;
-    u64 N = b->cw_len, n0 = N >> 1;
-    if (int e = dp_dev_alloc((void **)&b->level0, 32 * n0)) return e;
-    {
-        DpProfScope prof("k_merkle_batch_l0(poseidon2 sponge + compress)", (u64)n * N * (b->is_base ? 8 : 16) + 32 * n0);
-        const bool blake = blake_on();
-        if (blake) DP_CHECK((b->is_base ? n : 2 * n) <= 128, DP_ERR_UNSUPPORTED, "dp_pcs_batch_commit: BLAKE3 batch leaves are limited to one 1024-byte chunk (128 base / 64 extension polynomials)");
-        const auto kern = blake ? (b->is_base ? k_b3_batch_l0<false> : k_b3_batch_l0<true>) : (b->is_base ? k_merkle_batch_l0<false> : k_merkle_batch_l0<true>);
-        DP_CUDA(dp_launch(kern, (unsigned)((n0 + 127) / 128), 128, 0, c.stream, bp, n, n0, b->level0));
-    }
-    if (int e = tree_build(b->tree, b->parts[0]->codeword, !b->is_base, N, b->level0)) return e;
-    for (auto *part : b->parts) { part->tree = tree_view(b->tree); part->tree.leaves = part->codeword; }   // own leaves, the batch tree's digests
+    if (int e = tree_build(b->tree, codewords, !b->is_base, b->cw_len)) return e;
+    for (auto *part : b->parts) part->batch_tree = &b->tree;
     if (int e = dp_d2h(b->root, b->tree.root_dev, 32, c.stream)) return e;
     for (auto *part : b->parts) memcpy(part->root, b->root, 32);
     *out = b.release();
@@ -1004,7 +586,7 @@ int dp_pcs_comm_bh_evals(const dp_pcs_comm *cm, dp_mle **view) {
 }
 int dp_pcs_comm_free(dp_pcs_comm *cm) {
     if (!cm) return DP_OK;
-    if (dp_ctx().ready) { tree_free(cm->tree); if (!cm->trivial) dp_dev_free(cm->codeword); dp_dev_free(cm->bh_evals); dp_dev_free(cm->level0); tree_free(cm->top); dp_dev_free(cm->top_lvl0); }
+    if (dp_ctx().ready) { tree_free(cm->tree); if (!cm->trivial) dp_dev_free(cm->codeword); dp_dev_free(cm->bh_evals); tree_free(cm->top); }
     for (auto *p : cm->parts) dp_pcs_comm_free(p);
     delete cm;
     return DP_OK;
@@ -1035,7 +617,7 @@ int dp_pcs_open_begin(const dp_pcs_comm *const *comms, const uint64_t *coeffs, u
     }
     DP_CHECK(num_vars > BF_BASECODE_LOG, DP_ERR_INVALID, "minimum number of variables must be greater than basecode_msg_size_log");
     for (u32 i = 0; i < n_comms; i++) DP_CHECK(comms[i]->shard_log == 0 || (n_comms == 1 && !coeffs), DP_ERR_UNSUPPORTED, "dp_pcs_open_begin: a sharded commitment is opened alone");
-    if (cm->shard_log) DP_CHECK(cm->num_vars == num_vars && cm->top_lvl0, DP_ERR_STATE, "dp_pcs_open_begin: sharded commitment needs num_vars variables and its shard roots set");
+    if (cm->shard_log) DP_CHECK(cm->num_vars == num_vars && cm->top.level0, DP_ERR_STATE, "dp_pcs_open_begin: sharded commitment needs num_vars variables and its shard roots set");
     else if (!coeffs) DP_CHECK(n_comms == 1 && cm->num_vars == num_vars, DP_ERR_INVALID, "dp_pcs_open_begin: single open needs one commitment of num_vars variables");
 
     OpenPtr o(new dp_pcs_open());
@@ -1146,11 +728,11 @@ int dp_pcs_open_round(dp_pcs_open *o, const uint64_t challenge[2], uint64_t next
     if (i + 1 < o->num_rounds) {
         if (int e = dp_sc_round(o->sc, ch, ev3)) return e;       // sum_check_challenge_round
         msg_to_coeffs(ev3, next_msg);
-        OpenRound rd; rd.oracle = folded; rd.len = len >> 1;
+        OpenRound rd; rd.oracle = folded;
         if (!o->h_root) { void *hp = nullptr; if (int e = dp_pinned_alloc(&hp, 128)) return e; o->h_root = (u64 *)hp; o->h_root[8] = 0; o->root_seq = 0; }
-        RootOut ro{o->h_root, o->h_root + 8, ++o->root_seq}; bool published = false;
-        if (int e = tree_build(rd.tree, folded, true, rd.len, nullptr, &ro, &published)) return e;   // compute_inner_ext
-        if (published) {   // the tree's last launch stores the root and then the sequence number in mapped memory
+        RootOut ro{o->h_root, o->h_root + 8, ++o->root_seq};
+        if (int e = tree_build(rd.tree, {folded}, true, len >> 1, &ro)) return e;   // compute_inner_ext
+        if (rd.tree.root_published) {   // the tree's last launch stores the root and then the sequence number in mapped memory
             if (int e = dp_await(o->h_root + 8, o->root_seq, 30.0, "dp_pcs_open_round: tree kernel finished without publishing its root")) return e;
             memcpy(root, o->h_root, 32);
         } else if (int e = dp_d2h(root, rd.tree.root_dev, 32, c.stream)) return e;
@@ -1182,11 +764,8 @@ int dp_pcs_open_set_shard_roots(dp_pcs_open *o, const uint64_t *roots, uint64_t 
     DP_REQUIRE_CTX();
     DP_CHECK(o && roots && out_root && o->shard_log > 0 && !o->rounds.empty(), DP_ERR_INVALID, "dp_pcs_open_set_shard_roots: not a sharded opening with a pending round");
     OpenRound &rd = o->rounds.back();
-    DP_CHECK(!rd.top_lvl0, DP_ERR_STATE, "dp_pcs_open_set_shard_roots: roots of this round already set");
-    u64 rt[4];
-    if (int e = top_tree_build(rd.top, &rd.top_lvl0, roots, o->shard_log, rt)) return e;
-    for (int k = 0; k < 4; k++) out_root[k] = rt[k];
-    return DP_OK;
+    DP_CHECK(!rd.top.level0, DP_ERR_STATE, "dp_pcs_open_set_shard_roots: roots of this round already set");
+    return top_tree_build(rd.top, roots, o->shard_log, out_root);
 }
 
 // (sharded opening: this rank's (2^7 >> log world) entries of the BIT-REVERSED final message -- concatenate by rank, then un-bit-reverse)
@@ -1197,14 +776,16 @@ int dp_pcs_open_final_message(dp_pcs_open *o, uint64_t *out) {
     return DP_OK;
 }
 
-// u64 words one query occupies in dp_pcs_open_query's output
-uint64_t dp_pcs_open_query_words(const dp_pcs_open *o) {
-    if (!o) return 0;
-    u64 w = 0;
-    for (auto cm : o->comms) { u32 lg = 0; while ((1ULL << lg) < cm->cw_len) lg++; lg += o->shard_log; w += 4 + 4 * (u64)(lg - 1); }
-    for (auto &rd : o->rounds) w += 4 + 4 * (u64)(rd.tree.lg + o->shard_log - 1);
-    return w;
+// the trees a query opens, in the order of dp_pcs_open_query's output: every commitment's, then every round oracle's
+static std::vector<MkPath> query_paths(const dp_pcs_open *o) {
+    std::vector<MkPath> paths;   // a commitment of nv variables is queried at x >> (num_vars - nv)
+    for (auto cm : o->comms) paths.push_back({cm->batch_tree ? cm->batch_tree : &cm->tree, cm->codeword, o->num_vars - cm->num_vars, &cm->top});
+    for (size_t i = 0; i < o->rounds.size(); i++) paths.push_back({&o->rounds[i].tree, o->rounds[i].oracle, (u32)i + 1, &o->rounds[i].top});
+    return paths;
 }
+
+// u64 words one query occupies in dp_pcs_open_query's output
+uint64_t dp_pcs_open_query_words(const dp_pcs_open *o) { return o ? mk_query_words(query_paths(o), o->shard_log) : 0; }
 
 // K13 (query_phase.rs:373-474): for every x index, for every commitment then every round oracle:
 // [p0.c0 p0.c1 p1.c0 p1.c1] + Merkle path without leaf sibling or root (merkle_tree.rs:139-152).
@@ -1212,36 +793,8 @@ int dp_pcs_open_query(dp_pcs_open *o, const uint64_t *x_indices, uint32_t n, uin
     DP_REQUIRE_CTX();
     DP_CHECK(o && x_indices && out && n > 0, DP_ERR_INVALID, "dp_pcs_open_query: null argument");
     DP_CHECK(o->have_final, DP_ERR_STATE, "dp_pcs_open_query: commit phase not finished");
-    DpCtx &c = dp_ctx();
-    u32 nt = (u32)(o->comms.size() + o->rounds.size());
-    std::vector<QTree> qt(nt); std::vector<u64> off(nt);
-    u32 lgN = o->num_vars + BF_RATE_LOG; u64 w = 0; u32 k = 0;
-    const u32 logG = o->shard_log;
-    auto fill = [&](const DevTree &t, u32 shift, const DevTree *top, const u64 *top_lvl0) {
-        QTree &q = qt[k]; memset(&q, 0, sizeof q);
-        q.leaves = t.leaves; q.levels = t.levels; q.level0 = t.level0; q.lg = t.lg + logG; q.ext = t.ext; q.shift = shift;
-        for (u32 l = 1; l < t.lg && l < 34; l++) q.off[l] = t.lvl_off[l];
-        q.logG = logG; q.lg_local = t.lg; q.rank = o->shard_rank;
-        if (logG) { q.top_lvl0 = top_lvl0; q.top_levels = top->levels; for (u32 l = 1; l < top->lg && l < 9; l++) q.top_off[l] = top->lvl_off[l]; }
-        off[k] = w; w += 4 + 4 * (u64)(q.lg - 1); k++;
-    };
-    if (logG) for (auto &rd : o->rounds) DP_CHECK(rd.top_lvl0 != nullptr, DP_ERR_STATE, "dp_pcs_open_query: a round's shard roots were never set");
-    for (auto cm : o->comms) fill(cm->tree, lgN - (cm->tree.lg + logG), &cm->top, cm->top_lvl0);
-    for (size_t i = 0; i < o->rounds.size(); i++) fill(o->rounds[i].tree, (u32)i + 1, &o->rounds[i].top, o->rounds[i].top_lvl0);
-    QTree *dq = nullptr; u64 *doff = nullptr, *dx = nullptr, *dout = nullptr;
-    if (int e = dp_dev_alloc((void **)&dq, sizeof(QTree) * nt)) return e;
-    if (int e = dp_dev_alloc((void **)&doff, 8 * nt)) return e;
-    if (int e = dp_dev_alloc((void **)&dx, 8 * (size_t)n)) return e;
-    if (int e = dp_dev_alloc((void **)&dout, 8 * w * n)) return e;
-    DP_CUDA(cudaMemcpyAsync(dq, qt.data(), sizeof(QTree) * nt, cudaMemcpyHostToDevice, c.stream));
-    DP_CUDA(cudaMemcpyAsync(doff, off.data(), 8 * nt, cudaMemcpyHostToDevice, c.stream));
-    DP_CUDA(cudaMemcpyAsync(dx, x_indices, 8 * (size_t)n, cudaMemcpyHostToDevice, c.stream));
-    DP_CUDA(dp_stream_sync(c.stream));   // qt/off are stack-owned host buffers
-    if (logG) DP_CUDA(cudaMemsetAsync(dout, 0, 8 * w * n, c.stream));   // rows of queries other ranks own stay zero
-    DP_CUDA(dp_launch(k_query_gather, dim3(n, nt), 32, 0, c.stream, dq, nt, dx, doff, w, dout));
-    if (int e = dp_d2h(out, dout, 8 * w * n, c.stream)) return e;
-    dp_dev_free(dq); dp_dev_free(doff); dp_dev_free(dx); dp_dev_free(dout);
-    return DP_OK;
+    if (o->shard_log) for (auto &rd : o->rounds) DP_CHECK(rd.top.level0 != nullptr, DP_ERR_STATE, "dp_pcs_open_query: a round's shard roots were never set");
+    return mk_query_gather(query_paths(o), o->shard_log, o->shard_rank, x_indices, n, out);
 }
 
 int dp_pcs_open_free(dp_pcs_open *o) {
@@ -1249,7 +802,7 @@ int dp_pcs_open_free(dp_pcs_open *o) {
     if (dp_ctx().ready) {
         if (o->sc) dp_sc_destroy(o->sc);
         bool oracle_in_rounds = false;
-        for (auto &rd : o->rounds) { if (rd.oracle == o->oracle0) oracle_in_rounds = true; tree_free(rd.tree); dp_dev_free(rd.oracle); tree_free(rd.top); dp_dev_free(rd.top_lvl0); }
+        for (auto &rd : o->rounds) { if (rd.oracle == o->oracle0) oracle_in_rounds = true; tree_free(rd.tree); dp_dev_free(rd.oracle); tree_free(rd.top); }
         if (!oracle_in_rounds) dp_dev_free(o->oracle0);
         dp_dev_free(o->scratch_sum_evals);
     }

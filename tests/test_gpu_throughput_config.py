@@ -2,7 +2,7 @@
 (dp_set_wait_mode(1)) -- against the oracle.
 
 Several device paths exist only in that configuration:
-  * the Merkle builder changes shape with the wait mode (deep-prove_b200/csrc/basefold.cu tree_build, :470-550): in block mode
+  * the Merkle builder changes shape with the wait mode (deep-prove_b200/csrc/merkle.cu tree_build, :233-306): in block mode
     k_merkle_small takes 256-hash subtrees, hashes every level of >= 64 hashes one thread per hash (p2_compress_lat) and folds
     up to 8 subtree roots in the last block; in spin mode it takes 32-hash subtrees, always uses the 8-lane p2x8_compress and
     folds up to 64.  `tree_plan` below restates tree_build rule by rule; CASES is a matrix of commitments that, run through the
@@ -17,9 +17,9 @@ Several device paths exist only in that configuration:
   * the concurrent prover pool (host/capi.cpp): per-worker contexts, staggered starts from a pool's second call, the shared
     Merkle ticket ring.  dph_zkml_prove_concurrent_all returns every job's proof, and each must equal the oracle's.
 
-The ticket ring (basefold.cu:365-379, MK_TICKETS = 4096 counters handed out round robin) is safe only while fewer than 4096
+The ticket ring (merkle.cu:150-163, :280, MK_TICKETS = 4096 counters handed out round robin) is safe only while fewer than 4096
 k_merkle_small launches lie between one launch's enqueue and its completion.  A proof commits about 38 witness trees per
-dp_pcs_commit_many call (basefold.cu:964) and its thread waits for the call to finish, so 48 proofs in flight hold at most
+dp_pcs_commit_many call (basefold.cu:556) and its thread waits for the call to finish, so 48 proofs in flight hold at most
 about 48 x 38 = 1.8 k launches: a margin of about 2x.  Nothing here tries to provoke a collision.
 """
 import ctypes as C
@@ -40,22 +40,20 @@ import test_zkml as Z
 P = O.P
 SPIN, BLOCK = 0, 1
 
-# ---- constants of basefold.cu the model depends on -----------------------------------------------------------------------------
-MK_SMALL = 2048             # :293  k_merkle_small builds every remaining level once a level has <= this many hashes
-MK_SUB = 256                # :292  hashes of the first level per block in block mode
-SPIN_SUB = 32               # :519  ... and in spin mode
-TPH_MIN = 64                # :519  block mode: a block level with >= this many hashes runs one thread per hash
-MK_MID_MAX = 32768          # :528  k_merkle_mid up to this many hashes per level, k_merkle_l1 / k_merkle_up above
-B3_TAIL_MAX = 1024          # :496  BLAKE3: k_b3_tail takes every remaining level once a level has <= this many hashes
-LVL_MAX = 36                # :291  LvlOff holds 36 level offsets: the one-launch kernels need lg < 36
+# ---- constants of merkle.cu the model depends on ------------------------------------------------------------------------------
+MK_SMALL = 2048             # :81   k_merkle_small builds every remaining level once a level has <= this many hashes
+MK_SUB = 256                # :80   hashes of the first level per block in block mode
+SPIN_SUB = 32               # :278  ... and in spin mode
+TPH_MIN = 64                # :278  block mode: a block level with >= this many hashes runs one thread per hash
+MK_MID_MAX = 32768          # :287  k_merkle_mid up to this many hashes per level, k_merkle_wide above
+B3_TAIL_MAX = 1024          # :269  BLAKE3: k_b3_tail takes every remaining level once a level has <= this many hashes
 BF_BASECODE_LOG = 7         # nv <= 7: a trivial commitment, the tree is over the evaluations themselves
 BF_RATE_LOG = 1             # otherwise the tree is over the 2^(nv + 1) codeword entries
 
 PROFILE_NAME = {            # DpProfScope names of tree_build's kernels (k_leafpair_root has none)
     "k_merkle_small": "k_merkle_small(poseidon2 compress, all remaining levels)",
     "k_merkle_mid": "k_merkle_mid(poseidon2 compress, thread per hash)",
-    "k_merkle_l1": "k_merkle(poseidon2 compress)",
-    "k_merkle_up": "k_merkle(poseidon2 compress)",
+    "k_merkle_wide": "k_merkle(poseidon2 compress)",
     "k_leafpair_root": None,
     "k_b3_leaves": "k_b3_leaves(blake3)",
     "k_b3_up": "k_b3_up(blake3)",
@@ -65,48 +63,48 @@ TREE_PROFILE_NAMES = {v for v in PROFILE_NAME.values() if v}
 
 
 def tree_plan(n_leaves, ext, batch_lvl0, hasher, wait_mode):
-    """tree_build (basefold.cu:470-550) for a tree over n_leaves leaves.  batch_lvl0: the leaf-pair digests are given (a batch
+    """tree_build (merkle.cu:233-306) for a tree over n_leaves leaves.  batch_lvl0: the leaf-pair digests are given (a batch
     commitment); hasher: "poseidon2" or "blake3".  Returns dict(lg, launches: Counter of kernel names, route: [(kernel, level,
     hashes, source)], small: None or the k_merkle_small launch as dict(first_level, hashes, source, ext, grid, sub,
     levels: [(hashes per block, "thread" | "8 lanes")], fold: [hashes per fold level]))."""
     lg = 0
-    while (1 << lg) < n_leaves:                                                    # :474
+    while (1 << lg) < n_leaves:                                                    # :235
         lg += 1
-    assert lg >= 1                                                                 # :475
+    assert lg >= 1                                                                 # :236
     launches, route, small = Counter(), [], None
-    if hasher == "blake3":                                                         # :482-503
-        if not batch_lvl0:                                                         # :484-491  level 0 is stored
+    if hasher == "blake3":                                                         # :268-273
+        if not batch_lvl0:                                                         # :241-254  level 0 is stored
             launches["k_b3_leaves"] += 1
-        for l in range(1, lg):                                                     # :493
+        for l in range(1, lg):                                                     # :263
             nl = n_leaves >> (l + 1)
-            if nl <= B3_TAIL_MAX and lg < LVL_MAX:                                 # :496
+            if nl <= B3_TAIL_MAX:                                                  # :269
                 launches["k_b3_tail"] += 1
                 route.append(("k_b3_tail", l, nl, None))
                 break
-            launches["k_b3_up"] += 1                                               # :497-498
+            launches["k_b3_up"] += 1                                               # :270-271
             route.append(("k_b3_up", l, nl, None))
         return dict(lg=lg, launches=launches, route=route, small=None)
-    if lg == 1:                                                                    # :504-508
+    if lg == 1:                                                                    # :258-262
         if not batch_lvl0:
             launches["k_leafpair_root"] += 1
             route.append(("k_leafpair_root", 0, 1, "leaves"))
         return dict(lg=lg, launches=launches, route=route, small=None)
-    for l in range(1, lg):                                                         # :510
+    for l in range(1, lg):                                                         # :263
         nl = n_leaves >> (l + 1)
-        source = ("batch level 0" if batch_lvl0 else "leaves") if l == 1 else "digests"     # :512, :514
-        if nl <= MK_SMALL and lg < LVL_MAX:                                        # :516
-            many = wait_mode == BLOCK                                              # :518-519
+        source = ("batch level 0" if batch_lvl0 else "leaves") if l == 1 else "digests"     # :265-266
+        if nl <= MK_SMALL:                                                         # :275
+            many = wait_mode == BLOCK                                              # :277-278
             sub_max, tph_min = (MK_SUB, TPH_MIN) if many else (SPIN_SUB, None)
-            grid = (nl + sub_max - 1) // sub_max                                   # :520
-            sub = min(nl, sub_max)                                                 # kernel :308
+            grid = (nl + sub_max - 1) // sub_max                                   # :279
+            sub = min(nl, sub_max)                                                 # kernel :93
             levels, lv, k = [], l, 0
-            while (sub >> k) >= 1 and lv < lg:                                     # kernel :310-340
+            while (sub >> k) >= 1 and lv < lg:                                     # kernel :95-125
                 cnt = sub >> k
                 levels.append((cnt, "thread" if tph_min is not None and cnt >= tph_min else "8 lanes"))
                 k += 1
                 lv += 1
             fold = []
-            if grid > 1:                                                           # kernel :341, :349-361
+            if grid > 1:                                                           # kernel :126, :134-146
                 cnt = grid >> 1
                 while cnt >= 1 and lv < lg:
                     fold.append(cnt)
@@ -118,7 +116,7 @@ def tree_plan(n_leaves, ext, batch_lvl0, hasher, wait_mode):
             launches["k_merkle_small"] += 1
             route.append(("k_merkle_small", l, nl, source))
             break
-        kernel = "k_merkle_mid" if nl <= MK_MID_MAX else ("k_merkle_l1" if source == "leaves" else "k_merkle_up")   # :528, :542-543
+        kernel = "k_merkle_mid" if nl <= MK_MID_MAX else "k_merkle_wide"         # :287, :301
         launches[kernel] += 1
         route.append((kernel, l, nl, source))
     return dict(lg=lg, launches=launches, route=route, small=small)
@@ -159,15 +157,15 @@ CASES = [
     Case("p2_nv13_base", "poseidon2", 13, False, 1, 13),                 # mid from Base leaves, then small from digests
     Case("p2_nv14_ext", "poseidon2", 14, True, 1, 15),                   # mid from Ext leaves, mid from digests
     Case("p2_nv16_base", "poseidon2", 16, False, 1, 16),                 # four mid levels, then small from digests
-    Case("p2_nv17_base", "poseidon2", 17, False, 1, 17),                 # k_merkle_l1 Base
-    Case("p2_nv17_ext", "poseidon2", 17, True, 1, 17),                   # k_merkle_l1 Ext
-    Case("p2_nv18_base", "poseidon2", 18, False, 1, 19),                 # k_merkle_l1, then k_merkle_up
+    Case("p2_nv17_base", "poseidon2", 17, False, 1, 17),                 # k_merkle_wide from Base leaves
+    Case("p2_nv17_ext", "poseidon2", 17, True, 1, 17),                   # k_merkle_wide from Ext leaves
+    Case("p2_nv18_base", "poseidon2", 18, False, 1, 19),                 # k_merkle_wide from leaves, then from digests
     # Poseidon2, batch commitments (the leaf-pair digests of all polynomials are level 0)
     Case("p2_batch_lg1_nv1", "poseidon2", 1, False, 2, 8),               # the root is the level-0 digest
     Case("p2_batch_nv9_base", "poseidon2", 9, False, 3, 10),             # small from level 0 (block: threads, grid 1)
     Case("p2_batch_nv10_ext", "poseidon2", 10, True, 2, 10),             # small from level 0, grid > 1 in both modes
     Case("p2_batch_nv13_base", "poseidon2", 13, False, 3, 13),           # mid from level 0
-    Case("p2_batch_nv17_base", "poseidon2", 17, False, 2, 17),           # k_merkle_up from level 0
+    Case("p2_batch_nv17_base", "poseidon2", 17, False, 2, 17),           # k_merkle_wide from level 0
     # BLAKE3
     Case("b3_lg1_nv1_base", "blake3", 1, False, 1, 8),
     Case("b3_nv10_ext", "blake3", 10, True, 1, 10),                      # tail only
@@ -199,10 +197,8 @@ def cells_of(case, wait_mode):
     for kernel, _, _, source in plan["route"]:
         if kernel == "k_merkle_mid":
             cells.add(("k_merkle_mid", source, field) if source == "leaves" else ("k_merkle_mid", source))
-        elif kernel == "k_merkle_l1":
-            cells.add(("k_merkle_l1", field))
-        elif kernel == "k_merkle_up":
-            cells.add(("k_merkle_up", source))
+        elif kernel == "k_merkle_wide":
+            cells.add(("k_merkle_wide", source, field) if source == "leaves" else ("k_merkle_wide", source))
     s = plan["small"]
     if s is not None:
         grid = "grid 1" if s["grid"] == 1 else "grid > 1"
@@ -222,7 +218,7 @@ COMMON_CELLS = (
     | {("k_merkle_small", "leaves", f, g) for f in ("Base", "Ext") for g in ("grid 1", "grid > 1")}
     | {("k_merkle_small", "digests"), ("k_merkle_small", "batch level 0"), ("k_merkle_small", "8 lanes")}
     | {("k_merkle_mid", "leaves", f) for f in ("Base", "Ext")} | {("k_merkle_mid", "digests"), ("k_merkle_mid", "batch level 0")}
-    | {("k_merkle_l1", f) for f in ("Base", "Ext")} | {("k_merkle_up", "digests"), ("k_merkle_up", "batch level 0")}
+    | {("k_merkle_wide", "leaves", f) for f in ("Base", "Ext")} | {("k_merkle_wide", "digests"), ("k_merkle_wide", "batch level 0")}
     | {("blake3", c) for c in ("lg == 1", "tail only", "k_b3_up then tail", "batch level 0")}
 )
 REQUIRED_CELLS = {
@@ -248,7 +244,7 @@ def test_case_matrix_reaches_every_tree_cell(wait_mode):
 
 
 def test_model_restates_known_routes():
-    """routes derived by hand from basefold.cu"""
+    """routes derived by hand from merkle.cu"""
     # nv = 12 (Base): 2^13 leaves, level 1 has 2048 hashes -> k_merkle_small from the leaves
     r = tree_plan(1 << 13, False, False, "poseidon2", BLOCK)
     s = r["small"]
@@ -263,9 +259,9 @@ def test_model_restates_known_routes():
         r = tree_plan(1 << 17, False, False, "poseidon2", mode)
         assert [k for k, *_ in r["route"]] == ["k_merkle_mid"] * 4 + ["k_merkle_small"]
         assert r["small"]["source"] == "digests" and r["small"]["hashes"] == 2048
-    # nv = 17 starts with k_merkle_l1, then k_merkle_mid (32768 hashes is still a mid level)
+    # nv = 17 starts with k_merkle_wide, then k_merkle_mid (32768 hashes is still a mid level)
     r = tree_plan(1 << 18, True, False, "poseidon2", BLOCK)
-    assert r["route"][0][:3] == ("k_merkle_l1", 1, 1 << 16) and r["route"][1][:3] == ("k_merkle_mid", 2, 1 << 15)
+    assert r["route"][0][:3] == ("k_merkle_wide", 1, 1 << 16) and r["route"][1][:3] == ("k_merkle_mid", 2, 1 << 15)
     # a tree of two leaves: no launch from a batch level 0, k_leafpair_root otherwise; BLAKE3 stores its level 0
     assert not tree_plan(2, False, True, "poseidon2", BLOCK)["launches"]
     assert dict(tree_plan(2, False, False, "poseidon2", SPIN)["launches"]) == {"k_leafpair_root": 1}
@@ -444,7 +440,7 @@ VALUE_EDGE_CASES = ["p2_trivial_nv7_base",     # 8 lanes straight from the polyn
                     "p2_nv9_ext",              # block: thread per hash from Ext leaves
                     "p2_nv12_base",            # block: threads, 8 lanes and the fold over 8; spin: fold over 64
                     "p2_nv13_base",            # k_merkle_mid from leaves, small from digests
-                    "p2_nv17_ext",             # k_merkle_l1 Ext
+                    "p2_nv17_ext",             # k_merkle_wide from Ext leaves
                     "p2_batch_nv9_base"]       # a batch level 0
 
 
