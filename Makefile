@@ -2,6 +2,7 @@
 #   make            -> product library, host library, oracle
 #   make product    -> deep-prove_b200/libdeepprove_b200.so      (CUDA kernels + C ABI, sm_90a only)
 #   make oracle     -> oracle/libdp_oracle.so                     (CPU restatement: TEST INFRASTRUCTURE)
+#                      tests/libdp_oracle_model_io.so             (its model IO: output, verifier on a given output)
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
 ARCH      := -gencode arch=compute_90a,code=sm_90a
@@ -20,7 +21,7 @@ all: product host oracle tools
 
 product: $(PKG)/libdeepprove_b200.so
 host: $(PKG)/libdeepprove_host.so
-oracle: oracle/libdp_oracle.so
+oracle: oracle/libdp_oracle.so tests/libdp_oracle_model_io.so
 
 build/%.o: $(CSRC)/%.cu $(CU_HDRS)
 	@mkdir -p build
@@ -35,6 +36,9 @@ $(PKG)/libdeepprove_host.so: $(HOST_SRCS) $(HOST_HDRS) $(PKG)/libdeepprove_b200.
 oracle/libdp_oracle.so: $(ORC_SRCS) $(ORC_HDRS)
 	$(CXX) -O3 -march=x86-64-v3 -std=c++17 -fPIC -shared -Wall -o $@ $(ORC_SRCS) -lpthread
 
+tests/libdp_oracle_model_io.so: tests/oracle_model_io.cpp $(ORC_HDRS)
+	$(CXX) -O3 -march=x86-64-v3 -std=c++17 -fPIC -shared -Wall -o $@ tests/oracle_model_io.cpp -lpthread
+
 # device-vs-host self test of the field primitives and Poseidon2 (run by tests/test_gpu_baseline_size.py on the GPU box)
 tools: $(PKG)/gl_selftest_bin
 $(PKG)/gl_selftest_bin: tools/gl_selftest.cu $(CU_HDRS) $(HOST_HDRS)
@@ -48,6 +52,6 @@ $(PKG)/libdp_trace.so: tools/cupti_trace.cpp
 	$(CXX) -O2 -shared -fPIC -I/usr/local/cuda/include -I/usr/local/cuda/extras/CUPTI/include -o $@ tools/cupti_trace.cpp -L/usr/local/cuda/lib64 -L/usr/local/cuda/extras/CUPTI/lib64 -lcupti -lcudart -Wl,-rpath,/usr/local/cuda/lib64
 
 clean:
-	rm -rf build $(PKG)/*.so oracle/*.so $(PKG)/gl_selftest_bin
+	rm -rf build $(PKG)/*.so oracle/*.so tests/*.so $(PKG)/gl_selftest_bin
 
 .PHONY: all product host oracle tools devtools clean

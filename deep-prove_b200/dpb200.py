@@ -128,6 +128,10 @@ SIGNATURES = {
     "dph_zkml_pool_free": (None, [VP]),
     "dph_zkml_prove_concurrent": (INT, [VP, INT, U32, U32, INT, STR, VP, VP, U64, VP]),
     "dph_zkml_prove_concurrent_all": (INT, [VP, INT, U32, U32, INT, STR, VP, VP, U64, VP, VP]),
+    "dph_zkml_output_len": (INT, [VP, VP]),
+    "dph_zkml_trace_output": (INT, [VP, VP, U64, VP]),
+    "dph_zkml_prove_batch": (INT, [VP, INT, U32, VP, U32, STR, VP, U64, VP, VP, VP, VP]),
+    "dph_zkml_job_error": (STR, [VP, U32]),
     "dph_shm_mailbox_bytes": (U64, []),
     "dph_shm_allgather": (INT, [VP, U32, U32, VP, VP, U64, VP]),
     "dph_sumcheck_prove_sharded": (INT, [U32, U32, VP, U32, VP, U32, U32, STR, VP, VP, VP, VP, VP, VP, VP]),
@@ -594,6 +598,7 @@ class ZkmlContext:
         d = np.ascontiguousarray(desc, dtype=np.int64).reshape(-1, 9)
         w = np.ascontiguousarray(data, dtype=np.int64)
         self.h = C.c_void_p()
+        self.input_len = int(input_len)
         hcheck(host().dph_model_context_new(_ptr(d), d.shape[0], _ptr(w), int(input_len), C.byref(self.h)))
 
     def prove(self, x, label=b"m2vec"):
@@ -634,6 +639,50 @@ class ZkmlContext:
                                                     _ptr(out), int(stride), _ptr(lens), _ptr(workers)))
         out = out.reshape(int(n_proofs), int(stride))
         return sec.value, [out[j, : int(lens[j])] for j in range(int(n_proofs))], workers
+
+    @property
+    def output_len(self):
+        """elements of the model's output: the last node's output tensor in the padded layout"""
+        n = C.c_uint64()
+        hcheck(host().dph_zkml_output_len(self.h, C.byref(n)))
+        return n.value
+
+    def trace_output(self):
+        """the model output (int64) of the stored trace, after prove(x) or run_inference(x)"""
+        out = np.zeros(self.output_len, dtype=np.int64)
+        n = C.c_uint64()
+        hcheck(host().dph_zkml_trace_output(self.h, _ptr(out), out.size, C.byref(n)))
+        return out[: n.value].copy()
+
+    def prove_batch(self, inputs, n_workers, device=0, label=b"m2vec", stride=None):
+        """Prove n distinct inputs ([n, input_len] int64) end to end on the worker pool (dph_zkml_prove_batch).  Returns (seconds,
+        proofs, outputs, status, errors): proofs[j] is input j's flat proof (empty when it failed), outputs[j] its model output
+        ([n, output_len] int64), status[j] 0 or its error code, errors[j] None or its message.  The default stride is the length of
+        one proof of this model (measured once, on the first input, and kept)."""
+        x = np.ascontiguousarray(inputs, dtype=np.int64)
+        if x.ndim != 2 or x.shape[0] == 0 or x.shape[1] != self.input_len:
+            raise ValueError("prove_batch: inputs must be [n >= 1, %d]" % self.input_len)
+        n = x.shape[0]
+        if stride is None:
+            if getattr(self, "_proof_words", None) is None:
+                one = np.zeros(1 << 23, dtype=np.uint64)
+                lens, st = np.zeros(1, dtype=np.uint64), np.zeros(1, dtype=np.int32)
+                y = np.zeros(self.output_len, dtype=np.int64)
+                hcheck(host().dph_zkml_prove_batch(self.h, int(device), 1, _ptr(x[:1]), 1, label, _ptr(one), one.size, _ptr(lens), _ptr(y),
+                                                   _ptr(st), None))
+                if st[0] != 0:
+                    raise DpError(int(st[0]), "sizing the proof stride on input 0: %s" % host().dph_zkml_job_error(self.h, 0).decode())
+                self._proof_words = int(lens[0])
+            stride = self._proof_words
+        proofs = np.zeros((n, int(stride)), dtype=np.uint64)
+        lens = np.zeros(n, dtype=np.uint64)
+        outputs = np.zeros((n, self.output_len), dtype=np.int64)
+        status = np.zeros(n, dtype=np.int32)
+        sec = C.c_double()
+        hcheck(host().dph_zkml_prove_batch(self.h, int(device), int(n_workers), _ptr(x), n, label, _ptr(proofs), int(stride), _ptr(lens),
+                                           _ptr(outputs), _ptr(status), C.byref(sec)))
+        errors = [None if status[j] == 0 else host().dph_zkml_job_error(self.h, j).decode() for j in range(n)]
+        return sec.value, [proofs[j, : int(lens[j])] for j in range(n)], outputs, status, errors
 
     def free(self):
         if self.h:

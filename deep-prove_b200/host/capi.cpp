@@ -20,11 +20,12 @@ static ExtVec exts(const u64 *w, size_t n) {
     return v;
 }
 // The flat-output rule: *out_len = the words the output needs; a null `out` only asks for that length, a `cap` below it is refused.
-static int put_flat(const char *entry, const std::vector<u64> &words, uint64_t *out, uint64_t cap, uint64_t *out_len) {
+template <class W>
+static int put_flat(const char *entry, const std::vector<W> &words, W *out, uint64_t cap, uint64_t *out_len) {
     *out_len = words.size();
     if (!out) return 0;
     if (words.size() > cap) throw Error(DP_ERR_INVALID, std::string(entry) + ": output buffer too small");
-    memcpy(out, words.data(), 8 * words.size());
+    memcpy(out, words.data(), sizeof(W) * words.size());
     return 0;
 }
 
@@ -171,10 +172,30 @@ int dph_zkml_prove(void *handle, const int64_t *input, int mode, const char *lab
     DPH_CATCH
 }
 
+// The number of elements in the model's output: the last node's output tensor in the padded layout
+int dph_zkml_output_len(void *handle, uint64_t *len) {
+    DPH_TRY
+    if (!handle || !len) throw Error(DP_ERR_INVALID, "dph_zkml_output_len: null argument");
+    *len = ((ZkHandle *)handle)->model.output_len();
+    return 0;
+    DPH_CATCH
+}
+
+// The model output of the stored trace (dph_zkml_prove mode 0 or 1) as signed elements, by the flat-output rule
+int dph_zkml_trace_output(void *handle, int64_t *out, uint64_t cap, uint64_t *out_len) {
+    DPH_TRY
+    if (!handle || !out_len) throw Error(DP_ERR_INVALID, "dph_zkml_trace_output: null argument");
+    ZkHandle *h = (ZkHandle *)handle;
+    if (!h->trace.valid()) throw Error(DP_ERR_STATE, "dph_zkml_trace_output: no stored trace (run dph_zkml_prove mode 0 or 1 first)");
+    return put_flat("dph_zkml_trace_output", dp::zkml::to_elements(h->trace.outs.back()), out, cap, out_len);
+    DPH_CATCH
+}
+
 }  // extern "C"
 
 // ---- concurrent proving: a persistent pool of host threads, each with its own library context (stream + device
-// arena) on `device`, proves the stored trace; the GPU runs the threads' small latency-bound kernels side by side.
+// arena) on `device`, proves the stored trace, the stored input or a batch of caller inputs; the GPU runs the threads' small
+// latency-bound kernels side by side.  One call at a time per pool: a call on a busy pool is refused.
 #include <thread>
 #include <mutex>
 #include <atomic>
@@ -182,10 +203,13 @@ int dph_zkml_prove(void *handle, const int64_t *input, int mode, const char *lab
 namespace {
 struct ZkPool {
     std::vector<std::thread> th; std::mutex mu; std::condition_variable cv, done_cv;
-    ZkHandle *h = nullptr; int device = 0; bool stop = false; uint64_t pending = 0, inflight = 0; std::string label, err; bool failed = false; bool e2e = false;
+    ZkHandle *h = nullptr; int device = 0; bool stop = false, busy = false; uint64_t pending = 0, inflight = 0; std::string label, err; bool failed = false; bool e2e = false;
     uint64_t *out = nullptr, out_cap = 0, *out_len = nullptr;   // when set: the flat proof of the call's last job is copied here
     // when set: every job's flat proof goes to all_out + job * all_stride, its length to all_lens[job], its worker to all_worker[job]
     uint64_t *all_out = nullptr, all_stride = 0, *all_lens = nullptr; uint32_t *all_worker = nullptr; uint64_t next_job = 0;
+    // when set (dph_zkml_prove_batch): job j proves the caller's input j, in + j * input_len, end to end; its model output goes to
+    // outputs + j * output_len.  A failing job does not fail the call: it gets status[j] != 0, proof length 0 and job_err[j].
+    const int64_t *in = nullptr; int64_t *outputs = nullptr; int32_t *status = nullptr; std::vector<std::string> job_err;
     // Identical proofs started together stay in lockstep: all of them sit in the latency-bound layer sumchecks (GPU nearly idle)
     // and then all of them queue their GPU-filling opening kernels behind each other (CUPTI timeline).  So the
     // workers of one call start `stagger_s` apart (one proof duration spread over the workers; the duration is an average over the
@@ -195,8 +219,8 @@ struct ZkPool {
     void worker(uint32_t idx) {
         bool inited = false; uint64_t seen_gen = 0;
         for (;;) {
-            uint64_t gen, job; double delay = 0.0; bool keep = false, all = false;
-            { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || (pending > 0 && idx < active); }); if (stop) break; pending--; inflight++; keep = pending == 0 && out; all = all_out != nullptr; job = next_job++; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } }
+            uint64_t gen, job; double delay = 0.0; bool keep = false, all = false, batch = false;
+            { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || (pending > 0 && idx < active); }); if (stop) break; pending--; inflight++; keep = pending == 0 && out; all = all_out != nullptr; batch = in != nullptr; job = next_job++; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } }
             try {
                 const bool first_ever = !inited;     // grows this thread's device arena: not a representative duration
                 if (!inited) { dp::check(dp_init(device)); inited = true; }
@@ -205,7 +229,15 @@ struct ZkPool {
                 dp::DynTranscript t(label);
                 dp::zkml::Prover<dp::DynTranscript> prover(h->ctx, t);
                 std::vector<uint64_t> flat;
-                if (e2e) {   // from the host input vector: inference, prove, serialised proof in host memory
+                if (batch) {   // the caller's input `job`: inference, prove, serialised proof and model output in host memory
+                    const size_t w = h->model.input_len, ol = h->model.output_len();
+                    dp::zkml::DeviceTrace tr = dp::zkml::run_device(h->ctx, std::vector<dp::zkml::Element>(in + job * w, in + (job + 1) * w));
+                    flat = prover.prove(tr).flatten(h->model.nodes.size());
+                    const std::vector<dp::zkml::Element> y = dp::zkml::to_elements(tr.outs.back());
+                    if (y.size() != ol) throw dp::Error(DP_ERR_STATE, "dph_zkml_prove_batch: model output of unexpected length");
+                    if (flat.size() > all_stride) { std::lock_guard<std::mutex> lk(mu); failed = true; err = "dph_zkml_prove_batch: proof longer than the stride"; throw dp::Error(DP_ERR_INVALID, err); }
+                    memcpy(outputs + job * ol, y.data(), 8 * ol);
+                } else if (e2e) {   // from the host input vector: inference, prove, serialised proof in host memory
                     dp::zkml::Proof p = prover.prove(h->trace_input);
                     flat = p.flatten(h->model.nodes.size());
                     if (flat.empty()) throw dp::Error(DP_ERR_STATE, "empty proof");
@@ -222,7 +254,13 @@ struct ZkPool {
                 }
                 const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
                 if (!first_ever) { std::lock_guard<std::mutex> lk(mu); n_timed++; avg_proof_s += (sec - avg_proof_s) / (double)std::min<uint64_t>(n_timed, 64); }
-            } catch (const std::exception &e) { std::lock_guard<std::mutex> lk(mu); failed = true; err = e.what(); }
+            } catch (const std::exception &e) {
+                std::lock_guard<std::mutex> lk(mu);
+                if (batch) {   // this job's failure only
+                    const dp::Error *de = dynamic_cast<const dp::Error *>(&e);
+                    status[job] = de && de->code ? de->code : 1; all_lens[job] = 0; job_err[job] = e.what();
+                } else { failed = true; err = e.what(); }
+            }
             dp_profile_flush();   // per-kernel timing of the concurrent region (no-op unless dp_profile_enable(1))
             { std::lock_guard<std::mutex> lk(mu); inflight--; if (pending == 0 && inflight == 0) done_cv.notify_all(); }
         }
@@ -235,13 +273,15 @@ std::mutex g_pools_mu; std::map<void *, std::unique_ptr<ZkPool>> g_pools;
 extern "C" void dph_zkml_pool_free(void *handle) { std::lock_guard<std::mutex> lk(g_pools_mu); g_pools.erase(handle); }
 namespace {
 struct AllOut { uint64_t *out; uint64_t stride; uint64_t *lens; uint32_t *worker; };
+struct BatchIo { const int64_t *in; int64_t *outputs; int32_t *status; };
 int prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
-                     uint64_t *out, uint64_t cap, uint64_t *out_len, const AllOut &all) {
+                     uint64_t *out, uint64_t cap, uint64_t *out_len, const AllOut &all, const BatchIo &batch) {
     DPH_TRY
     ZkHandle *h = (ZkHandle *)handle;
-    if (!h->trace.valid()) throw dp::Error(DP_ERR_STATE, "dph_zkml_prove_concurrent: run inference first (mode 1)");
+    if (!batch.in && !h->trace.valid()) throw dp::Error(DP_ERR_STATE, "dph_zkml_prove_concurrent: run inference first (mode 1)");
     ZkPool *pool;
     { std::lock_guard<std::mutex> lk(g_pools_mu); auto &pp = g_pools[handle]; if (!pp) { pp = std::make_unique<ZkPool>(); pp->h = h; pp->device = device; } pool = pp.get(); }
+    { std::lock_guard<std::mutex> lk(pool->mu); if (pool->busy) throw dp::Error(DP_ERR_STATE, "the handle's worker pool is busy with another call"); pool->busy = true; }
     while (pool->th.size() < n_workers) { const uint32_t idx = (uint32_t)pool->th.size(); pool->th.emplace_back([pool, idx] { pool->worker(idx); }); }
     auto t0 = std::chrono::steady_clock::now();
     {
@@ -249,22 +289,24 @@ int prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_pr
         pool->label = label; pool->failed = false; pool->e2e = e2e != 0; pool->pending = n_proofs; pool->active = n_workers; pool->call_gen++;
         pool->out = out; pool->out_cap = cap; pool->out_len = out_len; if (out_len) *out_len = 0;
         pool->all_out = all.out; pool->all_stride = all.stride; pool->all_lens = all.lens; pool->all_worker = all.worker; pool->next_job = 0;
+        pool->in = batch.in; pool->outputs = batch.outputs; pool->status = batch.status;
+        if (batch.in) pool->job_err.assign(n_proofs, std::string());
         // stagger only when every worker gets several proofs (otherwise the ramps cost more than the overlap gains)
         pool->stagger_s = (n_workers > 1 && n_proofs >= 3 * n_workers && pool->n_timed > 0) ? pool->avg_proof_s / n_workers : 0.0;
     }
     // only the first n_workers threads are woken usefully: notify_all, extra threads just compete for the same jobs
     pool->cv.notify_all();
-    { std::unique_lock<std::mutex> lk(pool->mu); pool->done_cv.wait(lk, [&] { return pool->pending == 0 && pool->inflight == 0; }); }
+    bool failed;
+    { std::unique_lock<std::mutex> lk(pool->mu); pool->done_cv.wait(lk, [&] { return pool->pending == 0 && pool->inflight == 0; }); failed = pool->failed; if (failed) g_herr = pool->err; pool->busy = false; }
     if (out_seconds) *out_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    if (pool->failed) { g_herr = pool->err; return 1; }
-    return 0;
+    return failed ? 1 : 0;
     DPH_CATCH
 }
 }
 // out (optional, cap words): receives the flat proof of the last job handed out, *out_len its length in words.
 extern "C" int dph_zkml_prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
                                          uint64_t *out, uint64_t cap, uint64_t *out_len) {
-    return prove_concurrent(handle, device, n_workers, n_proofs, e2e, label, out_seconds, out, cap, out_len, AllOut{nullptr, 0, nullptr, nullptr});
+    return prove_concurrent(handle, device, n_workers, n_proofs, e2e, label, out_seconds, out, cap, out_len, AllOut{nullptr, 0, nullptr, nullptr}, BatchIo{nullptr, nullptr, nullptr});
 }
 // The same call, but every job's flat proof is kept: job j's proof is written to out + j * stride (n_proofs x stride words),
 // its length in words to out_lens[j] and, when out_worker is given, the index of the worker thread that proved it to out_worker[j].
@@ -274,7 +316,37 @@ extern "C" int dph_zkml_prove_concurrent_all(void *handle, int device, uint32_t 
                                              uint64_t *out, uint64_t stride, uint64_t *out_lens, uint32_t *out_worker) {
     if (!out || !out_lens) { g_herr = "dph_zkml_prove_concurrent_all: out and out_lens are required"; return 1; }
     for (uint32_t j = 0; j < n_proofs; j++) out_lens[j] = 0;
-    return prove_concurrent(handle, device, n_workers, n_proofs, e2e, label, out_seconds, nullptr, 0, nullptr, AllOut{out, stride, out_lens, out_worker});
+    return prove_concurrent(handle, device, n_workers, n_proofs, e2e, label, out_seconds, nullptr, 0, nullptr, AllOut{out, stride, out_lens, out_worker},
+                            BatchIo{nullptr, nullptr, nullptr});
+}
+// n distinct inputs (inputs: n x input_len), each proved end to end on the handle's worker pool (n_workers threads on `device`):
+// input j's flat proof goes to proofs + j * stride, its length in words to proof_lens[j], its model output (output_len elements,
+// dph_zkml_output_len) to outputs + j * output_len and its status to status[j].  Slots are indexed by input.  An input that fails
+// (a value outside its lookup table, say) fails alone: status[j] != 0, proof_lens[j] = 0, and dph_zkml_job_error(handle, j) holds
+// its message until the next batch call on the handle.  Non-zero only for call-level errors: an argument refused, no device, a
+// busy pool (DP_ERR_STATE), or a proof longer than `stride` (DP_ERR_INVALID, after the batch).  The stored trace is not touched.
+extern "C" int dph_zkml_prove_batch(void *handle, int device, uint32_t n_workers, const int64_t *inputs, uint32_t n, const char *label,
+                                    uint64_t *proofs, uint64_t stride, uint64_t *proof_lens, int64_t *outputs, int32_t *status, double *out_seconds) {
+    DPH_TRY
+    if (n == 0 || n_workers == 0) throw Error(DP_ERR_INVALID, "dph_zkml_prove_batch: no inputs or no workers");
+    if (!inputs || !label || !proofs || !proof_lens || !outputs || !status) throw Error(DP_ERR_INVALID, "dph_zkml_prove_batch: null argument");
+    const int n_dev = dp_device_count();
+    if (n_dev <= 0) throw Error(DP_ERR_NO_DEVICE, "dph_zkml_prove_batch: no CUDA device visible (no CPU fallback)");
+    if (device < 0 || device >= n_dev) throw Error(DP_ERR_INVALID, "dph_zkml_prove_batch: device index out of range");
+    if (!handle) throw Error(DP_ERR_INVALID, "dph_zkml_prove_batch: null handle");
+    for (uint32_t j = 0; j < n; j++) { proof_lens[j] = 0; status[j] = 0; }
+    return prove_concurrent(handle, device, n_workers, n, 0, label, out_seconds, nullptr, 0, nullptr, AllOut{proofs, stride, proof_lens, nullptr},
+                            BatchIo{inputs, outputs, status});
+    DPH_CATCH
+}
+// The message of job j of the handle's last batch call, or NULL when job j succeeded (or there is no such job)
+extern "C" const char *dph_zkml_job_error(void *handle, uint32_t j) {
+    std::lock_guard<std::mutex> lk(g_pools_mu);
+    auto it = g_pools.find(handle);
+    if (it == g_pools.end()) return nullptr;
+    std::lock_guard<std::mutex> pl(it->second->mu);
+    const std::vector<std::string> &e = it->second->job_err;
+    return j < e.size() && !e[j].empty() ? e[j].c_str() : nullptr;
 }
 
 // One proof sharded over `world` ranks: `mles` are THIS rank's slices (nv_total - log2(world) variables each).
@@ -386,7 +458,7 @@ extern "C" int dph_conv_prove(uint32_t kw, uint32_t kx, uint32_t n_x, uint32_t r
 // (kind 5 MatMul {rows, inner, cols, transposed, has_bias}: the constant right matrix then the bias; kind 0 Dense {nrows, ncols}: weights then bias; 1 Requant {right_shift, fp_scale, multiplier, intermediate_bits};
 //  2 ReLU; 3 Conv {kw, kx, nw, real_nw, unpadded_out[3]}: filter then bias; 4 Maxpool {C, H, W}).  Builds the Context: uploads
 // weights, bias and tables and commits them (CommitmentContext::new) -- setup, not proving.  dph_zkml_prove /
-// dph_zkml_prove_concurrent / dph_zkml_context_free take the handle.
+// dph_zkml_prove_concurrent / dph_zkml_prove_batch / dph_zkml_context_free take the handle.
 extern "C" int dph_model_context_new(const int64_t *desc, uint32_t n_nodes, const int64_t *data, uint64_t input_len, void **out) {
     DPH_TRY
     using namespace dp::zkml;

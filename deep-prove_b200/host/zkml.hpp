@@ -44,7 +44,20 @@ struct Node {
     // constant right matrix [mm_k][mm_c] ([mm_c][mm_k] with Config::TransposeB), `bias` (optional) one value per output column
     size_t mm_r = 0, mm_k = 0, mm_c = 0; bool mm_t = false, mm_bias = false;
 };
-struct Model { std::vector<Node> nodes; size_t input_len = 0; };
+struct Model {
+    std::vector<Node> nodes; size_t input_len = 0;
+    // elements of the last node's output tensor in the padded layout (DeviceTrace::outs.back() of run_device)
+    size_t output_len() const {
+        size_t len = input_len;
+        for (auto &n : nodes) {
+            if (n.op == Op::Dense) len = n.nrows;
+            else if (n.op == Op::MatMul) len = n.mm_r * n.mm_c;
+            else if (n.op == Op::Conv) len = n.kw * n.nw * n.nw;
+            else if (n.op == Op::Pool) len = n.pool_c * (n.pool_h / 2) * (n.pool_w / 2);
+        }
+        return len;
+    }
+};
 
 // TableType with the enum's derive(Ord) order (lookup/context.rs:53-63): Relu < Range < Clamping(size)
 struct TableType {
