@@ -703,6 +703,28 @@ class ModelContext(ZkmlContext):
     def __init__(self, desc, data, input_len):
         self._new(desc, data, input_len)
         self._out = np.zeros(1 << 23, dtype=np.uint64)
+        self.metadata = None
+
+    @classmethod
+    def from_onnx(cls, path):
+        """import a float ONNX model (onnx_import.py: AbsoluteMax quantisation and padding as the reference's default loader does);
+        .metadata quantises float inputs (quantize_input) and dequantises outputs (dequantize_output)"""
+        import onnx_import
+        desc, data, input_len, md, _, _ = onnx_import.import_onnx(path)
+        ctx = cls(desc, data, input_len)
+        ctx.metadata = md
+        return ctx
+
+    def prove_batch_float(self, inputs, n_workers, device=0, label=b"m2vec", stride=None):
+        """prove_batch on float inputs ([n, *input shape] in [-1, 1]) of a model made by from_onnx: quantises each input with
+        .metadata, proves them all, and returns (proofs, outputs, float_outputs, status, errors) -- outputs are the integer model
+        outputs in the padded layout, float_outputs their real entries dequantised"""
+        if self.metadata is None:
+            raise ValueError("prove_batch_float: the context has no quantisation metadata (build it with ModelContext.from_onnx)")
+        x = np.asarray(inputs, dtype=np.float32)
+        x = self.metadata.quantize_input(x.reshape((-1,) + self.metadata.input_shape))
+        _, proofs, outputs, status, errors = self.prove_batch(x, n_workers, device, label, stride)
+        return proofs, outputs, self.metadata.dequantize_output(outputs), status, errors
 
 
 def sumcheck_prove_batch_polys(T, mles, products, max_nv, label=b"m2vec"):

@@ -28,6 +28,38 @@ def _requant(int_part_log, intermediate_bits):
     return [REQUANT, int_part_log, fp, 3 << (fp - 2), intermediate_bits, 0, 0, 0, 0]
 
 
+def conv_layer(filt_u, bias_u, n_p, n_u):
+    """A Convolution node in the padded layout: filter [kw_u, kx_u, k, k] and bias [kw_u] over a [kx_u, n_u, n_u] image held in
+    [p2(kx_u), n_p, n_p].  The filter is padded to [p2(kw_u), p2(kx_u), p2(k), p2(k)], the bias to p2(kw_u) (zeros).
+    Returns (descriptor row, padded filter, padded bias, h_out = n_u - k + 1)."""
+    kw_u, kx_u, k, _ = filt_u.shape
+    kw, kx, rn = _p2(kw_u), _p2(kx_u), _p2(k)
+    filt = np.zeros((kw, kx, rn, rn), dtype=np.int64)
+    filt[:kw_u, :kx_u, :k, :k] = filt_u
+    bias = np.zeros(kw, dtype=np.int64)
+    bias[:kw_u] = bias_u
+    h_out = n_u - k + 1
+    return [CONV, kw, kx, n_p, rn, kw_u, h_out, h_out, 0], filt, bias, h_out
+
+
+def flatten_mask(c_u, n_u, n_p):
+    """The real columns of a flatten of [p2(c_u)][n_p][n_p] (padding.rs pad_matrix_to_ignore_garbage): c < c_u, row < n_u, col < n_u"""
+    mask = np.zeros((_p2(c_u), n_p, n_p), dtype=bool)
+    mask[:c_u, :n_u, :n_u] = True
+    return mask.reshape(-1)
+
+
+def dense_layer(w_u, b_u, real, nrows):
+    """A Dense node in the padded layout: the [out_u, real.sum()] matrix spread over the columns where `real` is True (zeros
+    elsewhere) and over the first out_u of `nrows` rows, the bias likewise.  Returns (descriptor row, padded matrix, padded bias)."""
+    out_u = w_u.shape[0]
+    w = np.zeros((nrows, real.size), dtype=np.int64)
+    w[:out_u, real] = w_u
+    b = np.zeros(nrows, dtype=np.int64)
+    b[:out_u] = b_u
+    return [DENSE, nrows, real.size, 0, 0, 0, 0, 0, 0], w, b
+
+
 def cnn(seed=1, img=32, c0=3, c1=12, c2=33, f1=247, f2=173, f3=10, k=5):
     """returns (desc [n_nodes, 9] int64, data int64, input int64 [padded c0 * img^2], n_real_params)"""
     rng = np.random.Generator(np.random.PCG64(seed))
@@ -36,14 +68,11 @@ def cnn(seed=1, img=32, c0=3, c1=12, c2=33, f1=247, f2=173, f3=10, k=5):
     x = np.zeros((_p2(c0), n_p, n_p), dtype=np.int64)
     x[:c0, :img, :img] = rng.integers(-127, 128, size=(c0, img, img))
     for kw_u in (c1, c2):
-        kx, kw, rn = _p2(kx_u), _p2(kw_u), _p2(k)
-        filt = np.zeros((kw, kx, rn, rn), dtype=np.int64)
-        filt[:kw_u, :kx_u, :k, :k] = rng.integers(-127, 128, size=(kw_u, kx_u, k, k))
-        bias = np.zeros(kw, dtype=np.int64)
-        bias[:kw_u] = rng.integers(-1000, 1001, size=kw_u)
+        filt_u = rng.integers(-127, 128, size=(kw_u, kx_u, k, k))
+        row, filt, bias, h_out = conv_layer(filt_u, rng.integers(-1000, 1001, size=kw_u), n_p, n_u)
+        kw = row[1]
         n_params += kw_u * kx_u * k * k + kw_u
-        h_out = n_u - k + 1
-        desc.append([CONV, kw, kx, n_p, rn, kw_u, h_out, h_out, 0])
+        desc.append(row)
         data += [filt.reshape(-1), bias]
         terms = k * k * kx_u
         desc.append(_requant(_clog2(terms) + 2, 2 * (BIT_LEN - 1) + _clog2(terms + 1)))   # convolution.rs:362-366 output_bitsize
@@ -53,18 +82,11 @@ def cnn(seed=1, img=32, c0=3, c1=12, c2=33, f1=247, f2=173, f3=10, k=5):
     ncols, prev_real = _p2(c2) * n_p * n_p, None
     for li, out_u in enumerate((f1, f2, f3)):
         nrows = _p2(out_u)
-        w = np.zeros((nrows, ncols), dtype=np.int64)
-        if li == 0:   # flatten of [C][n_p][n_p]: real entries are c < c2, row < n_u, col < n_u
-            mask = np.zeros((_p2(c2), n_p, n_p), dtype=bool)
-            mask[:c2, :n_u, :n_u] = True
-            real = mask.reshape(-1)
-        else:
-            real = np.arange(ncols) < prev_real
-        w[:out_u, real] = rng.integers(-127, 128, size=(out_u, int(real.sum())))
-        b = np.zeros(nrows, dtype=np.int64)
-        b[:out_u] = rng.integers(-127, 128, size=out_u)
+        real = flatten_mask(c2, n_u, n_p) if li == 0 else np.arange(ncols) < prev_real
+        w_u = rng.integers(-127, 128, size=(out_u, int(real.sum())))
+        row, w, b = dense_layer(w_u, rng.integers(-127, 128, size=out_u), real, nrows)
         n_params += out_u * int(real.sum()) + out_u
-        desc.append([DENSE, nrows, ncols, 0, 0, 0, 0, 0, 0])
+        desc.append(row)
         data += [w.reshape(-1), b]
         if li < 2:
             desc.append(_requant(_clog2(ncols), 2 * (BIT_LEN - 1) + _clog2(ncols) + 1))   # dense.rs:416-421
@@ -92,14 +114,11 @@ def covid(seed=1, img=224, channels=(32, 64, 64, 128, 128), fc=64, k=3):
     x = np.zeros((_p2(c0), n_p, n_p), dtype=np.int64)
     x[:c0, :img, :img] = rng.integers(-127, 128, size=(c0, img, img))
     for li, kw_u in enumerate(channels):
-        kx, kw, rn = _p2(kx_u), _p2(kw_u), _p2(k)
-        filt = np.zeros((kw, kx, rn, rn), dtype=np.int64)
-        filt[:kw_u, :kx_u, :k, :k] = rng.integers(-127, 128, size=(kw_u, kx_u, k, k))
-        bias = np.zeros(kw, dtype=np.int64)
-        bias[:kw_u] = rng.integers(-1000, 1001, size=kw_u)
+        filt_u = rng.integers(-127, 128, size=(kw_u, kx_u, k, k))
+        row, filt, bias, h_out = conv_layer(filt_u, rng.integers(-1000, 1001, size=kw_u), n_p, n_u)
+        kw = row[1]
         n_params += kw_u * kx_u * k * k + kw_u
-        h_out = n_u - k + 1
-        desc.append([CONV, kw, kx, n_p, rn, kw_u, h_out, h_out, 0])
+        desc.append(row)
         data += [filt.reshape(-1), bias]
         terms = k * k * kx_u
         desc.append(_requant(_clog2(terms) + 2, 2 * (BIT_LEN - 1) + _clog2(terms + 1)))
@@ -111,18 +130,11 @@ def covid(seed=1, img=224, channels=(32, 64, 64, 128, 128), fc=64, k=3):
     ncols, prev_real = _p2(kx_u) * n_p * n_p, None
     for li, out_u in enumerate((fc, 1)):
         nrows = max(4, _p2(out_u))
-        w = np.zeros((nrows, ncols), dtype=np.int64)
-        if li == 0:
-            mask = np.zeros((_p2(kx_u), n_p, n_p), dtype=bool)
-            mask[:kx_u, :n_u, :n_u] = True
-            real = mask.reshape(-1)
-        else:
-            real = np.arange(ncols) < prev_real
-        w[:out_u, real] = rng.integers(-127, 128, size=(out_u, int(real.sum())))
-        b = np.zeros(nrows, dtype=np.int64)
-        b[:out_u] = rng.integers(-127, 128, size=out_u)
+        real = flatten_mask(kx_u, n_u, n_p) if li == 0 else np.arange(ncols) < prev_real
+        w_u = rng.integers(-127, 128, size=(out_u, int(real.sum())))
+        row, w, b = dense_layer(w_u, rng.integers(-127, 128, size=out_u), real, nrows)
         n_params += out_u * int(real.sum()) + out_u
-        desc.append([DENSE, nrows, ncols, 0, 0, 0, 0, 0, 0])
+        desc.append(row)
         data += [w.reshape(-1), b]
         desc.append(_requant(_clog2(ncols), 2 * (BIT_LEN - 1) + _clog2(ncols) + 1))
         desc.append([RELU] + [0] * 8)
