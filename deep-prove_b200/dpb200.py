@@ -706,11 +706,12 @@ class ModelContext(ZkmlContext):
         self.metadata = None
 
     @classmethod
-    def from_onnx(cls, path):
-        """import a float ONNX model (onnx_import.py: AbsoluteMax quantisation and padding as the reference's default loader does);
+    def from_onnx(cls, path, calibration=None):
+        """import a float ONNX model (onnx_import.py: AbsoluteMax quantisation and padding as the reference's default loader does,
+        or, given calibration samples [n, *input shape] in [-1, 1], the reference's InferenceObserver on them);
         .metadata quantises float inputs (quantize_input) and dequantises outputs (dequantize_output)"""
         import onnx_import
-        desc, data, input_len, md, _, _ = onnx_import.import_onnx(path)
+        desc, data, input_len, md, _, _ = onnx_import.import_onnx(path, calibration)
         ctx = cls(desc, data, input_len)
         ctx.metadata = md
         return ctx

@@ -2,7 +2,8 @@
 padded quantised layout the prover takes: the (desc, data, input_len) of dph_model_context_new plus a Metadata object that
 quantises float inputs and dequantises outputs.  Pure Python + numpy: the protobuf wire format is read directly.
 
-The quantisation restates the reference's default loader (zkml/src/parser/mod.rs:71-93: load, quantise with AbsoluteMax, pad):
+The quantisation restates the reference's default loader (zkml/src/parser/mod.rs:71-93: load, quantise with AbsoluteMax, pad),
+or, given calibration samples, its InferenceObserver (observe(); the strategy its benchmark uses with --quantization inference):
   - AbsoluteMax without a representative input (quantization/strategy.rs:190-249): the model input and the output of every node
     that has a scaling of its own use ScalingFactor::default(), i.e. [-1, 1] over [MIN, MAX] (quantization/mod.rs:155-165);
   - quantize_model (strategy.rs:251-295): each Dense / Convolution node is quantised from its input scaling and followed by the
@@ -173,6 +174,13 @@ class FloatModel:
 
     def forward(self, x):
         """float inference in numpy (float64 accumulation of the float32 weights) on one unpadded input"""
+        y = np.asarray(x, dtype=np.float64)
+        for y in self.outputs(x):
+            pass
+        return y.reshape(-1)
+
+    def outputs(self, x):
+        """the float inference of forward(), yielding each layer's output in its unpadded shape"""
         x = np.asarray(x, dtype=np.float64).reshape(self.input_shape)
         for l in self.layers:
             if l[0] == "dense":
@@ -190,7 +198,7 @@ class FloatModel:
                 x = x[:, :h // 2 * 2, :w // 2 * 2].reshape(c, h // 2, 2, w // 2, 2).max(axis=(2, 4))
             else:
                 x = x.reshape(-1)
-        return x.reshape(-1)
+            yield x
 
 
 def _node_label(n):
@@ -392,17 +400,58 @@ class Metadata:
 
 class QuantizedLayer:
     """one quantised layer before padding, for inspection and for the unpadded integer inference the tests run: kind "dense" / "conv"
-    with w, b (int64) and rq = (right_shift, fp_scale, fixed_point_multiplier, intermediate_bit_size) of the Requant after it"""
+    with w, b (int64), rq = (right_shift, fp_scale, fixed_point_multiplier, intermediate_bit_size) of the Requant after it and
+    out_sf, the ScalingFactor of the layer's output that the Requant targets"""
 
-    def __init__(self, kind, w=None, b=None, rq=None):
-        self.kind, self.w, self.b, self.rq = kind, w, b, rq
+    def __init__(self, kind, w=None, b=None, rq=None, out_sf=None):
+        self.kind, self.w, self.b, self.rq, self.out_sf = kind, w, b, rq, out_sf
 
 
-def quantize(fm):
-    """AbsoluteMax without a representative input: -> (list of QuantizedLayer with the requants, input scaling, output scaling)"""
-    sf = in_sf = ScalingFactor.default()
+def observe(fm, samples):
+    """InferenceObserver::new_with_representative_input (quantization/strategy.rs:72-146): run the float model on every sample and
+    take the input's and each node's output minimum and maximum over all samples (InferenceTracker, strategy.rs:148-187: plain
+    min / max as f32, the percentile lines there are commented out); each scaling is from_absolute_max(max(|min|, |max|)).
+    samples: [n, *input_shape] in [-1, 1] of the unpadded model, which is what the reference observes: it quantises before it
+    pads (parser/mod.rs:89-90).  -> (input scaling, [output scaling of each Dense / Conv layer, None for the others]).  The float
+    inference is forward()'s, in float64; only the extremes are rounded to f32."""
+    x = np.asarray(samples, dtype=np.float32)
+    if x.size == 0:
+        raise ValueError("calibration: no samples; the reference then draws 10 inputs from its own RNG, which is not reproduced here")
+    if x.shape[1:] != fm.input_shape:
+        raise ValueError("calibration: expected samples of shape [n, %s], got %s"
+                         % (", ".join(map(str, fm.input_shape)), list(x.shape)))
+    if not np.all((x >= -1.0) & (x <= 1.0)):
+        raise ValueError("calibration: sample values must lie in [-1, 1] (the reference's QUANTIZATION_RANGE)")
+    lo = np.full(len(fm.layers) + 1, np.inf)
+    hi = -lo
+    for s in x:
+        for i, y in enumerate([s] + list(fm.outputs(s))):
+            lo[i], hi[i] = min(lo[i], y.min()), max(hi[i], y.max())
+    sfs = []
+    for i, (a, b) in enumerate(zip(lo, hi)):
+        if i > 0 and fm.layers[i - 1][0] not in ("dense", "conv"):
+            sfs.append(None)                      # Relu, MaxPool and flatten keep their input's scaling: theirs is not used
+            continue
+        m = max(abs(F32(a)), abs(F32(b)))
+        if m == 0:
+            raise ValueError("calibration: %s is zero on every sample, which gives a zero scaling factor"
+                             % ("the input" if i == 0 else "the output of layer %d (%s)" % (i - 1, fm.layers[i - 1][0])))
+        sfs.append(ScalingFactor.from_absolute_max(m))
+    return sfs[0], sfs[1:]
+
+
+def quantize(fm, calibration=None):
+    """-> (list of QuantizedLayer with the requants, input scaling, output scaling).  Without calibration: AbsoluteMax without a
+    representative input.  With calibration samples ([n, *input_shape]): InferenceObserver (observe()); each Dense / Conv requant
+    targets that layer's own observed output scaling, taken before any Relu (layers/dense.rs:243-285, layers/convolution.rs:579-597),
+    and Relu, MaxPool and flatten keep their input's scaling (layers/mod.rs:729-747)."""
+    if calibration is None:
+        in_sf, layer_sf = ScalingFactor.default(), [ScalingFactor.default()] * len(fm.layers)
+    else:
+        in_sf, layer_sf = observe(fm, calibration)
+    sf = in_sf
     out = []
-    for l in fm.layers:
+    for l, out_sf in zip(fm.layers, layer_sf):
         if l[0] in ("dense", "conv"):
             w, b = l[1], l[2]
             model_sf = ScalingFactor.from_absolute_max(max(np.abs(w).max(initial=F32(0)), np.abs(b).max(initial=F32(0))))
@@ -411,9 +460,8 @@ def quantize(fm):
                 bits = 2 * (BIT_LEN - 1) + _clog2(w.shape[1]) + 1                                      # dense.rs:415-420
             else:
                 bits = 2 * (BIT_LEN - 1) + _clog2(w.shape[1] * w.shape[2] * w.shape[3] + 1)            # convolution.rs:362-366
-            out_sf = ScalingFactor.default()
             rq = requant_from_multiplier(sf.m(model_sf, out_sf), bits) + (bits,)
-            out.append(QuantizedLayer(l[0], model_sf.quantize(w), bias_sf.quantize(b), rq))
+            out.append(QuantizedLayer(l[0], model_sf.quantize(w), bias_sf.quantize(b), rq, out_sf))
             sf = out_sf
         else:
             out.append(QuantizedLayer(l[0]))
@@ -461,13 +509,15 @@ def pad(fm, qlayers):
     return np.asarray(desc, dtype=np.int64), np.concatenate(data).astype(np.int64), int(np.prod(padded_in)), padded_in, cols
 
 
-def import_onnx(path_or_bytes):
-    """-> (desc, data, input_len, Metadata, FloatModel, quantised layers)"""
+def import_onnx(path_or_bytes, calibration=None):
+    """-> (desc, data, input_len, Metadata, FloatModel, quantised layers).  calibration: None for AbsoluteMax without a
+    representative input (the reference's default loader), or float samples [n, *input_shape] in [-1, 1] to quantise with the
+    InferenceObserver on them (quantize()); Metadata then carries the calibrated input and output scalings."""
     raw = path_or_bytes if isinstance(path_or_bytes, (bytes, bytearray)) else open(path_or_bytes, "rb").read()
     fm = load_float(bytes(raw))
     if not [l for l in fm.layers if l[0] != "relu"] or [l for l in fm.layers if l[0] != "relu"][-1][0] != "dense":
         raise ValueError("ONNX: the model must end in a dense layer (Gemm / MatMul), optionally followed by Relu")
-    qlayers, in_sf, out_sf = quantize(fm)
+    qlayers, in_sf, out_sf = quantize(fm, calibration)
     desc, data, input_len, padded_in, padded_out = pad(fm, qlayers)
     md = Metadata(in_sf, out_sf, fm.input_shape, padded_in, _check_shapes(fm)[0], padded_out)
     return desc, data, input_len, md, fm, qlayers
