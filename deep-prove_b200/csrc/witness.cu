@@ -10,9 +10,9 @@
 // histograms into the multiplicity polynomials.  Per proof only the model input crosses PCIe.
 // Values outside a table (a broken model/trace) raise an error flag that dp_wit_finish reports -- the reference panics there.
 #include "common.cuh"
+#include "quant.cuh"
 #include <algorithm>
 
-static constexpr long long WQMIN = -127, WQMAX = 127;     // quantization/mod.rs:28-29
 static constexpr u32 W_BIT_LEN = 8;
 __device__ __forceinline__ long long f2i(u64 f) { return f > (GL_P >> 1) ? -(long long)(GL_P - f) : (long long)f; }
 __device__ __forceinline__ u64 i2f(long long v) { return v < 0 ? GL_P - (u64)(-v) : (u64)v; }
@@ -60,29 +60,27 @@ __global__ void k_wit_matmul(const u64 *__restrict__ left, const u64 *__restrict
     out[i] = i2f(acc);
 }
 
-// ---- Requant: tmp = v * m + 2^(shift-1); cin = tmp >> shift; cout = clamp(cin); chunks = bytes of (tmp & (2^shift - 1)) ----
+// ---- Requant (rq_rule): cin = the clamping input, cout = the output; chunks = bytes of (tmp & (2^shift - 1)) ----
 struct RqCols { u64 *cin, *cout, *chunk[8]; u32 n_chunks; };
-__global__ void k_wit_requant(const u64 *__restrict__ x, u64 n, u32 shift, long long fpm, long long lim, RqCols c, u32 *clamp_counts, u32 clamp_size, u32 *range_counts, u32 *err) {
+__global__ void k_wit_requant(const u64 *__restrict__ x, u64 n, RqRule r, RqCols c, u32 *clamp_counts, u32 *range_counts, u32 *err) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const long long v = f2i(x[i]);
-    if (v > lim || v < -lim) atomicOr(err, 1u);              // "Could not apply requantisation, tensor element had absolute value too large"
-    const long long tmp = v * fpm + (1LL << (shift - 1)), cl = tmp >> shift;
-    const long long co = cl < WQMIN ? WQMIN : (cl > WQMAX ? WQMAX : cl);
-    const u64 sh = (u64)tmp & ((1ULL << shift) - 1);
-    c.cin[i] = i2f(cl); c.cout[i] = i2f(co);
-    const long long idx = cl + (1LL << (clamp_size - 1));
-    if (idx < 0 || idx >= (1LL << clamp_size)) atomicOr(err, 2u); else atomicAdd(clamp_counts + idx, 1u);
+    u32 e = 0;
+    const RqVal q = rq_rule(f2i(x[i]), r, e);
+    const u64 sh = (u64)q.tmp & ((1ULL << r.shift) - 1);
+    c.cin[i] = i2f(q.cl); c.cout[i] = i2f(q.out);
+    if (e) atomicOr(err, e);
+    if (!(e & 2u)) atomicAdd(clamp_counts + (q.cl + (1LL << (r.clamp_size - 1))), 1u);
     for (u32 j = 0; j < c.n_chunks; j++) { const u32 b = (u32)(sh >> (j * W_BIT_LEN)) & 255u; c.chunk[j][i] = b; atomicAdd(range_counts + b, 1u); }
 }
-// ---- Relu: out = max(v, 0); table rows are v = QMIN-1 .. QMAX ----
+// ---- Relu (relu_rule) ----
 __global__ void k_wit_relu(const u64 *__restrict__ x, u64 n, u64 *__restrict__ out, u32 *relu_counts, u32 *err) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const long long v = f2i(x[i]);
-    out[i] = v < 0 ? 0ULL : (u64)v;
-    const long long idx = v - (WQMIN - 1);
-    if (idx < 0 || idx > WQMAX - (WQMIN - 1)) atomicOr(err, 4u); else atomicAdd(relu_counts + idx, 1u);
+    u32 e = 0;
+    out[i] = (u64)relu_rule(v, e);
+    if (e) atomicOr(err, e); else atomicAdd(relu_counts + (v - (WQMIN - 1)), 1u);
 }
 // ---- Maxpool2D (kernel = stride = 2) on [C][H][W]: out = max of the 2x2 window; columns out - in(2r+dr, 2c+dc), (dr,dc) = (0,0),(1,0),(0,1),(1,1) ----
 struct PoolCols { u64 *out, *diff[4]; };
@@ -97,7 +95,9 @@ __global__ void k_wit_pool(const u64 *__restrict__ x, u32 C, u32 H, u32 W, PoolC
     for (int k = 0; k < 4; k++) {
         const long long d = mx - v[k];
         p.diff[k][oi] = (u64)d;
-        if (d > 255) atomicOr(err, 8u); else atomicAdd(range_counts + d, 1u);
+        u32 e = 0;
+        pool_rule(d, e);
+        if (e) atomicOr(err, e); else atomicAdd(range_counts + d, 1u);
     }
 }
 // ---- multiplicity polynomials: every table row is distinct in these tables (table_count == 1), so m[i] = count[i] ----
@@ -186,9 +186,9 @@ int dp_wit_requant(dp_wit *w, const dp_mle *x, uint32_t shift, int64_t fixed_poi
     c.cin = (u64 *)own[0]->data; c.cout = (u64 *)own[1]->data;
     for (u32 j = 0; j < c.n_chunks; j++) c.chunk[j] = (u64 *)own[2 + j]->data;
     DpProfScope prof("k_wit_requant", x->bytes() * (1 + n_cols));
-    DP_CUDA(dp_launch(k_wit_requant, (unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream, (const u64 *)x->data, x->len, shift, (long long)fixed_point_multiplier,
-                      1LL << intermediate_bit_size, c, w->counts + w->off[clamp_table], w->size[clamp_table], w->counts + w->off[range_table],
-                      w->counts + w->off[w->n_tables]));
+    const RqRule r{shift, w->size[clamp_table], (long long)fixed_point_multiplier, 1LL << intermediate_bit_size};
+    DP_CUDA(dp_launch(k_wit_requant, (unsigned)((x->len + 255) / 256), 256, 0, dp_ctx().stream, (const u64 *)x->data, x->len, r, c,
+                      w->counts + w->off[clamp_table], w->counts + w->off[range_table], w->counts + w->off[w->n_tables]));
     wit_hand_over(own, cols);
     return DP_OK;
 }

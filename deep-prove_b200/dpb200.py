@@ -106,6 +106,9 @@ SIGNATURES = {
     "dp_wit_pool": (INT, [VP, VP, U32, U32, U32, U32, VP]),
     "dp_wit_finish": (INT, [VP, VP, VP]),
     "dp_wit_free": (INT, [VP]),
+    "dp_infer_plan": (INT, [VP, U32, U64, VP]),
+    "dp_infer_run": (INT, [VP, VP, U32, VP, VP]),
+    "dp_infer_free": (INT, [VP]),
     # test hook of libdeepprove_b200.so, not part of the ABI (csrc/context.cu)
     "dp_debug_wait_flag": (U64, [VP, U64, F64]),
     # ---- libdeepprove_host.so: host/capi.cpp ----
@@ -132,6 +135,7 @@ SIGNATURES = {
     "dph_zkml_trace_output": (INT, [VP, VP, U64, VP]),
     "dph_zkml_prove_batch": (INT, [VP, INT, U32, VP, U32, STR, VP, U64, VP, VP, VP, VP]),
     "dph_zkml_job_error": (STR, [VP, U32]),
+    "dph_zkml_infer_batch": (INT, [VP, VP, U32, VP, VP, VP]),
     "dph_shm_mailbox_bytes": (U64, []),
     "dph_shm_allgather": (INT, [VP, U32, U32, VP, VP, U64, VP]),
     "dph_sumcheck_prove_sharded": (INT, [U32, U32, VP, U32, VP, U32, U32, STR, VP, VP, VP, VP, VP, VP, VP]),
@@ -684,6 +688,21 @@ class ZkmlContext:
         errors = [None if status[j] == 0 else host().dph_zkml_job_error(self.h, j).decode() for j in range(n)]
         return sec.value, [proofs[j, : int(lens[j])] for j in range(n)], outputs, status, errors
 
+    def infer_batch(self, inputs):
+        """The model's outputs for n inputs ([n, input_len] int64, each value in [-128, 127]) without proving, on the int8 tensor
+        cores (dph_zkml_infer_batch): the same outputs and per-input failures as prove_batch.  Returns (seconds, outputs [n,
+        output_len] int64, status, errors)."""
+        x = np.ascontiguousarray(inputs, dtype=np.int64)
+        if x.ndim != 2 or x.shape[0] == 0 or x.shape[1] != self.input_len:
+            raise ValueError("infer_batch: inputs must be [n >= 1, %d]" % self.input_len)
+        n = x.shape[0]
+        outputs = np.zeros((n, self.output_len), dtype=np.int64)
+        status = np.zeros(n, dtype=np.int32)
+        sec = C.c_double()
+        hcheck(host().dph_zkml_infer_batch(self.h, _ptr(x), n, _ptr(outputs), _ptr(status), C.byref(sec)))
+        errors = [None if status[j] == 0 else host().dph_zkml_job_error(self.h, j).decode() for j in range(n)]
+        return sec.value, outputs, status, errors
+
     def free(self):
         if self.h:
             host().dph_zkml_context_free(self.h)
@@ -726,6 +745,16 @@ class ModelContext(ZkmlContext):
         x = self.metadata.quantize_input(x.reshape((-1,) + self.metadata.input_shape))
         _, proofs, outputs, status, errors = self.prove_batch(x, n_workers, device, label, stride)
         return proofs, outputs, self.metadata.dequantize_output(outputs), status, errors
+
+    def infer_batch_float(self, inputs):
+        """infer_batch on float inputs ([n, *input shape] in [-1, 1]) of a model made by from_onnx: quantises each input with
+        .metadata, infers them all without proving, and returns (outputs, float_outputs, status, errors) as prove_batch_float does"""
+        if self.metadata is None:
+            raise ValueError("infer_batch_float: the context has no quantisation metadata (build it with ModelContext.from_onnx)")
+        x = np.asarray(inputs, dtype=np.float32)
+        x = self.metadata.quantize_input(x.reshape((-1,) + self.metadata.input_shape))
+        _, outputs, status, errors = self.infer_batch(x)
+        return outputs, self.metadata.dequantize_output(outputs), status, errors
 
 
 def sumcheck_prove_batch_polys(T, mles, products, max_nv, label=b"m2vec"):

@@ -149,7 +149,10 @@ int dph_pcs_open(dp_mle *poly, uint32_t full_log, const uint64_t *point, const c
 #include "zkml.hpp"
 #include <chrono>
 namespace {
-struct ZkHandle { dp::zkml::Model model; dp::zkml::Context ctx; dp::zkml::DeviceTrace trace; std::vector<dp::zkml::Element> trace_input; };   // the stored trace lives in HBM
+struct ZkHandle {   // the stored trace lives in HBM; the batch-inference plan is built by the first dph_zkml_infer_batch
+    dp::zkml::Model model; dp::zkml::Context ctx; dp::zkml::DeviceTrace trace; std::vector<dp::zkml::Element> trace_input;
+    std::unique_ptr<dp::zkml::InferPlan> plan;
+};
 }
 extern "C" {
 
@@ -272,6 +275,15 @@ std::mutex g_pools_mu; std::map<void *, std::unique_ptr<ZkPool>> g_pools;
 }
 extern "C" void dph_zkml_pool_free(void *handle) { std::lock_guard<std::mutex> lk(g_pools_mu); g_pools.erase(handle); }
 namespace {
+// The handle's pool (made on first use, without threads), marked busy for the caller; refused when another call holds it
+ZkPool *acquire_pool(void *handle) {
+    ZkPool *pool;
+    { std::lock_guard<std::mutex> lk(g_pools_mu); auto &pp = g_pools[handle]; if (!pp) { pp = std::make_unique<ZkPool>(); pp->h = (ZkHandle *)handle; } pool = pp.get(); }
+    std::lock_guard<std::mutex> lk(pool->mu);
+    if (pool->busy) throw dp::Error(DP_ERR_STATE, "the handle's worker pool is busy with another call");
+    pool->busy = true;
+    return pool;
+}
 struct AllOut { uint64_t *out; uint64_t stride; uint64_t *lens; uint32_t *worker; };
 struct BatchIo { const int64_t *in; int64_t *outputs; int32_t *status; };
 int prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_proofs, int e2e, const char *label, double *out_seconds,
@@ -280,8 +292,8 @@ int prove_concurrent(void *handle, int device, uint32_t n_workers, uint32_t n_pr
     ZkHandle *h = (ZkHandle *)handle;
     if (!batch.in && !h->trace.valid()) throw dp::Error(DP_ERR_STATE, "dph_zkml_prove_concurrent: run inference first (mode 1)");
     ZkPool *pool;
-    { std::lock_guard<std::mutex> lk(g_pools_mu); auto &pp = g_pools[handle]; if (!pp) { pp = std::make_unique<ZkPool>(); pp->h = h; pp->device = device; } pool = pp.get(); }
-    { std::lock_guard<std::mutex> lk(pool->mu); if (pool->busy) throw dp::Error(DP_ERR_STATE, "the handle's worker pool is busy with another call"); pool->busy = true; }
+    pool = acquire_pool(handle);
+    { std::lock_guard<std::mutex> lk(pool->mu); if (pool->th.empty()) pool->device = device; }
     while (pool->th.size() < n_workers) { const uint32_t idx = (uint32_t)pool->th.size(); pool->th.emplace_back([pool, idx] { pool->worker(idx); }); }
     auto t0 = std::chrono::steady_clock::now();
     {
@@ -323,7 +335,7 @@ extern "C" int dph_zkml_prove_concurrent_all(void *handle, int device, uint32_t 
 // input j's flat proof goes to proofs + j * stride, its length in words to proof_lens[j], its model output (output_len elements,
 // dph_zkml_output_len) to outputs + j * output_len and its status to status[j].  Slots are indexed by input.  An input that fails
 // (a value outside its lookup table, say) fails alone: status[j] != 0, proof_lens[j] = 0, and dph_zkml_job_error(handle, j) holds
-// its message until the next batch call on the handle.  Non-zero only for call-level errors: an argument refused, no device, a
+// its message until the next batch or infer call on the handle.  Non-zero only for call-level errors: an argument refused, no device, a
 // busy pool (DP_ERR_STATE), or a proof longer than `stride` (DP_ERR_INVALID, after the batch).  The stored trace is not touched.
 extern "C" int dph_zkml_prove_batch(void *handle, int device, uint32_t n_workers, const int64_t *inputs, uint32_t n, const char *label,
                                     uint64_t *proofs, uint64_t stride, uint64_t *proof_lens, int64_t *outputs, int32_t *status, double *out_seconds) {
@@ -339,7 +351,40 @@ extern "C" int dph_zkml_prove_batch(void *handle, int device, uint32_t n_workers
                             BatchIo{inputs, outputs, status});
     DPH_CATCH
 }
-// The message of job j of the handle's last batch call, or NULL when job j succeeded (or there is no such job)
+// n inputs (inputs: n x input_len) through the model without proving (csrc/infer.cu): input j's model output goes to outputs + j *
+// output_len (dph_zkml_output_len), in the same padded layout and with the same values as the stored trace's, and its status to
+// status[j].  The calling thread's device context runs it; the plan is built on the first call and kept until the context is freed.
+// An input fails alone with the status and message dph_zkml_prove_batch gives it (dph_zkml_job_error(handle, j), until the next
+// batch or infer call on the handle), and so does an input with a value outside [-128, 127]: the batch inference takes 8-bit inputs.
+// Non-zero for call-level errors: an argument refused, no device, a busy pool (DP_ERR_STATE), a model the plan refuses
+// (DP_ERR_INVALID, naming the node).  *out_seconds (optional): the inference's wall time, plan building excluded.  The stored trace
+// is not touched.
+extern "C" int dph_zkml_infer_batch(void *handle, const int64_t *inputs, uint32_t n, int64_t *outputs, int32_t *status, double *out_seconds) {
+    DPH_TRY
+    if (n == 0) throw Error(DP_ERR_INVALID, "dph_zkml_infer_batch: no inputs");
+    if (!inputs || !outputs || !status) throw Error(DP_ERR_INVALID, "dph_zkml_infer_batch: null argument");
+    if (dp_device_count() <= 0) throw Error(DP_ERR_NO_DEVICE, "dph_zkml_infer_batch: no CUDA device visible (no CPU fallback)");
+    if (!handle) throw Error(DP_ERR_INVALID, "dph_zkml_infer_batch: null handle");
+    ZkHandle *h = (ZkHandle *)handle;
+    ZkPool *pool = acquire_pool(handle);
+    struct Release { ZkPool *p; ~Release() { std::lock_guard<std::mutex> lk(p->mu); p->busy = false; } } release{pool};
+    { std::lock_guard<std::mutex> lk(pool->mu); pool->job_err.assign(n, std::string()); }
+    if (!h->plan) h->plan = std::make_unique<dp::zkml::InferPlan>(h->model);
+    std::vector<uint32_t> bits(n);
+    auto t0 = std::chrono::steady_clock::now();
+    check(dp_infer_run(h->plan->get(), inputs, n, outputs, bits.data()));
+    if (out_seconds) *out_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    std::lock_guard<std::mutex> lk(pool->mu);
+    for (uint32_t j = 0; j < n; j++) {
+        status[j] = bits[j] ? DP_ERR_INVALID : 0;
+        if (bits[j] & 16) pool->job_err[j] = "dph_zkml_infer_batch: an input value lies outside [-128, 127] (the batch inference takes 8-bit inputs)";
+        else if (bits[j]) pool->job_err[j] = dp::zkml::lookup_error_message(bits[j]);
+    }
+    return 0;
+    DPH_CATCH
+}
+
+// The message of job j of the handle's last batch or infer call, or NULL when job j succeeded (or there is no such job)
 extern "C" const char *dph_zkml_job_error(void *handle, uint32_t j) {
     std::lock_guard<std::mutex> lk(g_pools_mu);
     auto it = g_pools.find(handle);

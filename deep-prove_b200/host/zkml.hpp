@@ -274,6 +274,12 @@ struct DeviceTrace {
     const DeviceMle &node_input(size_t id) const { return id == 0 ? input : outs[id - 1]; }
 };
 
+// The message of a non-zero lookup error word (dp_wit_finish, dp_infer_run)
+inline const char *lookup_error_message(uint32_t bits) {
+    return bits & 1 ? "Could not apply requantisation, tensor element had absolute value too large"
+                    : "lookup witness: a value is not in its table (clamping / relu / pooling range)";
+}
+
 // One lookup-witness pass (csrc/witness.cu): a dp_wit over the Context's tables in TableType order (the reference's BTreeMap
 // order), whose histograms the node kernels fill; finish() turns them into the multiplicity polynomials.
 class LookupPass {
@@ -309,8 +315,7 @@ class LookupPass {
         std::vector<dp_mle *> raw(index_.size(), nullptr); uint32_t bits = 0;
         check(dp_wit_finish(w_, raw.data(), &bits));
         std::map<TableType, DeviceMle> mults; for (auto &kv : index_) mults[kv.first] = DeviceMle(raw[kv.second]);
-        if (bits & 1) throw Error(DP_ERR_INVALID, "Could not apply requantisation, tensor element had absolute value too large");
-        if (bits) throw Error(DP_ERR_INVALID, "lookup witness: a value is not in its table (clamping / relu / pooling range)");
+        if (bits) throw Error(DP_ERR_INVALID, lookup_error_message(bits));
         return mults;
     }
   private:
@@ -336,6 +341,36 @@ inline DeviceTrace run_device(const Context &ctx, const std::vector<Element> &in
     wit.finish();
     return tr;
 }
+
+// The model's batch-inference plan (csrc/infer.cu): the nodes as dp_infer_node, handed over once; the device keeps what it needs
+class InferPlan {
+  public:
+    explicit InferPlan(const Model &m) {
+        std::vector<dp_infer_node> v(m.nodes.size());
+        for (size_t i = 0; i < m.nodes.size(); i++) {
+            const Node &n = m.nodes[i]; dp_infer_node &d = v[i];
+            d = dp_infer_node{}; d.kind = (uint32_t)n.op;    // Op follows the layer-descriptor kinds
+            auto dims = [&](std::initializer_list<size_t> l) { uint32_t k = 0; for (size_t x : l) d.dims[k++] = (uint32_t)x; };
+            if (n.op == Op::Dense) dims({n.nrows, n.ncols});
+            else if (n.op == Op::Conv) dims({n.kw, n.kx, n.nw, n.real_nw, n.unpadded_out[0], n.unpadded_out[1], n.unpadded_out[2]});
+            else if (n.op == Op::Pool) dims({n.pool_c, n.pool_h, n.pool_w});
+            else if (n.op == Op::MatMul) dims({n.mm_r, n.mm_k, n.mm_c, n.mm_t ? 1u : 0u});
+            else if (n.op == Op::Requant) {
+                d.shift = (uint32_t)n.rq.shift(); d.clamp_size = (uint32_t)n.rq.clamping_size();
+                d.intermediate_bits = (uint32_t)n.rq.intermediate_bit_size; d.multiplier = n.rq.fixed_point_multiplier;
+            }
+            d.weights = n.weights.empty() ? nullptr : n.weights.data();
+            d.bias = n.bias.empty() ? nullptr : n.bias.data();
+        }
+        check(dp_infer_plan(v.data(), (uint32_t)v.size(), m.input_len, &p_));
+    }
+    ~InferPlan() { if (p_) dp_infer_free(p_); }
+    InferPlan(const InferPlan &) = delete;
+    InferPlan &operator=(const InferPlan &) = delete;
+    dp_infer *get() const { return p_; }
+  private:
+    dp_infer *p_ = nullptr;
+};
 
 // Prover<'a, E, T, PCS> (iop/prover.rs:40-60)
 template <class T>

@@ -316,6 +316,32 @@ int dp_wit_pool(dp_wit *w, const dp_mle *x, uint32_t C, uint32_t H, uint32_t W, 
 int dp_wit_finish(dp_wit *w, dp_mle **mults, uint32_t *error_bits);
 int dp_wit_free(dp_wit *w);
 
+/* ---- batch inference without proving (csrc/infer.cu) ------------------------------------------------------------------
+ * The model's integer outputs for many inputs at once, exactly as the witness path computes them (same values, same error bits),
+ * with every Dense / MatMul / Convolution on the int8 tensor cores (int32 accumulation).  A plan is built once per model from its
+ * nodes; each run takes host inputs and writes host outputs in the padded layout of the last node's output tensor.
+ * The plan refuses (DP_ERR_INVALID, naming the node): a weight outside [-128, 127], a bias outside int32, a Dense / MatMul /
+ * Convolution whose input is not 8-bit (not the model input nor a Requant output, optionally through Relu and/or Maxpool), an
+ * output row or channel with 128 * sum|w| + |b| > 2^31 - 1 (int32 accumulation would not be exact), and shapes that do not chain. */
+typedef struct dp_infer dp_infer;
+typedef struct dp_infer_node {
+    uint32_t kind;        /* the layer-descriptor kinds: 0 Dense, 1 Requant, 2 Relu, 3 Convolution, 4 Maxpool (2x2, stride 2), 5 MatMul */
+    uint32_t dims[7];     /* Dense {nrows, ncols}; Convolution {kw, kx, nw, real_nw, unpadded_out[3]}; Maxpool {C, H, W};
+                             MatMul {R, K, C, transposed} */
+    uint32_t shift, clamp_size, intermediate_bits;   /* Requant: fp_scale + right_shift, the clamping table's bits, log2 of the input bound */
+    int64_t multiplier;                              /* Requant: fixed_point_multiplier */
+    const int64_t *weights, *bias;   /* Dense [nrows][ncols] + [nrows]; Convolution [kw][kx][real_nw][real_nw] + [kw];
+                                        MatMul [K][C] ([C][K] when transposed) + [C] or NULL; read during dp_infer_plan only */
+} dp_infer_node;
+/* Inputs per device pass: a run processes its batch in chunks of at most this many inputs, fewer when free device memory is short. */
+#define DP_INFER_MAX_CHUNK 4096
+int dp_infer_plan(const dp_infer_node *nodes, uint32_t n_nodes, uint64_t input_len, dp_infer **out);
+/* inputs: n x input_len; outputs: n x (the last node's output length); err_bits[j]: input j's lookup error bits as dp_wit_finish
+ * reports them (1 requant input too large, 2 clamping, 4 relu, 8 pooling), plus 16 when one of its values lies outside [-128, 127]
+ * (such an input is computed as zeros).  Runs on the calling thread's context and stream; returns when the outputs are written. */
+int dp_infer_run(dp_infer *p, const int64_t *inputs, uint32_t n, int64_t *outputs, uint32_t *err_bits);
+int dp_infer_free(dp_infer *p);
+
 #ifdef __cplusplus
 }
 #endif
