@@ -21,7 +21,7 @@ all: product host oracle tools
 
 product: $(PKG)/libdeepprove_b200.so
 host: $(PKG)/libdeepprove_host.so
-oracle: oracle/libdp_oracle.so tests/libdp_oracle_model_io.so
+oracle: oracle/libdp_oracle.so tests/libdp_oracle_model_io.so tests/libdp_stream_queue_io.so
 
 build/%.o: $(CSRC)/%.cu $(CU_HDRS)
 	@mkdir -p build
@@ -38,6 +38,10 @@ oracle/libdp_oracle.so: $(ORC_SRCS) $(ORC_HDRS)
 
 tests/libdp_oracle_model_io.so: tests/oracle_model_io.cpp $(ORC_HDRS)
 	$(CXX) -O3 -march=x86-64-v3 -std=c++17 -fPIC -shared -Wall -o $@ tests/oracle_model_io.cpp -lpthread
+
+# the proof stream's queue under a fake job (tests/test_prove_stream_abi.py): no device needed
+tests/libdp_stream_queue_io.so: tests/stream_queue_io.cpp $(PKG)/host/proof_queue.hpp include/deepprove_b200.h
+	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -o $@ tests/stream_queue_io.cpp -lpthread
 
 # device-vs-host self test of the field primitives and Poseidon2 (run by tests/test_gpu_baseline_size.py on the GPU box)
 tools: $(PKG)/gl_selftest_bin

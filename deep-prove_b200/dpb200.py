@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libdeepprove_b200.so")
 HOST_LIB_PATH = os.path.join(_HERE, "libdeepprove_host.so")
 
 P = 0xFFFFFFFF00000001
-DP_OK, DP_ERR_INVALID, DP_ERR_CUDA, DP_ERR_NO_DEVICE, DP_ERR_STATE, DP_ERR_UNSUPPORTED = range(6)
+DP_OK, DP_ERR_INVALID, DP_ERR_CUDA, DP_ERR_NO_DEVICE, DP_ERR_STATE, DP_ERR_UNSUPPORTED, DP_ERR_TIMEOUT = range(7)
 
 # Every entry point's C signature, applied once when lib() / host() load the library.  One rule: every pointer, handle, array,
 # out-parameter and callback is VP; a C string is STR; restype is given for every return (INT for `int`, None for `void`).
@@ -136,6 +136,10 @@ SIGNATURES = {
     "dph_zkml_prove_batch": (INT, [VP, INT, U32, VP, U32, STR, VP, U64, VP, VP, VP, VP]),
     "dph_zkml_job_error": (STR, [VP, U32]),
     "dph_zkml_infer_batch": (INT, [VP, VP, U32, VP, VP, VP]),
+    "dph_zkml_stream_open": (INT, [VP, INT, U32, STR, U64, U32, VP]),
+    "dph_zkml_stream_submit": (INT, [VP, VP, U32, I64, VP]),
+    "dph_zkml_stream_next": (INT, [VP, I64, VP, VP, VP, VP, VP, VP, U64]),
+    "dph_zkml_stream_close": (INT, [VP, VP]),
     "dph_shm_mailbox_bytes": (U64, []),
     "dph_shm_allgather": (INT, [VP, U32, U32, VP, VP, U64, VP]),
     "dph_sumcheck_prove_sharded": (INT, [U32, U32, VP, U32, VP, U32, U32, STR, VP, VP, VP, VP, VP, VP, VP]),
@@ -668,16 +672,7 @@ class ZkmlContext:
             raise ValueError("prove_batch: inputs must be [n >= 1, %d]" % self.input_len)
         n = x.shape[0]
         if stride is None:
-            if getattr(self, "_proof_words", None) is None:
-                one = np.zeros(1 << 23, dtype=np.uint64)
-                lens, st = np.zeros(1, dtype=np.uint64), np.zeros(1, dtype=np.int32)
-                y = np.zeros(self.output_len, dtype=np.int64)
-                hcheck(host().dph_zkml_prove_batch(self.h, int(device), 1, _ptr(x[:1]), 1, label, _ptr(one), one.size, _ptr(lens), _ptr(y),
-                                                   _ptr(st), None))
-                if st[0] != 0:
-                    raise DpError(int(st[0]), "sizing the proof stride on input 0: %s" % host().dph_zkml_job_error(self.h, 0).decode())
-                self._proof_words = int(lens[0])
-            stride = self._proof_words
+            stride = self._default_stride(x[0], device, label)
         proofs = np.zeros((n, int(stride)), dtype=np.uint64)
         lens = np.zeros(n, dtype=np.uint64)
         outputs = np.zeros((n, self.output_len), dtype=np.int64)
@@ -687,6 +682,29 @@ class ZkmlContext:
                                            _ptr(outputs), _ptr(status), C.byref(sec)))
         errors = [None if status[j] == 0 else host().dph_zkml_job_error(self.h, j).decode() for j in range(n)]
         return sec.value, [proofs[j, : int(lens[j])] for j in range(n)], outputs, status, errors
+
+    def _default_stride(self, x, device, label):
+        """the length of one proof of this model: measured once, by proving input x, and kept"""
+        if getattr(self, "_proof_words", None) is None:
+            one = np.zeros(1 << 23, dtype=np.uint64)
+            lens, st = np.zeros(1, dtype=np.uint64), np.zeros(1, dtype=np.int32)
+            y = np.zeros(self.output_len, dtype=np.int64)
+            x = np.ascontiguousarray(x, dtype=np.int64)
+            hcheck(host().dph_zkml_prove_batch(self.h, int(device), 1, _ptr(x), 1, label, _ptr(one), one.size, _ptr(lens), _ptr(y),
+                                               _ptr(st), None))
+            if st[0] != 0:
+                raise DpError(int(st[0]), "sizing the proof stride on input 0: %s" % host().dph_zkml_job_error(self.h, 0).decode())
+            self._proof_words = int(lens[0])
+        return self._proof_words
+
+    def open_stream(self, n_workers, device=0, label=b"m2vec", stride=None, capacity=None):
+        """A ProofStream on the handle's worker pool (dph_zkml_stream_open): submit inputs while proofs run and collect each result
+        when its proof finishes.  The pool is held until the stream closes.  stride: the longest proof a job may return (default:
+        prove_batch's, which proves one all-zero input the first time); capacity: jobs submitted and not yet collected (default
+        4 * n_workers)."""
+        if stride is None:
+            stride = self._default_stride(np.zeros(self.input_len, dtype=np.int64), device, label)
+        return ProofStream(self, n_workers, device, label, stride, 4 * int(n_workers) if capacity is None else capacity)
 
     def infer_batch(self, inputs):
         """The model's outputs for n inputs ([n, input_len] int64, each value in [-128, 127]) without proving, on the int8 tensor
@@ -705,6 +723,8 @@ class ZkmlContext:
 
     def free(self):
         if self.h:
+            if getattr(self, "_stream", None) is not None:     # dph_zkml_context_free closes it
+                self._stream.h, self._stream = C.c_void_p(), None
             host().dph_zkml_context_free(self.h)
             self.h = C.c_void_p()
 
@@ -713,6 +733,108 @@ class ZkmlContext:
             self.free()
         except Exception:
             pass
+
+
+class StreamTimeout(DpError):
+    """a ProofStream wait ran out (DP_ERR_TIMEOUT)"""
+
+
+class StreamResult:
+    """One finished stream job: ticket, proof (flat, empty when the job failed), output (int64, the padded layout; zeros when it
+    failed), status (0 or its error code), error (None or its message) and output_float (the dequantised real output entries for a
+    model made by ModelContext.from_onnx, else None)."""
+    __slots__ = ("ticket", "proof", "output", "status", "error", "output_float")
+
+    def __init__(self, ticket, proof, output, status, error, output_float):
+        self.ticket, self.proof, self.output, self.status, self.error, self.output_float = ticket, proof, output, status, error, output_float
+
+
+def _ms(timeout):
+    """seconds (None: for ever) as the C ABI's timeout_ms"""
+    return -1 if timeout is None else max(0, int(round(float(timeout) * 1000)))
+
+
+class ProofStream:
+    """dph_zkml_stream_*: inputs submitted while proofs run, each result collected when its proof finishes, in completion order.
+    Each job is what prove_batch does for one input, except that a proof longer than the stride fails that job alone.  Made by
+    ZkmlContext.open_stream; a context manager.  submit and next may be called from different threads at once."""
+
+    def __init__(self, ctx, n_workers, device, label, stride, capacity):
+        self.ctx, self.stride, self.capacity = ctx, int(stride), int(capacity)
+        self._output_len = ctx.output_len
+        self.h = C.c_void_p()
+        hcheck(host().dph_zkml_stream_open(ctx.h, int(device), int(n_workers), label, self.stride, self.capacity, C.byref(self.h)))
+        ctx._stream = self
+
+    def _check(self, rc):
+        if rc == DP_ERR_TIMEOUT:
+            raise StreamTimeout(rc, host().dph_last_error().decode())
+        hcheck(rc)
+
+    def _open(self):
+        if not self.h:
+            raise DpError(DP_ERR_STATE, "the stream is closed")
+
+    def submit(self, inputs, timeout=None):
+        """Queue inputs ([n, input_len] int64, or one [input_len]); all or nothing.  Waits up to `timeout` seconds (None: for ever, 0:
+        not at all) for room in the capacity, else raises StreamTimeout.  Returns their tickets (uint64, consecutive)."""
+        self._open()
+        x = np.ascontiguousarray(inputs, dtype=np.int64)
+        x = x[None] if x.ndim == 1 else x
+        if x.ndim != 2 or x.shape[0] == 0 or x.shape[1] != self.ctx.input_len:
+            raise ValueError("submit: inputs must be [n >= 1, %d]" % self.ctx.input_len)
+        first = C.c_uint64()
+        self._check(host().dph_zkml_stream_submit(self.h, _ptr(x), x.shape[0], _ms(timeout), C.byref(first)))
+        return np.arange(first.value, first.value + x.shape[0], dtype=np.uint64)
+
+    def submit_float(self, inputs, timeout=None):
+        """submit on float inputs ([n, *input shape] or one [*input shape], in [-1, 1]) of a model made by ModelContext.from_onnx,
+        quantised with its metadata as prove_batch_float does"""
+        md = getattr(self.ctx, "metadata", None)
+        if md is None:
+            raise ValueError("submit_float: the context has no quantisation metadata (build it with ModelContext.from_onnx)")
+        return self.submit(md.quantize_input(np.asarray(inputs, dtype=np.float32)), timeout)
+
+    def next(self, timeout=None):
+        """The next finished job as a StreamResult.  Raises StreamTimeout when none finishes within `timeout` seconds (None: for
+        ever), and DpError DP_ERR_STATE at once when nothing submitted is left to collect."""
+        self._open()
+        proof = np.empty(self.stride, dtype=np.uint64)
+        out = np.empty(self._output_len, dtype=np.int64)
+        ticket, plen, st = C.c_uint64(), C.c_uint64(), C.c_int32()
+        msg = C.create_string_buffer(1024)
+        self._check(host().dph_zkml_stream_next(self.h, _ms(timeout), C.byref(ticket), _ptr(proof), C.byref(plen), _ptr(out), C.byref(st),
+                                                C.cast(msg, C.c_void_p), len(msg)))
+        md = getattr(self.ctx, "metadata", None)
+        return StreamResult(ticket.value, proof[: plen.value].copy(), out, st.value, msg.value.decode() if st.value else None,
+                            None if md is None else md.dequantize_output(out))
+
+    def results(self, timeout=None):
+        """Yields results until everything submitted so far has been collected"""
+        while True:
+            try:
+                r = self.next(timeout)
+            except DpError as e:
+                if e.code == DP_ERR_STATE:
+                    return
+                raise
+            yield r
+
+    def close(self):
+        """Cancel the jobs no worker has started, wait for the running ones, drop uncollected results and release the pool.
+        Returns the number cancelled (0 when already closed)."""
+        if not self.h:
+            return 0
+        n = C.c_uint64()
+        hcheck(host().dph_zkml_stream_close(self.h, C.byref(n)))
+        self.h, self.ctx._stream = C.c_void_p(), None
+        return n.value
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class ModelContext(ZkmlContext):

@@ -203,7 +203,19 @@ int dph_zkml_trace_output(void *handle, int64_t *out, uint64_t cap, uint64_t *ou
 #include <mutex>
 #include <atomic>
 #include <condition_variable>
+#include "proof_queue.hpp"
 namespace {
+// Input x of the handle's model end to end, as one job of a batch or of a stream: inference, Prover::prove, the flat proof and the
+// model output in host memory
+void prove_input(ZkHandle *h, dp::zkml::Prover<dp::DynTranscript> &prover, const int64_t *x, std::vector<uint64_t> &flat,
+                 std::vector<dp::zkml::Element> &y) {
+    const size_t w = h->model.input_len;
+    dp::zkml::DeviceTrace tr = dp::zkml::run_device(h->ctx, std::vector<dp::zkml::Element>(x, x + w));
+    flat = prover.prove(tr).flatten(h->model.nodes.size());
+    y = dp::zkml::to_elements(tr.outs.back());
+    if (y.size() != h->model.output_len()) throw dp::Error(DP_ERR_STATE, "zkml prover: model output of unexpected length");
+}
+struct ZkStream;
 struct ZkPool {
     std::vector<std::thread> th; std::mutex mu; std::condition_variable cv, done_cv;
     ZkHandle *h = nullptr; int device = 0; bool stop = false, busy = false; uint64_t pending = 0, inflight = 0; std::string label, err; bool failed = false; bool e2e = false;
@@ -219,11 +231,25 @@ struct ZkPool {
     // proofs this pool has already run -- the first call of a pool is not staggered): latency-bound and GPU-bound phases of
     // different proofs then overlap.  The ramp-up and ramp-down this costs are inside the caller's timed region.
     uint32_t active = 0; uint64_t call_gen = 0; double stagger_s = 0.0, avg_proof_s = 0.0; uint64_t n_timed = 0;
+    // The open stream (dph_zkml_stream_open), which the first `active` threads serve until it closes; stream_gen counts streams,
+    // so each thread joins each stream once
+    ZkStream *stream = nullptr; bool stream_closing = false; uint64_t stream_gen = 0;
+    void serve_stream(uint32_t idx, ZkStream &s, bool &inited);
+    void time_proof(double sec) { std::lock_guard<std::mutex> lk(mu); n_timed++; avg_proof_s += (sec - avg_proof_s) / (double)std::min<uint64_t>(n_timed, 64); }
     void worker(uint32_t idx) {
-        bool inited = false; uint64_t seen_gen = 0;
+        bool inited = false; uint64_t seen_gen = 0, seen_stream = 0;
         for (;;) {
-            uint64_t gen, job; double delay = 0.0; bool keep = false, all = false, batch = false;
-            { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || (pending > 0 && idx < active); }); if (stop) break; pending--; inflight++; keep = pending == 0 && out; all = all_out != nullptr; batch = in != nullptr; job = next_job++; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } }
+            uint64_t gen, job; double delay = 0.0; bool keep = false, all = false, batch = false; ZkStream *joined = nullptr;
+            { std::unique_lock<std::mutex> lk(mu);
+              cv.wait(lk, [&] { return stop || (pending > 0 && idx < active) || (stream && !stream_closing && idx < active && stream_gen != seen_stream); });
+              if (stop) break;
+              if (pending == 0) { joined = stream; seen_stream = stream_gen; inflight++; }
+              else { pending--; inflight++; keep = pending == 0 && out; all = all_out != nullptr; batch = in != nullptr; job = next_job++; gen = call_gen; if (gen != seen_gen) { seen_gen = gen; delay = stagger_s * idx; } } }
+            if (joined) {
+                serve_stream(idx, *joined, inited);
+                std::lock_guard<std::mutex> lk(mu); inflight--; if (inflight == 0) done_cv.notify_all();
+                continue;
+            }
             try {
                 const bool first_ever = !inited;     // grows this thread's device arena: not a representative duration
                 if (!inited) { dp::check(dp_init(device)); inited = true; }
@@ -233,11 +259,9 @@ struct ZkPool {
                 dp::zkml::Prover<dp::DynTranscript> prover(h->ctx, t);
                 std::vector<uint64_t> flat;
                 if (batch) {   // the caller's input `job`: inference, prove, serialised proof and model output in host memory
-                    const size_t w = h->model.input_len, ol = h->model.output_len();
-                    dp::zkml::DeviceTrace tr = dp::zkml::run_device(h->ctx, std::vector<dp::zkml::Element>(in + job * w, in + (job + 1) * w));
-                    flat = prover.prove(tr).flatten(h->model.nodes.size());
-                    const std::vector<dp::zkml::Element> y = dp::zkml::to_elements(tr.outs.back());
-                    if (y.size() != ol) throw dp::Error(DP_ERR_STATE, "dph_zkml_prove_batch: model output of unexpected length");
+                    const size_t ol = h->model.output_len();
+                    std::vector<dp::zkml::Element> y;
+                    prove_input(h, prover, in + job * h->model.input_len, flat, y);
                     if (flat.size() > all_stride) { std::lock_guard<std::mutex> lk(mu); failed = true; err = "dph_zkml_prove_batch: proof longer than the stride"; throw dp::Error(DP_ERR_INVALID, err); }
                     memcpy(outputs + job * ol, y.data(), 8 * ol);
                 } else if (e2e) {   // from the host input vector: inference, prove, serialised proof in host memory
@@ -256,7 +280,7 @@ struct ZkPool {
                     memcpy(all_out + job * all_stride, flat.data(), 8 * flat.size());
                 }
                 const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-                if (!first_ever) { std::lock_guard<std::mutex> lk(mu); n_timed++; avg_proof_s += (sec - avg_proof_s) / (double)std::min<uint64_t>(n_timed, 64); }
+                if (!first_ever) time_proof(sec);
             } catch (const std::exception &e) {
                 std::lock_guard<std::mutex> lk(mu);
                 if (batch) {   // this job's failure only
@@ -271,9 +295,57 @@ struct ZkPool {
     }
     ~ZkPool() { { std::lock_guard<std::mutex> lk(mu); stop = true; } cv.notify_all(); for (auto &t : th) t.join(); }
 };
+struct ZkStream {
+    ZkPool *pool; uint32_t n_workers; uint64_t stride; std::string label; dp::ProofQueue q;
+    ZkStream(ZkPool *p, uint32_t nw, uint64_t st, const char *lb, uint64_t capacity)
+        : pool(p), n_workers(nw), stride(st), label(lb), q(p->h->model.input_len, capacity) {}
+};
+// One worker thread serving the stream: each job is one dph_zkml_prove_batch job (prove_input), except that a proof longer than the
+// stride fails that job alone.  Stagger rule: a thread delays only its first job of the stream, by the batch rule's stagger_s * idx,
+// and only when that job was taken from a backlog of at least 3 jobs per worker (the batch rule's bound); so a lone job on an idle
+// stream starts at once, and a large submit spreads the workers' phases as a large batch does.
+void ZkPool::serve_stream(uint32_t idx, ZkStream &s, bool &inited) {
+    bool first = true;
+    s.q.serve([&](const int64_t *x, uint64_t backlog, dp::QueueResult &r) {
+        try {
+            const bool first_ever = !inited;
+            if (!inited) { dp::check(dp_init(device)); inited = true; }
+            double delay = 0.0;
+            if (first && s.n_workers > 1 && backlog >= 3ull * s.n_workers) { std::lock_guard<std::mutex> lk(mu); if (n_timed > 0) delay = avg_proof_s / s.n_workers * idx; }
+            first = false;
+            if (delay > 0.0) std::this_thread::sleep_for(std::chrono::duration<double>(delay));
+            auto t0 = std::chrono::steady_clock::now();
+            dp::DynTranscript t(s.label);
+            dp::zkml::Prover<dp::DynTranscript> prover(h->ctx, t);
+            prove_input(h, prover, x, r.proof, r.output);
+            if (r.proof.size() > s.stride) throw dp::Error(DP_ERR_INVALID, "dph_zkml_stream_next: proof longer than the stream's stride");
+            if (!first_ever) time_proof(std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
+        } catch (const std::exception &e) {
+            const dp::Error *de = dynamic_cast<const dp::Error *>(&e);
+            r.status = de && de->code ? de->code : 1; r.error = e.what();
+        }
+        dp_profile_flush();
+    });
+}
+// Closes a stream: cancels its queued jobs (returns their count), waits for the running ones and for the threads to leave it, and
+// releases the pool
+uint64_t close_stream(ZkStream *s) {
+    ZkPool *p = s->pool;
+    { std::lock_guard<std::mutex> lk(p->mu); p->stream_closing = true; }
+    const uint64_t cancelled = s->q.close();
+    { std::unique_lock<std::mutex> lk(p->mu); p->done_cv.wait(lk, [&] { return p->inflight == 0; }); p->stream = nullptr; p->stream_closing = false; p->busy = false; }
+    delete s;
+    return cancelled;
+}
 std::mutex g_pools_mu; std::map<void *, std::unique_ptr<ZkPool>> g_pools;
 }
-extern "C" void dph_zkml_pool_free(void *handle) { std::lock_guard<std::mutex> lk(g_pools_mu); g_pools.erase(handle); }
+// Frees the handle's pool, closing its open stream first
+extern "C" void dph_zkml_pool_free(void *handle) {
+    std::unique_ptr<ZkPool> p;
+    { std::lock_guard<std::mutex> lk(g_pools_mu); auto it = g_pools.find(handle); if (it == g_pools.end()) return; p = std::move(it->second); g_pools.erase(it); }
+    ZkStream *s; { std::lock_guard<std::mutex> lk(p->mu); s = p->stream_closing ? nullptr : p->stream; }
+    if (s) close_stream(s);
+}
 namespace {
 // The handle's pool (made on first use, without threads), marked busy for the caller; refused when another call holds it
 ZkPool *acquire_pool(void *handle) {
@@ -392,6 +464,74 @@ extern "C" const char *dph_zkml_job_error(void *handle, uint32_t j) {
     std::lock_guard<std::mutex> pl(it->second->mu);
     const std::vector<std::string> &e = it->second->job_err;
     return j < e.size() && !e[j].empty() ? e[j].c_str() : nullptr;
+}
+
+// ---- proof stream: inputs submitted while proofs run, each result collected when its proof finishes (proof_queue.hpp) ----
+// Opens a stream on the handle's worker pool (n_workers threads on `device`), which it holds until dph_zkml_stream_close: meanwhile
+// dph_zkml_prove_batch, dph_zkml_prove_concurrent[_all] and dph_zkml_infer_batch on the handle are refused (DP_ERR_STATE), as for a
+// busy pool.  Every job proves one input as dph_zkml_prove_batch does, under `label`.  `capacity` bounds the jobs submitted and not
+// yet collected; `stride` is the longest proof a job may return.  Refused: a null argument, n_workers or capacity 0, no device
+// (DP_ERR_NO_DEVICE), a device index out of range, a busy pool (DP_ERR_STATE).
+extern "C" int dph_zkml_stream_open(void *handle, int device, uint32_t n_workers, const char *label, uint64_t stride, uint32_t capacity,
+                                    void **stream) {
+    DPH_TRY
+    if (!label || !stream) throw Error(DP_ERR_INVALID, "dph_zkml_stream_open: null argument");
+    if (n_workers == 0 || capacity == 0) throw Error(DP_ERR_INVALID, "dph_zkml_stream_open: no workers or no capacity");
+    const int n_dev = dp_device_count();
+    if (n_dev <= 0) throw Error(DP_ERR_NO_DEVICE, "dph_zkml_stream_open: no CUDA device visible (no CPU fallback)");
+    if (device < 0 || device >= n_dev) throw Error(DP_ERR_INVALID, "dph_zkml_stream_open: device index out of range");
+    if (!handle) throw Error(DP_ERR_INVALID, "dph_zkml_stream_open: null handle");
+    ZkPool *pool = acquire_pool(handle);
+    ZkStream *s;
+    try {
+        s = new ZkStream(pool, n_workers, stride, label, capacity);
+        { std::lock_guard<std::mutex> lk(pool->mu); if (pool->th.empty()) pool->device = device; }
+        while (pool->th.size() < n_workers) { const uint32_t idx = (uint32_t)pool->th.size(); pool->th.emplace_back([pool, idx] { pool->worker(idx); }); }
+    } catch (...) { std::lock_guard<std::mutex> lk(pool->mu); pool->busy = false; throw; }
+    { std::lock_guard<std::mutex> lk(pool->mu); pool->stream = s; pool->active = n_workers; pool->stream_gen++; }
+    pool->cv.notify_all();
+    *stream = s;
+    return 0;
+    DPH_CATCH
+}
+// Copies n inputs (n x input_len int64; the caller may reuse its buffer at once) and queues them with the consecutive tickets
+// *first_ticket, ... (tickets count up from 0 in submission order across the stream's calls).  All or nothing: when the capacity has
+// no room for all n, waits up to timeout_ms (0: no wait, < 0: for ever), then DP_ERR_TIMEOUT with nothing submitted.
+// n > capacity is DP_ERR_INVALID.
+extern "C" int dph_zkml_stream_submit(void *stream, const int64_t *inputs, uint32_t n, int64_t timeout_ms, uint64_t *first_ticket) {
+    if (!stream) { g_herr = "dph_zkml_stream_submit: null stream"; return DP_ERR_INVALID; }
+    return ((ZkStream *)stream)->q.submit(inputs, n, timeout_ms, first_ticket, g_herr);
+}
+// One finished job, in completion order: its ticket, its flat proof (at most stride words) and length, its model output (output_len
+// elements, dph_zkml_output_len) and its status.  A job fails alone, as in dph_zkml_prove_batch: status != 0, proof_len 0, output
+// zeros, and msg (msg_cap bytes, NUL-terminated, optional) holds the message dph_zkml_prove_batch gives that input; msg is empty for a
+// proved job.  Unlike dph_zkml_prove_batch, a proof longer than the stride fails only its own job (DP_ERR_INVALID).  The call returns
+// DP_ERR_STATE at once when nothing is queued, running or waiting to be collected, and DP_ERR_TIMEOUT after timeout_ms (0: no wait,
+// < 0: for ever).  Several threads may call it, and submit, at once: each result goes to exactly one caller.
+extern "C" int dph_zkml_stream_next(void *stream, int64_t timeout_ms, uint64_t *ticket, uint64_t *proof, uint64_t *proof_len, int64_t *output,
+                                    int32_t *status, char *msg, uint64_t msg_cap) {
+    DPH_TRY
+    if (!stream || !ticket || !proof || !proof_len || !output || !status) throw Error(DP_ERR_INVALID, "dph_zkml_stream_next: null argument");
+    ZkStream *s = (ZkStream *)stream;
+    dp::QueueResult r;
+    if (const int rc = s->q.next(timeout_ms, r, g_herr)) return rc;
+    const size_t ol = s->pool->h->model.output_len();
+    *ticket = r.ticket; *status = r.status; *proof_len = r.proof.size();
+    memcpy(proof, r.proof.data(), 8 * r.proof.size());
+    if (r.status) memset(output, 0, 8 * ol); else memcpy(output, r.output.data(), 8 * ol);
+    if (msg && msg_cap) snprintf(msg, msg_cap, "%s", r.error.c_str());
+    return 0;
+    DPH_CATCH
+}
+// Closes the stream: the jobs no worker has started are cancelled, never proved, and counted in *n_cancelled (optional); the running
+// jobs are waited for, uncollected results dropped, and the pool released.  A submit or next waiting on the stream returns
+// DP_ERR_STATE before close returns; no call may use the stream pointer after it.  dph_zkml_context_free on the handle closes an
+// open stream first, and the stream pointer is then invalid.
+extern "C" int dph_zkml_stream_close(void *stream, uint64_t *n_cancelled) {
+    if (!stream) { g_herr = "dph_zkml_stream_close: null stream"; return DP_ERR_INVALID; }
+    const uint64_t n = close_stream((ZkStream *)stream);
+    if (n_cancelled) *n_cancelled = n;
+    return 0;
 }
 
 // One proof sharded over `world` ranks: `mles` are THIS rank's slices (nv_total - log2(world) variables each).

@@ -33,6 +33,7 @@ extern "C" {
 #define DP_ERR_NO_DEVICE 3    /* no usable GPU / dp_init not called */
 #define DP_ERR_STATE 4        /* call out of protocol order ("Prover is not active", ...) */
 #define DP_ERR_UNSUPPORTED 5  /* e.g. product degree > 5 (sumcheck/src/prover.rs:710) */
+#define DP_ERR_TIMEOUT 6      /* a timed wait ran out (dph_zkml_stream_submit / dph_zkml_stream_next) */
 
 typedef struct dp_mle dp_mle; /* device-resident DenseMultilinearExtension */
 typedef struct dp_sc dp_sc;   /* IOPProverState (sumcheck/src/structs.rs:37-48) on device */
