@@ -604,9 +604,9 @@ class ZkmlContext:
 
     def _new(self, desc, data, input_len):
         d = np.ascontiguousarray(desc, dtype=np.int64).reshape(-1, 9)
-        w = np.ascontiguousarray(data, dtype=np.int64)
+        w = np.ascontiguousarray(data, dtype=np.int64).reshape(-1)
         self.h = C.c_void_p()
-        self.input_len = int(input_len)
+        self.desc, self.data, self.input_len = d, w, int(input_len)     # kept so that stacked() can derive the stacked model
         hcheck(host().dph_model_context_new(_ptr(d), d.shape[0], _ptr(w), int(input_len), C.byref(self.h)))
 
     def prove(self, x, label=b"m2vec"):
@@ -720,6 +720,11 @@ class ZkmlContext:
         hcheck(host().dph_zkml_infer_batch(self.h, _ptr(x), n, _ptr(outputs), _ptr(status), C.byref(sec)))
         errors = [None if status[j] == 0 else host().dph_zkml_job_error(self.h, j).decode() for j in range(n)]
         return sec.value, outputs, status, errors
+
+    def stacked(self, rows):
+        """A StackedContext that proves up to `rows` inputs of this model in one proof (models.stack_rows).  It is a model of its own,
+        set up and committed on its own handle; this context stays usable and screens the stacked proofs' inputs."""
+        return StackedContext(self, rows)
 
     def free(self):
         if self.h:
@@ -877,6 +882,70 @@ class ModelContext(ZkmlContext):
         x = self.metadata.quantize_input(x.reshape((-1,) + self.metadata.input_shape))
         _, outputs, status, errors = self.infer_batch(x)
         return outputs, self.metadata.dequantize_output(outputs), status, errors
+
+
+class StackedContext(ModelContext):
+    """Many inputs of one model in one proof: the base model's Dense layers as the reference's MatMul of an input matrix [R][K] by the
+    constant weight matrix (models.stack_rows), with R = p2(rows) and row r of the input matrix holding one input.  The proof is an
+    ordinary proof of that stacked model; its public output is the whole [R][output_len] matrix.  Made by ZkmlContext.stacked(rows);
+    keeps the base context, which screens inputs before they are proved.  rows, R, base_input_len, base_output_len and the base's
+    metadata (None unless made by ModelContext.from_onnx) are attributes."""
+
+    def __init__(self, base, rows):
+        import models
+        desc, data, input_len, R = models.stack_rows(base.desc, base.data, base.input_len, rows)
+        ModelContext.__init__(self, desc, data, input_len)
+        self.base, self.rows, self.R = base, int(rows), R
+        self.base_input_len, self.base_output_len = base.input_len, base.output_len
+        self.metadata = getattr(base, "metadata", None)
+
+    def prove_stacked(self, inputs, n_workers, device=0, label=b"m2vec", stride=None):
+        """Prove n inputs ([n, base_input_len] int64, each value in [-128, 127]), `rows` per proof.
+          1. Screen every input with the base context's infer_batch, on the calling thread (which, as for infer_batch, needs init()):
+             an input it fails keeps that status and message and is not proved, since one failing row would fail every input of its
+             proof.
+          2. Group the others in order, `rows` per proof; the last group is padded to R rows with copies of its last input (an input
+             that passed screening, so the padding cannot fail a lookup; a zero row's bias chain could).
+          3. Prove each group as one input of this model with prove_batch (its worker pool, stride, refusals and wait modes).
+        Returns (seconds, proofs[g], group_outputs [G, R * base_output_len] (the public output of proof g), outputs [n,
+        base_output_len] (zeros where the input failed), status[n], errors[n], proof_of[n] (-1 when screened out), row_of[n]).
+        seconds is the screening plus the proving time.  Should a proof fail after screening, every input of its group gets its
+        status and message."""
+        import models
+        x = np.ascontiguousarray(inputs, dtype=np.int64)
+        if x.ndim != 2 or x.shape[0] == 0 or x.shape[1] != self.base_input_len:
+            raise ValueError("prove_stacked: inputs must be [n >= 1, %d]" % self.base_input_len)
+        n, R, out_len = x.shape[0], self.R, self.base_output_len
+        sec, _, status, errors = self.base.infer_batch(x)
+        status, errors = status.copy(), list(errors)
+        ok = np.flatnonzero(status == 0)
+        groups = [ok[g: g + self.rows] for g in range(0, ok.size, self.rows)]
+        outputs = np.zeros((n, out_len), dtype=np.int64)
+        proof_of, row_of = np.full(n, -1, dtype=np.int64), np.full(n, -1, dtype=np.int64)
+        if not groups:
+            return sec, [], np.zeros((0, R * out_len), dtype=np.int64), outputs, status, errors, proof_of, row_of
+        stacked = np.stack([models.pad_rows(x[idx], R) for idx in groups])
+        prove_sec, proofs, group_outputs, gstatus, gerrors = self.prove_batch(stacked, n_workers, device, label, stride)
+        for g, idx in enumerate(groups):
+            proof_of[idx], row_of[idx] = g, np.arange(idx.size)
+            if gstatus[g] == 0:
+                outputs[idx] = group_outputs[g].reshape(R, out_len)[: idx.size]
+            else:
+                status[idx] = gstatus[g]
+                for j in idx:
+                    errors[j] = gerrors[g]
+        return sec + prove_sec, proofs, group_outputs, outputs, status, errors, proof_of, row_of
+
+    def prove_stacked_float(self, inputs, n_workers, device=0, label=b"m2vec", stride=None):
+        """prove_stacked on float inputs ([n, *input shape] in [-1, 1]) of a model made by from_onnx: quantises each input with the
+        base's metadata and returns (proofs, group_outputs, outputs, float_outputs, status, errors, proof_of, row_of), float_outputs
+        being each input's real output entries dequantised"""
+        if self.metadata is None:
+            raise ValueError("prove_stacked_float: the base context has no quantisation metadata (build it with ModelContext.from_onnx)")
+        x = np.asarray(inputs, dtype=np.float32)
+        x = self.metadata.quantize_input(x.reshape((-1,) + self.metadata.input_shape))
+        _, proofs, group_outputs, outputs, status, errors, proof_of, row_of = self.prove_stacked(x, n_workers, device, label, stride)
+        return proofs, group_outputs, outputs, self.metadata.dequantize_output(outputs), status, errors, proof_of, row_of
 
 
 def sumcheck_prove_batch_polys(T, mles, products, max_nv, label=b"m2vec"):

@@ -142,6 +142,56 @@ def covid(seed=1, img=224, channels=(32, 64, 64, 128, 128), fc=64, k=3):
     return np.asarray(desc, dtype=np.int64), np.concatenate(data).astype(np.int64), x.reshape(-1), n_params
 
 
+_KIND_NAMES = {DENSE: "Dense", REQUANT: "Requant", RELU: "ReLU", CONV: "Conv", POOL: "Maxpool2D", MATMUL: "MatMul"}
+
+
+def stack_rows(desc, data, input_len, rows):
+    """The model that proves `rows` inputs of (desc, data, input_len) at once, as the rows of one input matrix (the reference's MatMul
+    with OperandMatrix::Input x OperandMatrix::Weight, zkml/src/layers/matrix_mul.rs).  With R = p2(rows): a Dense {nrows, ncols}
+    becomes MatMul {R, ncols, nrows, TransposeB, bias} -- its [nrows][ncols] weights are the [C][K] right matrix and its bias the
+    MatMul bias, so `data` is returned unchanged -- and a MatMul {r, k, c, t, b} becomes {R*r, k, c, t, b}; Requant and ReLU work
+    element by element and stay.  Row r of the stacked input ([R][input_len], row-major) is input r in the base model's padded
+    layout, and row r of the stacked output ([R][output_len]) is that input's output.  Returns (desc', data, R * input_len, R).
+    Raises ValueError for rows < 1, a Conv or Maxpool2D node (the reference's Convolution takes one image), an unknown node kind,
+    or nodes whose shapes do not chain."""
+    d = np.asarray(desc, dtype=np.int64).reshape(-1, 9)
+    if int(rows) < 1:
+        raise ValueError("stack_rows: rows must be at least 1, got %d" % int(rows))
+    R = _p2(int(rows))
+    out = d.copy()
+    cur = int(input_len)                       # elements of one input row's tensor before node i
+    for i, row in enumerate(d):
+        kind = int(row[0])
+        name = _KIND_NAMES.get(kind, "kind %d" % kind)
+        if kind in (CONV, POOL):
+            raise ValueError("stack_rows: node %d (%s) does not stack: the reference's Convolution and Maxpool2D take one image" % (i, name))
+        if kind == DENSE:
+            nrows, ncols = int(row[1]), int(row[2])
+            if ncols != cur:
+                raise ValueError("stack_rows: node %d (%s) takes %d inputs but follows a tensor of %d" % (i, name, ncols, cur))
+            out[i] = [MATMUL, R, ncols, nrows, 1, 1, 0, 0, 0]
+            cur = nrows
+        elif kind == MATMUL:
+            r, k, c = int(row[1]), int(row[2]), int(row[3])
+            if r * k != cur:
+                raise ValueError("stack_rows: node %d (%s) takes a [%d][%d] matrix but follows a tensor of %d" % (i, name, r, k, cur))
+            out[i, 1] = R * r
+            cur = r * c
+        elif kind not in (REQUANT, RELU):
+            raise ValueError("stack_rows: node %d has an unknown kind (%s)" % (i, name))
+    return out, data, R * int(input_len), R
+
+
+def pad_rows(xs, R):
+    """The input of one stacked proof: m <= R inputs ([m, input_len]) as the first m rows of an [R][input_len] matrix, the rest filled
+    with copies of the last input, flattened row-major.  Copies, not zeros: an input that passed screening cannot fail a lookup,
+    while nothing keeps a zero row's outputs (the bias chain) inside the tables."""
+    xs = np.asarray(xs, dtype=np.int64)
+    if xs.ndim != 2 or not 1 <= xs.shape[0] <= R:
+        raise ValueError("pad_rows: expected [1..%d, input_len] inputs, got shape %s" % (R, xs.shape))
+    return np.concatenate([xs, np.repeat(xs[-1:], R - xs.shape[0], axis=0)]).reshape(-1)
+
+
 def token_mlp(seed=1, tokens=8, d_model=64, d_hidden=128, transposed=(False, True), bias=(True, False)):
     """A token-wise MLP as the transformer feed-forward block uses it (zkml/src/layers/matrix_mul.rs: OperandMatrix::Input x
     OperandMatrix::Weight): X [tokens, d_model] -> MatMul(W1 [d_model, d_hidden] or its transpose, + bias) -> requant -> relu
