@@ -241,6 +241,9 @@ int dp_infer_plan(const dp_infer_node *nodes, uint32_t n_nodes, uint64_t input_l
             } else {
                 const u64 kw = nd.dims[0], kx = nd.dims[1], nw = nd.dims[2], rn = nd.dims[3];
                 if (kx * nw * nw != cur.len || kw == 0 || rn == 0 || (nw & (nw - 1)) || cur.len > (u64)INT32_MAX) return plan_fail(id, name, "shape does not match its input");
+                // a filter wider than the image has taps (b >= nw) that the FFT convolution drops and this gather would wrap into the
+                // next row; the prover refuses such a layer (dp_pad_rows), so the plan does too
+                if (rn > nw) return plan_fail(id, name, "filter width " + std::to_string(rn) + " exceeds the padded image width " + std::to_string(nw));
                 const u64 P = nw * nw, T = kx * rn * rn;
                 // keep the taps (c, a, b) with a non-zero weight for some output channel
                 std::vector<u64> keep;

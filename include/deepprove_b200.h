@@ -323,7 +323,8 @@ int dp_wit_free(dp_wit *w);
  * nodes; each run takes host inputs and writes host outputs in the padded layout of the last node's output tensor.
  * The plan refuses (DP_ERR_INVALID, naming the node): a weight outside [-128, 127], a bias outside int32, a Dense / MatMul /
  * Convolution whose input is not 8-bit (not the model input nor a Requant output, optionally through Relu and/or Maxpool), an
- * output row or channel with 128 * sum|w| + |b| > 2^31 - 1 (int32 accumulation would not be exact), and shapes that do not chain. */
+ * output row or channel with 128 * sum|w| + |b| > 2^31 - 1 (int32 accumulation would not be exact), a Convolution filter wider than
+ * its padded image (real_nw > nw: the prover refuses it too), and shapes that do not chain. */
 typedef struct dp_infer dp_infer;
 typedef struct dp_infer_node {
     uint32_t kind;        /* the layer-descriptor kinds: 0 Dense, 1 Requant, 2 Relu, 3 Convolution, 4 Maxpool (2x2, stride 2), 5 MatMul */
