@@ -12,6 +12,7 @@
 #include <algorithm>
 
 // ---- fft(v, flag) on rows (tensor.rs:261-323): natural order in/out, w = get_root_of_unity(log n) (inverse when flag) ----
+constexpr u32 FFT_ROWS_MAX_LOG = 13;
 __global__ void __launch_bounds__(256) k_fft_rows(gle *data, u32 lg, int inverse, PowTab tab) {
     extern __shared__ unsigned char smem_raw[];
     gle *sm = reinterpret_cast<gle *>(smem_raw);
@@ -37,10 +38,14 @@ __global__ void __launch_bounds__(256) k_fft_rows(gle *data, u32 lg, int inverse
 extern "C" int dp_fft_rows(dp_mle *m, uint32_t log_n, int inverse) {
     DP_REQUIRE_CTX();
     DP_CHECK(m && m->is_ext, DP_ERR_INVALID, "dp_fft_rows: need an Ext MLE");
-    DP_CHECK(log_n >= 1 && log_n <= 13 && (m->len >> log_n) >= 1 && (m->len & ((1ULL << log_n) - 1)) == 0, DP_ERR_INVALID, "dp_fft_rows: row length must be 2^1..2^13 and divide the MLE length");
+    DP_CHECK(log_n >= 1 && log_n <= FFT_ROWS_MAX_LOG && (m->len >> log_n) >= 1 && (m->len & ((1ULL << log_n) - 1)) == 0, DP_ERR_INVALID,
+             "dp_fft_rows: row length must be 2^1..2^13 and divide the MLE length");
     PowTab tab; if (int e = dp_root_powtab(&tab)) return e;
     size_t smem = sizeof(gle) << log_n;
-    if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_fft_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // the largest request of any row length (2^13 values, 128 KB), never the call's own: proving threads transform rows of 2^12 and
+    // 2^13 concurrently, and lowering the function's limit under another thread's launch would refuse that launch
+    const int smem_max = (int)(sizeof(gle) << FFT_ROWS_MAX_LOG);
+    if (smem > 48 * 1024) DP_CUDA(cudaFuncSetAttribute(k_fft_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
     DpProfScope prof("k_fft_rows", m->bytes() * 2);
     DP_CUDA(dp_launch(k_fft_rows, (unsigned)(m->len >> log_n), 256, smem, dp_ctx().stream, (gle *)m->data, log_n, inverse, tab));
     return DP_OK;
