@@ -3,8 +3,13 @@ libdeepprove_host.so (C++ host mirror of the reference crates).  Plumbing for te
 a Rust host binds the same C ABI directly (INTEGRATION.md).  Never imports anything from oracle/.
 Fails loudly when the CUDA library is missing: there is no CPU fallback.
 """
+import collections
+import contextlib
 import ctypes as C
+import math
 import os
+import threading
+import time
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -589,6 +594,9 @@ class ZkmlContext:
     """Context::generate for n_layers x [Dense(width x width)+bias -> Requant -> ReLU]: weights, bias and lookup
     tables uploaded once and committed (setup).  rq: (n_layers, 4) int64 = right_shift, fp_scale,
     fixed_point_multiplier, intermediate_bit_size."""
+    _stream = None      # the open ProofStream on this handle
+    _holder = None      # the StackedStream that holds this handle (StackedStream._hold)
+    _calls = 0          # calls on this handle's pool in progress (_pool_call)
 
     def __init__(self, n_layers, width, weights, bias, rq):
         self.n_layers, self.width = n_layers, width
@@ -606,8 +614,23 @@ class ZkmlContext:
         d = np.ascontiguousarray(desc, dtype=np.int64).reshape(-1, 9)
         w = np.ascontiguousarray(data, dtype=np.int64).reshape(-1)
         self.h = C.c_void_p()
+        self._mu = threading.Lock()
         self.desc, self.data, self.input_len = d, w, int(input_len)     # kept so that stacked() can derive the stacked model
         hcheck(host().dph_model_context_new(_ptr(d), d.shape[0], _ptr(w), int(input_len), C.byref(self.h)))
+
+    @contextlib.contextmanager
+    def _pool_call(self, name):
+        """Brackets a call on the handle's worker pool: refused (DP_ERR_STATE) while a StackedStream holds the handle, and counted
+        while it runs, so that a StackedStream opened meanwhile finds the pool busy"""
+        with self._mu:
+            if self._holder is not None:
+                raise DpError(DP_ERR_STATE, "%s: the handle's worker pool is busy: an open stacked stream holds it" % name)
+            self._calls += 1
+        try:
+            yield
+        finally:
+            with self._mu:
+                self._calls -= 1
 
     def prove(self, x, label=b"m2vec"):
         """inference + Prover::prove + flat proof, from a host input vector (end to end)"""
@@ -632,8 +655,9 @@ class ZkmlContext:
         trace; e2e=True: inference + prove + serialised proof per job."""
         sec, n = C.c_double(), C.c_uint64()
         out = _ptr(self._out) if want_proof else None
-        hcheck(host().dph_zkml_prove_concurrent(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
-                                                out, self._out.size, C.byref(n)))
+        with self._pool_call("prove_concurrent"):
+            hcheck(host().dph_zkml_prove_concurrent(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
+                                                    out, self._out.size, C.byref(n)))
         return (sec.value, self._out[: n.value].copy()) if want_proof else sec.value
 
     def prove_concurrent_all(self, n_workers, n_proofs, stride, device=0, e2e=False, label=b"m2vec"):
@@ -643,8 +667,9 @@ class ZkmlContext:
         lens = np.zeros(int(n_proofs), dtype=np.uint64)
         workers = np.zeros(int(n_proofs), dtype=np.uint32)
         sec = C.c_double()
-        hcheck(host().dph_zkml_prove_concurrent_all(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
-                                                    _ptr(out), int(stride), _ptr(lens), _ptr(workers)))
+        with self._pool_call("prove_concurrent_all"):
+            hcheck(host().dph_zkml_prove_concurrent_all(self.h, int(device), int(n_workers), int(n_proofs), int(bool(e2e)), label, C.byref(sec),
+                                                        _ptr(out), int(stride), _ptr(lens), _ptr(workers)))
         out = out.reshape(int(n_proofs), int(stride))
         return sec.value, [out[j, : int(lens[j])] for j in range(int(n_proofs))], workers
 
@@ -671,16 +696,17 @@ class ZkmlContext:
         if x.ndim != 2 or x.shape[0] == 0 or x.shape[1] != self.input_len:
             raise ValueError("prove_batch: inputs must be [n >= 1, %d]" % self.input_len)
         n = x.shape[0]
-        if stride is None:
-            stride = self._default_stride(x[0], device, label)
-        proofs = np.zeros((n, int(stride)), dtype=np.uint64)
-        lens = np.zeros(n, dtype=np.uint64)
-        outputs = np.zeros((n, self.output_len), dtype=np.int64)
-        status = np.zeros(n, dtype=np.int32)
-        sec = C.c_double()
-        hcheck(host().dph_zkml_prove_batch(self.h, int(device), int(n_workers), _ptr(x), n, label, _ptr(proofs), int(stride), _ptr(lens),
-                                           _ptr(outputs), _ptr(status), C.byref(sec)))
-        errors = [None if status[j] == 0 else host().dph_zkml_job_error(self.h, j).decode() for j in range(n)]
+        with self._pool_call("prove_batch"):
+            if stride is None:
+                stride = self._default_stride(x[0], device, label)
+            proofs = np.zeros((n, int(stride)), dtype=np.uint64)
+            lens = np.zeros(n, dtype=np.uint64)
+            outputs = np.zeros((n, self.output_len), dtype=np.int64)
+            status = np.zeros(n, dtype=np.int32)
+            sec = C.c_double()
+            hcheck(host().dph_zkml_prove_batch(self.h, int(device), int(n_workers), _ptr(x), n, label, _ptr(proofs), int(stride), _ptr(lens),
+                                               _ptr(outputs), _ptr(status), C.byref(sec)))
+            errors = [None if status[j] == 0 else host().dph_zkml_job_error(self.h, j).decode() for j in range(n)]
         return sec.value, [proofs[j, : int(lens[j])] for j in range(n)], outputs, status, errors
 
     def _default_stride(self, x, device, label):
@@ -702,14 +728,20 @@ class ZkmlContext:
         when its proof finishes.  The pool is held until the stream closes.  stride: the longest proof a job may return (default:
         prove_batch's, which proves one all-zero input the first time); capacity: jobs submitted and not yet collected (default
         4 * n_workers)."""
-        if stride is None:
-            stride = self._default_stride(np.zeros(self.input_len, dtype=np.int64), device, label)
-        return ProofStream(self, n_workers, device, label, stride, 4 * int(n_workers) if capacity is None else capacity)
+        with self._pool_call("open_stream"):
+            if stride is None:
+                stride = self._default_stride(np.zeros(self.input_len, dtype=np.int64), device, label)
+            return ProofStream(self, n_workers, device, label, stride, 4 * int(n_workers) if capacity is None else capacity)
 
     def infer_batch(self, inputs):
         """The model's outputs for n inputs ([n, input_len] int64, each value in [-128, 127]) without proving, on the int8 tensor
         cores (dph_zkml_infer_batch): the same outputs and per-input failures as prove_batch.  Returns (seconds, outputs [n,
         output_len] int64, status, errors)."""
+        with self._pool_call("infer_batch"):
+            return self._infer_batch(inputs)
+
+    def _infer_batch(self, inputs):
+        """infer_batch without the _pool_call bracket: the screening of the StackedStream that holds this handle"""
         x = np.ascontiguousarray(inputs, dtype=np.int64)
         if x.ndim != 2 or x.shape[0] == 0 or x.shape[1] != self.input_len:
             raise ValueError("infer_batch: inputs must be [n >= 1, %d]" % self.input_len)
@@ -728,6 +760,8 @@ class ZkmlContext:
 
     def free(self):
         if self.h:
+            if self._holder is not None:                       # a stacked stream proving on this handle or screening on it
+                self._holder.close()
             if getattr(self, "_stream", None) is not None:     # dph_zkml_context_free closes it
                 self._stream.h, self._stream = C.c_void_p(), None
             host().dph_zkml_context_free(self.h)
@@ -764,9 +798,10 @@ class ProofStream:
     Each job is what prove_batch does for one input, except that a proof longer than the stride fails that job alone.  Made by
     ZkmlContext.open_stream; a context manager.  submit and next may be called from different threads at once."""
 
-    def __init__(self, ctx, n_workers, device, label, stride, capacity):
+    def __init__(self, ctx, n_workers, device, label, stride, capacity, dequantize=True):
         self.ctx, self.stride, self.capacity = ctx, int(stride), int(capacity)
         self._output_len = ctx.output_len
+        self._metadata = getattr(ctx, "metadata", None) if dequantize else None
         self.h = C.c_void_p()
         hcheck(host().dph_zkml_stream_open(ctx.h, int(device), int(n_workers), label, self.stride, self.capacity, C.byref(self.h)))
         ctx._stream = self
@@ -810,7 +845,7 @@ class ProofStream:
         msg = C.create_string_buffer(1024)
         self._check(host().dph_zkml_stream_next(self.h, _ms(timeout), C.byref(ticket), _ptr(proof), C.byref(plen), _ptr(out), C.byref(st),
                                                 C.cast(msg, C.c_void_p), len(msg)))
-        md = getattr(self.ctx, "metadata", None)
+        md = self._metadata
         return StreamResult(ticket.value, proof[: plen.value].copy(), out, st.value, msg.value.decode() if st.value else None,
                             None if md is None else md.dequantize_output(out))
 
@@ -834,6 +869,258 @@ class ProofStream:
         hcheck(host().dph_zkml_stream_close(self.h, C.byref(n)))
         self.h, self.ctx._stream = C.c_void_p(), None
         return n.value
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+class StackedResult:
+    """One input's result from a StackedStream: ticket; proof (the flat proof of its group, one array shared by every input of that
+    proof; empty when screened out or failed); public_output (that proof's [R][base_output_len] output matrix, padding rows included,
+    shared likewise; [0][base_output_len] when screened out); proof_id (-1 when screened out); row (its row in the proof, or -1);
+    output (its row of public_output; zeros when it failed); status (0 or its error code); error (None or its message); output_float
+    (the dequantised real output entries for a model made by ModelContext.from_onnx, else None)."""
+    __slots__ = ("ticket", "proof", "public_output", "proof_id", "row", "output", "status", "error", "output_float")
+
+    def __init__(self, ticket, proof, public_output, proof_id, row, output, status, error, output_float):
+        self.ticket, self.proof, self.public_output, self.proof_id, self.row = ticket, proof, public_output, proof_id, row
+        self.output, self.status, self.error, self.output_float = output, status, error, output_float
+
+
+class StackedStream:
+    """Arriving inputs grouped into stacked proofs.  Made by StackedContext.open_stream; a context manager.  submit and next may be
+    called from several threads at once, and each result goes to exactly one next.
+
+    One grouping thread closes a group when `rows` inputs are pending, or when the oldest pending input has waited max_wait seconds.
+    It screens the group's inputs in one screen() call (infer_batch: (seconds, outputs, status, errors)); an input that fails gets its
+    result at once, with that status and message.  The survivors, in submission order, are padded to R rows with copies of the last
+    (models.pad_rows) and submitted to the prover (a ProofStream of the stacked model) as one job; a group is never topped up from
+    later arrivals.  open_prover(x) returns that prover; it is called once, with the first group's padded input.  A collector thread
+    takes each finished job and gives every input of its group its own result.  The class touches no device itself, so that tests
+    can drive it with a fake screener and prover.  screen_calls and screen_seconds count the groups screened and the seconds screen()
+    reported for them."""
+    POLL_S = 0.05       # the collector's longest wait inside the prover's next before it looks whether the stream is closing
+
+    def __init__(self, rows, R, input_len, output_len, n_workers, max_wait, capacity, screen, open_prover, metadata=None, thread_init=None):
+        import models
+        self.rows, self.R, self.input_len, self.output_len = int(rows), int(R), int(input_len), int(output_len)
+        self.max_wait, self.capacity = float(max_wait), (4 * int(n_workers) * int(rows) if capacity is None else int(capacity))
+        if int(n_workers) < 1:
+            raise ValueError("open_stream: n_workers must be >= 1")
+        if not (math.isfinite(self.max_wait) and self.max_wait >= 0):
+            raise ValueError("open_stream: max_wait must be a finite number of seconds >= 0")
+        if self.capacity < self.rows:
+            raise ValueError("open_stream: capacity (%d) must be at least rows (%d)" % (self.capacity, self.rows))
+        self._screen, self._open_prover, self._pad, self._metadata, self._thread_init = screen, open_prover, models.pad_rows, metadata, thread_init
+        self._prover = None
+        self._cv = threading.Condition()
+        self._pending = collections.deque()      # (ticket, input, arrival time), not yet in a group
+        self._ready = collections.deque()        # results not yet collected by next
+        self._groups = {}                        # proof_id -> tickets of the group's survivors, while its proof is out
+        self._next_ticket = self._uncollected = self._next_proof = self._cancelled = self._jobs = 0     # _jobs: submitted, uncollected
+        self._closed = False
+        self._holds = ()
+        self.screen_calls, self.screen_seconds = 0, 0.0
+        self._threads = [threading.Thread(target=f, daemon=True) for f in (self._group_loop, self._collect_loop)]
+        for t in self._threads:
+            t.start()
+
+    def _hold(self, ctxs):
+        """Reserves the handles for this stream: refused (DP_ERR_STATE) when a call or a stream is on any of their pools"""
+        for c in ctxs:
+            c._mu.acquire()
+        try:
+            for c in ctxs:
+                if c._holder is not None or c._stream is not None or c._calls:
+                    raise DpError(DP_ERR_STATE, "open_stream: the handle's worker pool is busy with another call or stream")
+            for c in ctxs:
+                c._holder = self
+            self._holds = tuple(ctxs)
+        finally:
+            for c in ctxs:
+                c._mu.release()
+
+    # ---- the grouping thread ----
+    def _group_loop(self):
+        while True:
+            with self._cv:
+                while len(self._pending) < self.rows:
+                    if self._closed:
+                        return
+                    left = None if not self._pending else self._pending[0][2] + self.max_wait - time.monotonic()
+                    if left is not None and left <= 0:
+                        break
+                    self._cv.wait(left)
+                if self._closed:
+                    return
+                take = [self._pending.popleft() for _ in range(min(self.rows, len(self._pending)))]
+            self._run_group(np.array([t[0] for t in take], dtype=np.uint64), np.stack([t[1] for t in take]))
+
+    def _run_group(self, tickets, x):
+        n = len(tickets)
+        try:
+            if self._thread_init is not None:
+                self._thread_init()
+                self._thread_init = None
+            sec, _, status, errors = self._screen(x)
+            self.screen_calls += 1
+            self.screen_seconds += sec
+        except Exception as e:                   # a call-level failure fails the whole group
+            status, errors = np.full(n, getattr(e, "code", DP_ERR_INVALID)), [str(e)] * n
+        ok = np.flatnonzero(np.asarray(status) == 0)
+        self._post([self._result(tickets[j], -1, -1, None, None, int(status[j]), errors[j]) for j in range(n) if status[j] != 0])
+        if ok.size == 0:
+            return
+        padded = self._pad(x[ok], self.R)
+        with self._cv:
+            if self._closed:
+                self._cancelled += ok.size
+                return
+            pid = self._next_proof                    # the prover's tickets count up from 0 as groups are submitted: ticket == proof_id
+            self._groups[pid] = tickets[ok]
+            self._next_proof += 1
+        try:
+            if self._prover is None:
+                self._prover = self._open_prover(padded)
+            self._prover.submit(padded)
+        except Exception as e:
+            with self._cv:
+                del self._groups[pid]
+                self._next_proof -= 1
+            code = getattr(e, "code", DP_ERR_INVALID)
+            self._post([self._result(t, -1, -1, None, None, code, str(e)) for t in tickets[ok]])
+            return
+        with self._cv:
+            self._jobs += 1
+            self._cv.notify_all()
+
+    # ---- the collector thread ----
+    def _collect_loop(self):
+        while True:
+            with self._cv:
+                self._cv.wait_for(lambda: self._closed or self._jobs > 0)
+                if self._closed:                      # close() closes the prover once this thread is out of its next
+                    return
+            try:
+                r = self._prover.next(self.POLL_S)
+            except StreamTimeout:
+                continue
+            except Exception as e:                    # the prover failed as a whole: fail every group still out, and stop
+                with self._cv:
+                    lost, self._groups, self._jobs = self._groups, {}, 0
+                self._post([self._result(t, -1, -1, None, None, getattr(e, "code", DP_ERR_INVALID), str(e))
+                            for ts in lost.values() for t in ts])
+                return
+            with self._cv:
+                tickets = self._groups.pop(int(r.ticket))
+                self._jobs -= 1
+            public = r.output.reshape(self.R, self.output_len)
+            self._post([self._result(t, int(r.ticket), row, r.proof, public, r.status, r.error) for row, t in enumerate(tickets)])
+
+    def _result(self, ticket, proof_id, row, proof, public, status, error):
+        if proof is None:
+            proof, public = np.zeros(0, dtype=np.uint64), np.zeros((0, self.output_len), dtype=np.int64)
+        out = public[row] if row >= 0 else np.zeros(self.output_len, dtype=np.int64)
+        return StackedResult(int(ticket), proof, public, proof_id, row, out, int(status), error if status else None,
+                             None if self._metadata is None else self._metadata.dequantize_output(out))
+
+    def _post(self, results):
+        if results:
+            with self._cv:
+                self._ready.extend(results)
+                self._cv.notify_all()
+
+    # ---- the caller's side ----
+    def _wait(self, deadline, what):
+        left = None if deadline is None else deadline - time.monotonic()
+        if left is not None and left <= 0:
+            raise StreamTimeout(DP_ERR_TIMEOUT, what)
+        self._cv.wait(left)
+
+    def submit(self, inputs, timeout=None):
+        """Queue inputs ([n, base_input_len] int64, or one [base_input_len]); all or nothing.  Waits up to `timeout` seconds (None: for
+        ever, 0: not at all) for room in the capacity (inputs submitted and not yet collected), else raises StreamTimeout; n > capacity
+        is DP_ERR_INVALID.  Returns their tickets (uint64, consecutive, counted from 0 across the stream)."""
+        x = np.array(inputs, dtype=np.int64)     # a copy: the caller may reuse its buffer at once
+        x = x[None] if x.ndim == 1 else x
+        if x.ndim != 2 or x.shape[0] == 0 or x.shape[1] != self.input_len:
+            raise ValueError("submit: inputs must be [n >= 1, %d]" % self.input_len)
+        n = x.shape[0]
+        if n > self.capacity:
+            raise DpError(DP_ERR_INVALID, "submit: %d inputs exceed the stream's capacity of %d" % (n, self.capacity))
+        deadline = None if timeout is None else time.monotonic() + max(0.0, float(timeout))
+        with self._cv:
+            while self._uncollected + n > self.capacity and not self._closed:
+                self._wait(deadline, "submit: no room for %d inputs before the timeout" % n)
+            if self._closed:
+                raise DpError(DP_ERR_STATE, "the stream is closed")
+            first = self._next_ticket
+            self._next_ticket += n
+            self._uncollected += n
+            now = time.monotonic()
+            self._pending.extend((first + j, x[j], now) for j in range(n))
+            self._cv.notify_all()
+        return np.arange(first, first + n, dtype=np.uint64)
+
+    def submit_float(self, inputs, timeout=None):
+        """submit on float inputs ([n, *input shape] or one [*input shape], in [-1, 1]) of a model made by ModelContext.from_onnx,
+        quantised with the base's metadata as prove_stacked_float does"""
+        if self._metadata is None:
+            raise ValueError("submit_float: the base context has no quantisation metadata (build it with ModelContext.from_onnx)")
+        return self.submit(self._metadata.quantize_input(np.asarray(inputs, dtype=np.float32)), timeout)
+
+    def next(self, timeout=None):
+        """One input's StackedResult, in completion order.  Raises StreamTimeout when none is ready within `timeout` seconds (None: for
+        ever), and DpError DP_ERR_STATE at once when nothing submitted is left to collect."""
+        deadline = None if timeout is None else time.monotonic() + max(0.0, float(timeout))
+        with self._cv:
+            while not self._ready:
+                if self._closed:
+                    raise DpError(DP_ERR_STATE, "the stream is closed")
+                if self._uncollected == 0:
+                    raise DpError(DP_ERR_STATE, "next: nothing submitted is left to collect")
+                self._wait(deadline, "next: no result before the timeout")
+            self._uncollected -= 1
+            self._cv.notify_all()
+            return self._ready.popleft()
+
+    def results(self, timeout=None):
+        """Yields results until everything submitted so far has been collected"""
+        while True:
+            try:
+                r = self.next(timeout)
+            except DpError as e:
+                if e.code == DP_ERR_STATE:
+                    return
+                raise
+            yield r
+
+    def close(self):
+        """Cancel the inputs not yet in a submitted group and the groups no worker has started, wait for the running proofs, drop the
+        uncollected results and release both handles.  Returns the number of inputs cancelled (0 when already closed)."""
+        with self._cv:
+            if self._closed:
+                return 0
+            self._closed = True
+            cancelled = len(self._pending)
+            self._pending.clear()
+            self._cv.notify_all()
+        for t in self._threads:
+            t.join()
+        if self._prover is not None:
+            n_jobs = self._prover.close()             # the prover starts jobs in ticket order: the cancelled ones are the last
+            ids = sorted(self._groups)
+            cancelled += sum(self._groups[i].size for i in ids[len(ids) - n_jobs:]) if n_jobs else 0
+        self._ready.clear()
+        self._groups.clear()
+        for c in self._holds:
+            with c._mu:
+                if c._holder is self:
+                    c._holder = None
+        return cancelled + self._cancelled
 
     def __enter__(self):
         return self
@@ -946,6 +1233,28 @@ class StackedContext(ModelContext):
         x = self.metadata.quantize_input(x.reshape((-1,) + self.metadata.input_shape))
         _, proofs, group_outputs, outputs, status, errors, proof_of, row_of = self.prove_stacked(x, n_workers, device, label, stride)
         return proofs, group_outputs, outputs, self.metadata.dequantize_output(outputs), status, errors, proof_of, row_of
+
+    def open_stream(self, n_workers, max_wait, device=0, label=b"m2vec", stride=None, capacity=None):
+        """A StackedStream: inputs submitted one by one are grouped, up to `rows` per proof, and proved as prove_stacked proves a group,
+        on a ProofStream of this handle with n_workers workers.  A group closes when `rows` inputs are pending or when its oldest input
+        has waited max_wait seconds.  Both handles are held until the stream closes: this handle's pool proves for it and the base
+        context screens for it, so calls on either pool are refused (DP_ERR_STATE) meanwhile.  stride: the longest proof a job may
+        return; by default the proof length this context measured before, else that of the first group's proof, measured on that
+        group (screened and copy-padded) before its job is submitted.  capacity: inputs submitted and not yet collected (default 4 *
+        n_workers * rows).  The calling thread needs no device; the grouping thread calls init(device) itself."""
+        def open_prover(x):
+            words = stride if stride is not None else self._default_stride(x, device, label)
+            return ProofStream(self, n_workers, device, label, words, s.capacity, dequantize=False)   # metadata is the base's
+        s = StackedStream(self.rows, self.R, self.base_input_len, self.base_output_len, n_workers, max_wait, capacity,
+                          self.base._infer_batch, open_prover, self.metadata, lambda: init(device))
+        try:
+            s._hold((self.base, self))
+            if stride is not None or getattr(self, "_proof_words", None) is not None:
+                s._prover = open_prover(None)          # the stride is known: open now, so that a busy pool refuses the open itself
+        except BaseException:
+            s.close()
+            raise
+        return s
 
 
 def sumcheck_prove_batch_polys(T, mles, products, max_nv, label=b"m2vec"):
